@@ -4,8 +4,8 @@ import numpy as np
 # float tolerance of the parity contract (BASELINE.json north_star: "within 1e-5
 # relative float tolerance"; SURVEY.md 0.3 shows it can only be norm-wise because
 # two builds of the reference itself differ by 2e-4 element-wise on stop-band
-# outputs).  Norm-wise: max|d| <= RTOL * max|ref|.  Element-wise:
-# |d| <= RTOL*|ref| + RTOL*max|ref|.
+# outputs): max|d| <= RTOL * max|ref| over a client's stream.  Bit-exact checks on
+# stimuli that every summation order reproduces live in tests/exact.py.
 RTOL = 1e-5
 
 
@@ -46,9 +46,6 @@ def assert_cf32_close(got, ref, what=""):
     worst = int(np.argmax(d))
     assert d.max() <= RTOL * scale, (f"{what}: norm-wise error {d.max() / scale:.3e} > {RTOL} at k={worst} "
                                      f"(got {got[worst]}, ref {ref[worst]})")
-    bound = RTOL * np.abs(ref) + RTOL * scale
-    bad = np.nonzero(d > bound)[0]
-    assert bad.size == 0, f"{what}: {bad.size} outputs beyond element-wise bound, first k={bad[0]}"
     return float(d.max() / scale)
 
 
