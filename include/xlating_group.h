@@ -96,6 +96,19 @@ typedef struct {
  * state == NULL is xlg_add_client (a fresh filter: hist = taps_len-1 zeros, oscillator 1+0i). */
 int xlg_add_client_ex(xlg_group *g, uint32_t decimation, const float *taps, size_t taps_len, int32_t center_freq,
                       const xlg_client_state *state, int *client_id);
+/* Attach a client at the rational rate fs * interp / decim.  It is exactly the reference filter
+ * create_frequency_xlating_filter(decim, taps, taps_len, center_freq, interp * fs, ...) fed the
+ * zero-stuffed stream u[interp * n] = x[n], u[m] = 0 for every m not divisible by interp: taps,
+ * oscillator increment and renormalisation are those of a filter at interp * fs, and its history,
+ * window starts and output counts are in upsampled samples.  Taps are designed at interp * fs with
+ * gain interp.  Every output k sums only the ceil(taps_len / interp) taps that meet nonzero samples
+ * (one polyphase branch), never a stuffed zero.  interp == 1 is xlg_add_client(g, decim, ...).
+ * -EINVAL (logged) unless interp, decim >= 1, interp * fs <= UINT32_MAX and
+ * interp * max_input_len / 2 < 2^31.  A group with a rational client refuses XLG_PATH_Q15 submits
+ * (-ENOTSUP, nothing enqueued).  With XLG_TRACK_STATE, the hist of a rational client is in
+ * upsampled samples. */
+int xlg_add_client_rational(xlg_group *g, uint32_t interp, uint32_t decim, const float *taps, size_t taps_len,
+                            int32_t center_freq, int *client_id);
 int xlg_remove_client(xlg_group *g, int client_id);
 /* Size the per-ticket result arenas (device and pinned host) for `output_samples_per_block` complex output
  * samples per block summed over all clients (a client at decimation D produces about max_input_len/2/D + 2).
@@ -178,8 +191,21 @@ typedef struct {
 int xlg_profile_enable(xlg_group *g, int on);
 int xlg_profile_read(xlg_group *g, xlg_profile *p, int reset);
 
-/* Introspection for tests: history length (src/xlating.c:29 history_offset) and
- * which kernel currently serves the client (0 = generic, 1 = tiled, 2 = long-filter split-K). */
+/* Kernels of rational clients (xlg_add_client_rational), counted like xlg_profile's while profiling
+ * is enabled.  xlg_profile's algo_macs counts n_out * ceil(taps_len / interp) for them. */
+typedef struct {
+  double fir_poly_tile_ms;    /* tiled classes: the tiled FIR over their polyphase branches + the placement */
+  double fir_poly_generic_ms; /* polyphase generic FIR kernel */
+  uint64_t fir_poly_tile_launches, fir_poly_generic_launches;
+  uint64_t poly_macs;         /* complex MACs of rational clients: sum n_out * ceil(taps_len / interp) */
+} xlg_poly_profile;
+int xlg_poly_profile_read(xlg_group *g, xlg_poly_profile *p, int reset);
+
+/* Introspection for tests: history length (src/xlating.c:29 history_offset; upsampled samples for a
+ * rational client) and which kernel currently serves the client (0 = generic, 1 = tiled,
+ * 2 = long-filter split-K, 3 = rational, polyphase generic, 4 = rational, tiled: at least 8 clients with
+ * identical (interp, decim, taps_len, window alignment), gcd(interp, decim) = 1, whose branches fit the tiled
+ * kernel's shared memory). */
 int xlg_client_info(const xlg_group *g, int client_id, size_t *history, int *kernel_kind);
 
 /* Counters of the per-filter drop-in ABI (include/xlating.h) on `device`: process_*

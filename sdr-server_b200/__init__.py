@@ -21,6 +21,7 @@ The directory name contains a hyphen; import it with
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 import subprocess
 
@@ -51,7 +52,7 @@ REFERENCE_SYMBOLS = (
 GROUP_SYMBOLS = [
     "xlg_create", "xlg_create_ex", "xlg_destroy", "xlg_add_client", "xlg_add_client_ex", "xlg_remove_client", "xlg_reserve", "xlg_client_count", "xlg_submit",
     "xlg_wait", "xlg_input_consumed", "xlg_output", "xlg_read_output", "xlg_copy_output", "xlg_alloc_pinned", "xlg_free_pinned", "xlg_wait_stream", "xlg_partition_active", "xlg_timer_start",
-    "xlg_timer_stop", "xlg_profile_enable", "xlg_profile_read", "xlg_client_info", "xlg_dropin_stats", "xlg_dropin_stream_stats", "xlg_dropin_stream_times",
+    "xlg_timer_stop", "xlg_profile_enable", "xlg_profile_read", "xlg_client_info", "xlg_add_client_rational", "xlg_poly_profile_read", "xlg_dropin_stats", "xlg_dropin_stream_stats", "xlg_dropin_stream_times",
 ]
 
 
@@ -63,6 +64,12 @@ class XlgProfile(C.Structure):
                 ("in_samples", C.c_uint64), ("tile_macs", C.c_uint64), ("algo_macs", C.c_uint64),
                 ("fir_long_ms", C.c_double), ("fir_long_launches", C.c_uint64),
                 ("host_submit_ms", C.c_double), ("host_wait_ms", C.c_double), ("submits", C.c_uint64)]
+
+
+class XlgPolyProfile(C.Structure):
+    _fields_ = [("fir_poly_tile_ms", C.c_double), ("fir_poly_generic_ms", C.c_double),
+                ("fir_poly_tile_launches", C.c_uint64), ("fir_poly_generic_launches", C.c_uint64),
+                ("poly_macs", C.c_uint64)]
 
 
 def build(verbose: bool = False) -> None:
@@ -104,6 +111,12 @@ def lib() -> C.CDLL:
     L.xlg_destroy.restype = None
     L.xlg_add_client.argtypes = [vp, u32, C.POINTER(C.c_float), sz, i32, C.POINTER(C.c_int)]
     L.xlg_add_client.restype = C.c_int
+    L.xlg_add_client_rational.argtypes = [vp, u32, u32, C.POINTER(C.c_float), sz, i32, C.POINTER(C.c_int)]
+    L.xlg_add_client_rational.restype = C.c_int
+    L.xlg_poly_profile_read.argtypes = [vp, C.POINTER(XlgPolyProfile), C.c_int]
+    L.xlg_poly_profile_read.restype = C.c_int
+    L.xl_poly_pack.argtypes = [C.POINTER(C.c_float), sz, u32, C.POINTER(C.c_float)]
+    L.xl_poly_pack.restype = None
     L.xlg_reserve.argtypes = [vp, sz]
     L.xlg_reserve.restype = C.c_int
     L.xlg_remove_client.argtypes = [vp, C.c_int]
@@ -268,6 +281,17 @@ class Group:
             raise ValueError(code)
         return cid.value
 
+    def add_client_rational(self, interp: int, decim: int, taps, center_freq: int) -> int:
+        """A client at fs * interp / decim: the reference filter at interp * fs fed the zero-stuffed
+        stream (include/xlating_group.h, xlg_add_client_rational)."""
+        taps = np.ascontiguousarray(taps, dtype=np.float32)
+        cid = C.c_int(-1)
+        code = self._L.xlg_add_client_rational(self._h, interp, decim, taps.ctypes.data_as(C.POINTER(C.c_float)),
+                                               len(taps), center_freq, C.byref(cid))
+        if code != 0:
+            raise ValueError(code)
+        return cid.value
+
     def remove_client(self, cid: int) -> None:
         code = self._L.xlg_remove_client(self._h, cid)
         if code != 0:
@@ -372,6 +396,11 @@ class Group:
         self._L.xlg_profile_read(self._h, C.byref(p), 1 if reset else 0)
         return {k: getattr(p, k) for k, _ in XlgProfile._fields_}
 
+    def poly_profile_read(self, reset: bool = True) -> dict:
+        p = XlgPolyProfile()
+        self._L.xlg_poly_profile_read(self._h, C.byref(p), 1 if reset else 0)
+        return {k: getattr(p, k) for k, _ in XlgPolyProfile._fields_}
+
     def close(self):
         if self._h:
             self._L.xlg_destroy(self._h)
@@ -425,6 +454,31 @@ def client_plan(fs: int, rates, tw=None):
             center = -312000 if fs > 700000 else -fs // 4
         plan.append({"rate": rate, "decimation": fs // rate, "center": center,
                      "cutoff": rate // 2, "tw": tw if tw is not None else rate // 5})
+    return plan
+
+
+def poly_pack(rev, interp: int) -> np.ndarray:
+    """The library's polyphase packer (csrc/taps_host.c): reversed complex taps -> branch-major
+    (interp, ceil(T / interp)) complex64 array, zero-padded."""
+    rev = np.ascontiguousarray(rev, dtype=np.complex64)
+    T = rev.size
+    Tb = -(-T // interp)
+    out = np.zeros(interp * Tb, dtype=np.complex64)
+    fp = C.POINTER(C.c_float)
+    lib().xl_poly_pack(rev.ctypes.data_as(fp), T, interp, out.ctypes.data_as(fp))
+    return out.reshape(interp, Tb)
+
+
+def rational_plan(fs: int, rates, lpf_cutoff_rate: int = 5):
+    """Clients at any rate: rate / fs reduced to interp / decim, taps designed at interp * fs with gain
+    interp (so every polyphase branch has unit DC gain), cutoff rate / 2 and transition width
+    rate / lpf_cutoff_rate.  Centres as client_plan places them."""
+    plan = []
+    for p, rate in zip(client_plan(fs, rates), rates):
+        g = math.gcd(int(rate), int(fs))
+        L, M = int(rate) // g, int(fs) // g
+        taps = create_low_pass_filter(float(L), L * fs, int(rate) // 2, int(rate) // lpf_cutoff_rate)
+        plan.append({"rate": rate, "interp": L, "decim": M, "center": p["center"], "taps": taps})
     return plan
 
 

@@ -70,6 +70,17 @@ void xl_client_consts_free(xl_client_consts *c) {
   c->rev_q15 = NULL;
 }
 
+void xl_poly_pack(const float *rev_cf32, size_t taps_len, uint32_t interp, float *out) {
+  const size_t L = interp, Tb = (taps_len + L - 1) / L;
+  for (size_t r = 0; r < L; r++)
+    for (size_t t = 0; t < Tb; t++) {
+      const size_t j = r + t * L;
+      float *slot = out + 2 * (r * Tb + t);
+      slot[0] = j < taps_len ? rev_cf32[2 * j] : 0.0f;
+      slot[1] = j < taps_len ? rev_cf32[2 * j + 1] : 0.0f;
+    }
+}
+
 void xl_osc_chain_cf32(float *phase_re, float *phase_im, float incr_re, float incr_im, float *table, int n_out) {
   float pr = *phase_re, pi = *phase_im;
   for (int k = 0; k < n_out; k++) {

@@ -25,6 +25,12 @@ int xl_client_consts_build(const float *lpf_taps, size_t taps_len, uint32_t deci
                            int32_t center_freq, uint32_t sampling_freq, xl_client_consts *out);
 void xl_client_consts_free(xl_client_consts *c);
 
+/* Polyphase branches of a rational (L/M) client, branch-major: for r < L and t < Tb = ceil(T/L),
+ * out[r][t] = rev[r + t*L] ((re, im) interleaved), zero where r + t*L >= T.  Branch r holds the
+ * taps that meet the nonzero samples of a zero-stuffed window whose start is -r mod L.
+ * `out` has room for 2*L*Tb floats. */
+void xl_poly_pack(const float *rev_cf32, size_t taps_len, uint32_t interp, float *out);
+
 /* The float oscillator of one call on the host (src/xlating.c:70-73): n_out steps of
  * phase *= incr starting from *phase, the phase of every EVEN output k stored as
  * (re, im) at table[k] / table[k + 1], then -- if n_out > 0 -- the once-per-call

@@ -36,6 +36,7 @@
 #include <chrono>
 #include <map>
 #include <mutex>
+#include <numeric>
 #include <tuple>
 #include <array>
 #include <cstdint>
@@ -69,12 +70,13 @@ constexpr int kSmSmem = 228 * 1024;
 struct HostClient {
   bool active = false;
   uint32_t D = 0;
+  uint32_t L = 1;                // interpolation of a rational client (xlg_add_client_rational)
   size_t T = 0;
-  std::vector<float> rev;        // 2*T
+  std::vector<float> rev;        // 2*T; a rational client's polyphase branches, 2*L*ceil(T/L)
   std::vector<int16_t> rev_q15;  // 2*T
   float incr_re = 0, incr_im = 0;
   int16_t qincr_re = 0, qincr_im = 0;
-  long long hist = 0;            // mirror of ClientDev::hist
+  long long hist = 0;            // mirror of ClientDev::hist (upsampled samples for L > 1)
   long long zero_before = 0, qzero_before = 0;
   bool is_new = true;            // dynamic state not yet on the device
   float init_ph_re = 1.0f, init_ph_im = 0.0f;  // oscillator at attach (src/xlating.c:543, or xlg_add_client_ex)
@@ -84,6 +86,7 @@ struct HostClient {
   int ph_off = 0;
   bool tile_ineligible = false;  // its class cannot use the tiled kernel (shared memory, too few outputs)
   bool pending_settle = false;   // still inside its zero-history window at the last layout rebuild
+  int poly_off = 0, poly_rowcap = 0;  // kind 4: its branches' rows in the slot's polyphase scratch
 };
 
 struct Slot {
@@ -100,6 +103,11 @@ struct Slot {
   cudaEvent_t pf[10] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   cudaEvent_t tl_ph[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // timeline: pre-pass stamps, by occupancy parity (it runs a block ahead)
   bool pf_conv = false, pf_phase = false, pf_tile = false, pf_gen = false, pf_long = false;
+  cudaEvent_t pf_poly[4] = {nullptr, nullptr, nullptr, nullptr};  // around the polyphase generic / tiled kernels
+  bool pf_pg = false, pf_pt = false;
+  float2 *d_pscratch = nullptr;  // kind 4: unrotated outputs per branch (ClientDev::poly_off)
+  BlkInfo *d_vblk = nullptr, *h_vblk = nullptr;  // kind 4: per branch class, this block's window start and count
+  uint64_t poly_macs = 0;
   std::atomic<int64_t> ticket{-1};
   bool q15 = false;
   bool harvested = true;
@@ -201,6 +209,9 @@ struct TileClassHost {
   std::vector<int> real;     // the real client ids
   size_t T;
   bool merged = false;       // members may have different window alignments (natural layout only)
+  int branch = -1;           // rational (kind 4) classes: the polyphase branch r this class computes
+  uint32_t interp = 1;
+  long long minv = 0;        // decimation^-1 mod interp
 };
 
 }  // namespace
@@ -284,6 +295,13 @@ struct xlg_group {
 
   std::vector<TileClassHost> classes;
   std::vector<TileClassHost> long_classes;  // split-K long-filter classes (fir_long_cf32_kernel)
+  std::vector<TileClassHost> poly_classes;  // kind 4: one class per (rational class, polyphase branch)
+  bool poly_tile = true;                    // XLATING_B200_POLY_TILE=0: every rational client on the generic kernel
+  int *d_poly3 = nullptr, *d_poly4 = nullptr;  // ids of the kind-3 / kind-4 clients
+  size_t cap_poly3 = 0, cap_poly4 = 0;
+  int n_poly3 = 0, n_poly4 = 0;
+  float2 *d_ones = nullptr;                 // phase 1 + 0i for the kind-4 classes' tiled launch
+  size_t ones_cap = 0, pscratch_cap = 0;
   size_t partial_cap = 0;                   // float2 per slot partial-sum buffer
   int n_generic = 0;
   int max_client = 0;     // highest active id + 1
@@ -311,6 +329,7 @@ struct xlg_group {
 
   bool profiling = false;
   xlg_profile prof;
+  xlg_poly_profile poly_prof;
   uint64_t host_submit_ns = 0, host_wait_ns = 0, host_count_base = 0;
   std::mutex mu;  // guards slots' harvest + profile
 };
@@ -337,6 +356,11 @@ static void slot_free(Slot &s) {
   if (s.d_qphases) cudaFree(s.d_qphases);
   if (s.d_blk) cudaFree(s.d_blk);
   if (s.d_endph) cudaFree(s.d_endph);
+  if (s.d_pscratch) cudaFree(s.d_pscratch);
+  if (s.d_vblk) cudaFree(s.d_vblk);
+  if (s.h_vblk) cudaFreeHost(s.h_vblk);
+  s.d_pscratch = nullptr;
+  s.d_vblk = s.h_vblk = nullptr;
   s.d_endph = nullptr;
   s.d_raw = s.h_raw = nullptr;
   s.d_out = nullptr;
@@ -395,6 +419,15 @@ static void harvest_locked(xlg_group *g, Slot &s) {
     g->prof.fir_long_ms += ms;
     g->prof.fir_long_launches++;
   }
+  if (s.pf_pg && cudaEventElapsedTime(&ms, s.pf_poly[0], s.pf_poly[1]) == cudaSuccess) {
+    g->poly_prof.fir_poly_generic_ms += ms;
+    g->poly_prof.fir_poly_generic_launches++;
+  }
+  if (s.pf_pt && cudaEventElapsedTime(&ms, s.pf_poly[2], s.pf_poly[3]) == cudaSuccess) {
+    g->poly_prof.fir_poly_tile_ms += ms;
+    g->poly_prof.fir_poly_tile_launches++;
+  }
+  g->poly_prof.poly_macs += s.poly_macs;
   g->prof.blocks++;
   g->prof.out_samples += s.out_samples;
   g->prof.in_samples += s.in_samples;
@@ -519,6 +552,15 @@ static int dev_assign(T **dptr, size_t *cap_bytes, const void *src, size_t bytes
   CU_OK(cudaMemcpy(*dptr, src, bytes, cudaMemcpyHostToDevice));
   return 0;
 }
+// first input sample a client's next window reads: floor((L*S - hist) / L)  (S - hist for integer clients)
+static long long first_input(const HostClient &h, long long S) {
+  const long long fu = S * h.L - h.hist;
+  return fu >= 0 ? fu / h.L : -((-fu + h.L - 1) / h.L);
+}
+// its zero-history window has passed (or the ring itself is still zero there): it may join a tiled class
+static bool poly_settled(const xlg_group *g, const HostClient &h) {
+  return (h.zero_before == 0 && g->S < (long long)g->ring_cap / 2) || h.zero_before <= first_input(h, g->S);
+}
 static int rebuild_layout(xlg_group *g) {
   // XLATING_B200_REBUILD_TIMING=1: where a re-layout spends its time (logged per call)
   static const bool timing = getenv("XLATING_B200_REBUILD_TIMING") != nullptr;
@@ -551,13 +593,14 @@ static int rebuild_layout(xlg_group *g) {
   for (int i = 0; i < nc; i++) {
     HostClient &h = g->clients[i];
     if (!h.active) continue;
-    h.out_cap = (int)(g->max_input_len / 2 / h.D + 2);
+    h.out_cap = (int)((uint64_t)g->max_input_len / 2 * h.L / h.D + 2);
     h.out_off = (int)out_total;
     out_total += (size_t)h.out_cap;
     out_total = (out_total + 3) & ~(size_t)3;  // keep rows 32-byte aligned
     h.taps_off = (int)taps_total;
-    taps_total += h.T;
-    max_hist = std::max(max_hist, h.T - 1);
+    taps_total += h.rev.size() / 2;
+    // a rational client's history of at most T - 1 upsampled samples reaches back ceil((T-1)/L) + 1 inputs
+    max_hist = std::max(max_hist, h.L == 1 ? h.T - 1 : (h.T - 1 + h.L - 1) / h.L + 1);
   }
   if (ensure_ring(g, max_hist, g->qring != nullptr)) return -EIO;
   if (ensure_arenas(g, out_total, g->q_alloc)) return -EIO;
@@ -569,8 +612,8 @@ static int rebuild_layout(xlg_group *g) {
   for (int i = 0; i < nc; i++) {
     const HostClient &h = g->clients[i];
     if (!h.active) continue;
-    memcpy(&taps[h.taps_off], h.rev.data(), h.T * sizeof(float2));        // both interleaved (re, im)
-    memcpy(&qtaps[h.taps_off], h.rev_q15.data(), h.T * sizeof(short2));
+    memcpy(&taps[h.taps_off], h.rev.data(), h.rev.size() * sizeof(float));  // both interleaved (re, im)
+    memcpy(&qtaps[h.taps_off], h.rev_q15.data(), h.rev_q15.size() * sizeof(int16_t));
   }
   if (dev_assign(&g->d_taps, &g->cap_taps, taps.data(), taps.size() * sizeof(float2)) ||
       dev_assign(&g->d_qtaps, &g->cap_qtaps, qtaps.data(), qtaps.size() * sizeof(short2)))
@@ -615,12 +658,28 @@ static int rebuild_layout(xlg_group *g) {
     return m;
   };
   std::map<std::tuple<uint32_t, size_t, long long>, std::vector<int>> buckets;
+  std::map<std::tuple<uint32_t, uint32_t, size_t, long long>, std::vector<int>> pbuckets;  // (L, M, T, hist)
+  g->poly_classes.clear();
   for (int i = 0; i < nc; i++) {
     HostClient &h = g->clients[i];
     if (!h.active) continue;
-    h.kind = 0;
+    h.kind = h.L > 1 ? 3 : 0;
     h.tile_ineligible = false;
     h.pending_settle = false;
+    if (h.L > 1) {
+      // rational: a tiled class per (L, M, T, alignment) where every branch is an integer class the tiled
+      // kernel takes (gcd(L, M) = 1: each block uses every branch, outputs L apart)
+      const size_t Tb = (h.T + h.L - 1) / h.L;
+      const Mode m = mode_of(h.D, Tb);
+      if ((g->flags & XLG_FORCE_GENERIC) || !g->poly_tile || std::gcd(h.L, h.D) != 1 || !m.eligible || m.as_long)
+        continue;
+      if (!poly_settled(g, h)) {
+        h.pending_settle = true;
+        continue;
+      }
+      pbuckets[std::make_tuple(h.L, h.D, h.T, h.hist)].push_back(i);
+      continue;
+    }
     const long long first = g->S - h.hist;
     const bool settled = (h.zero_before == 0 && g->S < (long long)g->ring_cap / 2) || h.zero_before <= first;
     if (g->flags & XLG_FORCE_GENERIC) continue;
@@ -741,6 +800,75 @@ static int rebuild_layout(xlg_group *g) {
     }
     dest.push_back(ch);
   }
+  // rational tiled classes: one tiled class per polyphase branch r, members in the same slots of every branch
+  size_t pscratch = 0;
+  int max_rowcap = 0;
+  for (auto &kv : pbuckets) {
+    const uint32_t L = std::get<0>(kv.first), M = std::get<1>(kv.first);
+    const size_t T = std::get<2>(kv.first), Tb = (T + L - 1) / L;
+    std::vector<int> &real = kv.second;
+    if ((int)real.size() < kTileMinClients || g->poly_classes.size() + L > (size_t)T_MAX_CLASSES) continue;
+    const Mode m = mode_of(M, Tb);
+    std::vector<int> slots(real);
+    while (slots.size() % T_CG != 0) slots.push_back(-1);
+    long long minv = 0;  // M^-1 mod L (extended Euclid)
+    {
+      long long a = M % L, b = L, x0 = 1, x1 = 0;
+      while (b != 0) {
+        const long long q = a / b, t = a - q * b, tx = x0 - q * x1;
+        a = b;
+        b = t;
+        x0 = x1;
+        x1 = tx;
+      }
+      minv = ((x0 % (long long)L) + L) % L;
+    }
+    for (int id : real) {
+      HostClient &h = g->clients[id];
+      h.kind = 4;
+      h.poly_rowcap = (h.out_cap + (int)L - 1) / (int)L + 1;
+      h.poly_off = (int)pscratch;
+      pscratch += (size_t)L * h.poly_rowcap;
+      max_rowcap = std::max(max_rowcap, h.poly_rowcap);
+    }
+    for (uint32_t r = 0; r < L; r++) {
+      TileClassHost ch;
+      memset(&ch.k, 0, sizeof(ch.k));
+      ch.T = Tb;
+      ch.members = slots;
+      ch.real = real;
+      ch.branch = (int)r;
+      ch.interp = L;
+      ch.minv = minv;
+      ch.k.D = (int)M;
+      ch.k.Dp = m.Dp;
+      ch.k.L = m.L;
+      ch.k.n_groups = (int)(slots.size() / T_CG);
+      ch.k.n_members = (int)real.size();
+      ch.k.natural = m.natural ? 1 : 0;
+      ch.k.members_off = (int)members.size();
+      ch.k.taps_off = (long long)tile_taps.size();
+      const int v = (int)g->poly_classes.size();  // the tiled kernel reads this class's BlkInfo at d_vblk[v]
+      for (int id : slots) {
+        member_cid.push_back(id < 0 ? -1 : v);
+        members.push_back(id < 0 ? -1 : g->clients[id].poly_off + (int)r * g->clients[id].poly_rowcap);
+        member_incr.push_back(make_float2(1.f, 0.f));
+      }
+      const size_t base = tile_taps.size();
+      tile_taps.resize(base + slots.size() * (size_t)m.L, make_float2(0.f, 0.f));
+      for (size_t gi = 0; gi < slots.size() / T_CG; gi++) {
+        float2 *dst = tile_taps.data() + base + gi * (size_t)m.L * T_CG;
+        for (int sl = 0; sl < T_CG; sl++) {
+          const int id = slots[gi * T_CG + sl];
+          if (id < 0) continue;
+          const float *src = g->clients[id].rev.data() + 2 * (size_t)r * Tb;  // branch r (xl_poly_pack)
+          for (size_t t = 0; t < Tb; t++)
+            dst[((t / M) * m.Dp + t % M) * T_CG + sl] = make_float2(src[2 * t], src[2 * t + 1]);
+        }
+      }
+      g->poly_classes.push_back(ch);
+    }
+  }
   tick(2);
   // heaviest classes first: their CTAs are scheduled first and the lighter ones
   // fill the tail of the launch
@@ -819,7 +947,7 @@ static int rebuild_layout(xlg_group *g) {
     }
     std::vector<int> loose;
     for (int i = 0; i < nc; i++)
-      if (g->clients[i].active && g->clients[i].kind == 0) loose.push_back(i);
+      if (g->clients[i].active && (g->clients[i].kind == 0 || g->clients[i].kind >= 3)) loose.push_back(i);
     for (size_t base = 0; base < loose.size(); base += 32) {
       int cap = 0;
       for (size_t m = base; m < std::min(base + 32, loose.size()); m++) cap = std::max(cap, g->clients[loose[m]].out_cap);
@@ -861,6 +989,24 @@ static int rebuild_layout(xlg_group *g) {
         }
       }
     }
+    if (pscratch > g->pscratch_cap) {
+      g->pscratch_cap = pscratch + pscratch / 4 + 1024;
+      for (Slot &sl : g->slots) {
+        if (sl.d_pscratch) cudaFree(sl.d_pscratch);
+        sl.d_pscratch = nullptr;
+        CU_OK(cudaMalloc(&sl.d_pscratch, g->pscratch_cap * sizeof(float2)));
+      }
+    }
+    // the tiled kernel reads the phase of output j at [32 * (j / 2) + client slot]: a table of ones that long
+    const size_t ones = ((size_t)max_rowcap / 2 + 2) * 32;
+    if (!g->poly_classes.empty() && ones > g->ones_cap) {
+      if (g->d_ones) cudaFree(g->d_ones);
+      g->d_ones = nullptr;
+      g->ones_cap = ones;
+      std::vector<float2> one(ones, make_float2(1.f, 0.f));
+      CU_OK(cudaMalloc(&g->d_ones, ones * sizeof(float2)));
+      CU_OK(cudaMemcpy(g->d_ones, one.data(), ones * sizeof(float2), cudaMemcpyHostToDevice));
+    }
     if (table > g->phase_cap) {
       g->phase_cap = table + table / 4 + 1024;
       for (Slot &sl : g->slots) {
@@ -893,6 +1039,7 @@ static int rebuild_layout(xlg_group *g) {
       h.is_new = false;
     }
     d.D = (int)h.D;
+    d.L = (int)h.L;
     d.T = (int)h.T;
     d.taps_off = h.taps_off;
     d.qtaps_off = h.taps_off;
@@ -902,7 +1049,20 @@ static int rebuild_layout(xlg_group *g) {
     d.kind = h.kind;
     d.renorm = (g->flags & XLG_NO_RENORM) ? 0 : 1;
     d.ph_off = h.ph_off;
+    d.poly_off = h.poly_off;
+    d.poly_rowcap = h.poly_rowcap;
     if (h.kind == 0) g->n_generic++;
+  }
+  {
+    std::vector<int> p3, p4;
+    for (int i = 0; i < nc; i++)
+      if (g->clients[i].active && g->clients[i].kind == 3) p3.push_back(i);
+      else if (g->clients[i].active && g->clients[i].kind == 4) p4.push_back(i);
+    g->n_poly3 = (int)p3.size();
+    g->n_poly4 = (int)p4.size();
+    if (dev_assign(&g->d_poly3, &g->cap_poly3, p3.data(), p3.size() * sizeof(int)) ||
+        dev_assign(&g->d_poly4, &g->cap_poly4, p4.data(), p4.size() * sizeof(int)))
+      return -EIO;
   }
   if ((size_t)nc > g->d_clients_cap) {
     if (g->d_clients) cudaFree(g->d_clients);
@@ -973,9 +1133,9 @@ static void choose_partition(xlg_group *g) {
     double steps = 0, fma = 0;
     for (const HostClient &h : g->clients) {
       if (!h.active) continue;
-      const double n_out = n / (double)h.D;
+      const double n_out = n * h.L / (double)h.D;
       steps = std::max(steps, n_out);
-      fma += 4.0 * n_out * (double)h.T;
+      fma += 4.0 * n_out * (double)((h.T + h.L - 1) / h.L);
     }
     const double t_chain_us = 6.0 + steps * 10.75 / g->sm_mhz * 1.15;
     const double fma_per_us = 128.0 * g->sm_mhz * (double)g->part.big_sms;
@@ -1100,6 +1260,7 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
   xlg_group *g = new (std::nothrow) xlg_group();
   if (g == nullptr) return -ENOMEM;
   memset(&g->prof, 0, sizeof(g->prof));
+  memset(&g->poly_prof, 0, sizeof(g->poly_prof));
   g->device = device;
   g->fs = sampling_freq;
   g->max_input_len = max_input_len;
@@ -1153,6 +1314,11 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
       if (cudaEventCreateWithFlags(ev, cudaEventDisableTiming) != cudaSuccess) return fail(-EIO);
     for (int i = 0; i < 10; i++)
       if (cudaEventCreate(&s.pf[i]) != cudaSuccess) return fail(-EIO);
+    for (cudaEvent_t &ev : s.pf_poly)
+      if (cudaEventCreate(&ev) != cudaSuccess) return fail(-EIO);
+    if (cudaMalloc(&s.d_vblk, T_MAX_CLASSES * sizeof(BlkInfo)) != cudaSuccess ||
+        cudaHostAlloc(&s.h_vblk, T_MAX_CLASSES * sizeof(BlkInfo), cudaHostAllocDefault) != cudaSuccess)
+      return fail(-ENOMEM);
   }
   if (cudaEventCreate(&g->ev_t0) != cudaSuccess || cudaEventCreate(&g->ev_t1) != cudaSuccess) return fail(-EIO);
   // the tiled kernel needs > 48 KiB of dynamic shared memory
@@ -1170,6 +1336,8 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
     if (tm != nullptr) g->long_tmap = atoi(tm) != 0;
     const char *sv = getenv("XLATING_B200_SPECULATE");
     if (sv != nullptr) g->speculate = atoi(sv) != 0;
+    const char *pt = getenv("XLATING_B200_POLY_TILE");
+    if (pt != nullptr) g->poly_tile = atoi(pt) != 0;
     const char *cv = getenv("XLATING_B200_CSTREAMS");
     if (cv != nullptr) g->n_cs = std::min(std::max(atoi(cv), 1), (int)xlg_group::kMaxCs);
   }
@@ -1268,6 +1436,8 @@ extern "C" void xlg_destroy(xlg_group *g) {
       if (ev) cudaEventDestroy(ev);
     for (int i = 0; i < 10; i++)
       if (s.pf[i]) cudaEventDestroy(s.pf[i]);
+    for (cudaEvent_t ev : s.pf_poly)
+      if (ev) cudaEventDestroy(ev);
   }
   for (HostOut &h : g->ring_out) {
     if (h.h_out) cudaFreeHost(h.h_out);
@@ -1293,6 +1463,9 @@ extern "C" void xlg_destroy(xlg_group *g) {
   if (g->d_member_incr) cudaFree(g->d_member_incr);
   if (g->d_member_cid) cudaFree(g->d_member_cid);
   if (g->d_order) cudaFree(g->d_order);
+  if (g->d_poly3) cudaFree(g->d_poly3);
+  if (g->d_poly4) cudaFree(g->d_poly4);
+  if (g->d_ones) cudaFree(g->d_ones);
   if (g->ev_user) cudaEventDestroy(g->ev_user);
   if (g->s_in) cudaStreamDestroy(g->s_in);
   for (const xlg_group::StreamSet *ss : {&g->set_part, &g->set_plain}) {
@@ -1317,14 +1490,12 @@ extern "C" int xlg_add_client(xlg_group *g, uint32_t decimation, const float *ta
   return xlg_add_client_ex(g, decimation, taps, taps_len, center_freq, nullptr, client_id);
 }
 
-extern "C" int xlg_add_client_ex(xlg_group *g, uint32_t decimation, const float *taps, size_t taps_len,
-                                 int32_t center_freq, const xlg_client_state *state, int *client_id) {
-  if (g == nullptr || client_id == nullptr) return -EINVAL;
-  if (state != nullptr && (state->hist < 0 || state->valid_history < 0 || (size_t)state->hist > taps_len)) return -EINVAL;
-  if (taps_len == 0 || taps == nullptr) return -1;  // src/xlating.c:496
-  if (decimation == 0) return -EINVAL;
+// Attach a client: the reference filter with `decimation` at `rate` (fs, or interp * fs for a rational client,
+// whose taps are kept as polyphase branches).  The callers have validated their arguments.
+static int attach_client(xlg_group *g, uint32_t interp, uint32_t decimation, uint32_t rate, const float *taps,
+                         size_t taps_len, int32_t center_freq, const xlg_client_state *state, int *client_id) {
   xl_client_consts k;
-  int rc = xl_client_consts_build(taps, taps_len, decimation, center_freq, g->fs, &k);
+  int rc = xl_client_consts_build(taps, taps_len, decimation, center_freq, rate, &k);
   if (rc) return rc;
   int id = -1;
   for (size_t i = 0; i < g->clients.size(); i++)
@@ -1340,14 +1511,20 @@ extern "C" int xlg_add_client_ex(xlg_group *g, uint32_t decimation, const float 
   h = HostClient();
   h.active = true;
   h.D = decimation;
+  h.L = interp;
   h.T = taps_len;
-  h.rev.assign(k.rev_cf32, k.rev_cf32 + 2 * taps_len);
-  h.rev_q15.assign(k.rev_q15, k.rev_q15 + 2 * taps_len);
+  if (interp == 1) {
+    h.rev.assign(k.rev_cf32, k.rev_cf32 + 2 * taps_len);
+    h.rev_q15.assign(k.rev_q15, k.rev_q15 + 2 * taps_len);
+  } else {
+    h.rev.resize(2 * (size_t)interp * ((taps_len + interp - 1) / interp));  // no Q15 path for rational clients
+    xl_poly_pack(k.rev_cf32, taps_len, interp, h.rev.data());
+  }
   h.incr_re = k.incr_re;
   h.incr_im = k.incr_im;
   h.qincr_re = k.qincr_re;
   h.qincr_im = k.qincr_im;
-  h.hist = (long long)taps_len - 1;  // src/xlating.c:552
+  h.hist = (long long)taps_len - 1;  // src/xlating.c:552 (upsampled samples for a rational client)
   h.zero_before = g->S;
   h.qzero_before = g->qS;
   if (state != nullptr) {
@@ -1364,6 +1541,36 @@ extern "C" int xlg_add_client_ex(xlg_group *g, uint32_t decimation, const float 
   g->dirty = true;
   *client_id = id;
   return 0;
+}
+
+extern "C" int xlg_add_client_ex(xlg_group *g, uint32_t decimation, const float *taps, size_t taps_len,
+                                 int32_t center_freq, const xlg_client_state *state, int *client_id) {
+  if (g == nullptr || client_id == nullptr) return -EINVAL;
+  if (state != nullptr && (state->hist < 0 || state->valid_history < 0 || (size_t)state->hist > taps_len)) return -EINVAL;
+  if (taps_len == 0 || taps == nullptr) return -1;  // src/xlating.c:496
+  if (decimation == 0) return -EINVAL;
+  return attach_client(g, 1, decimation, g->fs, taps, taps_len, center_freq, state, client_id);
+}
+
+extern "C" int xlg_add_client_rational(xlg_group *g, uint32_t interp, uint32_t decim, const float *taps,
+                                       size_t taps_len, int32_t center_freq, int *client_id) {
+  if (g == nullptr || client_id == nullptr) return -EINVAL;
+  if (interp == 0 || decim == 0) {
+    XL_LOG("rational client: interpolation %u and decimation %u must both be at least 1", interp, decim);
+    return -EINVAL;
+  }
+  if ((uint64_t)interp * g->fs > UINT32_MAX) {
+    XL_LOG("rational client: %u x %u Hz upsampled rate exceeds UINT32_MAX", interp, g->fs);
+    return -EINVAL;
+  }
+  if ((uint64_t)interp * (g->max_input_len / 2) >= (1ull << 31)) {
+    XL_LOG("rational client: %u x %u samples per block upsampled exceed 2^31", interp, g->max_input_len / 2);
+    return -EINVAL;
+  }
+  if (interp == 1) return xlg_add_client(g, decim, taps, taps_len, center_freq, client_id);
+  if (taps_len == 0 || taps == nullptr) return -1;  // as xlg_add_client (src/xlating.c:496)
+  if (taps_len > (size_t)INT32_MAX) return -EINVAL;
+  return attach_client(g, interp, decim, interp * g->fs, taps, taps_len, center_freq, nullptr, client_id);
 }
 
 extern "C" int xlg_reserve(xlg_group *g, size_t output_samples_per_block) {
@@ -1422,15 +1629,21 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     XL_LOG("block of %zu elements exceeds max_input_len %u", input_len, g->max_input_len);
     return -EINVAL;
   }
-  CU_OK(cudaSetDevice(g->device));
   const bool q15 = (flags & XLG_PATH_Q15) != 0;
+  if (q15)
+    for (const HostClient &h : g->clients)
+      if (h.active && h.L > 1) {
+        XL_LOG("the Q15 path does not serve rational clients; submit without XLG_PATH_Q15");
+        return -ENOTSUP;
+      }
+  CU_OK(cudaSetDevice(g->device));
   const bool dev_in = (flags & XLG_INPUT_DEVICE) != 0;
   const bool dev_out = (g->flags & XLG_OUT_DEVICE) != 0;
 
   // clients whose zero-history window has passed may move to a tiled / long class
   if (!g->dirty && !q15) {
     for (const HostClient &h : g->clients)
-      if (h.active && h.pending_settle && h.zero_before <= g->S - h.hist) {
+      if (h.active && h.pending_settle && h.zero_before <= first_input(h, g->S)) {
         g->dirty = true;
         break;
       }
@@ -1489,23 +1702,33 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     ho.q15 = q15;
   }
   s.q15 = q15;
-  s.tile_macs = s.algo_macs = s.out_samples = 0;
+  s.tile_macs = s.algo_macs = s.out_samples = s.poly_macs = 0;
   s.in_samples = (uint64_t)n;
-  int max_generic_out = 0;
+  int max_generic_out = 0, poly_warps = 0, max_poly4_out = 0;
   for (size_t i = 0; i < g->clients.size(); i++) {
     HostClient &h = g->clients[i];
     if (!h.active) continue;
-    const long long first = S - h.hist;
-    const long long last_ok = S + n - (long long)h.T;
+    // upsampled coordinates (the same integers for L = 1)
+    const long long Su = S * h.L, Eu = (S + n) * h.L;
+    const long long first = Su - h.hist;
+    const long long last_ok = Eu - (long long)h.T;
     int n_out = 0;
     if (last_ok >= first) n_out = (int)((last_ok - first) / (long long)h.D) + 1;
     if (n_out > h.out_cap) n_out = h.out_cap;
     ho.n_out[i] = n_out;
     ho.out_off[i] = h.out_off;
-    h.hist = (S + n) - (first + (long long)n_out * (long long)h.D);
+    h.hist = Eu - (first + (long long)n_out * (long long)h.D);
     if (g->flags & XLG_TRACK_STATE) ho.hist_after[i] = h.hist;
     s.out_samples += (uint64_t)n_out;
-    s.algo_macs += (uint64_t)n_out * h.T;
+    const uint64_t macs = (uint64_t)n_out * ((h.T + h.L - 1) / h.L);
+    s.algo_macs += macs;
+    if (h.kind >= 3) s.poly_macs += macs;
+    if (h.kind == 4) max_poly4_out = std::max(max_poly4_out, n_out);
+    if (h.kind == 3) {
+      // warps of fir_poly_generic_cf32_kernel: min(L, n_out) residues x groups of G_OPW outputs
+      const int per = (int)((n_out + (long long)h.L - 1) / h.L);
+      poly_warps = std::max(poly_warps, (int)std::min<long long>(h.L, n_out) * ((per + G_OPW - 1) / G_OPW));
+    }
     if (q15 || h.kind == 0) max_generic_out = std::max(max_generic_out, n_out);
   }
 
@@ -1829,6 +2052,87 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
                                                               s.d_phases, s.d_out);
     if (g->profiling) CU_OK(cudaEventRecord(s.pf[7], cs));
   }
+  // ---- rational tiled classes: the tiled kernel over one class per polyphase branch, then the placement ----
+  s.pf_pt = false;
+  if (!q15 && !g->poly_classes.empty() && max_poly4_out > 0) {
+    TileLaunch P;
+    memset(&P, 0, sizeof(P));
+    // largest tile that still gives about two CTAs per SM (every shape fits: eligibility was checked at 64)
+    static const int kPolyShapes[][2] = {{16, 4}, {16, 2}, {16, 1}};
+    int lo = 16, rk = 1;
+    for (const auto &sh : kPolyShapes) {
+      int ctas = 0;
+      for (const TileClassHost &ch : g->poly_classes)
+        ctas += ((ho.n_out[ch.real[0]] / (int)ch.interp + 1 + sh[0] * sh[1] - 1) / (sh[0] * sh[1])) * ch.k.n_groups;
+      if (ctas >= 2 * g->fir_sms) {
+        lo = sh[0];
+        rk = sh[1];
+        break;
+      }
+    }
+    const int KT = lo * rk;
+    int ctas = 0;
+    size_t smem = 0;
+    for (size_t v = 0; v < g->poly_classes.size(); v++) {
+      const TileClassHost &ch = g->poly_classes[v];
+      const HostClient &h0 = g->clients[ch.real[0]];
+      const int n_out = ho.n_out[ch.real[0]];
+      const long long L = ch.interp, M = h0.D;
+      // this block's first upsampled window (hist was advanced above); branch r serves k = rho + j*L
+      const long long first_u = (S + n) * L - h0.hist - (long long)n_out * M;
+      const long long a = (((-(first_u + ch.branch)) % L) + L) % L;
+      const long long rho = (a * ch.minv) % L;
+      const int nv = rho < n_out ? (int)((n_out - 1 - rho) / L) + 1 : 0;
+      s.h_vblk[v].first = (first_u + rho * M + ch.branch) / L;  // exact: the window start is -r mod L
+      s.h_vblk[v].n_out = nv;
+      s.h_vblk[v].pad_ = 0;
+      if (nv <= 0) continue;
+      TileClass k = ch.k;
+      k.first = s.h_vblk[v].first;
+      k.n_out = nv;
+      k.tiles = (nv + KT - 1) / KT;
+      k.xs_len = (KT - 1) * k.Dp + k.L;
+      k.cta_begin = ctas;
+      ctas += k.tiles * k.n_groups;
+      smem = std::max(smem, (size_t)T_SMEM_FIXED + ((size_t)k.xs_len + 10) * sizeof(float2));
+      P.cls[P.n_classes++] = k;
+      s.tile_macs += (uint64_t)k.tiles * KT * (uint64_t)k.L * (uint64_t)ch.members.size();
+    }
+    if (ctas > 0) {
+      if (g->profiling) {
+        CU_OK(cudaEventRecord(s.pf_poly[2], cs));
+        s.pf_pt = true;
+      }
+      CU_OK(cudaMemcpyAsync(s.d_vblk, s.h_vblk, g->poly_classes.size() * sizeof(BlkInfo), cudaMemcpyHostToDevice, cs));
+      const float2 *tt = (const float2 *)g->d_tile_taps;
+#define XL_LAUNCH_PTILE(RK_)                                                                                     \
+  fir_tile_cf32_kernel<16, RK_, 1><<<ctas, TileShape<16, RK_, 1>::kThreads, smem, cs>>>(                          \
+      P, g->ring, mask, tt, g->d_members, g->d_member_cid, g->d_member_incr, s.d_vblk, g->d_ones, s.d_pscratch, nullptr)
+      if (rk == 4)
+        XL_LAUNCH_PTILE(4);
+      else if (rk == 2)
+        XL_LAUNCH_PTILE(2);
+      else
+        XL_LAUNCH_PTILE(1);
+#undef XL_LAUNCH_PTILE
+      dim3 pgrid((max_poly4_out + 255) / 256, g->n_poly4);
+      poly_tile_place_cf32_kernel<<<pgrid, 256, 0, cs>>>(g->d_clients, g->d_poly4, s.d_blk, s.d_pscratch, s.d_phases,
+                                                         s.d_out);
+      if (g->profiling) CU_OK(cudaEventRecord(s.pf_poly[3], cs));
+    }
+  }
+  s.pf_pg = false;
+  if (!q15 && g->n_poly3 > 0 && poly_warps > 0) {
+    constexpr int warps_per_cta = G_THREADS / 32;
+    dim3 grid((poly_warps + warps_per_cta - 1) / warps_per_cta, g->n_poly3);
+    if (g->profiling) {
+      CU_OK(cudaEventRecord(s.pf_poly[0], cs));
+      s.pf_pg = true;
+    }
+    fir_poly_generic_cf32_kernel<<<grid, G_THREADS, 0, cs>>>(g->d_clients, g->d_poly3, s.d_blk, g->ring, mask, g->d_taps,
+                                                             s.d_phases, s.d_out);
+    if (g->profiling) CU_OK(cudaEventRecord(s.pf_poly[1], cs));
+  }
   CU_OK(cudaGetLastError());
   CU_OK(cudaEventRecord(s.ev_fir, cs));
 
@@ -2054,6 +2358,14 @@ extern "C" int xlg_profile_enable(xlg_group *g, int on) {
   std::lock_guard<std::mutex> lk(g->mu);
   for (Slot &s : g->slots) harvest_locked(g, s);
   g->profiling = on != 0;
+  return 0;
+}
+
+extern "C" int xlg_poly_profile_read(xlg_group *g, xlg_poly_profile *p, int reset) {
+  if (g == nullptr || p == nullptr) return -EINVAL;
+  std::lock_guard<std::mutex> lk(g->mu);
+  *p = g->poly_prof;
+  if (reset) memset(&g->poly_prof, 0, sizeof(g->poly_prof));
   return 0;
 }
 

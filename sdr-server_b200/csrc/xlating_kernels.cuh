@@ -45,22 +45,26 @@ namespace xl {
 // device-resident tables
 // ---------------------------------------------------------------------------
 struct ClientDev {
-  long long hist;         // history_offset of the reference (src/xlating.c:29), shared by both paths
+  long long hist;         // history_offset of the reference (src/xlating.c:29), shared by both paths;
+                          // in upsampled samples for a rational client (L > 1)
   long long zero_before;  // cf32 ring: samples with absolute index < this read as 0 (attach point)
   long long qzero_before; // same for the Q15 ring
   float2 phase;           // oscillator (src/xlating.c:36)
   float2 incr;            // (src/xlating.c:37)
   short qph_re, qph_im, qinc_re, qinc_im;  // Q15 oscillator (:39-42)
-  int D;                  // decimation
+  int D;                  // decimation (M of a rational client)
   int T;                  // taps_len
-  int taps_off;           // float2 offset of rev taps in the natural arena
+  int taps_off;           // float2 offset of rev taps in the natural arena (polyphase branches for L > 1)
   int qtaps_off;          // short2 offset in the Q15 arena
   int out_off;            // complex-sample offset in the per-slot output / phase arenas
   int out_cap;
   int active;
-  int kind;               // 0 = generic kernel, 1 = tiled kernel
+  int kind;               // 0 = generic kernel, 1 = tiled kernel, 2 = split-K, 3 / 4 = polyphase generic / tiled
   int renorm;             // 1 = native behaviour (:73), 0 = AVX behaviour (:336-339)
   int ph_off;             // cf32 oscillator table: phase of EVEN output k lives at phases[ph_off + 32*(k/2)]
+  int L;                  // interpolation: the client filters the stream zero-stuffed by L (1 = integer client)
+  int poly_off;           // kind 4: branch r's unrotated outputs at scratch[poly_off + r * poly_rowcap + k / L]
+  int poly_rowcap;
 };
 
 struct SpecSave {
@@ -169,8 +173,10 @@ phase_cf32_kernel(ClientDev *__restrict__ cl, const int *__restrict__ order, Blk
     save[c].phase = d->phase;
   }
   const int D = d->D;
-  const long long first = S - d->hist;
-  const int n_out = outputs_of_call(first, S, n_in, d->T, D, d->out_cap);
+  // stream positions in the client's (upsampled) coordinates: identical integers for L = 1
+  const long long Su = S * d->L, Eu = (S + n_in) * d->L;
+  const long long first = Su - d->hist;
+  const int n_out = outputs_of_call(first, Su, (int)(Eu - Su), d->T, D, d->out_cap);
   BlkInfo b;
   b.first = first;
   b.n_out = n_out;
@@ -179,7 +185,7 @@ phase_cf32_kernel(ClientDev *__restrict__ cl, const int *__restrict__ order, Blk
   const float2 after = osc_chain_cf32<32>(d->phase, d->incr, phases + d->ph_off, n_out, d->renorm);
   d->phase = after;
   if (endph != nullptr) endph[c] = after;  // XLG_TRACK_STATE: the oscillator after this block, per client id
-  d->hist = (S + n_in) - (first + (long long)n_out * D);  // src/xlating.c:76
+  d->hist = Eu - (first + (long long)n_out * D);  // src/xlating.c:76
 }
 
 // undo a speculative pre-pass that guessed the wrong block length
@@ -238,6 +244,77 @@ fir_generic_cf32_kernel(const ClientDev *__restrict__ cl, const BlkInfo *__restr
     if (k & 1) ph = cmul_unfused(ph, d->incr);     // odd outputs: one step from the stored even phase
     out[d->out_off + k] = cmul_unfused(mine, ph);  // src/xlating.c:70
   }
+}
+
+// ---------------------------------------------------------------------------
+// rational L/M client, any state (kind 3).  The client is the reference filter with
+// decimation M fed the zero-stuffed stream u[L*n] = x[n], u[m] = 0 otherwise.  Output
+// k's upsampled window starts at w = first + k*M; with r = (-w) mod L and n0 = (w + r)/L
+// only the taps rev[r + t*L] meet nonzero samples:
+//     y[k] = phase_k * sum_{t < Tb} x[n0 + t] * P[r][t],   P[r][t] = rev[r + t*L] (0 past T),
+// Tb = ceil(T / L) taps per output instead of T.  Outputs k and k + L share the branch
+// r and their inputs lie M samples apart, so a warp takes G_OPW outputs k0 + i*L and
+// runs the integer generic FIR on branch r with decimation M.  Warp q of a client
+// serves residue rho = q / groups (outputs rho, rho + L, ...), output group q % groups.
+// A padding tap reads one sample past the window; it is finite and weighted by zero.
+// ---------------------------------------------------------------------------
+__global__ void __launch_bounds__(G_THREADS)
+fir_poly_generic_cf32_kernel(const ClientDev *__restrict__ cl, const int *__restrict__ ids,
+                             const BlkInfo *__restrict__ blk, const float2 *__restrict__ ring, unsigned mask,
+                             const float2 *__restrict__ taps, const float2 *__restrict__ phases,
+                             float2 *__restrict__ out) {
+  const int c = ids[blockIdx.y];  // the kind-3 clients only
+  const ClientDev *d = cl + c;
+  const BlkInfo b = blk[c];
+  const int L = d->L, M = d->D;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int per = (b.n_out + L - 1) / L;           // outputs of residue 0 (the most of any residue)
+  const int groups = (per + G_OPW - 1) / G_OPW;
+  const int q = blockIdx.x * (G_THREADS / 32) + warp;
+  if (q >= min(L, b.n_out) * groups) return;       // warp-uniform
+  const int rho = q / groups;
+  const int k0 = rho + (q - rho * groups) * G_OPW * L;
+  if (k0 >= b.n_out) return;
+  const long long w = b.first + (long long)k0 * M;
+  const int r = (int)((((-w) % L) + L) % L);       // floor semantics: w < 0 inside the first block
+  const long long n0 = (w + r) / L;
+  const int Tb = (d->T + L - 1) / L;
+  const float2 mine = fir_warp_cf32(ring, mask, d->zero_before, taps + d->taps_off + (size_t)r * Tb, Tb, M, n0, lane);
+  const int k = k0 + lane * L;
+  if (lane < G_OPW && k < b.n_out) {
+    float2 ph = phases[d->ph_off + (size_t)(k >> 1) * 32];
+    if (k & 1) ph = cmul_unfused(ph, d->incr);
+    out[d->out_off + k] = cmul_unfused(mine, ph);
+  }
+}
+
+// ---------------------------------------------------------------------------
+// rational L/M clients of a tiled class (kind 4): clients with identical (L, M, T, window
+// alignment) and gcd(L, M) = 1.  In a block every branch r serves the outputs
+// k = rho_r + j*L (rho_r: the k < L whose window start -(first + k*M) is r mod L) from inputs
+// x[n0_r + j*M + t], t < Tb: an integer decimator with decimation M over the Tb taps of
+// branch r.  The host launches fir_tile_cf32_kernel with one class per branch (the branch's
+// taps packed for its 32-client groups, the class's BlkInfo at blk[class], phase 1 + 0i), which
+// leaves y_r[j] unrotated at scratch[poly_off + r * poly_rowcap + j]; this kernel rotates every
+// output with the client's oscillator and puts it at k.  Same arithmetic as the polyphase
+// generic kernel up to the order of the additions.
+// ---------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+poly_tile_place_cf32_kernel(const ClientDev *__restrict__ cl, const int *__restrict__ ids,
+                            const BlkInfo *__restrict__ blk, const float2 *__restrict__ scratch,
+                            const float2 *__restrict__ phases, float2 *__restrict__ out) {
+  const int c = ids[blockIdx.y];  // the kind-4 clients only
+  const ClientDev *d = cl + c;
+  const BlkInfo b = blk[c];
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= b.n_out) return;
+  const int L = d->L;
+  const long long w = b.first + (long long)k * d->D;
+  const int r = (int)((((-w) % L) + L) % L);
+  const float2 y = scratch[d->poly_off + (size_t)r * d->poly_rowcap + k / L];
+  float2 ph = phases[d->ph_off + (size_t)(k >> 1) * 32];
+  if (k & 1) ph = cmul_unfused(ph, d->incr);
+  out[d->out_off + k] = cmul_unfused(y, ph);
 }
 
 __global__ void __launch_bounds__(G_THREADS)
