@@ -109,6 +109,12 @@ int xlg_add_client_ex(xlg_group *g, uint32_t decimation, const float *taps, size
  * upsampled samples. */
 int xlg_add_client_rational(xlg_group *g, uint32_t interp, uint32_t decim, const float *taps, size_t taps_len,
                             int32_t center_freq, int *client_id);
+/* xlg_add_client_rational for a client that CONTINUES, as xlg_add_client_ex is for xlg_add_client: state->hist
+ * is in upsampled samples, state->valid_history in input samples (the stream's ring counts those).
+ * state == NULL is a fresh client.  -EINVAL for hist < 0, hist > taps_len or valid_history < 0, besides
+ * xlg_add_client_rational's checks; interp == 1 is xlg_add_client_ex. */
+int xlg_add_client_rational_ex(xlg_group *g, uint32_t interp, uint32_t decim, const float *taps, size_t taps_len,
+                               int32_t center_freq, const xlg_client_state *state, int *client_id);
 int xlg_remove_client(xlg_group *g, int client_id);
 /* Size the per-ticket result arenas (device and pinned host) for `output_samples_per_block` complex output
  * samples per block summed over all clients (a client at decimation D produces about max_input_len/2/D + 2).

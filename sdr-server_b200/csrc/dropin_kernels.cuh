@@ -17,9 +17,11 @@
  *   dropin_fir_kernel     the generic FIR (xlating_common.cuh) per request; each
  *                         CTA writes its 32 outputs as one 256-byte line straight
  *                         into the filter's pinned host output buffer.
+ *   dropin_fir_poly_kernel  the same for rational (L/M) filters, one polyphase branch
+ *                         per output (launched only when the batch has such a request).
  *
- * So a batch costs one (batched) input copy, two launches and one stream
- * synchronisation however many filters are in it.
+ * So a batch costs one (batched) input copy, two launches (three with rational
+ * filters in it) and one stream synchronisation however many filters are in it.
  */
 #pragma once
 
@@ -47,6 +49,8 @@ struct FilterDev {
   short2 qphase, qincr;   // (:39-42)
   unsigned mask;
   int D, T, out_cap;
+  int L;                  // interpolation of a rational filter (1 = integer filter); taps are then its
+                          // polyphase branches (xl_poly_pack), hist / blk.first in upsampled samples
 };
 
 // One process_* call.  The table lives in pinned host memory and is read by the
@@ -139,10 +143,13 @@ dropin_front_kernel(FilterDev *__restrict__ filters, const DropinReq *__restrict
     if (r >= n_req) return;
     const DropinReq q = req[r];
     FilterDev *d = filters + q.filter;
-    batch[r] = make_int2(q.filter, q.q15 | (q.osc_host == 2 ? 2 : 0));
+    batch[r] = make_int2(q.filter, q.q15 | (q.osc_host == 2 ? 2 : 0) | (d->L > 1 ? 4 : 0));
     const int D = d->D;
-    const long long first = q.S - d->hist;
-    const int n_out = outputs_of_call(first, q.S, q.n, d->T, D, d->out_cap);
+    // stream positions in the filter's (upsampled) coordinates, as the batch engine's pre-pass
+    // computes them: identical integers for L = 1
+    const long long Su = q.S * d->L, Eu = (q.S + q.n) * d->L;
+    const long long first = Su - d->hist;
+    const int n_out = outputs_of_call(first, Su, (int)(Eu - Su), d->T, D, d->out_cap);
     BlkInfo b;
     b.first = first;
     b.n_out = n_out;
@@ -152,7 +159,7 @@ dropin_front_kernel(FilterDev *__restrict__ filters, const DropinReq *__restrict
       d->qphase = osc_chain_q15(d->qphase, d->qincr, d->qphases, n_out);
     else if (q.osc_host == 0)
       d->phase = osc_chain_cf32<1>(d->phase, d->incr, d->phases, n_out, 1);
-    d->hist = (q.S + q.n) - (first + (long long)n_out * D);  // src/xlating.c:76, :133
+    d->hist = Eu - (first + (long long)n_out * D);  // src/xlating.c:76, :133
     return;
   }
   // ---- conversion blocks ----
@@ -182,11 +189,20 @@ dropin_front_kernel(FilterDev *__restrict__ filters, const DropinReq *__restrict
     dropin_convert8<2>(q, d, base);
 }
 
-// grid = (ceil(max n_out / G_OPC), n_req)
+// Outputs one CTA owns: G_OPC of an integer request (dropin_fir_kernel); for a rational one
+// (dropin_fir_poly_kernel) the G_OPC outputs of each of up to DF_POLY_RES residues mod L, so that every
+// residue of the span fills whole G_OPW-output groups.
+constexpr int DF_POLY_RES = 16;
+__host__ __device__ __forceinline__ int dropin_fir_span(int L) {
+  return G_OPC * (L < DF_POLY_RES ? L : DF_POLY_RES);
+}
+
+// grid = (max over integer requests of ceil(n_out / G_OPC), n_req); rational requests are skipped
 __global__ void __launch_bounds__(G_THREADS)
 dropin_fir_kernel(const FilterDev *__restrict__ filters, const int2 *__restrict__ batch) {
   __shared__ float2 so[G_OPC];
   const int2 bq = batch[blockIdx.y];
+  if (bq.y & 4) return;  // rational: dropin_fir_poly_kernel
   const FilterDev *d = filters + bq.x;
   const BlkInfo b = d->blk;
   const int kbase = blockIdx.x * G_OPC;
@@ -213,6 +229,53 @@ dropin_fir_kernel(const FilterDev *__restrict__ filters, const int2 *__restrict_
     __syncthreads();
     if (threadIdx.x < G_OPC && kbase + (int)threadIdx.x < b.n_out) d->out[kbase + threadIdx.x] = so[threadIdx.x];
   }
+}
+
+// Rational requests (L > 1), grid = (max over them of ceil(n_out / dropin_fir_span(L)), n_req); the
+// integer requests are skipped.  A CTA owns a contiguous span of outputs and computes them as the batch
+// engine's polyphase generic kernel (fir_poly_generic_cf32_kernel) does: outputs k0 + i*L (i < G_OPW)
+// share the branch r of k0 and read inputs M samples apart, so a warp runs the generic FIR warp on
+// branch r with decimation M; the warps loop over the span's (residue, output group) pairs.  Per output
+// the arithmetic is that kernel's, so a private rational filter equals the same client in a group bit for
+// bit.  A branch's padding tap reads one sample past its window with weight 0: the private ring starts
+// zeroed and only ever holds converted samples, so that sample is finite.  The span leaves through
+// shared memory as contiguous lines into the filter's pinned output buffer.  (A separate kernel: inlined
+// next to the integer path, this loop changed how the compiler scheduled that path's loads.)
+__global__ void __launch_bounds__(G_THREADS)
+dropin_fir_poly_kernel(const FilterDev *__restrict__ filters, const int2 *__restrict__ batch) {
+  __shared__ float2 so[G_OPC * DF_POLY_RES];
+  const int2 bq = batch[blockIdx.y];
+  if (!(bq.y & 4)) return;
+  const FilterDev *d = filters + bq.x;
+  const BlkInfo b = d->blk;
+  const int L = d->L, M = d->D;
+  const int kbase = blockIdx.x * dropin_fir_span(L);
+  if (kbase >= b.n_out) return;  // CTA-uniform
+  const int n_span = min(dropin_fir_span(L), b.n_out - kbase);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int per = (n_span + L - 1) / L;  // outputs of residue 0 (the most of any residue)
+  const int groups = (per + G_OPW - 1) / G_OPW;
+  const int pairs = min(L, n_span) * groups;
+  const int Tb = (d->T + L - 1) / L;
+  const float2 *ph_table = (bq.y & 2) ? d->phases_host : d->phases;
+  for (int p = warp; p < pairs; p += G_THREADS / 32) {
+    const int rho = p / groups;
+    const int kl = rho + (p - rho * groups) * G_OPW * L;  // span-local index of the group's first output
+    if (kl >= n_span) continue;                           // warp-uniform
+    const int k0 = kbase + kl;
+    long long n0;
+    const int r = poly_branch(b.first + (long long)k0 * M, L, &n0);
+    const float2 mine = fir_warp_cf32(d->ring, d->mask, 0, d->taps + (size_t)r * Tb, Tb, M, n0, lane);
+    const int kk = kl + lane * L;
+    if (lane < G_OPW && kk < n_span) {
+      const int k = kbase + kk;
+      float2 ph = ph_table[k >> 1];
+      if (k & 1) ph = cmul_unfused(ph, d->incr);  // odd outputs: one step from the stored even phase
+      so[kk] = cmul_unfused(mine, ph);             // src/xlating.c:70
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < n_span; i += G_THREADS) d->out[kbase + i] = so[i];
 }
 
 }  // namespace xl

@@ -112,6 +112,15 @@ __device__ __forceinline__ int outputs_of_call(long long first, long long S, int
   return n_out > out_cap ? out_cap : n_out;  // cannot clamp for input_len <= max_input_len
 }
 
+// rational L/M filter (the filter at L * fs fed the zero-stuffed stream u[L*n] = x[n]): the output
+// whose upsampled window starts at w reads only polyphase branch r = (-w) mod L (floor semantics:
+// w < 0 inside the first block), whose first tap meets input sample n0 = (w + r) / L
+__device__ __forceinline__ int poly_branch(long long w, int L, long long *n0) {
+  const int r = (int)((((-w) % L) + L) % L);
+  *n0 = (w + r) / L;
+  return r;
+}
+
 // ---------------------------------------------------------------------------
 // generic FIR, one warp = G_OPW consecutive outputs starting at window w0.  Lane i
 // (< G_OPW) returns the dot product of output i; other lanes return output 0's.

@@ -55,6 +55,11 @@
  *
  * XLATING_B200_DROPIN=group selects the older model instead (each filter a private
  * one-client batch group with its own streams), kept for A/B measurements.
+ *
+ * Rational filters (create_rational_frequency_xlating_filter, interpolation L > 1) are the
+ * filter with decimation M at L * fs fed the zero-stuffed stream, as the batch group's
+ * rational clients are: history and output counts in upsampled samples, polyphase taps, no
+ * Q15 path.  They share their band's group with the integer filters.
  */
 #include <cuda_runtime.h>
 #include <errno.h>
@@ -215,9 +220,10 @@ struct xlating_t {
   int slot = -1;
   bool counted = false;  // in Engine::live_filters
   uint32_t D = 0, max_in = 0;
+  uint32_t L = 1;           // interpolation (create_rational_frequency_xlating_filter); 1 = integer filter
   long long T = 0;
   int out_cap = 0;
-  long long hist = 0;       // host mirror of FilterDev::hist (same integer formula)
+  long long hist = 0;       // host mirror of FilterDev::hist (same integer formula; upsampled samples)
   long long S = 0, qS = 0;  // samples consumed so far by the cf32 / Q15 path
   void *d_mem = nullptr;    // ring | qring | taps | qtaps | phases | qphases
   void *h_mem = nullptr;    // pinned: staged input | cf32 output | Q15 output
@@ -237,8 +243,10 @@ struct xlating_t {
   int32_t center_freq = 0;
   uint32_t fs = 0;
   bool as_disabled = false;   // a Q15 call was made: the two paths share history_offset, stay private
+  bool q15_refused = false;   // a Q15 call on a rational filter was refused (and logged, once)
   bool dev_stale = false;     // the private device state is behind the mirror (group served the last blocks)
-  std::vector<float2> tail;   // the last T-1 samples consumed (cf32), oldest first, zeros before the first
+  std::vector<float2> tail;   // the last floor((T-1)/L) samples consumed (cf32), oldest first, zeros before
+                              // the first: all that the next window can reach
   float2 *d_ring = nullptr;   // the filter's private cf32 ring (inside d_mem) and its size
   size_t ring_cap = 0;
   // the call in flight
@@ -283,6 +291,8 @@ int stream_add(void *ctx, void *filter, int64_t valid_history, int *client) {
   st.hist = f->hist;
   st.phase_re = f->ph_re;
   st.phase_im = f->ph_im;
+  if (f->L > 1)
+    return xlg_add_client_rational_ex(sh->g, f->L, f->D, f->adopted_taps, (size_t)f->T, f->center_freq, &st, client);
   return xlg_add_client_ex(sh->g, f->D, f->adopted_taps, (size_t)f->T, f->center_freq, &st, client);
 }
 int stream_remove(void *ctx, int client) { return xlg_remove_client(((StreamHost *)ctx)->g, client); }
@@ -348,13 +358,18 @@ int run_batch(void *ctx, int lane, CombinerCall *const *batch, int n_req) {
   Lane &L = e->lanes[lane];
   cudaError_t err = cudaSetDevice(e->device);
   if (err == cudaSuccess) {
-    int max_n = 0, max_out = 0;
+    int max_n = 0, max_out = 0, max_poly_ctas = 0;
     unsigned slots = 0;  // shared inputs this batch reads: wait for their H2D
     for (int i = 0; i < n_req; i++) {
       const xlating *b = (const xlating *)batch[i]->user;
       L.h_req[i] = b->req;
       if (b->req.n > max_n) max_n = b->req.n;
-      if (b->req_out > max_out) max_out = b->req_out;
+      if (b->L > 1) {
+        const int span = dropin_fir_span((int)b->L);
+        max_poly_ctas = std::max(max_poly_ctas, (b->req_out + span - 1) / span);
+      } else if (b->req_out > max_out) {
+        max_out = b->req_out;
+      }
       if (b->req_slot >= 0) slots |= 1u << b->req_slot;
     }
     for (int sl = 0; sl < BlockCache::kSlots && err == cudaSuccess; sl++)
@@ -375,6 +390,8 @@ int run_batch(void *ctx, int lane, CombinerCall *const *batch, int n_req) {
       if (max_out > 0)
         dropin_fir_kernel<<<dim3((max_out + G_OPC - 1) / G_OPC, n_req), G_THREADS, 0, L.stream>>>(e->d_filters,
                                                                                                   L.d_batch);
+      if (max_poly_ctas > 0)
+        dropin_fir_poly_kernel<<<dim3(max_poly_ctas, n_req), G_THREADS, 0, L.stream>>>(e->d_filters, L.d_batch);
       err = cudaGetLastError();
     }
     if (err == cudaSuccess) err = cudaStreamSynchronize(L.stream);
@@ -558,8 +575,11 @@ void filter_release(xlating *f) {
   delete f;
 }
 
-int filter_build(xlating *f, int device, uint32_t decimation, const float *taps, size_t taps_len, int32_t center_freq,
-                 uint32_t sampling_freq, uint32_t max_in) {
+// A filter with interpolation L > 1 is the filter with decimation M = `decimation` at L * fs fed the
+// zero-stuffed stream (create_rational_frequency_xlating_filter): its constants are built at L * fs, its
+// taps are kept as polyphase branches and it has no Q15 ring or taps.  L = 1 is the integer filter.
+int filter_build(xlating *f, int device, uint32_t interp, uint32_t decimation, const float *taps, size_t taps_len,
+                 int32_t center_freq, uint32_t sampling_freq, uint32_t max_in) {
   if (decimation == 0 || sampling_freq == 0) return -EINVAL;
   int rc = engine_get(device, &f->e);
   if (rc != 0) {
@@ -567,26 +587,36 @@ int filter_build(xlating *f, int device, uint32_t decimation, const float *taps,
     return rc;
   }
   xl_client_consts k;
-  rc = xl_client_consts_build(taps, taps_len, decimation, center_freq, sampling_freq, &k);
+  rc = xl_client_consts_build(taps, taps_len, decimation, center_freq, interp * sampling_freq, &k);
   if (rc != 0) return rc;
+  const bool q15 = interp == 1;  // rational filters refuse the Q15 path
+  const size_t Tb = (taps_len + interp - 1) / interp;  // taps per polyphase branch (T for L = 1)
+  std::vector<float> branches;
+  if (!q15) {
+    branches.resize(2 * (size_t)interp * Tb);
+    xl_poly_pack(k.rev_cf32, taps_len, interp, branches.data());
+  }
   f->D = decimation;
+  f->L = interp;
   f->T = (long long)taps_len;
   f->max_in = max_in;
-  f->hist = (long long)taps_len - 1;                 // src/xlating.c:552
-  f->out_cap = (int)(max_in / 2 / decimation + 2);   // >= any call's output count (hist <= T-1)
+  f->hist = (long long)taps_len - 1;  // src/xlating.c:552 (upsampled samples)
+  // >= any call's output count (hist <= T-1)
+  f->out_cap = (int)((uint64_t)(max_in / 2) * interp / decimation + 2);
   const size_t max_n = max_in / 2;
+  const size_t hist_in = (taps_len - 1) / interp + 1;  // input samples the oldest window can reach
   size_t cap = 1024;
-  while (cap < taps_len + max_n + 64) cap <<= 1;     // history + one block, power of two
+  while (cap < hist_in + max_n + 64) cap <<= 1;      // history + one block, power of two
   FilterDev d;
   memset(&d, 0, sizeof(d));
   // device arena
   const size_t o_ring = 0;
   const size_t o_qring = align_up(o_ring + cap * sizeof(float2), 256);
-  const size_t o_taps = align_up(o_qring + cap * sizeof(short2), 256);
-  const size_t o_qtaps = align_up(o_taps + taps_len * sizeof(float2), 256);
-  const size_t o_ph = align_up(o_qtaps + taps_len * sizeof(short2), 256);
+  const size_t o_taps = align_up(o_qring + (q15 ? cap * sizeof(short2) : 0), 256);
+  const size_t o_qtaps = align_up(o_taps + interp * Tb * sizeof(float2), 256);
+  const size_t o_ph = align_up(o_qtaps + (q15 ? taps_len * sizeof(short2) : 0), 256);
   const size_t o_qph = align_up(o_ph + ((size_t)f->out_cap / 2 + 2) * sizeof(float2), 256);
-  const size_t d_bytes = align_up(o_qph + ((size_t)f->out_cap + 2) * sizeof(short2), 256);
+  const size_t d_bytes = align_up(o_qph + (q15 ? ((size_t)f->out_cap + 2) * sizeof(short2) : 0), 256);
   // pinned host arena
   const size_t h_in_bytes = align_up((size_t)max_in * sizeof(int16_t), 256);  // cs16 is the widest input
   const size_t h_out_bytes = align_up((size_t)f->out_cap * sizeof(float2), 256);
@@ -617,8 +647,12 @@ int filter_build(xlating *f, int device, uint32_t decimation, const float *taps,
   }
   dm = (char *)f->d_mem;
   CU_TRY(cudaMemset(dm, 0, o_taps));  // both rings start as the reference's zeroed working buffers (:556-565)
-  CU_TRY(cudaMemcpy(dm + o_taps, k.rev_cf32, taps_len * sizeof(float2), cudaMemcpyHostToDevice));
-  CU_TRY(cudaMemcpy(dm + o_qtaps, k.rev_q15, taps_len * sizeof(short2), cudaMemcpyHostToDevice));
+  if (q15) {
+    CU_TRY(cudaMemcpy(dm + o_taps, k.rev_cf32, taps_len * sizeof(float2), cudaMemcpyHostToDevice));
+    CU_TRY(cudaMemcpy(dm + o_qtaps, k.rev_q15, taps_len * sizeof(short2), cudaMemcpyHostToDevice));
+  } else {
+    CU_TRY(cudaMemcpy(dm + o_taps, branches.data(), branches.size() * sizeof(float), cudaMemcpyHostToDevice));
+  }
   if (f->h_mem == nullptr) {
     f->h_bytes = h_in_bytes + h_out_bytes + h_qout_bytes + h_ph_bytes;
     CU_TRY(cudaHostAlloc(&f->h_mem, f->h_bytes, cudaHostAllocMapped));
@@ -634,16 +668,16 @@ int filter_build(xlating *f, int device, uint32_t decimation, const float *taps,
   f->inc_im = k.incr_im;
   f->center_freq = center_freq;
   f->fs = sampling_freq;
-  f->tail.assign(taps_len - 1, make_float2(0.f, 0.f));  // src/xlating.c:552-565: zero history
+  f->tail.assign((taps_len - 1) / interp, make_float2(0.f, 0.f));  // src/xlating.c:552-565: zero history
   f->d_ring = (float2 *)(dm + o_ring);
   f->ring_cap = cap;
   d.ring = (float2 *)(dm + o_ring);
-  d.qring = (short2 *)(dm + o_qring);
+  d.qring = q15 ? (short2 *)(dm + o_qring) : nullptr;
   d.taps = (const float2 *)(dm + o_taps);
-  d.qtaps = (const short2 *)(dm + o_qtaps);
+  d.qtaps = q15 ? (const short2 *)(dm + o_qtaps) : nullptr;
   d.phases = (float2 *)(dm + o_ph);
   d.phases_host = (const float2 *)(hm_dev + h_in_bytes + h_out_bytes + h_qout_bytes);
-  d.qphases = (short2 *)(dm + o_qph);
+  d.qphases = q15 ? (short2 *)(dm + o_qph) : nullptr;
   d.out = (float2 *)(hm_dev + h_in_bytes);
   d.qout = (short2 *)(hm_dev + h_in_bytes + h_out_bytes);
   d.hist = f->hist;
@@ -655,6 +689,7 @@ int filter_build(xlating *f, int device, uint32_t decimation, const float *taps,
   d.D = (int)decimation;
   d.T = (int)taps_len;
   d.out_cap = f->out_cap;
+  d.L = (int)interp;
   {
     std::lock_guard<std::mutex> lk(f->e->mu);
     if (f->e->free_slots.empty()) {
@@ -707,6 +742,14 @@ void run_block_group(xlating *f, int fmt, const void *input, size_t input_len, u
 void run_block(xlating *f, int fmt, const void *input, size_t input_len, bool q15, void **output,
                size_t *output_len) {
   *output_len = 0;
+  if (q15 && f->L > 1) {
+    // the Q15 path serves integer filters only: refuse before anything is consumed, so that the
+    // filter's cf32 stream (and its place in the band's group) carries on as if this call never happened
+    if (!f->q15_refused) XL_LOG("Q15 output is not available for a rational (L = %u) filter; use process_*_cf32", f->L);
+    f->q15_refused = true;
+    *output = (void *)f->h_qout;
+    return;
+  }
   if (f->group != nullptr) {
     run_block_group(f, fmt, input, input_len, q15 ? XLG_PATH_Q15 : 0, output, output_len);
     return;
@@ -735,8 +778,8 @@ void run_block(xlating *f, int fmt, const void *input, size_t input_len, bool q1
     const uint64_t t_call = AutoStream::now_ns();
     if (f->as_m.member && as->member_call(f->as_m, input, bytes, fmt, elems, &sv) == 1) {
       // the group computed this block for every member; take this filter's row and state
-      const long long first = f->S - f->hist;
-      const long long last_ok = f->S + n - f->T;
+      const long long first = f->S * f->L - f->hist;
+      const long long last_ok = (f->S + n) * f->L - f->T;
       size_t want = 0, got = 0;
       if (last_ok >= first) want = (size_t)((last_ok - first) / (long long)f->D) + 1;
       xlg_client_state st;
@@ -769,9 +812,10 @@ void run_block(xlating *f, int fmt, const void *input, size_t input_len, bool q1
   if (e->share_inputs && bytes >= kShareMinBytes && e->live_filters.load() >= 2) slot = e->cache->acquire(input, bytes);
   if (slot < 0) memcpy(f->h_in, input, bytes);
   const long long S = q15 ? f->qS : f->S;
-  // host mirror of the output count (the oscillator lane uses the same integers)
-  const long long first = S - f->hist;
-  const long long last_ok = S + n - f->T;
+  // host mirror of the output count (the oscillator lane uses the same integers, in upsampled
+  // samples: L = 1 for the Q15 path)
+  const long long first = S * f->L - f->hist;
+  const long long last_ok = (S + n) * f->L - f->T;
   int n_out = 0;
   if (last_ok >= first) n_out = (int)((last_ok - first) / (long long)f->D) + 1;
   if (n_out > f->out_cap) n_out = f->out_cap;
@@ -800,7 +844,7 @@ void run_block(xlating *f, int fmt, const void *input, size_t input_len, bool q1
   const int rc = e->combiner->run(&f->call);
   if (slot >= 0) e->cache->release(slot);
   // the samples are consumed whatever happened to the launch
-  f->hist = (S + n) - (first + (long long)n_out * (long long)f->D);
+  f->hist = (S + n) * f->L - (first + (long long)n_out * (long long)f->D);
   if (q15)
     f->qS += n;
   else
@@ -809,7 +853,7 @@ void run_block(xlating *f, int fmt, const void *input, size_t input_len, bool q1
     tail_push(f, fmt, input, (size_t)n);
     if (as != nullptr && rc == 0) {
       if (!observed) as->private_observe(f->as_m, input, bytes, fmt, (size_t)n * 2, /*retry=*/true);
-      as->try_join(f->as_m, (int64_t)f->T - 1, (int64_t)f->S, f);
+      as->try_join(f->as_m, ((int64_t)f->T - 1) / f->L, (int64_t)f->S, f);  // the mirror's tail
     }
   }
   if (rc != 0) {
@@ -817,6 +861,39 @@ void run_block(xlating *f, int fmt, const void *input, size_t input_len, bool q1
     return;
   }
   *output_len = (size_t)n_out;
+}
+
+// Both constructors after their argument checks: adopts `taps`.
+int create_filter(uint32_t interp, uint32_t decimation, float *taps, size_t taps_len, int32_t center_freq,
+                  uint32_t sampling_freq, uint32_t max_input_buffer_length, xlating **filter) {
+  xlating *f = new (std::nothrow) xlating_t();
+  if (f == NULL) {
+    return -ENOMEM;
+  }
+  f->adopted_taps = taps;
+  f->call.user = f;
+  f->L = interp;
+  int device = 0;
+  const char *env = getenv("XLATING_B200_DEVICE");
+  if (env != NULL) {
+    device = atoi(env);
+  }
+  const uint32_t max_in = max_input_buffer_length < 2 ? 2 : max_input_buffer_length;
+  int rc;
+  if (use_group_model()) {
+    rc = xlg_create(device, sampling_freq, max_in, 0, &f->group);
+    if (rc == 0)
+      rc = interp == 1 ? xlg_add_client(f->group, decimation, taps, taps_len, center_freq, &f->client)
+                       : xlg_add_client_rational(f->group, interp, decimation, taps, taps_len, center_freq, &f->client);
+  } else {
+    rc = filter_build(f, device, interp, decimation, taps, taps_len, center_freq, sampling_freq, max_in);
+  }
+  if (rc != 0) {
+    filter_release(f);
+    return rc;
+  }
+  *filter = f;
+  return 0;
 }
 
 }  // namespace
@@ -833,31 +910,34 @@ int create_frequency_xlating_filter(uint32_t decimation, float *taps, size_t tap
   if (filter == NULL || taps == NULL) {
     return -EINVAL;
   }
-  xlating *f = new (std::nothrow) xlating_t();
-  if (f == NULL) {
-    return -ENOMEM;
+  return create_filter(1, decimation, taps, taps_len, center_freq, sampling_freq, max_input_buffer_length, filter);
+}
+
+int create_rational_frequency_xlating_filter(uint32_t interpolation, uint32_t decimation, float *taps,
+                                             size_t taps_len, int32_t center_freq, uint32_t sampling_freq,
+                                             uint32_t max_input_buffer_length, xlating **filter) {
+  if (taps_len == 0) {
+    return -1;  // as create_frequency_xlating_filter (taps NOT adopted on this path)
   }
-  f->adopted_taps = taps;
-  f->call.user = f;
-  int device = 0;
-  const char *env = getenv("XLATING_B200_DEVICE");
-  if (env != NULL) {
-    device = atoi(env);
+  if (filter == NULL || taps == NULL) {
+    return -EINVAL;
   }
+  // the batch group's rules (xlg_add_client_rational), checked before any CUDA call
   const uint32_t max_in = max_input_buffer_length < 2 ? 2 : max_input_buffer_length;
-  int rc;
-  if (use_group_model()) {
-    rc = xlg_create(device, sampling_freq, max_in, 0, &f->group);
-    if (rc == 0) rc = xlg_add_client(f->group, decimation, taps, taps_len, center_freq, &f->client);
-  } else {
-    rc = filter_build(f, device, decimation, taps, taps_len, center_freq, sampling_freq, max_in);
+  const char *why = NULL;
+  if (interpolation == 0 || decimation == 0)
+    why = "interpolation and decimation must both be at least 1";
+  else if ((uint64_t)interpolation * sampling_freq > UINT32_MAX)
+    why = "the upsampled rate interpolation x sampling_freq exceeds UINT32_MAX";
+  else if ((uint64_t)interpolation * (max_in / 2) >= (1ull << 31))
+    why = "interpolation x max_input_buffer_length / 2 upsampled samples per call reach 2^31";
+  if (why != NULL) {
+    XL_LOG("rational filter %u/%u at %u Hz, blocks of %u: %s", interpolation, decimation, sampling_freq, max_in, why);
+    free(taps);  // adopted, as on every other failure but taps_len == 0
+    return -EINVAL;
   }
-  if (rc != 0) {
-    filter_release(f);
-    return rc;
-  }
-  *filter = f;
-  return 0;
+  return create_filter(interpolation, decimation, taps, taps_len, center_freq, sampling_freq,
+                       max_input_buffer_length, filter);
 }
 
 void destroy_xlating(xlating *filter) {

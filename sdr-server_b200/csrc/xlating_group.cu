@@ -1554,6 +1554,12 @@ extern "C" int xlg_add_client_ex(xlg_group *g, uint32_t decimation, const float 
 
 extern "C" int xlg_add_client_rational(xlg_group *g, uint32_t interp, uint32_t decim, const float *taps,
                                        size_t taps_len, int32_t center_freq, int *client_id) {
+  return xlg_add_client_rational_ex(g, interp, decim, taps, taps_len, center_freq, nullptr, client_id);
+}
+
+extern "C" int xlg_add_client_rational_ex(xlg_group *g, uint32_t interp, uint32_t decim, const float *taps,
+                                          size_t taps_len, int32_t center_freq, const xlg_client_state *state,
+                                          int *client_id) {
   if (g == nullptr || client_id == nullptr) return -EINVAL;
   if (interp == 0 || decim == 0) {
     XL_LOG("rational client: interpolation %u and decimation %u must both be at least 1", interp, decim);
@@ -1567,10 +1573,12 @@ extern "C" int xlg_add_client_rational(xlg_group *g, uint32_t interp, uint32_t d
     XL_LOG("rational client: %u x %u samples per block upsampled exceed 2^31", interp, g->max_input_len / 2);
     return -EINVAL;
   }
-  if (interp == 1) return xlg_add_client(g, decim, taps, taps_len, center_freq, client_id);
+  if (interp == 1) return xlg_add_client_ex(g, decim, taps, taps_len, center_freq, state, client_id);
+  // state->hist is in upsampled samples, state->valid_history in input samples (the ring's unit)
+  if (state != nullptr && (state->hist < 0 || state->valid_history < 0 || (size_t)state->hist > taps_len)) return -EINVAL;
   if (taps_len == 0 || taps == nullptr) return -1;  // as xlg_add_client (src/xlating.c:496)
   if (taps_len > (size_t)INT32_MAX) return -EINVAL;
-  return attach_client(g, interp, decim, interp * g->fs, taps, taps_len, center_freq, nullptr, client_id);
+  return attach_client(g, interp, decim, interp * g->fs, taps, taps_len, center_freq, state, client_id);
 }
 
 extern "C" int xlg_reserve(xlg_group *g, size_t output_samples_per_block) {

@@ -275,9 +275,8 @@ fir_poly_generic_cf32_kernel(const ClientDev *__restrict__ cl, const int *__rest
   const int rho = q / groups;
   const int k0 = rho + (q - rho * groups) * G_OPW * L;
   if (k0 >= b.n_out) return;
-  const long long w = b.first + (long long)k0 * M;
-  const int r = (int)((((-w) % L) + L) % L);       // floor semantics: w < 0 inside the first block
-  const long long n0 = (w + r) / L;
+  long long n0;
+  const int r = poly_branch(b.first + (long long)k0 * M, L, &n0);
   const int Tb = (d->T + L - 1) / L;
   const float2 mine = fir_warp_cf32(ring, mask, d->zero_before, taps + d->taps_off + (size_t)r * Tb, Tb, M, n0, lane);
   const int k = k0 + lane * L;

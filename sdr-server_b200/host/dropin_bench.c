@@ -5,7 +5,11 @@
  * batch binding.  Measures what sdr-server gets by only re-linking against
  * libxlating_b200.so (INTEGRATION.md section 1).
  *
- * usage: dropin_bench <clients> <blocks> [window [warmup_blocks]]     (2.016 Msps cu8, 48/96 ksps mixed)
+ * usage: dropin_bench <clients> <blocks> [window [warmup_blocks [rational]]]
+ *
+ * Default workload: 2.016 Msps cu8, 48/96 ksps clients mixed.  With `rational` as the fifth argument:
+ * 48 ksps clients of a 2.048 Msps cu8 stream, each a rational 3/128 filter
+ * (create_rational_frequency_xlating_filter) with taps designed at 3 x 2.048 MHz with gain 3.
  *
  * The timed region starts after `warmup_blocks` (default 16) blocks have gone through the same
  * threads: a server's one-time start-up work -- the first CUDA call of every dsp thread, the
@@ -90,6 +94,7 @@ int main(int argc, char **argv) {
   g_window = argc > 3 ? atoi(argv[3]) : 0;
   g_warmup = argc > 4 ? atoi(argv[4]) : 16;
   if (g_warmup < 1) g_warmup = 1;
+  const int rational = argc > 5 && strcmp(argv[5], "rational") == 0;
   g_clients = n_clients;
   g_blocks = n_blocks + g_warmup; /* warm-up blocks first, then the timed ones */
   pthread_barrier_init(&g_warm_barrier, NULL, (unsigned)n_clients + 1);
@@ -97,7 +102,8 @@ int main(int argc, char **argv) {
   g_queue = (sem_t *)calloc((size_t)n_clients, sizeof(sem_t));
   for (int c = 0; c < n_clients; c++) sem_init(&g_queue[c], 0, 0);
   sem_init(&g_sdr, 0, 0);
-  const uint32_t fs = 2016000;
+  const uint32_t fs = rational ? 2048000 : 2016000;
+  const uint32_t interp = 3, decim = 128; /* rational: 2.048 MHz * 3 / 128 = 48 kHz */
   uint8_t *master[4];
   uint64_t s = 0x9E3779B97F4A7C15ull;
   for (int i = 0; i < 4; i++) {
@@ -111,13 +117,20 @@ int main(int argc, char **argv) {
   }
   client_t *clients = (client_t *)calloc((size_t)n_clients, sizeof(client_t));
   for (int c = 0; c < n_clients; c++) {
-    const uint32_t rate = (c % 2 == 0) ? 48000 : 96000;
+    const uint32_t rate = (rational || c % 2 == 0) ? 48000 : 96000;
     float *taps = NULL;
     size_t len = 0;
-    if (create_low_pass_filter(1.0f, fs, rate / 2, rate / 5, &taps, &len) != 0) return 1;
     const int32_t center = (int32_t)(-(int32_t)fs / 2 + (int32_t)rate / 2 +
                                      (int64_t)c * (fs - rate) / (n_clients > 1 ? n_clients - 1 : 1));
-    if (create_frequency_xlating_filter(fs / rate, taps, len, center, fs, BLOCK, &clients[c].filter) != 0) {
+    int rc;
+    if (rational) {
+      if (create_low_pass_filter((float)interp, interp * fs, rate / 2, rate / 5, &taps, &len) != 0) return 1;
+      rc = create_rational_frequency_xlating_filter(interp, decim, taps, len, center, fs, BLOCK, &clients[c].filter);
+    } else {
+      if (create_low_pass_filter(1.0f, fs, rate / 2, rate / 5, &taps, &len) != 0) return 1;
+      rc = create_frequency_xlating_filter(fs / rate, taps, len, center, fs, BLOCK, &clients[c].filter);
+    }
+    if (rc != 0) {
       fprintf(stderr, "create failed for client %d\n", c);
       return 1;
     }
@@ -168,12 +181,12 @@ int main(int argc, char **argv) {
                     "block: copy %.1f us, submit %.1f us, wait GPU %.1f us\n",
             ns[0] / 1e3 / st[0], ns[2] / 1e3 / st[0], ns[3] / 1e3 / st[0], ns[1] / 1e3 / st[0], ns[4] / 1e3 / st[1],
             ns[5] / 1e3 / st[1], ns[6] / 1e3 / st[1]);
-  printf("{\"bench\": \"dropin_thread_per_client\", \"simd_status\": \"%s\", \"clients\": %d, \"blocks\": %d, \"window\": %d, "
+  printf("{\"bench\": \"dropin_thread_per_client\", \"workload\": \"%s\", \"simd_status\": \"%s\", \"clients\": %d, \"blocks\": %d, \"window\": %d, "
          "\"seconds\": %.4f, \"input_msps\": %.2f, \"calls_per_s\": %.0f, \"us_per_call_per_thread\": %.1f, "
          "\"outputs\": %llu, \"launch_batches\": %llu, \"engine_calls\": %llu, \"shared_inputs\": %llu, "
          "\"stream_served\": %llu, \"stream_blocks\": %llu, \"stream_hits\": %llu, \"stream_desyncs\": %llu, "
          "\"stream_joins\": %llu, \"stream_members\": %llu}\n",
-         SIMD_STATUS, n_clients, n_blocks, g_window, dt, n_blocks * (BLOCK / 2) / dt / 1e6, (double)n_clients * n_blocks / dt,
+         rational ? "rational_3_128_of_2048k" : "integer_48k_96k_of_2016k", SIMD_STATUS, n_clients, n_blocks, g_window, dt, n_blocks * (BLOCK / 2) / dt / 1e6, (double)n_clients * n_blocks / dt,
          dt / n_blocks * 1e6, (unsigned long long)outputs, (unsigned long long)batches, (unsigned long long)calls,
          (unsigned long long)shared, (unsigned long long)st[0], (unsigned long long)st[1], (unsigned long long)st[2],
          (unsigned long long)st[3], (unsigned long long)st[4], (unsigned long long)st[6]);
