@@ -15,6 +15,10 @@ usage: _dropin_rational_worker.py <scenario> [arg]   -> one JSON line, exit code
   neighbours               integer filters give the same bits with rational filters alive
   overlay steady|drops|late|lag   24 rational + 4 integer filters of one band, exact stimuli
   q15refuse                a refused Q15 call leaves a member filter's stream untouched
+  wide                     exact stimuli at L from 4 to 441 (L >= 16: a call's span of residues is cut at 16;
+                           calls with fewer outputs than L), every output equal to the float64 sum
+  phase                    branch-one-hot filters at nonzero centres on a real cs16 stream: every output equal
+                           to the strict oracle on the zero-stuffed stream bit for bit (oscillator included)
 """
 import importlib
 import json
@@ -29,8 +33,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from oracle import pyoracle as po  # noqa: E402  (checker)
-from exact import assert_exact, dyadic_taps, exact_input, grid_step, ref_f64  # noqa: E402
-from rational import ROWS, oracle_filter, stuff  # noqa: E402
+from exact import assert_exact, dyadic_taps, exact_input, grid_step  # noqa: E402
+from rational import (ROWS, branch_one_hot_taps, oracle_filter, real_grid_input, ref_rational_f64,  # noqa: E402
+                      stuff)
 from util import assert_cf32_close, rand_block  # noqa: E402
 
 pkg = importlib.import_module("sdr-server_b200")
@@ -69,9 +74,18 @@ class F:
 
     def check_exact(self, what):
         L = max(self.L, 1)
-        assert_exact(self.got, ref_f64(self.taps, self.M, "cs16", [stuff(self.fmt, x, L) for x in self.seen]),
+        assert_exact(self.got, ref_rational_f64(self.taps, L, self.M, self.fmt, self.seen),
                      f"{what} L={L} M={self.M} T={self.taps.size} {self.fmt}", self.taps.size, self.M,
                      grid_step(self.taps, self.fmt))
+
+    def check_oracle_exact(self, fs, max_in, what):
+        L = max(self.L, 1)
+        assert self.taps.size >= self.M  # the oracle's history bookkeeping underflows with fewer taps
+        o = oracle_filter(po, L, self.M, self.taps, self.center, fs, max_in)
+        ref = [o.process_cf32("cs16", stuff(self.fmt, x, L)) for x in self.seen]
+        o.close()
+        assert_exact(self.got, ref, f"{what} L={L} M={self.M} T={self.taps.size} centre {self.center}",
+                     self.taps.size, self.M)
 
     def check_oracle(self, fs, max_in, what):
         L = max(self.L, 1)
@@ -296,6 +310,45 @@ def scenario_q15refuse():
         checked(errors, f.check_exact, f"filter {i}")
         f.close()
     return {"errors": errors, "refused": refused, "stream": stream}
+
+
+# (L, M, T): the drop-in span boundary (16, 17), the batch engine's class budget (36, 37), gcd(L, M) = 2,
+# 48 kHz from 44.1 kHz and back, 44.1 kHz from 2.048 Msps (T < M, fewer outputs than L per call), T < L
+WIDE = [(16, 15, 97), (17, 16, 200), (36, 35, 300), (37, 36, 300), (6, 256, 400), (4, 2, 9), (160, 147, 1000),
+        (147, 160, 1000), (441, 20480, 2000), (17, 16, 5)]
+# T >= M for the strict oracle
+PHASE = [(3, 128, 385), (7, 320, 431), (17, 16, 200), (6, 256, 401), (16, 15, 97), (36, 35, 300), (37, 36, 300),
+         (160, 147, 1000)]
+
+
+def scenario_wide():
+    errors, spans = [], 0
+    for fmt in ("cu8", "cs8", "cs16"):
+        rng = np.random.default_rng(59)
+        filters = exact_filters(rng, fmt, 2048000, 16384, WIDE, 2)
+        blocks = [exact_input(rng, fmt, n) for n in SMALL * 2]
+        errors += run_threads(filters, lambda i, b: blocks[b], len(blocks))
+        for i, f in enumerate(filters):
+            checked(errors, f.check_exact, f"filter {i}")
+            spans += sum(len(y) > f.L > 16 for y in f.got)
+            f.close()
+    few = sum(0 < len(y) < 441 for y in filters[WIDE.index((441, 20480, 2000))].got)
+    return {"errors": errors, "long_spans": spans, "fewer_than_L": few}
+
+
+def scenario_phase():
+    fs, max_in = 2048000, 16384
+    rng = np.random.default_rng(67)
+    filters = []
+    for k, (L, M, T) in enumerate(PHASE * 2):
+        center = int(rng.integers(-fs // 2 + 30000, fs // 2 - 30000))
+        filters.append(F(L, M, branch_one_hot_taps(rng, T, L), center, fs, max_in, "cs16"))
+    blocks = [real_grid_input(rng, n) for n in SMALL * 2]
+    errors = run_threads(filters, lambda i, b: blocks[b], len(blocks))
+    for i, f in enumerate(filters):
+        checked(errors, f.check_oracle_exact, fs, max_in, f"filter {i}")
+        f.close()
+    return {"errors": errors, "stream": pkg.dropin_stream_stats()}
 
 
 def main():

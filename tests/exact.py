@@ -206,6 +206,45 @@ def oracle_phases(inc, counts, renorm=True):
     return np.array(out, dtype=np.complex128)
 
 
+def _f32(v):
+    return np.asarray(v, dtype=np.float32)
+
+
+def _fma(a, b, c):
+    # exact product of two float32 numbers in float64, one rounding to float32 (exact for the sums here:
+    # one of the addends is always zero)
+    return _f32(a.astype(np.float64) * b.astype(np.float64) + c.astype(np.float64))
+
+
+def _cmul(a_re, a_im, b_re, b_im):
+    return (_f32(_f32(a_re * b_re) - _f32(a_im * b_im)), _f32(_f32(a_re * b_im) + _f32(a_im * b_re)))
+
+
+def gpu_model(rev, inc, D, blocks, renorm=True):
+    """What the kernels compute: fmaf chains per accumulator, then the unfused derotation by the
+    float32 oscillator recursion."""
+    T = rev.size
+    tr, ti = _f32(rev.real), _f32(rev.imag)
+    x = np.concatenate([np.zeros(T - 1, np.complex64)] + [to_complex("cs16", b).astype(np.complex64) for b in blocks])
+    n_in = np.cumsum([b.size // 2 for b in blocks])
+    done = np.where(n_in >= 1, (n_in - 1) // D + 1, 0)
+    total = int(done[-1])
+    W = np.lib.stride_tricks.sliding_window_view(x, T)[np.arange(total) * D]
+    xr, xi = _f32(W.real), _f32(W.imag)
+    are = np.zeros(total, np.float32)
+    aim = np.zeros(total, np.float32)
+    for j in range(T):
+        are = _fma(xr[:, j], np.full(total, tr[j]), are)
+        are = _fma(-xi[:, j], np.full(total, ti[j]), are)
+        aim = _fma(xr[:, j], np.full(total, ti[j]), aim)
+        aim = _fma(xi[:, j], np.full(total, tr[j]), aim)
+    ph = oracle_phases(inc, np.diff(np.concatenate([[0], done])), renorm)
+    yr, yi = _cmul(are, aim, _f32(ph.real), _f32(ph.imag))
+    y = (yr + 1j * yi.astype(np.complex64)).astype(np.complex64)
+    out = np.split(y, np.cumsum(np.diff(np.concatenate([[0], done])))[:-1])
+    return out
+
+
 def assert_exact(got, ref, what="", T=None, D=None, step=None):
     """Bit-for-bit equality of per-block outputs (+0 and -0 count as equal).
 

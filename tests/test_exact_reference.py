@@ -12,8 +12,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from exact import (assert_exact, dyadic_taps, exact_input, grid_step, one_hot_taps, real_input, ref_f64,
-                   oracle_phases, oscillator_increment, ref_q15, reversed_taps, tap_bits, to_complex)
+from exact import (assert_exact, dyadic_taps, exact_input, gpu_model, grid_step, one_hot_taps, real_input, ref_f64,
+                   oscillator_increment, ref_q15, reversed_taps, tap_bits, to_complex)
 from oracle import pyoracle as po
 from util import assert_cf32_close, rand_block
 
@@ -98,45 +98,6 @@ def test_ref_f64_history_equals_oracle_state():
 # ---------------------------------------------------------------------------
 # one-hot taps, real input, any centre: FMA accumulation == the oracle's unfused sums
 # ---------------------------------------------------------------------------
-def _f32(v):
-    return np.asarray(v, dtype=np.float32)
-
-
-def _fma(a, b, c):
-    # exact product of two float32 numbers in float64, one rounding to float32 (exact for the sums here:
-    # one of the addends is always zero)
-    return _f32(a.astype(np.float64) * b.astype(np.float64) + c.astype(np.float64))
-
-
-def _cmul(a_re, a_im, b_re, b_im):
-    return (_f32(_f32(a_re * b_re) - _f32(a_im * b_im)), _f32(_f32(a_re * b_im) + _f32(a_im * b_re)))
-
-
-def gpu_model(rev, inc, D, blocks, renorm=True):
-    """What the kernels compute: fmaf chains per accumulator, then the unfused derotation by the
-    float32 oscillator recursion."""
-    T = rev.size
-    tr, ti = _f32(rev.real), _f32(rev.imag)
-    x = np.concatenate([np.zeros(T - 1, np.complex64)] + [to_complex("cs16", b).astype(np.complex64) for b in blocks])
-    n_in = np.cumsum([b.size // 2 for b in blocks])
-    done = np.where(n_in >= 1, (n_in - 1) // D + 1, 0)
-    total = int(done[-1])
-    W = np.lib.stride_tricks.sliding_window_view(x, T)[np.arange(total) * D]
-    xr, xi = _f32(W.real), _f32(W.imag)
-    are = np.zeros(total, np.float32)
-    aim = np.zeros(total, np.float32)
-    for j in range(T):
-        are = _fma(xr[:, j], np.full(total, tr[j]), are)
-        are = _fma(-xi[:, j], np.full(total, ti[j]), are)
-        aim = _fma(xr[:, j], np.full(total, ti[j]), aim)
-        aim = _fma(xi[:, j], np.full(total, tr[j]), aim)
-    ph = oracle_phases(inc, np.diff(np.concatenate([[0], done])), renorm)
-    yr, yi = _cmul(are, aim, _f32(ph.real), _f32(ph.imag))
-    y = (yr + 1j * yi.astype(np.complex64)).astype(np.complex64)
-    out = np.split(y, np.cumsum(np.diff(np.concatenate([[0], done])))[:-1])
-    return out
-
-
 @pytest.mark.parametrize("center", [-987654, -312000, 1, 400123, 1007999])
 @pytest.mark.parametrize("j", [0, 100, 252])
 def test_one_hot_real_input_fma_matches_oracle(center, j):

@@ -71,6 +71,22 @@ def test_exact_stimuli_every_format(env):
         assert line["stream"]["served_by_group"] > 0
 
 
+@pytest.mark.parametrize("env", [None, PRIVATE], ids=["overlay", "private"])
+def test_wide_interpolations_exact(env):
+    """L from 4 to 441 on exact stimuli: dropin_fir_poly_kernel's span of residues cut at 16 (L >= 16) and
+    calls with fewer outputs than L (441/20480)."""
+    line = run("wide", env=env)
+    assert line["long_spans"] > 0 and line["fewer_than_L"] > 0
+
+
+@pytest.mark.parametrize("stream", ["1", "0"], ids=["overlay", "private"])
+@pytest.mark.parametrize("osc", ["host", "device", "lanes"])
+def test_phase_one_hot_at_any_centre(osc, stream):
+    """Branch-one-hot filters at nonzero centres on a real input equal the strict oracle bit for bit under
+    every oscillator walk (the host one mirrors the output count in upsampled coordinates)."""
+    run("phase", env={"XLATING_B200_OSC": osc, "XLATING_B200_STREAM": stream})
+
+
 def test_combined_calls_mix_rational_integer_and_q15():
     """24 threads released together; one launch lane, so calls that overlap must share a batch."""
     line = run("combined", env={**PRIVATE, "XLATING_B200_LANES": "1"})
