@@ -67,6 +67,29 @@ constexpr int kTileMaxSmem = 200 * 1024;
 // shared memory of an SM (CTAs get kSmSmem / n - 1 KiB each at n per SM)
 constexpr int kSmSmem = 228 * 1024;
 
+// The tiled FIR's shapes, largest tile first.  min_ctas = CTAs per SM whose shared memory the
+// shape needs (0: any); code = LO*100 + RK*10 + OS, the value XLATING_B200_TILE pins it by.
+struct TileShapeHost {
+  int lo, rk, os, min_ctas;
+  decltype(&fir_tile_cf32_kernel<16, 1, 1>) kernel;
+  int threads;
+  int kt() const { return lo * rk * os; }
+  int code() const { return lo * 100 + rk * 10 + os; }
+};
+#define XL_TILE_SHAPE(LO_, RK_, OS_, MIN_CTAS_) \
+  {LO_, RK_, OS_, MIN_CTAS_, fir_tile_cf32_kernel<LO_, RK_, OS_>, TileShape<LO_, RK_, OS_>::kThreads}
+const TileShapeHost kTileShapes[] = {XL_TILE_SHAPE(16, 4, 2, 3), XL_TILE_SHAPE(16, 4, 1, 0), XL_TILE_SHAPE(16, 2, 1, 0),
+                                     XL_TILE_SHAPE(16, 1, 1, 0)};
+#undef XL_TILE_SHAPE
+constexpr int kTileSmallest = sizeof(kTileShapes) / sizeof(kTileShapes[0]) - 1;
+
+// index into kTileShapes of the shape with this code, -1 if none has it
+int tile_shape_index(int code) {
+  for (int i = 0; i <= kTileSmallest; i++)
+    if (kTileShapes[i].code() == code) return i;
+  return -1;
+}
+
 struct HostClient {
   bool active = false;
   uint32_t D = 0;
@@ -272,17 +295,13 @@ struct xlg_group {
   std::vector<float2> h_taps, h_tile_taps;  // host staging of the tap arenas, kept between re-layouts (no fresh pages)
   std::vector<short2> h_qtaps;
   size_t cap_taps = 0, cap_qtaps = 0, cap_tile_taps = 0, cap_members = 0, cap_member_cid = 0, cap_member_incr = 0;
-  int tile_force = 0;     // XLATING_B200_TILE=<LO*100+RK*10+OS> pins the tile shape (e.g. 3241, 1642, 1641, 1621, 1611)
-  int long_kt = W2_KT;    // output tile of the long-filter kernel: 56 (fir_long3 / fir_long2) or 64 (XLATING_B200_LONG=1)
+  int tile_force = 0;     // XLATING_B200_TILE=<LO*100+RK*10+OS> pins the tile shape (1642, 1641, 1621 or 1611)
   // long4's input strips through a TMA tensor map over the ring (XLATING_B200_LONG_TMAP=0: 28 bulk copies per stage)
   bool long_tmap = true;
   CUtensorMap strip_map;          // valid for (strip_ring, strip_cap, strip_D)
   const void *strip_ring = nullptr;
   size_t strip_cap = 0;
   int strip_D = 0, strip_w = 0;   // strip_w: inner width of the map in samples (0 = could not be encoded)
-  bool long_pk_active = false;  // this layout's long classes ARE packed (packed_long, generation 4, every long D even)
-  bool packed_long = false;  // XLATING_B200_LONG_FFMA2=1: long4 on packed FFMA2 (long classes' taps packed per client pair)
-  int long_gen = 4;       // XLATING_B200_LONG=1|2|3|4: which long-filter kernel (4 = pipelined 28 x 64 tile, the default)
   int fir_sms = 0;        // SMs the FIR kernels can use (all, or all minus the reserved partition)
   int *d_members = nullptr;
   int *d_member_cid = nullptr;      // client id per member slot (-1 = padding)
@@ -294,7 +313,7 @@ struct xlg_group {
   bool q_alloc = false;
 
   std::vector<TileClassHost> classes;
-  std::vector<TileClassHost> long_classes;  // split-K long-filter classes (fir_long_cf32_kernel)
+  std::vector<TileClassHost> long_classes;  // split-K long-filter classes (fir_long4 / fir_long2)
   std::vector<TileClassHost> poly_classes;  // kind 4: one class per (rational class, polyphase branch)
   bool poly_tile = true;                    // XLATING_B200_POLY_TILE=0: every rational client on the generic kernel
   int *d_poly3 = nullptr, *d_poly4 = nullptr;  // ids of the kind-3 / kind-4 clients
@@ -695,12 +714,6 @@ static int rebuild_layout(xlg_group *g) {
     const bool merge = m.natural && !m.as_long && !env_no_merge;
     buckets[std::make_tuple(h.D, h.T, merge ? -1ll : h.hist)].push_back(i);
   }
-  {
-    bool all_even = true;
-    for (auto &kv : buckets)
-      if (mode_of(std::get<0>(kv.first), std::get<1>(kv.first)).as_long && (std::get<0>(kv.first) & 1u)) all_even = false;
-    g->long_pk_active = g->packed_long && g->long_gen == 4 && all_even;
-  }
   std::vector<int> members;       // output row offset per member slot
   std::vector<int> member_cid;    // client id per member slot
   std::vector<float2> member_incr;
@@ -767,7 +780,6 @@ static int rebuild_layout(xlg_group *g) {
     }
     // taps into [group][flat tap f][32 slots]: one 256-byte line (all 32 slots of a tap) at a time -- slot-major
     // packing touched a new cache line for every tap of every client (1.5 ms per re-layout at 1000 clients)
-    const bool pk = m.as_long && g->long_pk_active;
     for (size_t gi = 0; gi < slots.size() / T_CG; gi++) {
       float2 *dst = tile_taps.data() + base + gi * (size_t)m.L * T_CG;
       const float *src[T_CG];
@@ -782,20 +794,9 @@ static int rebuild_layout(xlg_group *g) {
           r = 0;
           q++;
         }
-        if (pk) {
-          // packed long4: a client PAIR's tap is (re0, re1, im0, im1) -- one 128-bit load = two FFMA2 operands
-          float *row = reinterpret_cast<float *>(dst + f * T_CG);
-          for (int sl = 0; sl < T_CG; sl++)
-            if (src[sl]) {
-              float *q4 = row + (sl & ~1) * 2;
-              q4[sl & 1] = src[sl][2 * j];
-              q4[2 + (sl & 1)] = src[sl][2 * j + 1];
-            }
-        } else {
-          float2 *row = dst + f * T_CG;
-          for (int sl = 0; sl < T_CG; sl++)
-            if (src[sl]) row[sl] = make_float2(src[sl][2 * j], src[sl][2 * j + 1]);
-        }
+        float2 *row = dst + f * T_CG;
+        for (int sl = 0; sl < T_CG; sl++)
+          if (src[sl]) row[sl] = make_float2(src[sl][2 * j], src[sl][2 * j + 1]);
       }
     }
     dest.push_back(ch);
@@ -974,7 +975,7 @@ static int rebuild_layout(xlg_group *g) {
       for (TileClassHost &ch : g->long_classes) {
         int cap = 0;
         for (int id : ch.real) cap = std::max(cap, g->clients[id].out_cap);
-        const size_t kt = (size_t)g->long_kt;
+        const size_t kt = (size_t)W2_KT;
         const size_t kpad_max = ((size_t)cap + kt - 1) / kt * kt;
         ch.k.part_off = (long long)part;
         ch.k.kpad = (int)kpad_max;
@@ -1324,14 +1325,15 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
   // the tiled kernel needs > 48 KiB of dynamic shared memory
   {
     const char *tv = getenv("XLATING_B200_TILE");
-    if (tv != nullptr) g->tile_force = atoi(tv);
-    const char *lv = getenv("XLATING_B200_LONG");
-    if (lv != nullptr && atoi(lv) >= 1 && atoi(lv) <= 4) g->long_gen = atoi(lv);  // A/B of the long-filter kernels
-    if (g->long_gen == 1) g->long_kt = W_KT;
+    if (tv != nullptr) {
+      g->tile_force = atoi(tv);
+      if (tile_shape_index(g->tile_force) < 0) {
+        XL_LOG("XLATING_B200_TILE=%s is not a tile shape (1642, 1641, 1621 or 1611); choosing automatically", tv);
+        g->tile_force = 0;
+      }
+    }
     const char *cvs = getenv("XLATING_B200_CONV_STREAM");
     if (cvs != nullptr) g->conv_own_stream = atoi(cvs) != 0;
-    const char *pl = getenv("XLATING_B200_LONG_FFMA2");
-    if (pl != nullptr) g->packed_long = atoi(pl) != 0;
     const char *tm = getenv("XLATING_B200_LONG_TMAP");
     if (tm != nullptr) g->long_tmap = atoi(tm) != 0;
     const char *sv = getenv("XLATING_B200_SPECULATE");
@@ -1341,18 +1343,13 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
     const char *cv = getenv("XLATING_B200_CSTREAMS");
     if (cv != nullptr) g->n_cs = std::min(std::max(atoi(cv), 1), (int)xlg_group::kMaxCs);
   }
-  if (cudaFuncSetAttribute(fir_tile_cf32_kernel<32, 4, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem) != cudaSuccess ||
-      cudaFuncSetAttribute(fir_tile_cf32_kernel<16, 4, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem) != cudaSuccess ||
-      cudaFuncSetAttribute(fir_tile_cf32_kernel<16, 4, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem) != cudaSuccess ||
-      cudaFuncSetAttribute(fir_tile_cf32_kernel<16, 2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem) != cudaSuccess ||
-      cudaFuncSetAttribute(fir_tile_cf32_kernel<16, 1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem) != cudaSuccess ||
-      cudaFuncSetAttribute(fir_long_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(fir_long2_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W2_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(fir_long3_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W3_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(fir_long4_cf32_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, W4_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(fir_long4_cf32_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, W4_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(fir_long4_cf32_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, W4_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(fir_long4_cf32_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, W4_SMEM) != cudaSuccess) {
+  for (const TileShapeHost &sh : kTileShapes)
+    if (cudaFuncSetAttribute(sh.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem) != cudaSuccess) {
+      XL_LOG("cannot raise dynamic shared memory to %d bytes", kTileMaxSmem);
+      return fail(-EIO);
+    }
+  if (cudaFuncSetAttribute(fir_long2_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W2_SMEM) != cudaSuccess ||
+      cudaFuncSetAttribute(fir_long4_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W4_SMEM) != cudaSuccess) {
     XL_LOG("cannot raise dynamic shared memory to %d bytes", kTileMaxSmem);
     return fail(-EIO);
   }
@@ -1859,47 +1856,40 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     // Measured on cfg2: an isolated launch takes ~94 us with every shape -- finer tiles
     // balance better but pay more shared loads per FMA -- while in steady state, where
     // consecutive blocks overlap, RK = 4 is 25 % faster than RK = 1.)
-    // {LO, RK, OS, CTAs per SM whose shared memory the shape needs (0: any)}.  The 128-output tile of
-    // 4 warps (two output sets) must fit 3 CTAs per SM, and it is taken only when its waves are at
-    // least 70 % full: its CTAs are twice as long, so a thin last wave idles SMs for longer
-    // (measured on H100: cfg2 at 0.80 and c1000 at 0.72 run faster with it, c512 at 0.54 ran 4 % slower).
-    static const int kShapes[][4] = {{16, 4, 2, 3}, {16, 4, 1, 0}, {16, 2, 1, 0}, {16, 1, 1, 0}};
+    // The 128-output tile of 4 warps (two output sets) must fit 3 CTAs per SM, and it is taken only
+    // when its waves are at least 70 % full: its CTAs are twice as long, so a thin last wave idles SMs
+    // for longer (measured on H100: cfg2 at 0.80 and c1000 at 0.72 run faster with it, c512 at 0.54
+    // ran 4 % slower).
     // input tile + tap stages of a class at KT outputs per CTA (the merged layout reads D more samples)
     auto tile_smem = [](const TileClassHost &ch, int KT) {
       return (size_t)T_SMEM_FIXED + ((size_t)(KT - 1) * ch.k.Dp + ch.k.L + ch.k.D + 10) * sizeof(float2);
     };
-    int lo = 16, rk = 1, os = 1;
-    for (const auto &sh : kShapes) {
-      const int kt = sh[0] * sh[1] * sh[2];
+    int si = kTileSmallest;
+    for (int i = 0; i <= kTileSmallest; i++) {
+      const TileShapeHost &sh = kTileShapes[i];
+      const int kt = sh.kt();
       int ctas = 0;
       bool fits = true;
       for (TileClassHost &ch : g->classes) {
         int n_out = 0;
         for (int id : ch.real) n_out = std::max(n_out, ho.n_out[id]);
         if (n_out > 0) ctas += ((n_out + kt - 1) / kt) * ch.k.n_groups;
-        if (sh[3] > 0 && tile_smem(ch, kt) > (size_t)(kSmSmem / sh[3] - 1024)) fits = false;
+        if (sh.min_ctas > 0 && tile_smem(ch, kt) > (size_t)(kSmSmem / sh.min_ctas - 1024)) fits = false;
       }
-      const int slots = sh[3] * g->fir_sms;  // resident CTAs per wave
-      if (sh[3] > 0 && ctas > 0 && 10 * ctas < 7 * ((ctas + slots - 1) / slots) * slots) fits = false;
+      const int slots = sh.min_ctas * g->fir_sms;  // resident CTAs per wave
+      if (sh.min_ctas > 0 && ctas > 0 && 10 * ctas < 7 * ((ctas + slots - 1) / slots) * slots) fits = false;
       if (fits && ctas >= 2 * g->fir_sms) {
-        lo = sh[0];
-        rk = sh[1];
-        os = sh[2];
+        si = i;
         break;
       }
     }
-    if (g->tile_force > 0) {
-      lo = g->tile_force / 100;
-      rk = g->tile_force / 10 % 10;
-      os = g->tile_force % 10;
+    if (g->tile_force > 0) {  // a shape of kTileShapes (checked in xlg_create_ex)
+      si = tile_shape_index(g->tile_force);
       for (TileClassHost &ch : g->classes)  // an experiment must not overflow shared memory
-        if (tile_smem(ch, lo * rk * os) > (size_t)kTileMaxSmem) {
-          lo = 16;
-          rk = 1;
-          os = 1;
-        }
+        if (tile_smem(ch, kTileShapes[si].kt()) > (size_t)kTileMaxSmem) si = kTileSmallest;
     }
-    const int KT = lo * rk * os;
+    const TileShapeHost &shape = kTileShapes[si];
+    const int KT = shape.kt();
     TileLaunch P;
     memset(&P, 0, sizeof(P));
     int ctas = 0;
@@ -1941,20 +1931,8 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
         g->trace_launches++;
         g->trace_ctas = ctas;
       }
-#define XL_LAUNCH_TILE(LO_, RK_, OS_)                                                                        \
-  fir_tile_cf32_kernel<LO_, RK_, OS_><<<ctas, TileShape<LO_, RK_, OS_>::kThreads, smem, cs>>>(                 \
-      P, g->ring, mask, tt, g->d_members, g->d_member_cid, g->d_member_incr, s.d_blk, s.d_phases, s.d_out, trace_ptr)
-      if (lo == 32 && rk == 4 && os == 1)
-        XL_LAUNCH_TILE(32, 4, 1);
-      else if (lo == 16 && rk == 4 && os == 2)
-        XL_LAUNCH_TILE(16, 4, 2);
-      else if (lo == 16 && rk == 4 && os == 1)
-        XL_LAUNCH_TILE(16, 4, 1);
-      else if (lo == 16 && rk == 2 && os == 1)
-        XL_LAUNCH_TILE(16, 2, 1);
-      else
-        XL_LAUNCH_TILE(16, 1, 1);
-#undef XL_LAUNCH_TILE
+      shape.kernel<<<ctas, shape.threads, smem, cs>>>(P, g->ring, mask, tt, g->d_members, g->d_member_cid,
+                                                      g->d_member_incr, s.d_blk, s.d_phases, s.d_out, trace_ptr);
       if (g->profiling || g->timeline) CU_OK(cudaEventRecord(s.pf[5], cs));
     }
   }
@@ -1964,18 +1942,12 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     TileLaunch P;
     memset(&P, 0, sizeof(P));
     int ctas = 0, max_out = 0, max_groups = 0;
-    // the pipelined kernel needs 16-byte aligned strips (even decimation and window start) for its TMA
-    // bulk copies; fir_long2 takes over otherwise (it can fall back to 8-byte cp.async)
-    bool pipelined = g->long_gen >= 3;
-    const bool wide = g->long_gen == 4;  // 28 outputs x 2 groups per CTA instead of 56 x 1
-    for (TileClassHost &ch : g->long_classes) {
-      const HostClient &h0 = g->clients[ch.real[0]];
-      const int n_out = ho.n_out[ch.real[0]];
-      if (n_out <= 0) continue;
-      const long long first = (S + n) - h0.hist - (long long)n_out * (long long)h0.D;
-      // (generation 4 fetches an odd window start from one sample earlier; generation 3 needs it even)
-      if ((h0.D & 1) != 0 || (!wide && (first & 1) != 0)) pipelined = false;
-    }
+    // fir_long4's TMA bulk copies need 16-byte aligned strips: with even D every strip has the parity of
+    // the window start, and an odd start is fetched from one sample earlier.  One odd-D class sends the
+    // whole launch to fir_long2, which falls back to 8-byte cp.async for unaligned strips.
+    bool pipelined = true;
+    for (TileClassHost &ch : g->long_classes)
+      if (ho.n_out[ch.real[0]] > 0 && (g->clients[ch.real[0]].D & 1) != 0) pipelined = false;
     int n_live = 0;
     for (TileClassHost &ch : g->long_classes) n_live += ho.n_out[ch.real[0]] > 0 ? 1 : 0;
     for (TileClassHost &ch : g->long_classes) {
@@ -1985,16 +1957,15 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       TileClass k = ch.k;
       k.first = (S + n) - h0.hist - (long long)n_out * (long long)h0.D;
       k.n_out = n_out;
-      k.tiles = (n_out + g->long_kt - 1) / g->long_kt;
+      k.tiles = (n_out + W2_KT - 1) / W2_KT;
       k.cta_begin = ctas;
       k.nslab = k.nseg;
       k.ksplit = k.nseg;
       k.seg_per = 1;
       if (pipelined) {
         // one resident CTA per SM: as many CTAs along the tap axis as fill one wave of this class's share
-        const int units = wide ? ((n_out + W4_KT - 1) / W4_KT) * ((k.n_groups + W4_GROUPS - 1) / W4_GROUPS)
-                               : k.tiles * k.n_groups;
-        if (wide) k.tiles = (n_out + W4_KT - 1) / W4_KT;  // (kpad, a multiple of 56, covers 2 x 28 too)
+        const int units = ((n_out + W4_KT - 1) / W4_KT) * ((k.n_groups + W4_GROUPS - 1) / W4_GROUPS);
+        k.tiles = (n_out + W4_KT - 1) / W4_KT;  // (kpad, a multiple of 56, covers 2 x 28 too)
         const int share = std::max(1, g->fir_sms / std::max(n_live, 1));
         const int want = std::max(1, share / std::max(1, units));
         k.seg_per = (k.nseg + std::min(want, k.nseg) - 1) / std::min(want, k.nseg);
@@ -2007,39 +1978,24 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       max_out = std::max(max_out, n_out);
       max_groups = std::max(max_groups, k.n_groups);
       P.cls[P.n_classes++] = k;
-      s.tile_macs += (uint64_t)k.tiles * g->long_kt * (uint64_t)k.L * (uint64_t)ch.members.size();
+      s.tile_macs += (uint64_t)k.tiles * W2_KT * (uint64_t)k.L * (uint64_t)ch.members.size();
     }
     if (ctas > 0) {
       if (g->profiling) {
         CU_OK(cudaEventRecord(s.pf[8], cs));
         s.pf_long = true;
       }
-      if (pipelined && wide) {
-        // the first class gets the tensor map for its strips (all long clients of a stream normally share one D)
+      if (pipelined) {
+        // the first class gets the tensor map for its strips (all long clients of a stream normally share one D);
+        // tmap_w = 0 (no map) sends every stage down the per-strip bulk copies
         strip_map_update(g, P.cls[0].D);
         P.cls[0].tmap_w = g->strip_w;
-#define XL_LAUNCH_LONG4(TM_, PK_)                                                                                  \
-  fir_long4_cf32_kernel<TM_, PK_><<<ctas, W3_THREADS, W4_SMEM, cs>>>(P, g->ring, mask, (const float2 *)g->d_tile_taps, \
-                                                                    s.d_partial, g->strip_map)
-        if (g->strip_w > 0 && g->long_pk_active)
-          XL_LAUNCH_LONG4(true, true);
-        else if (g->strip_w > 0)
-          XL_LAUNCH_LONG4(true, false);
-        else if (g->long_pk_active)
-          XL_LAUNCH_LONG4(false, true);
-        else
-          XL_LAUNCH_LONG4(false, false);
-#undef XL_LAUNCH_LONG4
-      }
-      else if (pipelined)
-        fir_long3_cf32_kernel<<<ctas, W3_THREADS, W3_SMEM, cs>>>(P, g->ring, mask, (const float2 *)g->d_tile_taps,
-                                                                s.d_partial);
-      else if (g->long_kt == W2_KT)
+        fir_long4_cf32_kernel<<<ctas, W4_THREADS, W4_SMEM, cs>>>(P, g->ring, mask, (const float2 *)g->d_tile_taps,
+                                                                s.d_partial, g->strip_map);
+      } else {
         fir_long2_cf32_kernel<<<ctas, W2_THREADS, W2_SMEM, cs>>>(P, g->ring, mask, (const float2 *)g->d_tile_taps,
                                                                 s.d_partial);
-      else
-        fir_long_cf32_kernel<<<ctas, W_THREADS, W_SMEM, cs>>>(P, g->ring, mask, (const float2 *)g->d_tile_taps,
-                                                             s.d_partial);
+      }
       dim3 rgrid((max_out + 7) / 8, max_groups, P.n_classes);
       fir_long_reduce_kernel<<<rgrid, 256, 0, cs>>>(P, s.d_partial, g->d_members, g->d_member_incr, s.d_phases,
                                                     s.d_out);

@@ -363,15 +363,12 @@ constexpr int T_MAX_CLASSES = 36;    // (D, T) classes per launch: 36 x 104 byte
 constexpr int T_TRACE_REC = 6;       // long long per CTA in the XLATING_B200_TRACE timeline
 constexpr int T_TRACE_LAUNCHES = 16; // launches kept (ring)
 constexpr int T_TRACE_CTAS = 4096;   // CTAs recorded per launch
-constexpr int T_RK_LONG = 4;         // outputs per thread in the long-filter kernel
 
 // Shape of the tile a CTA computes.  LO = number of output lanes in a warp, RK =
 // outputs per thread; the thread tile is RK outputs x 8 clients, the CTA tile
-// (LO*RK) outputs x 32 clients.
-//   LO = 32: lane = output column; warp = LO*RK outputs x 8 clients, 4 warps per CTA.
-//   LO = 16: lane = (h, o), o = lane & 15 the output column, h = lane >> 4 the client
-//            half; warp = LO*RK outputs x 16 clients, 2 warps per output set.  Both
-//            half-warps read the same x (one shared-memory wavefront instead of two).
+// (LO*RK) outputs x 32 clients.  With LO = 16, lane = (h, o), o = lane & 15 the output
+// column, h = lane >> 4 the client half; warp = LO*RK outputs x 16 clients, 2 warps per
+// output set.  Both half-warps read the same x (one shared-memory wavefront instead of two).
 // OS = output sets: OS groups of those warps take consecutive LO*RK-output ranges of
 // one input tile and share its tap stages.  OS = 2 with RK = 4 (128 outputs, 4 warps,
 // 72 KB at D = 42) runs 3 CTAs per SM with 3 warps on every scheduler, and a CTA that is
@@ -389,7 +386,7 @@ struct TileShape {
   static constexpr int kThreads = kWarps * 32;
   static constexpr int kKT = LO * RK * OS;                   // outputs per CTA
   // CTAs per SM the register budget is set for
-  static constexpr int kMinCtas = LO == 32 || OS == 2 ? 3 : XL_TILE_MINCTAS;
+  static constexpr int kMinCtas = OS == 2 ? 3 : XL_TILE_MINCTAS;
 };
 
 // One class = clients with identical (D, T, window alignment).  "Flat" tap index:
@@ -482,34 +479,6 @@ __device__ __forceinline__ void cp_async_8(void *dst, const void *src) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
 
-// FP32 pairs in one 64-bit register.  sm_90 has no packed FP32 FMA (fma.rn.f32x2 needs
-// sm_100), so a pair is two FFMA with the same rounding: the packed kernels keep their
-// tap layout and stay bit-identical to the scalar ones.
-typedef unsigned long long u64x;
-__device__ __forceinline__ u64x ffma2(u64x a, u64x b, u64x c) {
-  u64x d;
-  asm("{\n"
-      ".reg .f32 a0, a1, b0, b1, c0, c1;\n"
-      "mov.b64 {a0, a1}, %1;\n"
-      "mov.b64 {b0, b1}, %2;\n"
-      "mov.b64 {c0, c1}, %3;\n"
-      "fma.rn.f32 c0, a0, b0, c0;\n"
-      "fma.rn.f32 c1, a1, b1, c1;\n"
-      "mov.b64 %0, {c0, c1};\n"
-      "}"
-      : "=l"(d)
-      : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ u64x pack2f(float lo, float hi) {
-  u64x r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack2f(u64x v, float &lo, float &hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-
 template <int LO, int RK, int OS>
 __global__ void __launch_bounds__(TileShape<LO, RK, OS>::kThreads, TileShape<LO, RK, OS>::kMinCtas)
 fir_tile_cf32_kernel(const __grid_constant__ TileLaunch P, const float2 *__restrict__ ring, unsigned mask,
@@ -530,7 +499,7 @@ fir_tile_cf32_kernel(const __grid_constant__ TileLaunch P, const float2 *__restr
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int o = lane & (LO - 1);   // output column of this lane
-  const int h = lane / LO;         // client half of this lane (0 when LO == 32)
+  const int h = lane / LO;         // client half of this lane
   const int cbase = (warp % S::kClientWarps) * S::kWarpClients + h * T_RC;  // first of this thread's 8 clients in the group
   const int obase = (warp / S::kClientWarps) * (LO * RK);                  // first output of this warp's output set
 
@@ -767,147 +736,31 @@ fir_tile_cf32_kernel(const __grid_constant__ TileLaunch P, const float2 *__restr
 // only ~52 outputs per 256 KiB block: the window of ONE output (123 KB of cf32) does
 // not fit the tiled kernel's shared-memory tile, and (outputs x clients) alone is far
 // too little parallelism for 132 SMs.  So the tap range is cut into segments of W_JS
-// taps and every (segment, client group, output tile) is a CTA:
-//   * the x "strips" of the tile's 64 outputs for this segment (64 x W_JS samples, each
-//     strip contiguous in the ring) arrive by one TMA bulk copy per output row when
-//     the strips are 16-byte aligned (even D and window start), else by 8-byte
-//     cp.async; the segment's taps (W_JS x 32 clients, 32 KiB) by one TMA bulk copy;
-//   * the same 4-output x 8-client register tile and lane mapping (16 output lanes x
-//     2 client halves) as the tiled kernel accumulates the segment;
-//   * partial sums go to [segment][group][output][32 clients] (coalesced);
-// fir_long_reduce_kernel then adds the segments IN ORDER (deterministic), derotates
-// with the oscillator table and stores.  Same arithmetic as the other kernels up to
-// the order of the fp32 additions.
+// taps, CTAs along the tap axis write partial sums to [slab][group][output][32 clients]
+// (coalesced), and fir_long_reduce_kernel adds the slabs IN ORDER (deterministic),
+// derotates with the oscillator table and stores.  Same arithmetic as the other kernels
+// up to the order of the fp32 additions.  Two kernels compute the partial sums, both
+// with a 7-output x 8-client register tile per thread:
+//   * fir_long4 when every long class of the launch has even D (the strips can then be
+//     fetched 16-byte aligned by TMA bulk copies);
+//   * fir_long2 otherwise (it falls back to 8-byte cp.async for unaligned strips).
 // ---------------------------------------------------------------------------
 constexpr int W_JS = 128;             // taps per segment
-constexpr int W_KT = 64;              // outputs per CTA (16 lanes x 4)
-constexpr int W_THREADS = 64;
 constexpr int W_JSP = W_JS + 2;       // strip pitch: 16-byte aligned rows, 2-way conflicts at most
-constexpr int W_SMEM = W_JS * T_CG * 8 + 64 + W_KT * W_JSP * 8;  // 32 KiB taps + barrier + 65 KiB strips
-
-__global__ void __launch_bounds__(W_THREADS, 2)
-fir_long_cf32_kernel(const __grid_constant__ TileLaunch P, const float2 *__restrict__ ring, unsigned mask,
-                     const float2 *__restrict__ tile_taps, float2 *__restrict__ partial) {
-  extern __shared__ __align__(128) unsigned char smem[];
-  float2 *ts = reinterpret_cast<float2 *>(smem);
-  uint64_t *bar = reinterpret_cast<uint64_t *>(smem + W_JS * T_CG * 8);
-  float2 *xs = reinterpret_cast<float2 *>(smem + W_JS * T_CG * 8 + 64);
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int o = lane & 15, h = lane >> 4;
-  const int cbase = warp * 16 + h * T_RC;
-
-  const int ci = class_of_cta(P, (int)blockIdx.x);
-  const TileClass &K = P.cls[ci];
-  const int local = (int)blockIdx.x - K.cta_begin;
-  const int seg = local % K.nseg;
-  const int rest = local / K.nseg;
-  const int tile = rest % K.tiles;
-  const int grp = rest / K.tiles;
-  const int k0 = tile * W_KT;
-  const int f0 = seg * W_JS;
-  const int len = min(W_JS, K.L - f0);  // multiple of 8
-  const int D = K.D;
-
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  __syncthreads();
-
-  const long long w0 = K.first + (long long)k0 * D + f0;  // first sample of strip 0
-  const bool aligned = ((K.first | (long long)D) & 1) == 0;  // f0 and k0*D are even then
-  const unsigned strip_bytes = (unsigned)len * 8u;
-  if (tid == 0) {
-    const unsigned tap_bytes = (unsigned)len * T_CG * 8u;
-    mbar_expect_tx(bar, tap_bytes + (aligned ? W_KT * strip_bytes : 0u));
-    tma_bulk_g2s(ts, tile_taps + K.taps_off + ((long long)grp * K.L + f0) * T_CG, tap_bytes, bar);
-  }
-  __syncthreads();  // expect_tx is posted before any strip copy can complete
-  if (aligned) {
-    // one strip per thread: x[(k0 + tid)*D + f0 .. + len), contiguous in the ring
-    const unsigned idx = (unsigned)((unsigned long long)(w0 + (long long)tid * D)) & mask;
-    const unsigned n1 = min((unsigned)len, mask + 1u - idx);
-    tma_bulk_g2s(xs + tid * W_JSP, ring + idx, n1 * 8u, bar);
-    if (n1 < (unsigned)len) tma_bulk_g2s(xs + tid * W_JSP + n1, ring, ((unsigned)len - n1) * 8u, bar);
-  } else {
-    for (int e = tid; e < W_KT * W_JS; e += W_THREADS) {
-      const int k = e / W_JS, f = e - k * W_JS;
-      if (f < len) {
-        const long long ab = w0 + (long long)k * D + f;
-        cp_async_8(xs + k * W_JSP + f, ring + ((unsigned)((unsigned long long)ab) & mask));
-      }
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    __syncthreads();
-  }
-  mbar_wait(bar, 0);
-
-  float2 acc[T_RK_LONG][T_RC];
-#pragma unroll
-  for (int i = 0; i < T_RK_LONG; i++)
-#pragma unroll
-    for (int c = 0; c < T_RC; c++) acc[i][c] = make_float2(0.f, 0.f);
-  const float2 *xb[T_RK_LONG];
-#pragma unroll
-  for (int i = 0; i < T_RK_LONG; i++) xb[i] = xs + (o + 16 * i) * W_JSP;
-  const float4 *tp = reinterpret_cast<const float4 *>(ts + cbase);
-
-  const bool warp_active = grp * T_CG + warp * 16 < K.n_members;
-  if (warp_active) {
-#pragma unroll 1
-    for (int f = 0; f < len; f += T_UNROLL) {
-#pragma unroll
-      for (int u = 0; u < T_UNROLL; u++) {
-        float2 x[T_RK_LONG];
-        float4 tq[T_RC / 2];
-#pragma unroll
-        for (int i = 0; i < T_RK_LONG; i++) x[i] = xb[i][f + u];
-#pragma unroll
-        for (int q = 0; q < T_RC / 2; q++) tq[q] = tp[(f + u) * (T_CG / 2) + q];
-#pragma unroll
-        for (int i = 0; i < T_RK_LONG; i++) {
-#pragma unroll
-          for (int q = 0; q < T_RC / 2; q++) {
-            float2 &a0 = acc[i][2 * q], &a1 = acc[i][2 * q + 1];
-            a0.x = fmaf(x[i].x, tq[q].x, a0.x);
-            a0.x = fmaf(-x[i].y, tq[q].y, a0.x);
-            a0.y = fmaf(x[i].x, tq[q].y, a0.y);
-            a0.y = fmaf(x[i].y, tq[q].x, a0.y);
-            a1.x = fmaf(x[i].x, tq[q].z, a1.x);
-            a1.x = fmaf(-x[i].y, tq[q].w, a1.x);
-            a1.y = fmaf(x[i].x, tq[q].w, a1.y);
-            a1.y = fmaf(x[i].y, tq[q].z, a1.y);
-          }
-        }
-      }
-    }
-    // partial sums: [segment][group][output][32 clients]
-    float2 *pp = partial + K.part_off + (((long long)seg * K.n_groups + grp) * K.kpad + k0) * T_CG + cbase;
-#pragma unroll
-    for (int i = 0; i < T_RK_LONG; i++) {
-      float4 *row = reinterpret_cast<float4 *>(pp + (size_t)(o + 16 * i) * T_CG);
-#pragma unroll
-      for (int q = 0; q < T_RC / 2; q++)
-        row[q] = make_float4(acc[i][2 * q].x, acc[i][2 * q].y, acc[i][2 * q + 1].x, acc[i][2 * q + 1].y);
-    }
-  }
-}
 
 // ---------------------------------------------------------------------------
-// long filters, second generation (the default): the same split-K scheme with
-//   * 4 warps per CTA that split the CTA's 128-tap segment four ways (32 taps each) and
-//     add their partial sums through shared memory in a fixed order -- two CTAs = 8 warps
-//     per SM instead of 4 (the first kernel's one warp per scheduler left the FMA pipe
-//     half idle);
+// fir_long2: one CTA per (segment, client group, 56-output tile):
+//   * the x "strips" of the tile's 56 outputs for this segment (each strip contiguous in
+//     the ring) arrive by one TMA bulk copy per output row when the strips are 16-byte
+//     aligned (even D and window start), else by 8-byte cp.async; the segment's taps
+//     (W_JS x 32 clients, 32 KiB) by one TMA bulk copy;
+//   * 4 warps per CTA split the 128-tap segment four ways (32 taps each) and add their
+//     partial sums through shared memory in a fixed order -- two CTAs = 8 warps per SM
+//     (one warp per scheduler leaves the FMA pipe half idle);
 //   * a 56-output tile (8 output lanes x 7 outputs per thread; lane = (client octet,
 //     output column), a warp covers all 32 clients): BASELINE configs[4] produces 51-52
-//     outputs per 256 KiB block, which wasted 19 % of a 64-output tile and wastes 7 % of
-//     this one; per tap a thread issues 7 + 4 shared loads for 224 FFMA (8 for 128 before).
-// Partial sums, the reduction kernel and the arithmetic are unchanged (the order of the
-// fp32 additions inside a segment differs: four 32-tap runs instead of one 128-tap run).
+//     outputs per 256 KiB block, 7 % of the tile is waste; per tap a thread issues 7 + 4
+//     shared loads for 224 FFMA.
 // ---------------------------------------------------------------------------
 constexpr int W2_LO = 8;               // output lanes per warp
 constexpr int W2_RK = 7;               // outputs per thread
@@ -1061,204 +914,41 @@ fir_long2_cf32_kernel(const __grid_constant__ TileLaunch P, const float2 *__rest
 }
 
 // ---------------------------------------------------------------------------
-// long filters, pipelined (the default when the strips are 16-byte aligned): ONE resident CTA
-// per SM walks `seg_per` consecutive 128-tap segments of one (group, 56-output tile) through a
-// two-stage ring -- while its 8 warps (16 taps of the segment each, all 32 clients x 56 outputs)
-// accumulate segment i, warp 0 has already issued the TMA bulk copies of segment i+1 (57 copies:
-// the taps and one strip per output row).  Against fir_long2: no idle time while a CTA loads
-// (there the two CTAs of an SM were often both waiting), the prologue and the cross-warp
-// reduction are paid once per ~13 segments instead of once per segment, and the partial-sum
-// slabs shrink from one per segment (121 for BASELINE configs[4]) to one per CTA along the tap
-// axis (9): the reduction kernel and its traffic shrink with them.
+// fir_long4: ONE resident CTA per SM walks `seg_per` consecutive 128-tap segments of one (group
+// pair, 28-output tile) through a two-stage ring -- while its 8 warps (16 taps of the segment each)
+// accumulate segment i, warp 0 has already issued the TMA copies of segment i+1.  No idle time while
+// a CTA loads, the prologue and the cross-warp reduction are paid once per ~13 segments instead of
+// once per segment, and the partial-sum slabs shrink from one per segment (121 for BASELINE
+// configs[4]) to one per CTA along the tap axis (9): the reduction kernel and its traffic shrink
+// with them.
+// The tile is 28 outputs x 64 clients (4 output lanes x 7 outputs per thread, 8 client octets = TWO
+// 32-client groups per CTA), and ~52 outputs per block fit 2 x 28.  Small bulk copies, not FMAs, are
+// what a long-filter kernel waits for (~300 cycles per 1 KiB strip copy and SM whatever else it
+// does), so a stage is 28 strips + 2 tap blocks = 30 bulk copies where a 56 x 32 tile of the same
+// FLOPs needs 57 -- or 3 copies, when the 28 strips arrive as one tensor copy (below).
 // ---------------------------------------------------------------------------
-constexpr int W3_WARPS = 8;
-constexpr int W3_THREADS = 32 * W3_WARPS;
-constexpr int W3_STAGES = 2;
-constexpr int W3_JW = W_JS / W3_WARPS;                       // taps per warp per segment (16)
-constexpr int W3_STAGE_BYTES = W_JS * T_CG * 8 + W2_KT * W_JSP * 8;  // 32 KiB taps + 57 KiB strips
-constexpr int W3_SMEM = W3_STAGES * W3_STAGE_BYTES + 64;
-static_assert((W3_WARPS - 1) * 32 * W2_RK * T_RC * 2 * 4 <= W3_STAGES * W3_STAGE_BYTES, "reduction scratch reuses the stages");
-
-__global__ void __launch_bounds__(W3_THREADS, 1)
-fir_long3_cf32_kernel(const __grid_constant__ TileLaunch P, const float2 *__restrict__ ring, unsigned mask,
-                      const float2 *__restrict__ tile_taps, float2 *__restrict__ partial) {
-  extern __shared__ __align__(128) unsigned char smem[];
-  uint64_t *bars = reinterpret_cast<uint64_t *>(smem + W3_STAGES * W3_STAGE_BYTES);  // full[2], empty[2]
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int o = lane & (W2_LO - 1), h = lane / W2_LO;  // output column, client octet
-  const int cbase = h * T_RC;
-
-  const int ci = class_of_cta(P, (int)blockIdx.x);
-  const TileClass &K = P.cls[ci];
-  const int local = (int)blockIdx.x - K.cta_begin;
-  const int sp = local % K.ksplit;
-  const int rest = local / K.ksplit;
-  const int tile = rest % K.tiles;
-  const int grp = rest / K.tiles;
-  const int k0 = tile * W2_KT;
-  const int D = K.D;
-  const int seg_begin = sp * K.seg_per;
-  const int seg_end = min(seg_begin + K.seg_per, K.nseg);
-  const bool group_active = grp * T_CG < K.n_members;
-
-  if (tid == 0) {
-    for (int st = 0; st < W3_STAGES; st++) {
-      mbar_init(&bars[st], 1);
-      mbar_init(&bars[W3_STAGES + st], W3_WARPS);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  __syncthreads();
-
-  // warp 0 is also the producer: lane 0 announces the stage's bytes, then every lane issues
-  // its copies (strip rows lane and lane + 32, lane 0 also the taps)
-  auto load_segment = [&](int sg, int st) {
-    const int f0 = sg * W_JS;
-    const int len = min(W_JS, K.L - f0);
-    float2 *ts = reinterpret_cast<float2 *>(smem + st * W3_STAGE_BYTES);
-    float2 *xs = ts + W_JS * T_CG;
-    const unsigned strip_bytes = (unsigned)len * 8u, tap_bytes = (unsigned)len * T_CG * 8u;
-    if (lane == 0) {
-      mbar_expect_tx(&bars[st], tap_bytes + W2_KT * strip_bytes);
-      tma_bulk_g2s(ts, tile_taps + K.taps_off + ((long long)grp * K.L + f0) * T_CG, tap_bytes, &bars[st]);
-    }
-    __syncwarp();
-    const long long w0 = K.first + (long long)k0 * D + f0;
-    for (int r = lane; r < W2_KT; r += 32) {
-      const unsigned idx = (unsigned)((unsigned long long)(w0 + (long long)r * D)) & mask;
-      const unsigned n1 = min((unsigned)len, mask + 1u - idx);
-      tma_bulk_g2s(xs + r * W_JSP, ring + idx, n1 * 8u, &bars[st]);
-      if (n1 < (unsigned)len) tma_bulk_g2s(xs + r * W_JSP + n1, ring, ((unsigned)len - n1) * 8u, &bars[st]);
-    }
-  };
-
-  float2 acc[W2_RK][T_RC];
-#pragma unroll
-  for (int i = 0; i < W2_RK; i++)
-#pragma unroll
-    for (int c = 0; c < T_RC; c++) acc[i][c] = make_float2(0.f, 0.f);
-
-  if (group_active && seg_begin < seg_end) {
-    if (warp == 0) load_segment(seg_begin, 0);
-    for (int sg = seg_begin; sg < seg_end; sg++) {
-      const int it = sg - seg_begin, st = it % W3_STAGES;
-      if (warp == 0 && sg + 1 < seg_end) {
-        // the other stage held segment sg-1: every warp has released it before entering segment sg
-        // (or is about to); refill it with segment sg+1 while segment sg is being accumulated
-        const int ns = (it + 1) % W3_STAGES;
-        if (it >= 1) mbar_wait(&bars[W3_STAGES + ns], (unsigned)(((it - 1) / W3_STAGES) & 1));
-        load_segment(sg + 1, ns);
-      }
-      mbar_wait(&bars[st], (unsigned)((it / W3_STAGES) & 1));
-      const int len = min(W_JS, K.L - sg * W_JS);
-      const float2 *ts = reinterpret_cast<const float2 *>(smem + st * W3_STAGE_BYTES);
-      const float2 *xs = ts + W_JS * T_CG;
-      const float4 *tp = reinterpret_cast<const float4 *>(ts + cbase);
-      const float2 *xb[W2_RK];
-#pragma unroll
-      for (int i = 0; i < W2_RK; i++) xb[i] = xs + (o + W2_LO * i) * W_JSP;
-      const int f_end = min(len, (warp + 1) * W3_JW);
-#pragma unroll 1
-      for (int f = warp * W3_JW; f < f_end; f += T_UNROLL) {
-#pragma unroll
-        for (int u = 0; u < T_UNROLL; u++) {
-          float2 x[W2_RK];
-          float4 tq[T_RC / 2];
-#pragma unroll
-          for (int i = 0; i < W2_RK; i++) x[i] = xb[i][f + u];
-#pragma unroll
-          for (int q = 0; q < T_RC / 2; q++) tq[q] = tp[(f + u) * (T_CG / 2) + q];
-#pragma unroll
-          for (int i = 0; i < W2_RK; i++) {
-#pragma unroll
-            for (int q = 0; q < T_RC / 2; q++) {
-              float2 &a0 = acc[i][2 * q], &a1 = acc[i][2 * q + 1];
-              a0.x = fmaf(x[i].x, tq[q].x, a0.x);
-              a0.x = fmaf(-x[i].y, tq[q].y, a0.x);
-              a0.y = fmaf(x[i].x, tq[q].y, a0.y);
-              a0.y = fmaf(x[i].y, tq[q].x, a0.y);
-              a1.x = fmaf(x[i].x, tq[q].z, a1.x);
-              a1.x = fmaf(-x[i].y, tq[q].w, a1.x);
-              a1.y = fmaf(x[i].x, tq[q].w, a1.y);
-              a1.y = fmaf(x[i].y, tq[q].z, a1.y);
-            }
-          }
-        }
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars[W3_STAGES + st]);  // this warp is done with the stage
-    }
-  }
-  // warps 1..7 hand their sums to warp 0 through shared memory, layout [warp-1][value][lane]
-  __syncthreads();
-  float *red = reinterpret_cast<float *>(smem);
-  constexpr int NV = W2_RK * T_RC * 2;
-  if (warp > 0 && group_active) {
-    float *dst = red + (size_t)(warp - 1) * NV * 32 + lane;
-#pragma unroll
-    for (int i = 0; i < W2_RK; i++)
-#pragma unroll
-      for (int c = 0; c < T_RC; c++) {
-        dst[(size_t)((i * T_RC + c) * 2) * 32] = acc[i][c].x;
-        dst[(size_t)((i * T_RC + c) * 2 + 1) * 32] = acc[i][c].y;
-      }
-  }
-  __syncthreads();
-  if (warp == 0 && group_active) {
-#pragma unroll 1
-    for (int w = 0; w < W3_WARPS - 1; w++) {
-      const float *src = red + (size_t)w * NV * 32 + lane;
-#pragma unroll
-      for (int i = 0; i < W2_RK; i++)
-#pragma unroll
-        for (int c = 0; c < T_RC; c++) {
-          acc[i][c].x += src[(size_t)((i * T_RC + c) * 2) * 32];
-          acc[i][c].y += src[(size_t)((i * T_RC + c) * 2 + 1) * 32];
-        }
-    }
-    // partial sums: [tap split][group][output][32 clients]
-    float2 *pp = partial + K.part_off + (((long long)sp * K.n_groups + grp) * K.kpad + k0) * T_CG + cbase;
-#pragma unroll
-    for (int i = 0; i < W2_RK; i++) {
-      float4 *row = reinterpret_cast<float4 *>(pp + (size_t)(o + W2_LO * i) * T_CG);
-#pragma unroll
-      for (int q = 0; q < T_RC / 2; q++)
-        row[q] = make_float4(acc[i][2 * q].x, acc[i][2 * q].y, acc[i][2 * q + 1].x, acc[i][2 * q + 1].y);
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------
-// fir_long4: the pipelined kernel with a 28-output x 64-client tile (4 output lanes x 7 outputs
-// per thread, 8 client octets = TWO 32-client groups per CTA).  Same FLOPs per stage as fir_long3's
-// 56 x 32, but a stage is 28 strips + 2 tap blocks = 30 bulk copies instead of 57.  The three
-// earlier kernels all run at ~300 cycles per 1 KiB strip copy and SM whatever else they do
-// (745 copies per SM and block in 113-121 us): small bulk copies, not FMAs, are what they wait for.
-// ---------------------------------------------------------------------------
+constexpr int W4_WARPS = 8;
+constexpr int W4_THREADS = 32 * W4_WARPS;
+constexpr int W4_STAGES = 2;
+constexpr int W4_JW = W_JS / W4_WARPS;  // taps per warp per segment (16)
 constexpr int W4_LO = 4;
 constexpr int W4_KT = W4_LO * W2_RK;    // 28 outputs per CTA
 constexpr int W4_GROUPS = 2;            // client groups per CTA
 constexpr int W4_STAGE_BYTES = (W4_GROUPS * W_JS * T_CG * 8 + W4_KT * W_JSP * 8 + 127) / 128 * 128;  // 64 KiB taps + 28.4 KiB strips (128-byte aligned stages: TMA tensor destinations)
-constexpr int W4_SMEM = W3_STAGES * W4_STAGE_BYTES + 64;
-static_assert((W3_WARPS - 1) * 32 * W2_RK * T_RC * 2 * 4 <= W3_STAGES * W4_STAGE_BYTES, "reduction scratch reuses the stages");
+constexpr int W4_SMEM = W4_STAGES * W4_STAGE_BYTES + 64;
+static_assert((W4_WARPS - 1) * 32 * W2_RK * T_RC * 2 * 4 <= W4_STAGES * W4_STAGE_BYTES, "reduction scratch reuses the stages");
 
-// TM = the 28 input strips of a stage arrive as ONE 2-D tensor copy (box 130 x 28 eight-byte elements, row
-// pitch D in the ring) instead of 28 bulk copies of 1 KiB: the stage loads, not the FMAs, are what this
-// kernel waits for (ncu: 12 % of warp time on the stage's mbarrier), and small copies cost ~300 cycles each.
-// A stage whose box would cross the ring's wrap-around (or the map's inner width) uses the strip path.
-// PK = packed FFMA2 arithmetic on client pairs: the taps of a client PAIR are stored (re0, re1, im0, im1)
-// by the host, so that one 128-bit shared load yields TR = (re0, re1) and TI = (im0, im1); per pair and
-// output the four FMAs of the scalar path become four FFMA2 on RE = (re of client 0, re of client 1) and
-// IM likewise, in the SAME order per accumulator (+xr*tr, -xi*ti | +xr*ti, +xi*tr): bit-identical.
-template <bool TM, bool PK>
-__global__ void __launch_bounds__(W3_THREADS, 1)
+// With a tensor map (K.tmap_w > 0) the 28 input strips of a stage arrive as ONE 2-D tensor copy (box
+// 130 x 28 eight-byte elements, row pitch D in the ring) instead of 28 bulk copies of 1 KiB: the stage
+// loads, not the FMAs, are what this kernel waits for (ncu: 12 % of warp time on the stage's mbarrier).
+// A stage whose box would cross the ring's wrap-around (or the map's inner width), and every stage of a
+// class without a map, uses the per-strip copies.
+__global__ void __launch_bounds__(W4_THREADS, 1)
 fir_long4_cf32_kernel(const __grid_constant__ TileLaunch P, const float2 *__restrict__ ring, unsigned mask,
                       const float2 *__restrict__ tile_taps, float2 *__restrict__ partial,
                       const __grid_constant__ CUtensorMap strips) {
   extern __shared__ __align__(128) unsigned char smem[];
-  uint64_t *bars = reinterpret_cast<uint64_t *>(smem + W3_STAGES * W4_STAGE_BYTES);  // full[2], empty[2]
+  uint64_t *bars = reinterpret_cast<uint64_t *>(smem + W4_STAGES * W4_STAGE_BYTES);  // full[2], empty[2]
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int o = lane & (W4_LO - 1), h = lane / W4_LO;  // output column, client octet (0..7)
@@ -1281,9 +971,9 @@ fir_long4_cf32_kernel(const __grid_constant__ TileLaunch P, const float2 *__rest
   const bool mine_active = gsel < n_grp && (grp0 + gsel) * T_CG < K.n_members;
 
   if (tid == 0) {
-    for (int st = 0; st < W3_STAGES; st++) {
+    for (int st = 0; st < W4_STAGES; st++) {
       mbar_init(&bars[st], 1);
-      mbar_init(&bars[W3_STAGES + st], W3_WARPS);
+      mbar_init(&bars[W4_STAGES + st], W4_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -1304,7 +994,7 @@ fir_long4_cf32_kernel(const __grid_constant__ TileLaunch P, const float2 *__rest
     const long long w0 = K.first + (long long)k0 * D + f0 - (long long)xoff;
     bool boxed = false;
     unsigned q = 0, c0 = 0;
-    if (TM && K.tmap_w > 0) {
+    if (K.tmap_w > 0) {
       const unsigned idx0 = (unsigned)((unsigned long long)w0) & mask;
       q = idx0 / (unsigned)D;
       c0 = idx0 - q * (unsigned)D;
@@ -1328,25 +1018,21 @@ fir_long4_cf32_kernel(const __grid_constant__ TileLaunch P, const float2 *__rest
   };
 
   float2 acc[W2_RK][T_RC];
-  u64x RE[W2_RK][T_RC / 2], IM[W2_RK][T_RC / 2];  // PK only
 #pragma unroll
-  for (int i = 0; i < W2_RK; i++) {
+  for (int i = 0; i < W2_RK; i++)
 #pragma unroll
     for (int c = 0; c < T_RC; c++) acc[i][c] = make_float2(0.f, 0.f);
-#pragma unroll
-    for (int q = 0; q < T_RC / 2; q++) RE[i][q] = IM[i][q] = 0ull;
-  }
 
   if (seg_begin < seg_end) {
     if (warp == 0) load_segment(seg_begin, 0);
     for (int sg = seg_begin; sg < seg_end; sg++) {
-      const int it = sg - seg_begin, st = it % W3_STAGES;
+      const int it = sg - seg_begin, st = it % W4_STAGES;
       if (warp == 0 && sg + 1 < seg_end) {
-        const int ns = (it + 1) % W3_STAGES;
-        if (it >= 1) mbar_wait(&bars[W3_STAGES + ns], (unsigned)(((it - 1) / W3_STAGES) & 1));
+        const int ns = (it + 1) % W4_STAGES;
+        if (it >= 1) mbar_wait(&bars[W4_STAGES + ns], (unsigned)(((it - 1) / W4_STAGES) & 1));
         load_segment(sg + 1, ns);
       }
-      mbar_wait(&bars[st], (unsigned)((it / W3_STAGES) & 1));
+      mbar_wait(&bars[st], (unsigned)((it / W4_STAGES) & 1));
       if (mine_active) {
         const int len = min(W_JS, K.L - sg * W_JS);
         const float2 *ts = reinterpret_cast<const float2 *>(smem + st * W4_STAGE_BYTES);
@@ -1355,66 +1041,38 @@ fir_long4_cf32_kernel(const __grid_constant__ TileLaunch P, const float2 *__rest
         const float2 *xb[W2_RK];
 #pragma unroll
         for (int i = 0; i < W2_RK; i++) xb[i] = xs + (o + W4_LO * i) * W_JSP + xoff;
-        const int f_end = min(len, (warp + 1) * W3_JW);
+        const int f_end = min(len, (warp + 1) * W4_JW);
 #pragma unroll 1
-        for (int f = warp * W3_JW; f < f_end; f += T_UNROLL) {
+        for (int f = warp * W4_JW; f < f_end; f += T_UNROLL) {
 #pragma unroll
           for (int u = 0; u < T_UNROLL; u++) {
             float2 x[W2_RK];
 #pragma unroll
             for (int i = 0; i < W2_RK; i++) x[i] = xb[i][f + u];
-            if constexpr (PK) {
-              ulonglong2 tq[T_RC / 2];  // .x = (re0, re1), .y = (im0, im1)
+            float4 tq[T_RC / 2];
 #pragma unroll
-              for (int q = 0; q < T_RC / 2; q++)
-                tq[q] = reinterpret_cast<const ulonglong2 *>(tp)[(f + u) * (T_CG / 2) + q];
+            for (int q = 0; q < T_RC / 2; q++) tq[q] = tp[(f + u) * (T_CG / 2) + q];
 #pragma unroll
-              for (int i = 0; i < W2_RK; i++) {
-                const u64x XR = pack2f(x[i].x, x[i].x), XI = pack2f(x[i].y, x[i].y);
-                const u64x XN = XI ^ 0x8000000080000000ull;
+            for (int i = 0; i < W2_RK; i++) {
 #pragma unroll
-                for (int q = 0; q < T_RC / 2; q++) {
-                  RE[i][q] = ffma2(XR, tq[q].x, RE[i][q]);
-                  RE[i][q] = ffma2(XN, tq[q].y, RE[i][q]);
-                  IM[i][q] = ffma2(XR, tq[q].y, IM[i][q]);
-                  IM[i][q] = ffma2(XI, tq[q].x, IM[i][q]);
-                }
-              }
-            } else {
-              float4 tq[T_RC / 2];
-#pragma unroll
-              for (int q = 0; q < T_RC / 2; q++) tq[q] = tp[(f + u) * (T_CG / 2) + q];
-#pragma unroll
-              for (int i = 0; i < W2_RK; i++) {
-#pragma unroll
-                for (int q = 0; q < T_RC / 2; q++) {
-                  float2 &a0 = acc[i][2 * q], &a1 = acc[i][2 * q + 1];
-                  a0.x = fmaf(x[i].x, tq[q].x, a0.x);
-                  a0.x = fmaf(-x[i].y, tq[q].y, a0.x);
-                  a0.y = fmaf(x[i].x, tq[q].y, a0.y);
-                  a0.y = fmaf(x[i].y, tq[q].x, a0.y);
-                  a1.x = fmaf(x[i].x, tq[q].z, a1.x);
-                  a1.x = fmaf(-x[i].y, tq[q].w, a1.x);
-                  a1.y = fmaf(x[i].x, tq[q].w, a1.y);
-                  a1.y = fmaf(x[i].y, tq[q].z, a1.y);
-                }
+              for (int q = 0; q < T_RC / 2; q++) {
+                float2 &a0 = acc[i][2 * q], &a1 = acc[i][2 * q + 1];
+                a0.x = fmaf(x[i].x, tq[q].x, a0.x);
+                a0.x = fmaf(-x[i].y, tq[q].y, a0.x);
+                a0.y = fmaf(x[i].x, tq[q].y, a0.y);
+                a0.y = fmaf(x[i].y, tq[q].x, a0.y);
+                a1.x = fmaf(x[i].x, tq[q].z, a1.x);
+                a1.x = fmaf(-x[i].y, tq[q].w, a1.x);
+                a1.y = fmaf(x[i].x, tq[q].w, a1.y);
+                a1.y = fmaf(x[i].y, tq[q].z, a1.y);
               }
             }
           }
         }
       }
       __syncwarp();
-      if (lane == 0) mbar_arrive(&bars[W3_STAGES + st]);  // this warp is done with the stage
+      if (lane == 0) mbar_arrive(&bars[W4_STAGES + st]);  // this warp is done with the stage
     }
-  }
-  if constexpr (PK) {
-#pragma unroll
-    for (int i = 0; i < W2_RK; i++)
-#pragma unroll
-      for (int q = 0; q < T_RC / 2; q++) {
-        unpack2f(RE[i][q], acc[i][2 * q].x, acc[i][2 * q + 1].x);
-        unpack2f(IM[i][q], acc[i][2 * q].y, acc[i][2 * q + 1].y);
-      }
   }
   // warps 1..7 hand their sums to warp 0 through shared memory, layout [warp-1][value][lane]
   __syncthreads();
@@ -1433,7 +1091,7 @@ fir_long4_cf32_kernel(const __grid_constant__ TileLaunch P, const float2 *__rest
   __syncthreads();
   if (warp == 0 && mine_active) {
 #pragma unroll 1
-    for (int w = 0; w < W3_WARPS - 1; w++) {
+    for (int w = 0; w < W4_WARPS - 1; w++) {
       const float *src = red + (size_t)w * NV * 32 + lane;
 #pragma unroll
       for (int i = 0; i < W2_RK; i++)

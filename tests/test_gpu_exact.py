@@ -132,11 +132,12 @@ def test_generic_kernel(pkg, monkeypatch):
     assert kinds_of(cl) == {GENERIC}
 
 
-@pytest.mark.parametrize("shape", [None, "1642", "1641", "1621", "1611", "3241"])
+@pytest.mark.parametrize("shape", [None, "1642", "1641", "1621", "1611", "3241", "1651"])
 def test_tiled_kernel_shapes(pkg, monkeypatch, shape):
     """Every tile shape on the natural and the skewed layout, ragged and odd-length blocks, and a
     second wave of clients that attaches mid-stream (generic until its zero history has passed,
-    then its own window alignment inside a merged class)."""
+    then its own window alignment inside a merged class).  3241 (the retired LO = 32 shape) and
+    1651 are not shapes: they are ignored and the automatic choice runs."""
     env = {"XLATING_B200_TILE": shape} if shape else {}
     cl, prof = drive(pkg, monkeypatch, MIXED, RAGGED, env=env, attach={2: [(42, 505)] * 8 + [(21, 253)] * 8},
                      profile=True, seed=3)
@@ -165,14 +166,15 @@ LONG_PLAN = [(1280, 2561)] * 8 + [(1280, 1407)] * 12 + [(1280, 1281)] * 8 + [(12
 LONG_SIZES = [MAX_IN5, 50002, MAX_IN5, MAX_IN5, 30006, MAX_IN5, MAX_IN5, 131070, MAX_IN5, MAX_IN5, MAX_IN5, 2]
 
 
-@pytest.mark.parametrize("env", [{}, {"XLATING_B200_LONG": "1"}, {"XLATING_B200_LONG": "2"}, {"XLATING_B200_LONG": "3"},
-                                 {"XLATING_B200_LONG": "4"}, {"XLATING_B200_LONG_FFMA2": "1"}, {"XLATING_B200_LONG_TMAP": "0"},
-                                 {"XLATING_B200_LONG_FFMA2": "1", "XLATING_B200_LONG_TMAP": "0"}],
-                         ids=["default", "long1", "long2", "long3", "long4", "ffma2", "no_tmap", "ffma2_no_tmap"])
-def test_split_k_kernels(pkg, monkeypatch, env):
+@pytest.mark.parametrize("plan, env", [(LONG_PLAN, {}), (LONG_PLAN, {"XLATING_B200_LONG_TMAP": "0"}),
+                                       ([(1280, 2561)] * 8 + [(1279, 2561)] * 8, {})],
+                         ids=["default", "no_tmap", "mixed_parity"])
+def test_split_k_kernels(pkg, monkeypatch, plan, env):
     """The split-K long-filter kernels: T just above and below multiples of D and of the 128-tap
-    segment, odd window starts (odd block lengths), and a ring wrap-around."""
-    cl, prof = drive(pkg, monkeypatch, LONG_PLAN, LONG_SIZES, fmt="cs16", fs=FS5, max_in=MAX_IN5, env=env,
+    segment, odd window starts (odd block lengths), and a ring wrap-around.  fir_long4 with and without
+    its strip tensor map; an odd-D class in the group sends the even-D class to fir_long2 as well,
+    whose strips then alternate between aligned bulk copies and cp.async with the window start."""
+    cl, prof = drive(pkg, monkeypatch, plan, LONG_SIZES, fmt="cs16", fs=FS5, max_in=MAX_IN5, env=env,
                      profile=True, seed=6)
     assert kinds_of(cl) == {LONG}
     assert prof["fir_long_launches"] > 0 and prof["fir_tile_launches"] == 0

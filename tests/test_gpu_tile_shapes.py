@@ -57,7 +57,7 @@ def run_shape(pkg, monkeypatch, shape):
     return outs
 
 
-@pytest.mark.parametrize("shape", ["1641", "1621", "1611", "3241"])
+@pytest.mark.parametrize("shape", ["1641", "1621", "1611"])
 def test_tile_shapes_bit_identical(pkg, monkeypatch, shape):
     ref = run_shape(pkg, monkeypatch, "1642")
     got = run_shape(pkg, monkeypatch, shape)
