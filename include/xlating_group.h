@@ -115,9 +115,30 @@ int xlg_add_client_rational(xlg_group *g, uint32_t interp, uint32_t decim, const
  * xlg_add_client_rational's checks; interp == 1 is xlg_add_client_ex. */
 int xlg_add_client_rational_ex(xlg_group *g, uint32_t interp, uint32_t decim, const float *taps, size_t taps_len,
                                int32_t center_freq, const xlg_client_state *state, int *client_id);
+/* Attach a two-stage client: a wide, short first stage at the band rate, then a narrow second stage at
+ * fs / decim1, for the transition band of one long filter at a fraction of its multiply-adds (DESIGN.md
+ * section 5, "Cascade clients").  Per submitted block its output is, by definition:
+ *   stage A = create_frequency_xlating_filter(decim1, taps1, taps1_len, center_freq, fs, ...), fed the block
+ *             exactly as an xlg_add_client client is (same history, zero history before the attach point,
+ *             oscillator, renormalisation; XLG_NO_RENORM applies);
+ *   stage B = the float path (src/xlating.c:52-83) of create_frequency_xlating_filter(decim2, taps2, taps2_len,
+ *             0, fs / decim1, ...), fed the cf32 outputs of stage A for the same block, with taps2_len - 1
+ *             zeros of history at the attach point.
+ * At centre 0 stage B's rotated taps are (h, 0) (cexpf(0) = 1; the even-length reversal quirk of :530-534
+ * applies), its oscillator stays 1 + 0i and renormalisation divides by 1, so stage B is exactly a real-tap
+ * complex decimator with history.  The client's output per block is stage B's; *out_len is known when
+ * xlg_submit returns, as for every client.  xlg_client_info reports kind 5; xlg_cascade_info tells which
+ * kernel serves stage A.  -EINVAL (logged) for decim1, decim2, taps1_len or taps2_len of 0, or a stage B
+ * too long for the stage-B kernel's shared memory (about 16000 taps); -ENOTSUP (logged) on an
+ * XLG_TRACK_STATE group.  A group with a cascade client refuses XLG_PATH_Q15 submits (-ENOTSUP, nothing
+ * enqueued). */
+int xlg_add_client_cascade(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, int32_t center_freq,
+                           uint32_t decim2, const float *taps2, size_t taps2_len, int *client_id);
 int xlg_remove_client(xlg_group *g, int client_id);
 /* Size the per-ticket result arenas (device and pinned host) for `output_samples_per_block` complex output
  * samples per block summed over all clients (a client at decimation D produces about max_input_len/2/D + 2).
+ * A cascade client counts two rows, each rounded up to a multiple of 4 samples: its stage-A row of
+ * n1 = max_input_len/2/decim1 + 2 samples, which stays on the device, and its final row of n1/decim2 + 2.
  * Optional: the arenas grow on demand when clients are added, but a growth re-allocates every ring entry and
  * the results still waiting in the ring are lost (-ESTALE for consumers that had not read them yet, like a
  * block overwritten in the reference's queue).  A server that knows its client limit reserves once, up front. */
@@ -207,12 +228,26 @@ typedef struct {
 } xlg_poly_profile;
 int xlg_poly_profile_read(xlg_group *g, xlg_poly_profile *p, int reset);
 
+/* Stage B of cascade clients (xlg_add_client_cascade), counted like xlg_profile's while profiling is enabled.
+ * xlg_profile counts each cascade client's stage A as the integer client it is. */
+typedef struct {
+  double stage_b_ms;         /* the ring appends + the stage-B kernel */
+  uint64_t stage_b_launches;
+  uint64_t stage_b_macs;     /* complex-by-real MACs of stage B: sum n_out * taps2_len */
+  uint64_t d2h_bytes;        /* result bytes copied to the host, all clients (stage-A rows are never copied) */
+} xlg_cascade_profile;
+int xlg_cascade_profile_read(xlg_group *g, xlg_cascade_profile *p, int reset);
+
 /* Introspection for tests: history length (src/xlating.c:29 history_offset; upsampled samples for a
- * rational client) and which kernel currently serves the client (0 = generic, 1 = tiled,
- * 2 = long-filter split-K, 3 = rational, polyphase generic, 4 = rational, tiled: at least 8 clients with
- * identical (interp, decim, taps_len, window alignment), gcd(interp, decim) = 1, whose branches fit the tiled
- * kernel's shared memory). */
+ * rational client, stage A's for a cascade client) and which kernel currently serves the client
+ * (0 = generic, 1 = tiled, 2 = long-filter split-K, 3 = rational, polyphase generic, 4 = rational, tiled: at
+ * least 8 clients with identical (interp, decim, taps_len, window alignment), gcd(interp, decim) = 1, whose
+ * branches fit the tiled kernel's shared memory, 5 = cascade). */
 int xlg_client_info(const xlg_group *g, int client_id, size_t *history, int *kernel_kind);
+/* A cascade client's stages: the kind (0, 1 or 2, as xlg_client_info) of the kernel serving stage A, and the
+ * history_offset of each stage (stage B's in stage-A samples).  -EINVAL for any other client. */
+int xlg_cascade_info(const xlg_group *g, int client_id, int *stage_a_kind, size_t *stage_a_history,
+                     size_t *stage_b_history);
 
 /* Counters of the per-filter drop-in ABI (include/xlating.h) on `device`: process_*
  * calls served so far, the number of launches (batches) they were combined into, and

@@ -55,7 +55,7 @@ DROPIN_EXTENSION_SYMBOLS = ["create_rational_frequency_xlating_filter"]
 GROUP_SYMBOLS = [
     "xlg_create", "xlg_create_ex", "xlg_destroy", "xlg_add_client", "xlg_add_client_ex", "xlg_add_client_rational_ex", "xlg_remove_client", "xlg_reserve", "xlg_client_count", "xlg_submit",
     "xlg_wait", "xlg_input_consumed", "xlg_output", "xlg_read_output", "xlg_copy_output", "xlg_alloc_pinned", "xlg_free_pinned", "xlg_wait_stream", "xlg_partition_active", "xlg_timer_start",
-    "xlg_timer_stop", "xlg_profile_enable", "xlg_profile_read", "xlg_client_info", "xlg_add_client_rational", "xlg_poly_profile_read", "xlg_dropin_stats", "xlg_dropin_stream_stats", "xlg_dropin_stream_times",
+    "xlg_timer_stop", "xlg_profile_enable", "xlg_profile_read", "xlg_client_info", "xlg_add_client_rational", "xlg_poly_profile_read", "xlg_add_client_cascade", "xlg_cascade_info", "xlg_cascade_profile_read", "xlg_dropin_stats", "xlg_dropin_stream_stats", "xlg_dropin_stream_times",
 ]
 
 
@@ -78,6 +78,11 @@ class XlgPolyProfile(C.Structure):
     _fields_ = [("fir_poly_tile_ms", C.c_double), ("fir_poly_generic_ms", C.c_double),
                 ("fir_poly_tile_launches", C.c_uint64), ("fir_poly_generic_launches", C.c_uint64),
                 ("poly_macs", C.c_uint64)]
+
+
+class XlgCascadeProfile(C.Structure):
+    _fields_ = [("stage_b_ms", C.c_double), ("stage_b_launches", C.c_uint64), ("stage_b_macs", C.c_uint64),
+                ("d2h_bytes", C.c_uint64)]
 
 
 def build(verbose: bool = False) -> None:
@@ -128,6 +133,13 @@ def lib() -> C.CDLL:
     L.xlg_add_client_rational_ex.restype = C.c_int
     L.xlg_poly_profile_read.argtypes = [vp, C.POINTER(XlgPolyProfile), C.c_int]
     L.xlg_poly_profile_read.restype = C.c_int
+    fp = C.POINTER(C.c_float)
+    L.xlg_add_client_cascade.argtypes = [vp, u32, fp, sz, i32, u32, fp, sz, C.POINTER(C.c_int)]
+    L.xlg_add_client_cascade.restype = C.c_int
+    L.xlg_cascade_info.argtypes = [vp, C.c_int, C.POINTER(C.c_int), C.POINTER(sz), C.POINTER(sz)]
+    L.xlg_cascade_info.restype = C.c_int
+    L.xlg_cascade_profile_read.argtypes = [vp, C.POINTER(XlgCascadeProfile), C.c_int]
+    L.xlg_cascade_profile_read.restype = C.c_int
     L.xl_poly_pack.argtypes = [C.POINTER(C.c_float), sz, u32, C.POINTER(C.c_float)]
     L.xl_poly_pack.restype = None
     L.xlg_reserve.argtypes = [vp, sz]
@@ -324,6 +336,28 @@ class Group:
             raise ValueError(code)
         return cid.value
 
+    def add_client_cascade(self, decim1: int, taps1, center_freq: int, decim2: int, taps2) -> int:
+        """A two-stage client (include/xlating_group.h, xlg_add_client_cascade): the reference filter
+        (decim1, taps1, center_freq) at fs, followed by the reference filter (decim2, taps2, centre 0) at
+        fs / decim1 fed its outputs.  See cascade_plan for taps."""
+        t1 = np.ascontiguousarray(taps1, dtype=np.float32)
+        t2 = np.ascontiguousarray(taps2, dtype=np.float32)
+        cid = C.c_int(-1)
+        fp = C.POINTER(C.c_float)
+        code = self._L.xlg_add_client_cascade(self._h, decim1, t1.ctypes.data_as(fp), len(t1), center_freq, decim2,
+                                              t2.ctypes.data_as(fp), len(t2), C.byref(cid))
+        if code != 0:
+            raise ValueError(code)
+        return cid.value
+
+    def cascade_info(self, cid: int):
+        """(stage-A kernel kind, stage-A history, stage-B history in stage-A samples) of a cascade client."""
+        kind, h1, h2 = C.c_int(0), C.c_size_t(0), C.c_size_t(0)
+        code = self._L.xlg_cascade_info(self._h, cid, C.byref(kind), C.byref(h1), C.byref(h2))
+        if code != 0:
+            raise ValueError(code)
+        return kind.value, h1.value, h2.value
+
     def remove_client(self, cid: int) -> None:
         code = self._L.xlg_remove_client(self._h, cid)
         if code != 0:
@@ -433,6 +467,11 @@ class Group:
         self._L.xlg_poly_profile_read(self._h, C.byref(p), 1 if reset else 0)
         return {k: getattr(p, k) for k, _ in XlgPolyProfile._fields_}
 
+    def cascade_profile_read(self, reset: bool = True) -> dict:
+        p = XlgCascadeProfile()
+        self._L.xlg_cascade_profile_read(self._h, C.byref(p), 1 if reset else 0)
+        return {k: getattr(p, k) for k, _ in XlgCascadeProfile._fields_}
+
     def close(self):
         if self._h:
             self._L.xlg_destroy(self._h)
@@ -511,6 +550,49 @@ def rational_plan(fs: int, rates, lpf_cutoff_rate: int = 5):
         L, M = int(rate) // g, int(fs) // g
         taps = create_low_pass_filter(float(L), L * fs, int(rate) // 2, int(rate) // lpf_cutoff_rate)
         plan.append({"rate": rate, "interp": L, "decim": M, "center": p["center"], "taps": taps})
+    return plan
+
+
+def cascade_fmas(fs: int, rate: int, d1: int, t1: int, t2: int) -> float:
+    """Algorithmic real FMAs per input sample of a cascade client: 4 per complex tap of stage A at fs / d1,
+    2 per real tap of stage B at the client rate."""
+    return 4.0 * t1 / d1 + 2.0 * t2 / (fs // rate)
+
+
+def cascade_stages(fs: int, rate: int, d1: int):
+    """Taps of the two stages for D1 = d1: stage B is the server's own design at fs1 = fs / d1 (cutoff
+    rate / 2, transition rate / 5); stage A passes up to e = 3 * rate / 5 (stage B's passband edge plus half
+    its transition) and stops from fs1 - e, so everything it aliases onto the band lands in stage B's
+    stopband: create_low_pass_filter(1, fs, fs1 / 2, fs1 - 2e)."""
+    fs1 = fs // d1
+    e = 3 * rate // 5
+    return (create_low_pass_filter(1.0, fs, fs1 // 2, fs1 - 2 * e),
+            create_low_pass_filter(1.0, fs1, rate // 2, rate // 5))
+
+
+def cascade_plan(fs: int, rates):
+    """Two-stage clients for rates that divide fs: for D = fs / rate, the divisor D1 >= 2 of D (with
+    D2 = D / D1 >= 2) with the fewest estimated FMAs per input sample, 4*T1/D1 + 2*T2/D (cascade_fmas;
+    ties go to the smaller D1).  Taps from cascade_stages; centres as client_plan places them."""
+    plan = []
+    for p, rate in zip(client_plan(fs, rates), rates):
+        rate = int(rate)
+        if fs % rate != 0:
+            raise ValueError(f"{rate} does not divide {fs}")
+        D = fs // rate
+        best = None
+        for d1 in range(2, D // 2 + 1):
+            if D % d1 != 0 or fs % d1 != 0:
+                continue
+            t1, t2 = cascade_stages(fs, rate, d1)
+            cost = cascade_fmas(fs, rate, d1, t1.size, t2.size)
+            if best is None or cost < best[0]:
+                best = (cost, d1, t1, t2)
+        if best is None:
+            raise ValueError(f"decimation {D} has no divisor D1 >= 2 with D / D1 >= 2")
+        cost, d1, t1, t2 = best
+        plan.append({"rate": rate, "d1": d1, "d2": D // d1, "center": p["center"], "taps1": t1, "taps2": t2,
+                     "fmas": cost})
     return plan
 
 

@@ -70,6 +70,14 @@ void xl_client_consts_free(xl_client_consts *c) {
   c->rev_q15 = NULL;
 }
 
+int xl_walk(long long *hist, long long n_in, size_t taps_len, uint32_t decimation, int out_cap) {
+  const long long avail = *hist + n_in - (long long)taps_len; /* last admissible window start - first */
+  long long n_out = avail >= 0 ? avail / decimation + 1 : 0;
+  if (n_out > out_cap) n_out = out_cap;
+  *hist += n_in - n_out * (long long)decimation;
+  return (int)n_out;
+}
+
 void xl_poly_pack(const float *rev_cf32, size_t taps_len, uint32_t interp, float *out) {
   const size_t L = interp, Tb = (taps_len + L - 1) / L;
   for (size_t r = 0; r < L; r++)

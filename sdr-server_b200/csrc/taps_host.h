@@ -29,6 +29,12 @@ void xl_client_consts_free(xl_client_consts *c);
  * out[r][t] = rev[r + t*L] ((re, im) interleaved), zero where r + t*L >= T.  Branch r holds the
  * taps that meet the nonzero samples of a zero-stuffed window whose start is -r mod L.
  * `out` has room for 2*L*Tb floats. */
+/* The reference's walk over one call (src/xlating.c:58-60, :76): a filter whose next window starts *hist
+ * samples (history_offset) before the call's n_in new samples produces the returned number of outputs (at
+ * most out_cap) and leaves *hist for the next call.  Stage B of a cascade client walks its stage-A stream
+ * with it. */
+int xl_walk(long long *hist, long long n_in, size_t taps_len, uint32_t decimation, int out_cap);
+
 void xl_poly_pack(const float *rev_cf32, size_t taps_len, uint32_t interp, float *out);
 
 /* The float oscillator of one call on the host (src/xlating.c:70-73): n_out steps of

@@ -14,6 +14,8 @@
  *                    for the tiled kernel's TMA chunks
  *   per slot (XLG_SLOTS in flight): raw input staging, BlkInfo, per-output
  *                    oscillator table, output arena (+ pinned host mirrors)
+ *   cascade clients  a stage-A history ring each (HostClient::d_cring), their stage-B taps
+ *                    (d_taps2); stage-A rows follow the host-visible rows of the arena
  *
  * Streams: s_in (H2D), s_ph (oscillator pre-pass chain), s_cs[0..n_cs) (convert + FIR,
  * round-robin by block; 3 by default, XLATING_B200_CSTREAMS=1..4), s_out (D2H); events order them per block so block b+1's
@@ -110,6 +112,19 @@ struct HostClient {
   bool tile_ineligible = false;  // its class cannot use the tiled kernel (shared memory, too few outputs)
   bool pending_settle = false;   // still inside its zero-history window at the last layout rebuild
   int poly_off = 0, poly_rowcap = 0;  // kind 4: its branches' rows in the slot's polyphase scratch
+  // cascade client (xlg_add_client_cascade): everything above describes its stage A, an integer client
+  // whose out_off row lies after every host-visible row; stage B is described here
+  bool casc = false;
+  uint32_t D2 = 0;
+  size_t T2 = 0;
+  std::vector<float> rev2;       // stage B's reversed taps (the real parts of its rotated taps at centre 0)
+  long long hist2 = 0;           // stage B's history_offset, in stage-A samples
+  long long a_pos = 0;           // stage-A outputs produced since the attach: the ring's stream position
+  float2 *d_cring = nullptr;     // stage-A history ring, cring_cap samples (a power of two)
+  size_t cring_cap = 0;
+  int fin_off = 0, fin_cap = 0;  // final row of the slot's output arena
+  int taps2_off = 0;             // rev2 in the real tap arena
+  int last_n2 = 0;               // stage-B outputs of the block being submitted
 };
 
 struct Slot {
@@ -131,6 +146,12 @@ struct Slot {
   float2 *d_pscratch = nullptr;  // kind 4: unrotated outputs per branch (ClientDev::poly_off)
   BlkInfo *d_vblk = nullptr, *h_vblk = nullptr;  // kind 4: per branch class, this block's window start and count
   uint64_t poly_macs = 0;
+  CascBlk *d_cblk = nullptr, *h_cblk = nullptr;  // cascade clients: this block's ring positions, windows and counts
+  size_t cblk_cap = 0;
+  cudaEvent_t ev_casc = nullptr;                 // stage B of this block done (its rings' appends are ordered on it)
+  cudaEvent_t pf_casc[2] = {nullptr, nullptr};
+  bool pf_cb = false;
+  uint64_t casc_macs = 0, d2h_bytes = 0;
   std::atomic<int64_t> ticket{-1};
   bool q15 = false;
   bool harvested = true;
@@ -322,6 +343,12 @@ struct xlg_group {
   float2 *d_ones = nullptr;                 // phase 1 + 0i for the kind-4 classes' tiled launch
   size_t ones_cap = 0, pscratch_cap = 0;
   size_t partial_cap = 0;                   // float2 per slot partial-sum buffer
+  float *d_taps2 = nullptr;                 // cascade clients' stage-B taps (HostClient::taps2_off)
+  size_t cap_taps2 = 0;
+  int n_casc = 0;                           // active cascade clients
+  std::vector<float2 *> dead_rings;         // rings of removed cascade clients, freed once the pipeline is drained
+  cudaEvent_t ev_last_casc = nullptr;       // ev_casc of the last block with cascade clients
+  bool have_last_casc = false;
   int n_generic = 0;
   int max_client = 0;     // highest active id + 1
   bool dirty = true;
@@ -349,6 +376,7 @@ struct xlg_group {
   bool profiling = false;
   xlg_profile prof;
   xlg_poly_profile poly_prof;
+  xlg_cascade_profile casc_prof;
   uint64_t host_submit_ns = 0, host_wait_ns = 0, host_count_base = 0;
   std::mutex mu;  // guards slots' harvest + profile
 };
@@ -378,6 +406,10 @@ static void slot_free(Slot &s) {
   if (s.d_pscratch) cudaFree(s.d_pscratch);
   if (s.d_vblk) cudaFree(s.d_vblk);
   if (s.h_vblk) cudaFreeHost(s.h_vblk);
+  if (s.d_cblk) cudaFree(s.d_cblk);
+  if (s.h_cblk) cudaFreeHost(s.h_cblk);
+  s.d_cblk = s.h_cblk = nullptr;
+  s.cblk_cap = 0;
   s.d_pscratch = nullptr;
   s.d_vblk = s.h_vblk = nullptr;
   s.d_endph = nullptr;
@@ -447,6 +479,12 @@ static void harvest_locked(xlg_group *g, Slot &s) {
     g->poly_prof.fir_poly_tile_launches++;
   }
   g->poly_prof.poly_macs += s.poly_macs;
+  if (s.pf_cb && cudaEventElapsedTime(&ms, s.pf_casc[0], s.pf_casc[1]) == cudaSuccess) {
+    g->casc_prof.stage_b_ms += ms;
+    g->casc_prof.stage_b_launches++;
+  }
+  g->casc_prof.stage_b_macs += s.casc_macs;
+  g->casc_prof.d2h_bytes += s.d2h_bytes;
   g->prof.blocks++;
   g->prof.out_samples += s.out_samples;
   g->prof.in_samples += s.in_samples;
@@ -613,13 +651,56 @@ static int rebuild_layout(xlg_group *g) {
     HostClient &h = g->clients[i];
     if (!h.active) continue;
     h.out_cap = (int)((uint64_t)g->max_input_len / 2 * h.L / h.D + 2);
-    h.out_off = (int)out_total;
-    out_total += (size_t)h.out_cap;
+    if (h.casc) {
+      // n2 <= (n1 - 1) / D2 + 1 for any history
+      h.fin_cap = h.out_cap / (int)h.D2 + 2;
+      h.fin_off = (int)out_total;
+      out_total += (size_t)h.fin_cap;
+    } else {
+      h.out_off = (int)out_total;
+      out_total += (size_t)h.out_cap;
+    }
     out_total = (out_total + 3) & ~(size_t)3;  // keep rows 32-byte aligned
     h.taps_off = (int)taps_total;
     taps_total += h.rev.size() / 2;
     // a rational client's history of at most T - 1 upsampled samples reaches back ceil((T-1)/L) + 1 inputs
     max_hist = std::max(max_hist, h.L == 1 ? h.T - 1 : (h.T - 1 + h.L - 1) / h.L + 1);
+  }
+  // cascade clients: stage-A rows after every host-visible row (the D2H copy ends before them), stage-B taps,
+  // and a zeroed history ring for each new client (its positions before the attach read as zero)
+  {
+    std::vector<float> taps2;
+    g->n_casc = 0;
+    for (int i = 0; i < nc; i++) {
+      HostClient &h = g->clients[i];
+      if (!h.active || !h.casc) continue;
+      h.out_off = (int)out_total;
+      out_total += (size_t)h.out_cap;
+      out_total = (out_total + 3) & ~(size_t)3;
+      h.taps2_off = (int)taps2.size();
+      taps2.insert(taps2.end(), h.rev2.begin(), h.rev2.end());
+      taps2.resize((taps2.size() + 3) & ~(size_t)3, 0.f);  // 16-byte aligned bulk copies of whole float4s
+      if (h.d_cring == nullptr) {
+        // stage B of block b reads stage-A outputs of earlier blocks; the submit of block b + XLG_SLOTS waits
+        // for ticket b, so T2 - 1 + (XLG_SLOTS + 1) * max n1 samples are never overwritten while still needed
+        h.cring_cap = next_pow2(h.T2 - 1 + (size_t)(XLG_SLOTS + 1) * (size_t)h.out_cap);
+        CU_OK(cudaMalloc(&h.d_cring, h.cring_cap * sizeof(float2)));
+        CU_OK(cudaMemset(h.d_cring, 0, h.cring_cap * sizeof(float2)));
+      }
+      g->n_casc++;
+    }
+    if (dev_assign(&g->d_taps2, &g->cap_taps2, taps2.data(), taps2.size() * sizeof(float))) return -EIO;
+    for (float2 *p : g->dead_rings) cudaFree(p);
+    g->dead_rings.clear();
+    for (Slot &s : g->slots) {
+      if (s.cblk_cap >= (size_t)g->n_casc) continue;
+      if (s.d_cblk) cudaFree(s.d_cblk);
+      if (s.h_cblk) cudaFreeHost(s.h_cblk);
+      s.d_cblk = s.h_cblk = nullptr;
+      s.cblk_cap = std::max<size_t>((size_t)g->n_casc * 2, 16);
+      CU_OK(cudaMalloc(&s.d_cblk, s.cblk_cap * sizeof(CascBlk)));
+      CU_OK(cudaHostAlloc(&s.h_cblk, s.cblk_cap * sizeof(CascBlk), cudaHostAllocDefault));
+    }
   }
   if (ensure_ring(g, max_hist, g->qring != nullptr)) return -EIO;
   if (ensure_arenas(g, out_total, g->q_alloc)) return -EIO;
@@ -1262,6 +1343,7 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
   if (g == nullptr) return -ENOMEM;
   memset(&g->prof, 0, sizeof(g->prof));
   memset(&g->poly_prof, 0, sizeof(g->poly_prof));
+  memset(&g->casc_prof, 0, sizeof(g->casc_prof));
   g->device = device;
   g->fs = sampling_freq;
   g->max_input_len = max_input_len;
@@ -1317,6 +1399,9 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
       if (cudaEventCreate(&s.pf[i]) != cudaSuccess) return fail(-EIO);
     for (cudaEvent_t &ev : s.pf_poly)
       if (cudaEventCreate(&ev) != cudaSuccess) return fail(-EIO);
+    for (cudaEvent_t &ev : s.pf_casc)
+      if (cudaEventCreate(&ev) != cudaSuccess) return fail(-EIO);
+    if (cudaEventCreateWithFlags(&s.ev_casc, cudaEventDisableTiming) != cudaSuccess) return fail(-EIO);
     if (cudaMalloc(&s.d_vblk, T_MAX_CLASSES * sizeof(BlkInfo)) != cudaSuccess ||
         cudaHostAlloc(&s.h_vblk, T_MAX_CLASSES * sizeof(BlkInfo), cudaHostAllocDefault) != cudaSuccess)
       return fail(-ENOMEM);
@@ -1349,7 +1434,8 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
       return fail(-EIO);
     }
   if (cudaFuncSetAttribute(fir_long2_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W2_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(fir_long4_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W4_SMEM) != cudaSuccess) {
+      cudaFuncSetAttribute(fir_long4_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W4_SMEM) != cudaSuccess ||
+      cudaFuncSetAttribute(cascade_fir_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem) != cudaSuccess) {
     XL_LOG("cannot raise dynamic shared memory to %d bytes", kTileMaxSmem);
     return fail(-EIO);
   }
@@ -1435,6 +1521,9 @@ extern "C" void xlg_destroy(xlg_group *g) {
       if (s.pf[i]) cudaEventDestroy(s.pf[i]);
     for (cudaEvent_t ev : s.pf_poly)
       if (ev) cudaEventDestroy(ev);
+    for (cudaEvent_t ev : s.pf_casc)
+      if (ev) cudaEventDestroy(ev);
+    if (s.ev_casc) cudaEventDestroy(s.ev_casc);
   }
   for (HostOut &h : g->ring_out) {
     if (h.h_out) cudaFreeHost(h.h_out);
@@ -1463,6 +1552,10 @@ extern "C" void xlg_destroy(xlg_group *g) {
   if (g->d_poly3) cudaFree(g->d_poly3);
   if (g->d_poly4) cudaFree(g->d_poly4);
   if (g->d_ones) cudaFree(g->d_ones);
+  if (g->d_taps2) cudaFree(g->d_taps2);
+  for (HostClient &h : g->clients)
+    if (h.d_cring) cudaFree(h.d_cring);
+  for (float2 *p : g->dead_rings) cudaFree(p);
   if (g->ev_user) cudaEventDestroy(g->ev_user);
   if (g->s_in) cudaStreamDestroy(g->s_in);
   for (const xlg_group::StreamSet *ss : {&g->set_part, &g->set_plain}) {
@@ -1578,6 +1671,44 @@ extern "C" int xlg_add_client_rational_ex(xlg_group *g, uint32_t interp, uint32_
   return attach_client(g, interp, decim, interp * g->fs, taps, taps_len, center_freq, state, client_id);
 }
 
+extern "C" int xlg_add_client_cascade(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len,
+                                      int32_t center_freq, uint32_t decim2, const float *taps2, size_t taps2_len,
+                                      int *client_id) {
+  if (g == nullptr || client_id == nullptr) return -EINVAL;
+  if (decim1 == 0 || decim2 == 0 || taps1_len == 0 || taps2_len == 0 || taps1 == nullptr || taps2 == nullptr) {
+    XL_LOG("cascade client: decimations (%u, %u) and tap counts (%zu, %zu) must all be at least 1", decim1, decim2,
+           taps1_len, taps2_len);
+    return -EINVAL;
+  }
+  if (g->flags & XLG_TRACK_STATE) {
+    XL_LOG("cascade client: an XLG_TRACK_STATE group cannot carry the state of two stages");
+    return -ENOTSUP;
+  }
+  if (taps2_len > (size_t)INT32_MAX || cascade_smem(1, (int)decim2, (int)taps2_len) > (size_t)kTileMaxSmem) {
+    XL_LOG("cascade client: %zu stage-B taps exceed the stage-B kernel's shared memory", taps2_len);
+    return -EINVAL;
+  }
+  // stage B: the reference filter at fs / D1 with centre 0 -- its rotated taps are (h, +-0), so the real
+  // parts of the reversed taps (the even-length quirk included) are all it needs
+  xl_client_consts k2;
+  int rc = xl_client_consts_build(taps2, taps2_len, decim2, 0, std::max<uint32_t>(g->fs / decim1, 1), &k2);
+  if (rc) return rc;
+  std::vector<float> rev2(taps2_len);
+  for (size_t j = 0; j < taps2_len; j++) rev2[j] = k2.rev_cf32[2 * j];
+  xl_client_consts_free(&k2);
+  int id = -1;
+  rc = attach_client(g, 1, decim1, g->fs, taps1, taps1_len, center_freq, nullptr, &id);
+  if (rc) return rc;
+  HostClient &h = g->clients[id];
+  h.casc = true;
+  h.D2 = decim2;
+  h.T2 = taps2_len;
+  h.rev2.swap(rev2);
+  h.hist2 = (long long)taps2_len - 1;  // src/xlating.c:552
+  *client_id = id;
+  return 0;
+}
+
 extern "C" int xlg_reserve(xlg_group *g, size_t output_samples_per_block) {
   if (g == nullptr) return -EINVAL;
   CU_OK(cudaSetDevice(g->device));
@@ -1591,6 +1722,9 @@ extern "C" int xlg_remove_client(xlg_group *g, int client_id) {
   if (g == nullptr || client_id < 0 || client_id >= (int)g->clients.size() || !g->clients[client_id].active)
     return -EINVAL;
   g->clients[client_id].active = false;
+  if (g->clients[client_id].d_cring) g->dead_rings.push_back(g->clients[client_id].d_cring);  // in-flight tickets read it
+  g->clients[client_id].d_cring = nullptr;
+  g->clients[client_id].rev2.clear();
   g->clients[client_id].rev.clear();
   g->clients[client_id].rev_q15.clear();
   g->dirty = true;
@@ -1608,7 +1742,19 @@ extern "C" int xlg_client_info(const xlg_group *g, int client_id, size_t *histor
   if (g == nullptr || client_id < 0 || client_id >= (int)g->clients.size() || !g->clients[client_id].active)
     return -EINVAL;
   if (history) *history = (size_t)g->clients[client_id].hist;
-  if (kernel_kind) *kernel_kind = g->clients[client_id].kind;
+  if (kernel_kind) *kernel_kind = g->clients[client_id].casc ? 5 : g->clients[client_id].kind;
+  return 0;
+}
+
+extern "C" int xlg_cascade_info(const xlg_group *g, int client_id, int *stage_a_kind, size_t *stage_a_history,
+                                size_t *stage_b_history) {
+  if (g == nullptr || client_id < 0 || client_id >= (int)g->clients.size() || !g->clients[client_id].active ||
+      !g->clients[client_id].casc)
+    return -EINVAL;
+  const HostClient &h = g->clients[client_id];
+  if (stage_a_kind) *stage_a_kind = h.kind;
+  if (stage_a_history) *stage_a_history = (size_t)h.hist;
+  if (stage_b_history) *stage_b_history = (size_t)h.hist2;
   return 0;
 }
 
@@ -1637,8 +1783,8 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
   const bool q15 = (flags & XLG_PATH_Q15) != 0;
   if (q15)
     for (const HostClient &h : g->clients)
-      if (h.active && h.L > 1) {
-        XL_LOG("the Q15 path does not serve rational clients; submit without XLG_PATH_Q15");
+      if (h.active && (h.L > 1 || h.casc)) {
+        XL_LOG("the Q15 path does not serve rational or cascade clients; submit without XLG_PATH_Q15");
         return -ENOTSUP;
       }
   CU_OK(cudaSetDevice(g->device));
@@ -1707,9 +1853,10 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     ho.q15 = q15;
   }
   s.q15 = q15;
-  s.tile_macs = s.algo_macs = s.out_samples = s.poly_macs = 0;
+  s.tile_macs = s.algo_macs = s.out_samples = s.poly_macs = s.casc_macs = s.d2h_bytes = 0;
   s.in_samples = (uint64_t)n;
-  int max_generic_out = 0, poly_warps = 0, max_poly4_out = 0;
+  int max_generic_out = 0, poly_warps = 0, max_poly4_out = 0, n_casc = 0, max_n1 = 0, max_n2 = 0;
+  size_t casc_smem = 0;
   for (size_t i = 0; i < g->clients.size(); i++) {
     HostClient &h = g->clients[i];
     if (!h.active) continue;
@@ -1735,6 +1882,29 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       poly_warps = std::max(poly_warps, (int)std::min<long long>(h.L, n_out) * ((per + G_OPW - 1) / G_OPW));
     }
     if (q15 || h.kind == 0) max_generic_out = std::max(max_generic_out, n_out);
+    if (h.casc) {
+      // stage B: the reference's walk over this block's n_out stage-A samples
+      const long long first2 = h.a_pos - h.hist2;
+      const int n2 = xl_walk(&h.hist2, n_out, h.T2, h.D2, h.fin_cap);
+      CascBlk &cb = s.h_cblk[n_casc++];
+      cb.ring = h.d_cring;
+      cb.a_pos = h.a_pos;
+      cb.first = first2;
+      cb.mask = (unsigned)(h.cring_cap - 1);
+      cb.a_off = h.out_off;
+      cb.n1 = n_out;
+      cb.n2 = n2;
+      cb.D2 = (int)h.D2;
+      cb.T2 = (int)h.T2;
+      cb.taps_off = h.taps2_off;
+      cb.out_off = h.fin_off;
+      h.a_pos += n_out;
+      h.last_n2 = n2;
+      max_n1 = std::max(max_n1, n_out);
+      max_n2 = std::max(max_n2, n2);
+      casc_smem = std::max(casc_smem, cascade_smem(C_KO, cb.D2, cb.T2));
+      s.casc_macs += (uint64_t)n2 * h.T2;
+    }
   }
 
   // consecutive blocks alternate between two compute streams so that the tail of
@@ -2097,6 +2267,40 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
                                                              s.d_phases, s.d_out);
     if (g->profiling) CU_OK(cudaEventRecord(s.pf_poly[1], cs));
   }
+  // ---- cascade clients: append the stage-A outputs to their rings, then stage B ----
+  s.pf_cb = false;
+  if (!q15 && n_casc > 0) {
+    // the rings are appended in block order: after the previous block's stage B, whichever stream ran it
+    if (g->have_last_casc) CU_OK(cudaStreamWaitEvent(cs, g->ev_last_casc, 0));
+    if (g->profiling) {
+      CU_OK(cudaEventRecord(s.pf_casc[0], cs));
+      s.pf_cb = true;
+    }
+    CU_OK(cudaMemcpyAsync(s.d_cblk, s.h_cblk, (size_t)n_casc * sizeof(CascBlk), cudaMemcpyHostToDevice, cs));
+    if (max_n1 > 0) cascade_append_kernel<<<dim3((max_n1 + 255) / 256, n_casc), 256, 0, cs>>>(s.d_cblk, s.d_out);
+    if (max_n2 > 0) {
+      // fewer outputs per CTA where a long stage-B window would not fit (attach checked that one output fits)
+      int ko = C_KO;
+      while (ko > 1 && casc_smem > (size_t)kTileMaxSmem) {
+        ko /= 2;
+        casc_smem = 0;
+        for (int c = 0; c < n_casc; c++)
+          casc_smem = std::max(casc_smem, cascade_smem(ko, s.h_cblk[c].D2, s.h_cblk[c].T2));
+      }
+      cascade_fir_cf32_kernel<<<dim3((max_n2 + ko - 1) / ko, n_casc), C_THREADS, casc_smem, cs>>>(s.d_cblk, g->d_taps2,
+                                                                                                s.d_out, ko);
+    }
+    if (g->profiling) CU_OK(cudaEventRecord(s.pf_casc[1], cs));
+    CU_OK(cudaEventRecord(s.ev_casc, cs));
+    g->ev_last_casc = s.ev_casc;
+    g->have_last_casc = true;
+    // from here on the client's results are its final row
+    for (size_t i = 0; i < g->clients.size(); i++)
+      if (g->clients[i].active && g->clients[i].casc) {
+        ho.n_out[i] = g->clients[i].last_n2;
+        ho.out_off[i] = g->clients[i].fin_off;
+      }
+  }
   CU_OK(cudaGetLastError());
   CU_OK(cudaEventRecord(s.ev_fir, cs));
 
@@ -2104,13 +2308,14 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
   if (!dev_out && g->arena_cap > 0 && nc > 0) {
     size_t used = 0;
     for (size_t i = 0; i < g->clients.size(); i++)
-      if (g->clients[i].active) used = std::max(used, (size_t)g->clients[i].out_off + (size_t)ho.n_out[i]);
+      if (g->clients[i].active) used = std::max(used, (size_t)ho.out_off[i] + (size_t)ho.n_out[i]);  // final rows
     CU_OK(cudaStreamWaitEvent(g->s_out, s.ev_fir, 0));
     if (used > 0) {
       if (q15)
         CU_OK(cudaMemcpyAsync(ho.h_qout, s.d_qout, used * sizeof(short2), cudaMemcpyDeviceToHost, g->s_out));
       else
         CU_OK(cudaMemcpyAsync(ho.h_out, s.d_out, used * sizeof(float2), cudaMemcpyDeviceToHost, g->s_out));
+      s.d2h_bytes = used * (q15 ? sizeof(short2) : sizeof(float2));
     }
     if ((g->flags & XLG_TRACK_STATE) && !q15 && s.d_endph != nullptr && ho.h_endph != nullptr)
       CU_OK(cudaMemcpyAsync(ho.h_endph, s.d_endph, (size_t)nc * sizeof(float2), cudaMemcpyDeviceToHost, g->s_out));
@@ -2330,6 +2535,14 @@ extern "C" int xlg_poly_profile_read(xlg_group *g, xlg_poly_profile *p, int rese
   std::lock_guard<std::mutex> lk(g->mu);
   *p = g->poly_prof;
   if (reset) memset(&g->poly_prof, 0, sizeof(g->poly_prof));
+  return 0;
+}
+
+extern "C" int xlg_cascade_profile_read(xlg_group *g, xlg_cascade_profile *p, int reset) {
+  if (g == nullptr || p == nullptr) return -EINVAL;
+  std::lock_guard<std::mutex> lk(g->mu);
+  *p = g->casc_prof;
+  if (reset) memset(&g->casc_prof, 0, sizeof(g->casc_prof));
   return 0;
 }
 

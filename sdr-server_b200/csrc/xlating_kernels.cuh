@@ -25,6 +25,8 @@
  *                    (cp.async.bulk + mbarrier, 3 stages)
  *   fir_generic_*    any (T, D, alignment): one warp per 4 outputs, lanes split the
  *                    taps, warp-shuffle reduction; also the Q15 integer path
+ *   cascade_*        stage B of two-stage clients: a real-tap decimator over each
+ *                    client's stage-A history ring, TMA-staged window, register tile
  *
  * The arithmetic shared with the per-filter drop-in engine (conversions, oscillator
  * recursion, generic FIR warp) lives in xlating_common.cuh.
@@ -1152,6 +1154,103 @@ fir_long_reduce_kernel(const __grid_constant__ TileLaunch P, const float2 *__res
   float2 ph = phases[K.ph_base + (long long)grp * K.ph_stride + (size_t)(k >> 1) * 32 + lane];
   if (k & 1) ph = cmul_unfused(ph, __ldg(member_incr + K.members_off + grp * T_CG + lane));
   out[off + k] = cmul_unfused(acc, ph);  // src/xlating.c:70
+}
+
+// ---------------------------------------------------------------------------
+// cascade clients (xlg_add_client_cascade).  Stage A is an integer client of the kernels above whose
+// outputs land in a row of the slot's arena that is never copied to the host.  Stage B is the reference
+// filter at fs / D1 with centre 0: its rotated taps are (h, +-0), its oscillator stays 1 + 0i and the
+// renormalisation divides by 1, so it is a real-tap decimator with history,
+//     z[k] = sum_{j < T2} y[first + k*D2 + j] * rev2[j]          (2 real FMAs per tap),
+// over the client's stage-A stream y, kept in a per-client power-of-two ring in HBM: y at stage-A stream
+// position p lives at ring[p & mask], and positions before the attach point read as the ring's zeros.
+// ---------------------------------------------------------------------------
+struct CascBlk {
+  float2 *ring;     // the client's stage-A history ring
+  long long a_pos;  // stage-A stream position of this block's first stage-A output
+  long long first;  // stage-A stream position where this block's stage-B output 0 starts its window
+  unsigned mask;    // ring capacity - 1
+  int a_off;        // this block's stage-A outputs in the slot's output arena
+  int n1, n2;       // stage-A outputs appended / stage-B outputs computed by this block
+  int D2, T2;
+  int taps_off;     // float offset of rev2 in the real tap arena, a multiple of 4 (16-byte TMA source)
+  int out_off;      // final row in the slot's output arena
+};
+
+// companion copy: append this block's stage-A outputs to each client's ring (grid.y = client)
+__global__ void __launch_bounds__(256)
+cascade_append_kernel(const CascBlk *__restrict__ cb, const float2 *__restrict__ out) {
+  const CascBlk &b = cb[blockIdx.y];
+  const int n1 = b.n1;
+  for (int i = blockIdx.x * 256 + threadIdx.x; i < n1; i += gridDim.x * 256)
+    b.ring[(unsigned)((unsigned long long)(b.a_pos + i)) & b.mask] = out[b.a_off + i];
+}
+
+constexpr int C_THREADS = 128;
+constexpr int C_R = 2;                    // outputs per thread: t and t + C_THREADS
+constexpr int C_KO = C_THREADS * C_R;     // outputs per CTA at most (the host lowers it where shared memory runs out)
+// shared memory of a CTA with ko outputs: mbarrier, taps padded to 16 bytes, the window (+1 for an odd start, even)
+__host__ __device__ constexpr size_t cascade_smem(int ko, int D2, int T2) {
+  return 16 + (size_t)((T2 + 3) & ~3) * 4 + (((size_t)(ko - 1) * D2 + T2 + 2) & ~(size_t)1) * 8;
+}
+
+// Stage B: CTA (x, c) computes outputs [x*ko, x*ko + ko) of cascade client c.  One TMA bulk copy stages the
+// taps, one or two (the ring wraps) stage the window; every thread then keeps C_R outputs in registers.
+// Lane l walks the taps starting at j = l (mod T2) when D2 is even: the lanes' samples then lie D2 + 1
+// apart in shared memory, an odd stride, so neither the window nor the tap loads have bank conflicts
+// (with odd D2 every lane starts at j = 0 and the tap load is a broadcast).
+__global__ void __launch_bounds__(C_THREADS)
+cascade_fir_cf32_kernel(const CascBlk *__restrict__ cb, const float *__restrict__ taps2, float2 *__restrict__ out,
+                        int ko) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  uint64_t *bar = reinterpret_cast<uint64_t *>(smem);
+  const CascBlk &b = cb[blockIdx.y];
+  const int n2 = b.n2, k0 = blockIdx.x * ko;
+  if (k0 >= n2) return;
+  const int D2 = b.D2, T2 = b.T2, tpad = (T2 + 3) & ~3;
+  const int nk = min(ko, n2 - k0);
+  float *ts = reinterpret_cast<float *>(smem + 16);
+  float2 *xs = reinterpret_cast<float2 *>(smem + 16 + tpad * 4);
+  const unsigned idx = (unsigned)((unsigned long long)(b.first + (long long)k0 * D2)) & b.mask;
+  const unsigned shift = idx & 1u;  // an odd window start is fetched from one sample earlier (16-byte source)
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    mbar_init(bar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  __syncthreads();
+  if (tid == 0) {
+    const unsigned need = ((unsigned)((nk - 1) * D2 + T2) + shift + 1u) & ~1u;
+    const unsigned p1 = min(need, b.mask + 1u - (idx - shift));
+    mbar_expect_tx(bar, (unsigned)tpad * 4u + need * 8u);
+    tma_bulk_g2s(ts, taps2 + b.taps_off, (unsigned)tpad * 4u, bar);
+    tma_bulk_g2s(xs, b.ring + (idx - shift), p1 * 8u, bar);
+    if (p1 < need) tma_bulk_g2s(xs + p1, b.ring, (need - p1) * 8u, bar);
+  }
+  mbar_wait(bar, 0);
+  if (tid >= nk) return;
+  const float2 *x[C_R];
+#pragma unroll
+  for (int i = 0; i < C_R; i++) x[i] = xs + shift + (size_t)min(tid + C_THREADS * i, nk - 1) * D2;
+  float2 acc[C_R];
+#pragma unroll
+  for (int i = 0; i < C_R; i++) acc[i] = make_float2(0.f, 0.f);
+  int j = (D2 & 1) ? 0 : (tid & 31) % T2;
+#pragma unroll 4
+  for (int s = 0; s < T2; s++) {
+    const float h = ts[j];
+#pragma unroll
+    for (int i = 0; i < C_R; i++) {
+      const float2 v = x[i][j];
+      acc[i].x = fmaf(v.x, h, acc[i].x);
+      acc[i].y = fmaf(v.y, h, acc[i].y);
+    }
+    if (++j == T2) j = 0;
+  }
+#pragma unroll
+  for (int i = 0; i < C_R; i++)
+    if (tid + C_THREADS * i < nk) out[b.out_off + k0 + tid + C_THREADS * i] = acc[i];
 }
 
 }  // namespace xl
