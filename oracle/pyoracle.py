@@ -70,6 +70,8 @@ def orc() -> C.CDLL:
         lib.orc_xlating_phase.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float)]
         lib.orc_xlating_taps.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_float))]
         lib.orc_xlating_taps.restype = C.c_size_t
+        lib.orc_xlating_set_state.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_size_t, C.c_float, C.c_float]
+        lib.orc_xlating_set_state.restype = C.c_int
         _orc = lib
     return _orc
 
@@ -127,6 +129,15 @@ class OracleFilter:
         re, im = C.c_float(), C.c_float()
         self._lib.orc_xlating_phase(self._h, C.byref(re), C.byref(im))
         return complex(re.value, im.value)
+
+    def set_state(self, history: np.ndarray, phase: complex) -> None:
+        """Continue from a given state: `history` (complex, oldest first) is what the next window reaches
+        back to, its length the history offset; `phase` the oscillator."""
+        h = np.ascontiguousarray(np.asarray(history, dtype=np.complex64)).view(np.float32)
+        code = self._lib.orc_xlating_set_state(self._h, h.ctypes.data_as(C.POINTER(C.c_float)), h.size // 2,
+                                               float(phase.real), float(phase.imag))
+        if code != 0:
+            raise ValueError(f"orc_xlating_set_state -> {code}")
 
     @property
     def rev_taps(self) -> np.ndarray:

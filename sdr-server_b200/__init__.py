@@ -126,6 +126,9 @@ def lib() -> C.CDLL:
     L.xlg_destroy.restype = None
     L.xlg_add_client.argtypes = [vp, u32, C.POINTER(C.c_float), sz, i32, C.POINTER(C.c_int)]
     L.xlg_add_client.restype = C.c_int
+    L.xlg_add_client_ex.argtypes = [vp, u32, C.POINTER(C.c_float), sz, i32, C.POINTER(XlgClientState),
+                                    C.POINTER(C.c_int)]
+    L.xlg_add_client_ex.restype = C.c_int
     L.xlg_add_client_rational.argtypes = [vp, u32, u32, C.POINTER(C.c_float), sz, i32, C.POINTER(C.c_int)]
     L.xlg_add_client_rational.restype = C.c_int
     L.xlg_add_client_rational_ex.argtypes = [vp, u32, u32, C.POINTER(C.c_float), sz, i32, C.POINTER(XlgClientState),
@@ -158,6 +161,8 @@ def lib() -> C.CDLL:
     L.xlg_output.restype = C.c_int
     L.xlg_read_output.argtypes = [vp, C.c_int64, C.c_int, vp, sz, C.POINTER(sz)]
     L.xlg_read_output.restype = C.c_int
+    L.xlg_copy_output.argtypes = [vp, C.c_int64, C.c_int, vp, sz, C.POINTER(sz), C.POINTER(XlgClientState)]
+    L.xlg_copy_output.restype = C.c_int
     L.xlg_alloc_pinned.argtypes = [sz]
     L.xlg_alloc_pinned.restype = vp
     L.xlg_free_pinned.argtypes = [vp]
@@ -310,11 +315,17 @@ class Group:
         self.flags = flags
         self.fs = sampling_freq
 
-    def add_client(self, decimation: int, taps, center_freq: int) -> int:
+    def add_client(self, decimation: int, taps, center_freq: int, state=None) -> int:
+        """state: an XlgClientState for a client that continues a stream it consumed elsewhere
+        (xlg_add_client_ex); None for a fresh client."""
         taps = np.ascontiguousarray(taps, dtype=np.float32)
         cid = C.c_int(-1)
-        code = self._L.xlg_add_client(self._h, decimation, taps.ctypes.data_as(C.POINTER(C.c_float)), len(taps),
-                                      center_freq, C.byref(cid))
+        fp = taps.ctypes.data_as(C.POINTER(C.c_float))
+        if state is None:
+            code = self._L.xlg_add_client(self._h, decimation, fp, len(taps), center_freq, C.byref(cid))
+        else:
+            code = self._L.xlg_add_client_ex(self._h, decimation, fp, len(taps), center_freq, C.byref(state),
+                                             C.byref(cid))
         if code != 0:
             raise ValueError(code)
         return cid.value
@@ -432,6 +443,22 @@ class Group:
             raise RuntimeError(f"xlg_read_output -> {code}")
         assert got.value == n
         return buf
+
+    def copy_output(self, ticket: int, cid: int):
+        """xlg_copy_output of a completed ticket with its state_after (XLG_TRACK_STATE groups): (cf32 output,
+        XlgClientState after the ticket).  Raises ValueError(code) on a nonzero return."""
+        st, n = XlgClientState(), C.c_size_t(0)
+
+        def copy(buf):
+            code = self._L.xlg_copy_output(self._h, ticket, cid, buf.ctypes.data, buf.size, C.byref(n), C.byref(st))
+            if code != 0:
+                raise ValueError(code)
+            return buf
+
+        buf = copy(np.zeros(1, dtype=np.complex64))  # reports the count
+        if n.value > buf.size:
+            buf = copy(np.zeros(n.value, dtype=np.complex64))
+        return buf[:n.value].copy(), st
 
     def wait_stream(self, cuda_stream: int) -> None:
         code = self._L.xlg_wait_stream(self._h, cuda_stream)

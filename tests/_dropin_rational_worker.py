@@ -13,12 +13,15 @@ usage: _dropin_rational_worker.py <scenario> [arg]   -> one JSON line, exit code
   combined                 rational, integer cf32 and integer Q15 filters across formats and ragged
                            sizes meet at a barrier every block: every call within the contract
   neighbours               integer filters give the same bits with rational filters alive
-  overlay steady|drops|late|lag   24 rational + 4 integer filters of one band, exact stimuli
+  overlay steady|drops|late|lag   24 rational + 4 integer filters of one band on one real cs16 stream, half
+                           one-hot at centres across the band, half dyadic at centre 0
   q15refuse                a refused Q15 call leaves a member filter's stream untouched
   wide                     exact stimuli at L from 4 to 441 (L >= 16: a call's span of residues is cut at 16;
                            calls with fewer outputs than L), every output equal to the float64 sum
-  phase                    branch-one-hot filters at nonzero centres on a real cs16 stream: every output equal
-                           to the strict oracle on the zero-stuffed stream bit for bit (oscillator included)
+  phase [lone]             branch-one-hot rational and one-hot integer filters at nonzero centres and dyadic
+                           integer filters at centre 0 on one real cs16 stream, 108 calls each: every output
+                           equal to the strict oracle on the zero-stuffed stream, or to the float64 sum, bit for
+                           bit (oscillator included); lone: one filter alive at a time
 """
 import importlib
 import json
@@ -33,7 +36,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from oracle import pyoracle as po  # noqa: E402  (checker)
-from exact import assert_exact, dyadic_taps, exact_input, grid_step  # noqa: E402
+from exact import assert_exact, dyadic_taps, exact_input, grid_step, one_hot_taps  # noqa: E402
 from rational import (ROWS, branch_one_hot_taps, oracle_filter, real_grid_input, ref_rational_f64,  # noqa: E402
                       stuff)
 from util import assert_cf32_close, rand_block  # noqa: E402
@@ -65,6 +68,7 @@ class F:
         else:
             self.f = pkg.XlatingFilter.rational(max(L, 1), M, taps, center, fs, max_in)
         self.seen, self.got = [], []
+        self.dyadic = False  # dyadic taps at centre 0: checked against the float64 sum
 
     def call(self, x):
         y = self.f.process_q15(self.fmt, x) if self.q15 else self.f.process_cf32(self.fmt, x)
@@ -274,9 +278,11 @@ def scenario_neighbours():
 
 def scenario_overlay(mode):
     rng = np.random.default_rng(41)
-    n_blocks = 16
-    filters = exact_filters(rng, "cu8", FS, 65536, [(3, 128, 97), (7, 320, 431)] * 12, 4)
-    blocks = [exact_input(rng, "cu8", 65536) for _ in range(n_blocks)]
+    n_blocks, max_in = 16, 65536
+    # half of each class one-hot at centres across the band, half dyadic at centre 0, on one real stream
+    filters = [(hot_filter if k % 4 < 2 else dyadic_filter)(rng, L, M, T, FS, max_in)
+               for k, (L, M, T) in enumerate([(3, 128, 385), (7, 320, 431)] * 12 + [(0, 42, 97)] * 4)]
+    blocks = [real_grid_input(rng, max_in) for _ in range(n_blocks)]
     r = np.random.default_rng(5)
     drop = {(i, b) for i in range(len(filters)) for b in range(3, n_blocks) if i % 3 == 0 and r.integers(0, 5) == 0}
     skip = {"drops": lambda i, b: (i, b) in drop,
@@ -287,7 +293,7 @@ def scenario_overlay(mode):
     calls = sum(len(f.got) for f in filters)
     stream = pkg.dropin_stream_stats()
     for i, f in enumerate(filters):
-        checked(errors, f.check_exact, f"filter {i}")
+        check_mixed(errors, f, FS, max_in, f"filter {i}")
         f.close()
     return {"errors": errors, "stream": stream, "calls": calls, "filters": len(filters)}
 
@@ -336,19 +342,77 @@ def scenario_wide():
     return {"errors": errors, "long_spans": spans, "fewer_than_L": few}
 
 
-def scenario_phase():
+# integer (D, T) of the phase scenario: client_plan's 48 and 96 ksps classes at 2.016 Msps (8 filters each, so
+# that the band's group tiles them), D = 1, even T, T = D
+PHASE_INT = [(42, 505, 4), (21, 253, 4), (1, 1, 1), (8, 64, 1), (7, 7, 1)]
+# 108 calls: empty, 1-sample (2 and 3 elements: samples without outputs), odd and ragged sizes; the private
+# rings wrap many times
+PHASE_SIZES = [16384, 16384, 7001, 2, 0, 16384, 3, 16382, 5, 12345, 16384, 999] * 9
+
+
+def hot_filter(rng, L, M, T, fs, max_in, j=None):
+    """A filter at a centre drawn across the band whose accumulators are each one rounded product on a real
+    input: branch-one-hot taps (L > 0) or one hot tap at j (L = 0; random when None)."""
+    center = int(rng.integers(-fs // 2 + 30000, fs // 2 - 30000))
+    if L:
+        taps = branch_one_hot_taps(rng, T, L)
+    else:
+        taps = one_hot_taps(T, int(rng.integers(0, T)) if j is None else j, float(rng.choice([0.75, -0.5])))
+    return F(L, M, taps, center, fs, max_in, "cs16")
+
+
+def dyadic_filter(rng, L, M, T, fs, max_in):
+    f = F(L, M, dyadic_taps(rng, T, "cs16"), 0, fs, max_in, "cs16")
+    f.dyadic = True
+    return f
+
+
+def check_mixed(errors, f, fs, max_in, what):
+    if f.dyadic:
+        checked(errors, f.check_exact, f"{what} (dyadic)")
+    else:
+        checked(errors, f.check_oracle_exact, fs, max_in, what)
+
+
+def phase_filters(rng, fs, max_in):
+    """PHASE's rational filters and PHASE_INT's integer filters (one-hot at the first, the last and random
+    taps) at centres across the band, and as many dyadic integer filters at centre 0.  A generator: each
+    filter is created when it is taken."""
+    for L, M, T in PHASE * 2:
+        yield hot_filter(rng, L, M, T, fs, max_in)
+    for D, T, n in PHASE_INT:
+        for k in range(n):
+            yield hot_filter(rng, 0, D, T, fs, max_in, j=(0, T - 1, None)[k % 3])
+            yield dyadic_filter(rng, 0, D, T, fs, max_in)
+
+
+def scenario_phase(mode=None):
+    """lone: one filter alive at a time, so that each call walks its oscillator while the front kernel runs
+    (the engine does that while fewer than two filters are alive).  `alone` counts the filters that found no
+    band group when they had made all their calls: the group exists, and publishes the blocks it sees, from
+    the moment two filters of one band are alive until the last of them is destroyed."""
     fs, max_in = 2048000, 16384
     rng = np.random.default_rng(67)
-    filters = []
-    for k, (L, M, T) in enumerate(PHASE * 2):
-        center = int(rng.integers(-fs // 2 + 30000, fs // 2 - 30000))
-        filters.append(F(L, M, branch_one_hot_taps(rng, T, L), center, fs, max_in, "cs16"))
-    blocks = [real_grid_input(rng, n) for n in SMALL * 2]
-    errors = run_threads(filters, lambda i, b: blocks[b], len(blocks))
+    blocks = [real_grid_input(rng, n) for n in PHASE_SIZES]
+    errors = []
+    alone = 0
+    if mode == "lone":
+        filters = []
+        for f in phase_filters(rng, fs, max_in):  # created, run and closed one by one
+            errors += run_threads([f], lambda i, b: blocks[b], len(blocks))
+            alone += pkg.dropin_stream_stats()["published"] == 0
+            f.close()
+            filters.append(f)
+    else:
+        filters = list(phase_filters(rng, fs, max_in))
+        errors += run_threads(filters, lambda i, b: blocks[b], len(blocks))
+    batches, calls, shared = pkg.dropin_stats()  # this process's engine served only these filters
+    stream = pkg.dropin_stream_stats()
     for i, f in enumerate(filters):
-        checked(errors, f.check_oracle_exact, fs, max_in, f"filter {i}")
+        check_mixed(errors, f, fs, max_in, f"filter {i}")
         f.close()
-    return {"errors": errors, "stream": pkg.dropin_stream_stats()}
+    return {"errors": errors, "stream": stream, "filters": len(filters), "batches": batches, "calls": calls,
+            "shared": shared, "alone": alone}
 
 
 def main():

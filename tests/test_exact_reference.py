@@ -7,8 +7,6 @@
 * mutations that the float tolerance cannot see with designed (lpf.c) taps -- a dropped first or
   last tap, an un-zeroed oldest history sample, two clients' taps swapped -- fail assert_exact.
 """
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -86,11 +84,7 @@ def test_ref_f64_history_equals_oracle_state():
     hist = to_complex(fmt, exact_input(rng, fmt, 2 * (T - 1)))
     blocks = ragged_blocks(rng, fmt, [4096, 7, 2000])
     o = po.OracleFilter(D, taps, 0, 2016000, MAX_IN)
-    lib = po.orc()
-    lib.orc_xlating_set_state.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_size_t, C.c_float, C.c_float]
-    lib.orc_xlating_set_state.restype = C.c_int
-    h32 = np.ascontiguousarray(hist.astype(np.complex64)).view(np.float32)
-    assert lib.orc_xlating_set_state(o._h, h32.ctypes.data_as(C.POINTER(C.c_float)), T - 1, 1.0, 0.0) == 0
+    o.set_state(hist, 1 + 0j)
     got = [o.process_cf32(fmt, x) for x in blocks]
     assert_exact(ref_f64(taps, D, fmt, blocks, history=hist), got, "history", T, D, grid_step(taps, fmt))
 
@@ -98,17 +92,45 @@ def test_ref_f64_history_equals_oracle_state():
 # ---------------------------------------------------------------------------
 # one-hot taps, real input, any centre: FMA accumulation == the oracle's unfused sums
 # ---------------------------------------------------------------------------
-@pytest.mark.parametrize("center", [-987654, -312000, 1, 400123, 1007999])
-@pytest.mark.parametrize("j", [0, 100, 252])
-def test_one_hot_real_input_fma_matches_oracle(center, j):
+ONE_HOT_CENTRES = [-987654, -312000, 1, 400123, 1007999]
+
+
+def drawn_centres(fs, half_width, n=4, seed=5):
+    """Centres drawn the way the GPU phase tests draw theirs: uniformly in +-(fs / 2 - half_width)."""
+    band = fs // 2 - half_width
+    return [int(c) for c in np.random.default_rng(seed + fs % 1000003).integers(-band, band, n)]
+
+
+# (j, centre, D, T, fs): the (21, 253) class at every fixed centre; the other integer classes of the hand-over
+# and drop-in phase tests (D = 1, even T, T = D) with the first, a middle and the last tap, at the fixed
+# centres of the 2.016 Msps band and at centres drawn as the drop-in phase scenario (2.048 Msps) and the
+# split-K hand-over band (61.44 Msps) draw theirs (same distributions, not the same draws)
+ONE_HOT_CASES = ([(j, c, 21, 253, 2016000) for j in (0, 100, 252) for c in ONE_HOT_CENTRES] +
+                 [(j, c, D, T, 2016000) for D, T in ((42, 505), (8, 64), (7, 7), (1, 1), (42, 200))
+                  for j in sorted({0, T // 2, T - 1}) for c in ONE_HOT_CENTRES] +
+                 [(j, c, D, T, 2048000) for D, T in ((42, 505), (21, 253), (8, 64), (7, 7), (1, 1))
+                  for j in sorted({0, T // 2, T - 1}) for c in drawn_centres(2048000, 30000)] +
+                 [(j, c, 1280, 1407, 61440000) for j in (0, 703, 1406)
+                  for c in drawn_centres(61440000, 61440000 // 2560 + 1000)])
+
+
+def one_hot_id(j, c, D, T, fs):
+    if fs != 2016000:
+        return f"fs{fs}-D{D}T{T}-{j}-{c}"
+    return f"{j}-{c}" if (D, T) == (21, 253) else f"D{D}T{T}-{j}-{c}"
+
+
+@pytest.mark.parametrize("j,center,D,T,fs", ONE_HOT_CASES, ids=[one_hot_id(*case) for case in ONE_HOT_CASES])
+def test_one_hot_real_input_fma_matches_oracle(j, center, D, T, fs):
     rng = np.random.default_rng(j + 17)
-    fs, D, T = 2016000, 21, 253
     taps = one_hot_taps(T, j, 0.75)
     o = po.OracleFilter(D, taps, center, fs, MAX_IN)
     rev = o.rev_taps
     inc = oscillator_increment(D, center, fs)
-    blocks = [real_input(rng, n) for n in (4096, 2, 1001, 4096, 0, 3000)]
+    sizes = (4096, 2, 1001, 4096, 0, 3000) if D < 1000 else (MAX_IN, 2, 16001, MAX_IN, 0, 48000)
+    blocks = [real_input(rng, n) for n in sizes]
     want = [o.process_cf32("cs16", x) for x in blocks]
+    assert sum(len(w) for w in want) > 20
     assert_exact(gpu_model(rev, inc, D, blocks), want, f"centre {center} j={j}", T, D)
 
 

@@ -5,7 +5,6 @@ band's batch group.
 A rational filter is the filter with decimation M at L * fs fed the zero-stuffed stream
 (tests/rational.py).  The drop-in scenarios run in tests/_dropin_rational_worker.py, one subprocess per
 engine configuration (the engine reads its switches once per process)."""
-import ctypes as C
 import errno
 import json
 import os
@@ -82,9 +81,33 @@ def test_wide_interpolations_exact(env):
 @pytest.mark.parametrize("stream", ["1", "0"], ids=["overlay", "private"])
 @pytest.mark.parametrize("osc", ["host", "device", "lanes"])
 def test_phase_one_hot_at_any_centre(osc, stream):
-    """Branch-one-hot filters at nonzero centres on a real input equal the strict oracle bit for bit under
-    every oscillator walk (the host one mirrors the output count in upsampled coordinates)."""
-    run("phase", env={"XLATING_B200_OSC": osc, "XLATING_B200_STREAM": stream})
+    """Branch-one-hot rational and one-hot integer filters at nonzero centres on a real input equal the strict
+    oracle bit for bit under every oscillator walk (the host one mirrors the output count in upsampled
+    coordinates), and dyadic integer filters at centre 0 on the same stream the float64 sum.  With the
+    overlay on and the host walk, filters join the band's group: the phase is handed over and back."""
+    line = run("phase", env={"XLATING_B200_OSC": osc, "XLATING_B200_STREAM": stream})
+    if stream == "1" and osc == "host":
+        st = line["stream"]
+        assert st["joins"] > 0 and st["served_by_group"] > 0 and st["published"] > 0
+
+
+@pytest.mark.parametrize("case", ["lone", "lanes1", "no_share"])
+def test_phase_one_hot_engine_paths(case):
+    """The phase scenario on the private engine's other paths.  lone: one filter alive at a time, so each call
+    walks its host oscillator while the front kernel converts; lanes1: one launch lane, so calls share
+    batches; no_share: every call stages its own input."""
+    if case == "lone":
+        line = run("phase", "lone")
+        # no filter ever had a band group (which appears with a second live filter of the band, see the
+        # overlay case of test_phase_one_hot_at_any_centre) and every batch held one call
+        assert line["alone"] == line["filters"] > 0 and line["batches"] == line["calls"] > 0
+    elif case == "lanes1":
+        line = run("phase", env={**PRIVATE, "XLATING_B200_LANES": "1"})
+        assert 0 < line["batches"] < line["calls"]
+    else:
+        assert run("phase", env=PRIVATE)["shared"] > 0  # the same calls share staged inputs by default
+        line = run("phase", env={**PRIVATE, "XLATING_B200_SHARE": "0"})
+        assert line["shared"] == 0 and line["calls"] > 0
 
 
 def test_combined_calls_mix_rational_integer_and_q15():
@@ -133,17 +156,6 @@ def test_refused_q15_call_consumes_nothing():
 
 # ---- xlg_add_client_rational_ex ----
 
-def _copy_output(pkg, g, t, cid):
-    fn = pkg.lib().xlg_copy_output
-    fn.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t),
-                   C.POINTER(pkg.XlgClientState)]
-    fn.restype = C.c_int
-    buf = np.zeros(MAX_IN, dtype=np.complex64)
-    got, st = C.c_size_t(0), pkg.XlgClientState()
-    assert fn(g._h, t, cid, buf.ctypes.data, buf.size, C.byref(got), C.byref(st)) == 0
-    return buf[:got.value].copy(), st
-
-
 @pytest.mark.parametrize("interp_one", [False, True], ids=["rational", "interp1"])
 def test_reattach_continues_bit_for_bit(pkg, monkeypatch, interp_one):
     """A client re-attached mid-stream to a second group with the XLG_TRACK_STATE state of the first
@@ -167,7 +179,7 @@ def test_reattach_continues_bit_for_bit(pkg, monkeypatch, interp_one):
         ta, tb = a.submit("cu8", x), b.submit("cu8", x)
         a.wait(ta)
         b.wait(tb)
-        y, st = _copy_output(pkg, a, ta, ca)
+        y, st = a.copy_output(ta, ca)
         want.append(y)
         if i >= cut:
             got.append(b.output(tb, cb))
@@ -193,14 +205,7 @@ def test_interp_one_is_add_client_ex(pkg):
         if rational:
             cid = g.add_client_rational(1, 42, taps, -312000, state=st)
         else:
-            cid = C.c_int(-1)
-            fn = pkg.lib().xlg_add_client_ex
-            fn.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_float), C.c_size_t, C.c_int32,
-                           C.POINTER(pkg.XlgClientState), C.POINTER(C.c_int)]
-            fn.restype = C.c_int
-            assert fn(g._h, 42, taps.ctypes.data_as(C.POINTER(C.c_float)), taps.size, -312000, C.byref(st),
-                      C.byref(cid)) == 0
-            cid = cid.value
+            cid = g.add_client(42, taps, -312000, state=st)
         got = []
         for x in blocks:
             t = g.submit("cs16", x)

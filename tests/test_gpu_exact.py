@@ -327,23 +327,35 @@ def test_dropin_filters(pkg, fmt, variant):
         fq.close()
 
 
-def run_overlay(scenario, env=None, clients=24, blocks=16):
+def run_overlay(scenario, env=None, clients=24, blocks=16, stim="exact"):
     e = dict(os.environ)
     e.update(env or {})
     r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "_dropin_overlay_worker.py"), scenario,
-                        str(clients), str(blocks), "exact"], capture_output=True, text=True, timeout=600, env=e)
+                        str(clients), str(blocks), stim], capture_output=True, text=True, timeout=600, env=e)
     assert r.stdout.strip(), r.stderr[-2000:]
     line = json.loads(r.stdout.strip().splitlines()[-1])
     assert r.returncode == 0 and not line["errors"], (line, r.stderr[-1500:])
-    return line["stream"]
+    return line
 
 
-@pytest.mark.parametrize("scenario", ["steady", "drops", "late", "lag"])
-def test_dropin_overlay_exact(scenario):
+OVERLAY_SCENARIOS = ["steady", "drops", "late", "lag", "two_sources", "late_short"]
+
+
+@pytest.mark.parametrize("stim,scenario", [("exact", s) for s in OVERLAY_SCENARIOS] +
+                         [("phase", s) for s in OVERLAY_SCENARIOS],
+                         ids=OVERLAY_SCENARIOS + [f"phase-{s}" for s in OVERLAY_SCENARIOS])
+def test_dropin_overlay_exact(stim, scenario):
     """Filters of one band handed into and out of a batch group: the state handed over (history,
-    valid_history, phase) is right to the sample."""
-    st = run_overlay(scenario, env={"XLATING_B200_STREAM_RING": "4"} if scenario == "lag" else None)
-    assert st["joins"] > 0
+    valid_history and, with the phase stimuli at nonzero centres, the oscillator) is right to the sample
+    and to the bit.  Every scenario hands state over (joins); drops and lag also hand it back (desyncs)."""
+    line = run_overlay(scenario, env={"XLATING_B200_STREAM_RING": "4"} if scenario == "lag" else None, stim=stim)
+    st = line["stream"]
+    assert st["joins"] > 0 and st["served_by_group"] > 0
+    if scenario in ("drops", "lag"):
+        assert st["desyncs"] >= 1
+    if scenario == "late_short":
+        # late filters that have consumed 2 samples (fewer than taps - 1) are already members
+        assert st["desyncs"] == 0 and line["short"]["members"] > 12, line["short"]
 
 
 @pytest.mark.parametrize("env", [{"XLATING_B200_LANES": "1"}, {"XLATING_B200_LANES": "8"},

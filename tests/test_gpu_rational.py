@@ -6,7 +6,6 @@ on that stream; exact stimuli (tests/exact.py: centre 0, dyadic taps, inputs on 
 the float64 sum on it bit for bit, which sees a wrong branch, a window one sample off or a stuffed
 position that leaked a sample.
 """
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -212,14 +211,6 @@ def test_attach_detach_pipelined(pkg, monkeypatch, variant):
 
 def test_track_state_hist_and_oscillator(pkg):
     """XLG_TRACK_STATE: hist in upsampled samples and the oscillator equal the oracle's after every block."""
-    class State(C.Structure):
-        _fields_ = [("valid_history", C.c_int64), ("hist", C.c_int64), ("phase_re", C.c_float),
-                    ("phase_im", C.c_float)]
-
-    L_ = pkg.lib()
-    fn = L_.xlg_copy_output
-    fn.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(State)]
-    fn.restype = C.c_int
     fs = 2048000
     plan = pkg.rational_plan(fs, [48000] * 3)
     g = pkg.Group(fs, MAX_IN, flags=pkg.XLG_TRACK_STATE)
@@ -232,10 +223,8 @@ def test_track_state_hist_and_oscillator(pkg):
         g.wait(t)
         for c, o, p in zip(ids, oracles, plan):
             r = o.process_cf32("cs16", stuff("cu8", x, p["interp"]))
-            buf = np.zeros(max(len(r), 1), dtype=np.complex64)
-            got, st = C.c_size_t(0), State()
-            assert fn(g._h, t, c, buf.ctypes.data, buf.size, C.byref(got), C.byref(st)) == 0
-            assert got.value == len(r)
+            got, st = g.copy_output(t, c)
+            assert len(got) == len(r)
             assert st.hist == o.history == g.client_info(c)[0]
             assert complex(st.phase_re, st.phase_im) == complex(np.complex64(o.phase))
     g.close()
