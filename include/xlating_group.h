@@ -134,11 +134,28 @@ int xlg_add_client_rational_ex(xlg_group *g, uint32_t interp, uint32_t decim, co
  * enqueued). */
 int xlg_add_client_cascade(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, int32_t center_freq,
                            uint32_t decim2, const float *taps2, size_t taps2_len, int *client_id);
+/* A cascade client whose stage B resamples by interp2 / decim2, for client rates that do not divide the band
+ * rate (DESIGN.md section 5, "Rational cascade clients").  Stage A is xlg_add_client_cascade's.  Stage B is
+ * the float path of create_frequency_xlating_filter(decim2, taps2, taps2_len, 0, interp2 * fs / decim1, ...)
+ * fed the zero-stuffed stage-A stream of the same block, u[interp2 * n] = y[n] and u[m] = 0 for every other
+ * m (as for xlg_add_client_rational), with taps2_len - 1 upsampled zeros of history at the attach point.
+ * Every output sums only the ceil(taps2_len / interp2) taps that meet stage-A samples (one polyphase branch),
+ * never a stuffed zero.  Taps2 are designed at interp2 * fs / decim1 with gain interp2.  The output rate is
+ * fs * interp2 / (decim1 * decim2).  interp2 == 1 is xlg_add_client_cascade (same kernels, same bits).
+ * xlg_client_info reports kind 5, and xlg_cascade_info's stage_b_history is in upsampled samples.
+ * -EINVAL (logged) for xlg_add_client_cascade's refusals, interp2 of 0, interp2 * (max_input_len / 2 /
+ * decim1 + 2) >= 2^31, or a stage B whose branches and one output's window do not fit the stage-B kernel's
+ * shared memory; -ENOTSUP (logged) on an XLG_TRACK_STATE group.  Q15 submits are refused as for every
+ * cascade client. */
+int xlg_add_client_cascade_rational(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len,
+                                    int32_t center_freq, uint32_t interp2, uint32_t decim2,
+                                    const float *taps2, size_t taps2_len, int *client_id);
 int xlg_remove_client(xlg_group *g, int client_id);
 /* Size the per-ticket result arenas (device and pinned host) for `output_samples_per_block` complex output
  * samples per block summed over all clients (a client at decimation D produces about max_input_len/2/D + 2).
  * A cascade client counts two rows, each rounded up to a multiple of 4 samples: its stage-A row of
- * n1 = max_input_len/2/decim1 + 2 samples, which stays on the device, and its final row of n1/decim2 + 2.
+ * n1 = max_input_len/2/decim1 + 2 samples, which stays on the device, and its final row of
+ * floor(n1 * interp2 / decim2) + 2 (interp2 = 1 for xlg_add_client_cascade).
  * Optional: the arenas grow on demand when clients are added, but a growth re-allocates every ring entry and
  * the results still waiting in the ring are lost (-ESTALE for consumers that had not read them yet, like a
  * block overwritten in the reference's queue).  A server that knows its client limit reserves once, up front. */
@@ -228,12 +245,12 @@ typedef struct {
 } xlg_poly_profile;
 int xlg_poly_profile_read(xlg_group *g, xlg_poly_profile *p, int reset);
 
-/* Stage B of cascade clients (xlg_add_client_cascade), counted like xlg_profile's while profiling is enabled.
- * xlg_profile counts each cascade client's stage A as the integer client it is. */
+/* Stage B of cascade clients (xlg_add_client_cascade, _rational), counted like xlg_profile's while profiling
+ * is enabled.  xlg_profile counts each cascade client's stage A as the integer client it is. */
 typedef struct {
-  double stage_b_ms;         /* the ring appends + the stage-B kernel */
+  double stage_b_ms;         /* the ring appends + the stage-B kernels (integer and rational) */
   uint64_t stage_b_launches;
-  uint64_t stage_b_macs;     /* complex-by-real MACs of stage B: sum n_out * taps2_len */
+  uint64_t stage_b_macs;     /* complex-by-real MACs of stage B: sum n_out * ceil(taps2_len / interp2) */
   uint64_t d2h_bytes;        /* result bytes copied to the host, all clients (stage-A rows are never copied) */
 } xlg_cascade_profile;
 int xlg_cascade_profile_read(xlg_group *g, xlg_cascade_profile *p, int reset);
@@ -245,7 +262,8 @@ int xlg_cascade_profile_read(xlg_group *g, xlg_cascade_profile *p, int reset);
  * branches fit the tiled kernel's shared memory, 5 = cascade). */
 int xlg_client_info(const xlg_group *g, int client_id, size_t *history, int *kernel_kind);
 /* A cascade client's stages: the kind (0, 1 or 2, as xlg_client_info) of the kernel serving stage A, and the
- * history_offset of each stage (stage B's in stage-A samples).  -EINVAL for any other client. */
+ * history_offset of each stage (stage B's in stage-A samples, upsampled by interp2 for a rational cascade
+ * client).  -EINVAL for any other client. */
 int xlg_cascade_info(const xlg_group *g, int client_id, int *stage_a_kind, size_t *stage_a_history,
                      size_t *stage_b_history);
 

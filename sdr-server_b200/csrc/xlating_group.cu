@@ -115,10 +115,12 @@ struct HostClient {
   // cascade client (xlg_add_client_cascade): everything above describes its stage A, an integer client
   // whose out_off row lies after every host-visible row; stage B is described here
   bool casc = false;
-  uint32_t D2 = 0;
+  uint32_t L2 = 1, D2 = 0;       // stage B's interpolation (> 1: xlg_add_client_cascade_rational) and decimation
   size_t T2 = 0;
-  std::vector<float> rev2;       // stage B's reversed taps (the real parts of its rotated taps at centre 0)
-  long long hist2 = 0;           // stage B's history_offset, in stage-A samples
+  int Tb2 = 0, ko2 = 0;          // L2 > 1: taps per branch, outputs per CTA of cascade_fir_poly_cf32_kernel
+  std::vector<float> rev2;       // stage B's reversed taps (the real parts of its rotated taps at centre 0),
+                                 // packed branch-major (xl_poly_pack) when L2 > 1
+  long long hist2 = 0;           // stage B's history_offset, in stage-A samples (upsampled when L2 > 1)
   long long a_pos = 0;           // stage-A outputs produced since the attach: the ring's stream position
   float2 *d_cring = nullptr;     // stage-A history ring, cring_cap samples (a power of two)
   size_t cring_cap = 0;
@@ -147,7 +149,9 @@ struct Slot {
   BlkInfo *d_vblk = nullptr, *h_vblk = nullptr;  // kind 4: per branch class, this block's window start and count
   uint64_t poly_macs = 0;
   CascBlk *d_cblk = nullptr, *h_cblk = nullptr;  // cascade clients: this block's ring positions, windows and counts
-  size_t cblk_cap = 0;
+  size_t cblk_cap = 0;                           // (integer stage B first, then the rational ones)
+  CascPolyBlk *d_pblk = nullptr, *h_pblk = nullptr;  // rational cascade clients: this block's stage B
+  size_t pblk_cap = 0;
   cudaEvent_t ev_casc = nullptr;                 // stage B of this block done (its rings' appends are ordered on it)
   cudaEvent_t pf_casc[2] = {nullptr, nullptr};
   bool pf_cb = false;
@@ -346,6 +350,7 @@ struct xlg_group {
   float *d_taps2 = nullptr;                 // cascade clients' stage-B taps (HostClient::taps2_off)
   size_t cap_taps2 = 0;
   int n_casc = 0;                           // active cascade clients
+  int n_casc_int = 0;                       // of which integer stage B (their CascBlk entries come first)
   std::vector<float2 *> dead_rings;         // rings of removed cascade clients, freed once the pipeline is drained
   cudaEvent_t ev_last_casc = nullptr;       // ev_casc of the last block with cascade clients
   bool have_last_casc = false;
@@ -410,6 +415,10 @@ static void slot_free(Slot &s) {
   if (s.h_cblk) cudaFreeHost(s.h_cblk);
   s.d_cblk = s.h_cblk = nullptr;
   s.cblk_cap = 0;
+  if (s.d_pblk) cudaFree(s.d_pblk);
+  if (s.h_pblk) cudaFreeHost(s.h_pblk);
+  s.d_pblk = s.h_pblk = nullptr;
+  s.pblk_cap = 0;
   s.d_pscratch = nullptr;
   s.d_vblk = s.h_vblk = nullptr;
   s.d_endph = nullptr;
@@ -652,8 +661,8 @@ static int rebuild_layout(xlg_group *g) {
     if (!h.active) continue;
     h.out_cap = (int)((uint64_t)g->max_input_len / 2 * h.L / h.D + 2);
     if (h.casc) {
-      // n2 <= (n1 - 1) / D2 + 1 for any history
-      h.fin_cap = h.out_cap / (int)h.D2 + 2;
+      // n2 <= (L2 * n1 - 1) / D2 + 1 for any history
+      h.fin_cap = (int)((uint64_t)h.out_cap * h.L2 / h.D2 + 2);
       h.fin_off = (int)out_total;
       out_total += (size_t)h.fin_cap;
     } else {
@@ -670,7 +679,7 @@ static int rebuild_layout(xlg_group *g) {
   // and a zeroed history ring for each new client (its positions before the attach read as zero)
   {
     std::vector<float> taps2;
-    g->n_casc = 0;
+    g->n_casc = g->n_casc_int = 0;
     for (int i = 0; i < nc; i++) {
       HostClient &h = g->clients[i];
       if (!h.active || !h.casc) continue;
@@ -682,12 +691,16 @@ static int rebuild_layout(xlg_group *g) {
       taps2.resize((taps2.size() + 3) & ~(size_t)3, 0.f);  // 16-byte aligned bulk copies of whole float4s
       if (h.d_cring == nullptr) {
         // stage B of block b reads stage-A outputs of earlier blocks; the submit of block b + XLG_SLOTS waits
-        // for ticket b, so T2 - 1 + (XLG_SLOTS + 1) * max n1 samples are never overwritten while still needed
-        h.cring_cap = next_pow2(h.T2 - 1 + (size_t)(XLG_SLOTS + 1) * (size_t)h.out_cap);
+        // for ticket b, so T2 - 1 + (XLG_SLOTS + 1) * max n1 samples are never overwritten while still needed;
+        // a rational stage B's history of at most T2 - 1 upsampled samples reaches back ceil((T2 - 1) / L2)
+        // stage-A samples, and its last branch may read one zero-weighted sample past the block
+        const size_t back = h.L2 == 1 ? h.T2 - 1 : (h.T2 - 1 + h.L2 - 1) / h.L2 + 1;
+        h.cring_cap = next_pow2(back + (size_t)(XLG_SLOTS + 1) * (size_t)h.out_cap);
         CU_OK(cudaMalloc(&h.d_cring, h.cring_cap * sizeof(float2)));
         CU_OK(cudaMemset(h.d_cring, 0, h.cring_cap * sizeof(float2)));
       }
       g->n_casc++;
+      if (h.L2 == 1) g->n_casc_int++;
     }
     if (dev_assign(&g->d_taps2, &g->cap_taps2, taps2.data(), taps2.size() * sizeof(float))) return -EIO;
     for (float2 *p : g->dead_rings) cudaFree(p);
@@ -700,6 +713,16 @@ static int rebuild_layout(xlg_group *g) {
       s.cblk_cap = std::max<size_t>((size_t)g->n_casc * 2, 16);
       CU_OK(cudaMalloc(&s.d_cblk, s.cblk_cap * sizeof(CascBlk)));
       CU_OK(cudaHostAlloc(&s.h_cblk, s.cblk_cap * sizeof(CascBlk), cudaHostAllocDefault));
+    }
+    const int n_rat = g->n_casc - g->n_casc_int;
+    for (Slot &s : g->slots) {
+      if (s.pblk_cap >= (size_t)n_rat) continue;
+      if (s.d_pblk) cudaFree(s.d_pblk);
+      if (s.h_pblk) cudaFreeHost(s.h_pblk);
+      s.d_pblk = s.h_pblk = nullptr;
+      s.pblk_cap = std::max<size_t>((size_t)n_rat * 2, 16);
+      CU_OK(cudaMalloc(&s.d_pblk, s.pblk_cap * sizeof(CascPolyBlk)));
+      CU_OK(cudaHostAlloc(&s.h_pblk, s.pblk_cap * sizeof(CascPolyBlk), cudaHostAllocDefault));
     }
   }
   if (ensure_ring(g, max_hist, g->qring != nullptr)) return -EIO;
@@ -1435,7 +1458,8 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
     }
   if (cudaFuncSetAttribute(fir_long2_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W2_SMEM) != cudaSuccess ||
       cudaFuncSetAttribute(fir_long4_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W4_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(cascade_fir_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem) != cudaSuccess) {
+      cudaFuncSetAttribute(cascade_fir_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem) != cudaSuccess ||
+      cudaFuncSetAttribute(cascade_fir_poly_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem) != cudaSuccess) {
     XL_LOG("cannot raise dynamic shared memory to %d bytes", kTileMaxSmem);
     return fail(-EIO);
   }
@@ -1674,37 +1698,76 @@ extern "C" int xlg_add_client_rational_ex(xlg_group *g, uint32_t interp, uint32_
 extern "C" int xlg_add_client_cascade(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len,
                                       int32_t center_freq, uint32_t decim2, const float *taps2, size_t taps2_len,
                                       int *client_id) {
+  return xlg_add_client_cascade_rational(g, decim1, taps1, taps1_len, center_freq, 1, decim2, taps2, taps2_len,
+                                         client_id);
+}
+
+extern "C" int xlg_add_client_cascade_rational(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len,
+                                               int32_t center_freq, uint32_t interp2, uint32_t decim2,
+                                               const float *taps2, size_t taps2_len, int *client_id) {
   if (g == nullptr || client_id == nullptr) return -EINVAL;
   if (decim1 == 0 || decim2 == 0 || taps1_len == 0 || taps2_len == 0 || taps1 == nullptr || taps2 == nullptr) {
     XL_LOG("cascade client: decimations (%u, %u) and tap counts (%zu, %zu) must all be at least 1", decim1, decim2,
            taps1_len, taps2_len);
     return -EINVAL;
   }
+  if (interp2 == 0) {
+    XL_LOG("cascade client: stage-B interpolation must be at least 1");
+    return -EINVAL;
+  }
+  if (interp2 > 1 && (uint64_t)interp2 * ((uint64_t)g->max_input_len / 2 / decim1 + 2) >= (1ull << 31)) {
+    XL_LOG("cascade client: %u x %u stage-A samples per block upsampled exceed 2^31", interp2,
+           g->max_input_len / 2 / decim1 + 2);
+    return -EINVAL;
+  }
   if (g->flags & XLG_TRACK_STATE) {
     XL_LOG("cascade client: an XLG_TRACK_STATE group cannot carry the state of two stages");
     return -ENOTSUP;
   }
-  if (taps2_len > (size_t)INT32_MAX || cascade_smem(1, (int)decim2, (int)taps2_len) > (size_t)kTileMaxSmem) {
-    XL_LOG("cascade client: %zu stage-B taps exceed the stage-B kernel's shared memory", taps2_len);
+  const size_t Tb2 = (taps2_len + interp2 - 1) / interp2;
+  if (taps2_len > (size_t)INT32_MAX ||
+      (interp2 == 1 ? cascade_smem(1, (int)decim2, (int)taps2_len)
+                    : cascade_poly_smem(1, (int)interp2, (int)decim2, (int)Tb2)) > (size_t)kTileMaxSmem) {
+    XL_LOG("cascade client: %zu stage-B taps (interpolation %u) exceed the stage-B kernel's shared memory", taps2_len,
+           interp2);
     return -EINVAL;
   }
-  // stage B: the reference filter at fs / D1 with centre 0 -- its rotated taps are (h, +-0), so the real
-  // parts of the reversed taps (the even-length quirk included) are all it needs
+  // stage B: the reference filter at interp2 * fs / D1 with centre 0 -- its rotated taps are (h, +-0), so the
+  // real parts of the reversed taps (the even-length quirk included) are all it needs; at centre 0 the rate
+  // only enters the rotation, so clamping it changes nothing
+  const uint64_t rate2 = (uint64_t)interp2 * std::max<uint32_t>(g->fs / decim1, 1);
   xl_client_consts k2;
-  int rc = xl_client_consts_build(taps2, taps2_len, decim2, 0, std::max<uint32_t>(g->fs / decim1, 1), &k2);
+  int rc = xl_client_consts_build(taps2, taps2_len, decim2, 0, (uint32_t)std::min<uint64_t>(rate2, UINT32_MAX), &k2);
   if (rc) return rc;
   std::vector<float> rev2(taps2_len);
-  for (size_t j = 0; j < taps2_len; j++) rev2[j] = k2.rev_cf32[2 * j];
+  if (interp2 == 1) {
+    for (size_t j = 0; j < taps2_len; j++) rev2[j] = k2.rev_cf32[2 * j];
+  } else {
+    // branch-major P[r][t] = rev2[r + t * L2], zero-padded to Tb2 taps per branch
+    std::vector<float> packed(2 * (size_t)interp2 * Tb2);
+    xl_poly_pack(k2.rev_cf32, taps2_len, interp2, packed.data());
+    rev2.resize((size_t)interp2 * Tb2);
+    for (size_t j = 0; j < rev2.size(); j++) rev2[j] = packed[2 * j];
+  }
   xl_client_consts_free(&k2);
   int id = -1;
   rc = attach_client(g, 1, decim1, g->fs, taps1, taps1_len, center_freq, nullptr, &id);
   if (rc) return rc;
   HostClient &h = g->clients[id];
   h.casc = true;
+  h.L2 = interp2;
   h.D2 = decim2;
   h.T2 = taps2_len;
   h.rev2.swap(rev2);
-  h.hist2 = (long long)taps2_len - 1;  // src/xlating.c:552
+  h.hist2 = (long long)taps2_len - 1;  // src/xlating.c:552 (upsampled samples when L2 > 1)
+  if (interp2 > 1) {
+    h.Tb2 = (int)Tb2;
+    // about 2 * C_THREADS outputs per CTA, a whole number per branch where L2 <= C_THREADS; fewer where the
+    // window would not fit (the attach check above guarantees that one output fits)
+    int ko = interp2 <= (uint32_t)C_THREADS ? 2 * (int)interp2 * (C_THREADS / (int)interp2) : C_KO;
+    while (ko > 1 && cascade_poly_smem(ko, (int)interp2, (int)decim2, h.Tb2) > (size_t)kTileMaxSmem) ko /= 2;
+    h.ko2 = ko;
+  }
   *client_id = id;
   return 0;
 }
@@ -1856,7 +1919,8 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
   s.tile_macs = s.algo_macs = s.out_samples = s.poly_macs = s.casc_macs = s.d2h_bytes = 0;
   s.in_samples = (uint64_t)n;
   int max_generic_out = 0, poly_warps = 0, max_poly4_out = 0, n_casc = 0, max_n1 = 0, max_n2 = 0;
-  size_t casc_smem = 0;
+  int n_cint = 0, n_crat = 0, max_rat_ctas = 0;  // integer / rational stage B; CTAs per rational client
+  size_t casc_smem = 0, casc_poly_smem = 0;
   for (size_t i = 0; i < g->clients.size(); i++) {
     HostClient &h = g->clients[i];
     if (!h.active) continue;
@@ -1883,10 +1947,11 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     }
     if (q15 || h.kind == 0) max_generic_out = std::max(max_generic_out, n_out);
     if (h.casc) {
-      // stage B: the reference's walk over this block's n_out stage-A samples
-      const long long first2 = h.a_pos - h.hist2;
-      const int n2 = xl_walk(&h.hist2, n_out, h.T2, h.D2, h.fin_cap);
-      CascBlk &cb = s.h_cblk[n_casc++];
+      // stage B: the reference's walk over this block's n_out stage-A samples, upsampled by L2 (the
+      // zero-stuffed stream u[L2 * n] = y[n]; the same integers for L2 = 1)
+      const long long first2 = (long long)h.L2 * h.a_pos - h.hist2;
+      const int n2 = xl_walk(&h.hist2, (long long)h.L2 * n_out, h.T2, h.D2, h.fin_cap);
+      CascBlk &cb = s.h_cblk[h.L2 == 1 ? n_cint++ : g->n_casc_int + n_crat];
       cb.ring = h.d_cring;
       cb.a_pos = h.a_pos;
       cb.first = first2;
@@ -1898,12 +1963,31 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       cb.T2 = (int)h.T2;
       cb.taps_off = h.taps2_off;
       cb.out_off = h.fin_off;
+      if (h.L2 == 1) {
+        max_n2 = std::max(max_n2, n2);
+        casc_smem = std::max(casc_smem, cascade_smem(C_KO, cb.D2, cb.T2));
+        s.casc_macs += (uint64_t)n2 * h.T2;
+      } else {
+        // only the appends read this client's CascBlk; cascade_fir_poly_cf32_kernel reads its CascPolyBlk
+        CascPolyBlk &pb = s.h_pblk[n_crat++];
+        pb.ring = h.d_cring;
+        pb.first = first2;
+        pb.mask = cb.mask;
+        pb.n2 = n2;
+        pb.L2 = (int)h.L2;
+        pb.M2 = (int)h.D2;
+        pb.Tb2 = h.Tb2;
+        pb.ko = h.ko2;
+        pb.taps_off = h.taps2_off;
+        pb.out_off = h.fin_off;
+        max_rat_ctas = std::max(max_rat_ctas, (n2 + h.ko2 - 1) / h.ko2);
+        casc_poly_smem = std::max(casc_poly_smem, cascade_poly_smem(h.ko2, pb.L2, pb.M2, pb.Tb2));
+        s.casc_macs += (uint64_t)n2 * (uint64_t)h.Tb2;
+      }
+      n_casc++;
       h.a_pos += n_out;
       h.last_n2 = n2;
       max_n1 = std::max(max_n1, n_out);
-      max_n2 = std::max(max_n2, n2);
-      casc_smem = std::max(casc_smem, cascade_smem(C_KO, cb.D2, cb.T2));
-      s.casc_macs += (uint64_t)n2 * h.T2;
     }
   }
 
@@ -2277,6 +2361,8 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       s.pf_cb = true;
     }
     CU_OK(cudaMemcpyAsync(s.d_cblk, s.h_cblk, (size_t)n_casc * sizeof(CascBlk), cudaMemcpyHostToDevice, cs));
+    if (n_crat > 0)
+      CU_OK(cudaMemcpyAsync(s.d_pblk, s.h_pblk, (size_t)n_crat * sizeof(CascPolyBlk), cudaMemcpyHostToDevice, cs));
     if (max_n1 > 0) cascade_append_kernel<<<dim3((max_n1 + 255) / 256, n_casc), 256, 0, cs>>>(s.d_cblk, s.d_out);
     if (max_n2 > 0) {
       // fewer outputs per CTA where a long stage-B window would not fit (attach checked that one output fits)
@@ -2284,12 +2370,16 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       while (ko > 1 && casc_smem > (size_t)kTileMaxSmem) {
         ko /= 2;
         casc_smem = 0;
-        for (int c = 0; c < n_casc; c++)
+        for (int c = 0; c < n_cint; c++)
           casc_smem = std::max(casc_smem, cascade_smem(ko, s.h_cblk[c].D2, s.h_cblk[c].T2));
       }
-      cascade_fir_cf32_kernel<<<dim3((max_n2 + ko - 1) / ko, n_casc), C_THREADS, casc_smem, cs>>>(s.d_cblk, g->d_taps2,
+      cascade_fir_cf32_kernel<<<dim3((max_n2 + ko - 1) / ko, n_cint), C_THREADS, casc_smem, cs>>>(s.d_cblk, g->d_taps2,
                                                                                                 s.d_out, ko);
     }
+    // rational stage B: each client's CTA size was fixed at attach to fit the shared memory
+    if (max_rat_ctas > 0)
+      cascade_fir_poly_cf32_kernel<<<dim3(max_rat_ctas, n_crat), C_THREADS, casc_poly_smem, cs>>>(s.d_pblk, g->d_taps2,
+                                                                                                s.d_out);
     if (g->profiling) CU_OK(cudaEventRecord(s.pf_casc[1], cs));
     CU_OK(cudaEventRecord(s.ev_casc, cs));
     g->ev_last_casc = s.ev_casc;

@@ -25,8 +25,9 @@
  *                    (cp.async.bulk + mbarrier, 3 stages)
  *   fir_generic_*    any (T, D, alignment): one warp per 4 outputs, lanes split the
  *                    taps, warp-shuffle reduction; also the Q15 integer path
- *   cascade_*        stage B of two-stage clients: a real-tap decimator over each
- *                    client's stage-A history ring, TMA-staged window, register tile
+ *   cascade_*        stage B of two-stage clients: a real-tap decimator (or rational
+ *                    L2/M2 polyphase filter) over each client's stage-A history ring,
+ *                    TMA-staged window, register tile
  *
  * The arithmetic shared with the per-filter drop-in engine (conversions, oscillator
  * recursion, generic FIR warp) lives in xlating_common.cuh.
@@ -1251,6 +1252,104 @@ cascade_fir_cf32_kernel(const CascBlk *__restrict__ cb, const float *__restrict_
 #pragma unroll
   for (int i = 0; i < C_R; i++)
     if (tid + C_THREADS * i < nk) out[b.out_off + k0 + tid + C_THREADS * i] = acc[i];
+}
+
+// ---------------------------------------------------------------------------
+// rational cascade clients (xlg_add_client_cascade_rational, interp2 = L2 > 1).  Stage B is the reference
+// filter with decimation M2 at L2 * fs / D1, centre 0, fed the zero-stuffed stage-A stream u[L2*n] = y[n]:
+// output k's upsampled window starts at w = first + k*M2, and with r = (-w) mod L2, n0 = (w + r) / L2
+// (poly_branch) only the branch r of the real reversed taps meets stage-A samples,
+//     z[k] = sum_{t < Tb2} y[n0 + t] * P[r][t],   P[r][t] = rev2[r + t*L2] (0 past T2),  Tb2 = ceil(T2 / L2).
+// The ring, its positions and its zeros before the attach are the integer cascade's (CascBlk appends them).
+// ---------------------------------------------------------------------------
+struct CascPolyBlk {
+  float2 *ring;     // the client's stage-A history ring
+  long long first;  // upsampled stream position where this block's output 0 starts its window
+  unsigned mask;    // ring capacity - 1
+  int n2;           // outputs computed by this block
+  int L2, M2, Tb2;
+  int ko;           // outputs per CTA (the host sets it per client)
+  int taps_off;     // float offset of the branch-major taps P in the real tap arena, a multiple of 4
+  int out_off;      // final row in the slot's output arena
+};
+
+// shared memory of a CTA with ko outputs: mbarrier, the L2 branches padded to 16 bytes, the window: the
+// n0 of ko consecutive outputs span at most ceil((ko - 1) * M2 / L2) samples, plus Tb2 taps (+1 for an odd
+// start, even)
+__host__ __device__ constexpr size_t cascade_poly_smem(int ko, int L2, int M2, int Tb2) {
+  return 16 + (((size_t)L2 * Tb2 + 3) & ~(size_t)3) * 4 +
+         ((((size_t)(ko - 1) * M2 + L2 - 1) / L2 + Tb2 + 2) & ~(size_t)1) * 8;
+}
+
+// Stage B of rational cascade clients: CTA (x, c) computes outputs [x*ko, x*ko + ko) of client c.  One TMA
+// bulk copy stages the client's branches, one or two (the ring wraps) the stage-A window from n0 of the
+// first output to n0 of the last + Tb2.  Outputs k and k + L2 share a branch and their windows lie M2
+// samples apart, so threads take the CTA's outputs residue-major: pair slot (rho, p) computes relative
+// outputs rho + p*L2 and rho + (p + P)*L2 on branch r(rho), and consecutive lanes hold consecutive p of one
+// residue.  A warp therefore works on one branch (the tap load is a broadcast) wherever the CTA has at
+// least 64 outputs per branch, on a few branches otherwise.  Lanes of one residue read the window M2 apart;
+// with even M2 they walk the taps skewed (start at t = lane mod Tb2), an odd stride, as the integer stage B
+// does for even D2, and the window loads have no bank conflicts.  Two real FMAs per tap.
+__global__ void __launch_bounds__(C_THREADS)
+cascade_fir_poly_cf32_kernel(const CascPolyBlk *__restrict__ pb, const float *__restrict__ taps2,
+                             float2 *__restrict__ out) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  uint64_t *bar = reinterpret_cast<uint64_t *>(smem);
+  const CascPolyBlk &b = pb[blockIdx.y];
+  const int n2 = b.n2, ko = b.ko;
+  if ((long long)blockIdx.x * ko >= n2) return;
+  const int k0 = blockIdx.x * ko;
+  const int L2 = b.L2, M2 = b.M2, Tb2 = b.Tb2, tpad = (L2 * Tb2 + 3) & ~3;
+  const int nk = min(ko, n2 - k0);
+  float *ts = reinterpret_cast<float *>(smem + 16);
+  float2 *xs = reinterpret_cast<float2 *>(smem + 16 + tpad * 4);
+  long long base, nlast;
+  poly_branch(b.first + (long long)k0 * M2, L2, &base);
+  poly_branch(b.first + (long long)(k0 + nk - 1) * M2, L2, &nlast);
+  const unsigned idx = (unsigned)((unsigned long long)base) & b.mask;
+  const unsigned shift = idx & 1u;  // an odd window start is fetched from one sample earlier (16-byte source)
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    mbar_init(bar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  __syncthreads();
+  if (tid == 0) {
+    const unsigned need = ((unsigned)(nlast - base + Tb2) + shift + 1u) & ~1u;
+    const unsigned p1 = min(need, b.mask + 1u - (idx - shift));
+    mbar_expect_tx(bar, (unsigned)tpad * 4u + need * 8u);
+    tma_bulk_g2s(ts, taps2 + b.taps_off, (unsigned)tpad * 4u, bar);
+    tma_bulk_g2s(xs, b.ring + (idx - shift), p1 * 8u, bar);
+    if (p1 < need) tma_bulk_g2s(xs + p1, b.ring, (need - p1) * 8u, bar);
+  }
+  mbar_wait(bar, 0);
+  const int P = ((nk + L2 - 1) / L2 + 1) / 2;  // pair slots per residue: residue 0 has the most outputs
+  const int slots = min(L2, nk) * P;
+  for (int ps = tid; ps < slots; ps += C_THREADS) {
+    const int rho = ps / P, p = ps - rho * P;
+    const int ka = rho + p * L2, kb = ka + P * L2;
+    if (ka >= nk) continue;
+    long long n0;
+    const int r = poly_branch(b.first + (long long)(k0 + rho) * M2, L2, &n0);
+    const float *h = ts + r * Tb2;
+    const float2 *xa = xs + shift + (size_t)(n0 - base) + (size_t)p * M2;
+    const float2 *xb = kb < nk ? xa + (size_t)P * M2 : xa;
+    float2 acc_a = make_float2(0.f, 0.f), acc_b = make_float2(0.f, 0.f);
+    int t = (M2 & 1) ? 0 : (tid & 31) % Tb2;
+#pragma unroll 4
+    for (int s = 0; s < Tb2; s++) {
+      const float hv = h[t];
+      const float2 va = xa[t], vb = xb[t];
+      acc_a.x = fmaf(va.x, hv, acc_a.x);
+      acc_a.y = fmaf(va.y, hv, acc_a.y);
+      acc_b.x = fmaf(vb.x, hv, acc_b.x);
+      acc_b.y = fmaf(vb.y, hv, acc_b.y);
+      if (++t == Tb2) t = 0;
+    }
+    out[b.out_off + k0 + ka] = acc_a;
+    if (kb < nk) out[b.out_off + k0 + kb] = acc_b;
+  }
 }
 
 }  // namespace xl
