@@ -34,9 +34,10 @@
  *   variants   process_optimized_* == process_native_* (as in the reference's
  *              default x86-64 build where SIMD is "Not detected", :142-153).
  *
- * One extension, marked below, is not a reference symbol:
+ * Two extensions, marked below, are not reference symbols:
  * create_rational_frequency_xlating_filter, a filter whose output rate fs * L / M
- * does not divide the band rate.
+ * does not divide the band rate, and create_cascade_frequency_xlating_filter, a
+ * two-stage filter that reaches a narrow rate with fewer multiply-adds.
  *
  * Many clients sharing one wideband input should use the batch extension in
  * include/xlating_group.h: one H2D copy and one fused launch for all clients.
@@ -101,6 +102,34 @@ void process_optimized_cs16_cs16(const int16_t *input, size_t input_len, int16_t
 int create_rational_frequency_xlating_filter(uint32_t interpolation, uint32_t decimation, float *taps,
                                              size_t taps_len, int32_t center_freq, uint32_t sampling_freq,
                                              uint32_t max_input_buffer_length, xlating **filter);
+
+/* ---- extension (not in the reference) ----
+ * A two-stage (cascade) filter: stage A is create_frequency_xlating_filter(decimation1, taps1, taps1_len,
+ * center_freq, sampling_freq, ...); stage B is the filter with decimation decimation2 and centre 0 at
+ * interpolation2 * sampling_freq / decimation1, fed stage A's outputs zero-stuffed by interpolation2
+ * (interpolation2 == 1: plain decimation).  Call n gives exactly what block n gives for the client of
+ * xlg_add_client_cascade_rational(g, decimation1, taps1, taps1_len, center_freq, interpolation2, decimation2,
+ * taps2, taps2_len, &id) attached to a fresh group of the same sampling_freq and max_input_buffer_length
+ * before block 0, fed these calls as its blocks: stage A starts with taps1_len - 1 zeros of history, stage B
+ * with taps2_len - 1 (upsampled) zeros, and *output_len counts stage B's outputs.  taps2 is designed at
+ * interpolation2 * sampling_freq / decimation1 (with gain interpolation2); cascade_plan in the Python package
+ * designs both stages.
+ * Both tap vectors are adopted and freed by destroy_xlating; *output points into filter-owned pinned memory,
+ * valid until the next call on the filter.
+ * Errors, in this order: -1 when taps1_len or taps2_len is 0 (neither vector adopted); -EINVAL and one "<3>"
+ * line for what xlg_add_client_cascade_rational refuses as an argument -- decimation1, decimation2 or
+ * interpolation2 of 0, interpolation2 > 1 with interpolation2 * (max_input_buffer_length / 2 / decimation1 + 2)
+ * >= 2^31, or a stage B whose branches and one output's window do not fit the stage-B kernels' shared memory
+ * (all checked before any CUDA call; both vectors are freed); then -ENODEV, -EIO, -ENOMEM as
+ * create_frequency_xlating_filter.
+ * process_*_cs16 (Q15) calls are refused as on a rational filter: *output_len = 0, one "<3>" line per filter,
+ * nothing consumed.  A cascade filter is always served by the per-filter engine: it never joins the batch
+ * group that filters of one band share. */
+int create_cascade_frequency_xlating_filter(uint32_t decimation1, float *taps1, size_t taps1_len,
+                                            int32_t center_freq, uint32_t interpolation2,
+                                            uint32_t decimation2, float *taps2, size_t taps2_len,
+                                            uint32_t sampling_freq, uint32_t max_input_buffer_length,
+                                            xlating **filter);
 
 /* replaces src/xlating.c:584-616; NULL is a no-op */
 void destroy_xlating(xlating *filter);

@@ -9,8 +9,8 @@ callers do (``src/dsp_worker.c:98-124``, ``test/test_xlating.c``):
 * :func:`create_low_pass_filter`  -> ``create_low_pass_filter``  (src/lpf.h:6)
 * :class:`XlatingFilter`          -> ``create_frequency_xlating_filter`` /
   ``process_{native,optimized}_{cu8,cs8,cs16}_{cf32,cs16}`` / ``destroy_xlating``
-  (src/xlating.h:10-38); :meth:`XlatingFilter.rational` -> the extension
-  ``create_rational_frequency_xlating_filter``
+  (src/xlating.h:10-38); :meth:`XlatingFilter.rational` and :meth:`XlatingFilter.cascade` -> the
+  extensions ``create_rational_frequency_xlating_filter`` and ``create_cascade_frequency_xlating_filter``
 * :class:`Group`                  -> the batch extension ``xlg_*``
 
 There is no CPU fallback anywhere: if the shared library is missing, or no sm_90
@@ -51,7 +51,7 @@ REFERENCE_SYMBOLS = (
     + [f"process_{v}_{f}_{o}" for v in ("native", "optimized") for f in ("cu8", "cs8", "cs16") for o in ("cf32", "cs16")]
 )
 # include/xlating.h's extension of the reference's per-filter ABI
-DROPIN_EXTENSION_SYMBOLS = ["create_rational_frequency_xlating_filter"]
+DROPIN_EXTENSION_SYMBOLS = ["create_rational_frequency_xlating_filter", "create_cascade_frequency_xlating_filter"]
 GROUP_SYMBOLS = [
     "xlg_create", "xlg_create_ex", "xlg_destroy", "xlg_add_client", "xlg_add_client_ex", "xlg_add_client_rational_ex", "xlg_remove_client", "xlg_reserve", "xlg_client_count", "xlg_submit",
     "xlg_wait", "xlg_input_consumed", "xlg_output", "xlg_read_output", "xlg_copy_output", "xlg_alloc_pinned", "xlg_free_pinned", "xlg_wait_stream", "xlg_partition_active", "xlg_timer_start",
@@ -110,6 +110,8 @@ def lib() -> C.CDLL:
     L.create_frequency_xlating_filter.restype = C.c_int
     L.create_rational_frequency_xlating_filter.argtypes = [u32, u32, vp, sz, i32, u32, u32, C.POINTER(vp)]
     L.create_rational_frequency_xlating_filter.restype = C.c_int
+    L.create_cascade_frequency_xlating_filter.argtypes = [u32, vp, sz, i32, u32, u32, vp, sz, u32, u32, C.POINTER(vp)]
+    L.create_cascade_frequency_xlating_filter.restype = C.c_int
     L.destroy_xlating.argtypes = [vp]
     L.destroy_xlating.restype = None
     for v in ("native", "optimized"):
@@ -236,20 +238,32 @@ def create_low_pass_filter(gain: float, sampling_freq: int, cutoff_freq: int, tr
     return out
 
 
+def _adoptable(taps: np.ndarray):
+    """A malloc()ed copy of `taps` for a constructor that adopts (and later free()s) the vector, as the
+    reference does; None for an empty vector."""
+    if len(taps) == 0:
+        return None
+    mem = _libc.malloc(taps.nbytes)
+    C.memmove(mem, taps.ctypes.data, taps.nbytes)
+    return mem
+
+
 class XlatingFilter:
     """Per-client drop-in filter (reference API: src/xlating.h:10-38)."""
 
     def __init__(self, decimation: int, taps, center_freq: int, sampling_freq: int, max_input_buffer_length: int,
-                 interp: int | None = None):
+                 interp: int | None = None, stage_b=None):
         self._L = lib()
         taps = np.ascontiguousarray(taps, dtype=np.float32)
-        mem = None
-        if len(taps) > 0:
-            # create adopts (and later free()s) the vector, as the reference does
-            mem = _libc.malloc(taps.nbytes)
-            C.memmove(mem, taps.ctypes.data, taps.nbytes)
+        mem = _adoptable(taps)
         h = C.c_void_p()
-        if interp is None:
+        if stage_b is not None:
+            interp2, decim2, taps2 = stage_b
+            taps2 = np.ascontiguousarray(taps2, dtype=np.float32)
+            code = self._L.create_cascade_frequency_xlating_filter(decimation, mem, len(taps), center_freq, interp2,
+                                                                   decim2, _adoptable(taps2), len(taps2),
+                                                                   sampling_freq, max_input_buffer_length, C.byref(h))
+        elif interp is None:
             code = self._L.create_frequency_xlating_filter(decimation, mem, len(taps), center_freq, sampling_freq,
                                                            max_input_buffer_length, C.byref(h))
         else:
@@ -267,6 +281,16 @@ class XlatingFilter:
         create_rational_frequency_xlating_filter): the filter with decimation `decim` at
         interp * sampling_freq fed the zero-stuffed stream.  Taps are designed at interp * sampling_freq."""
         return cls(decim, taps, center_freq, sampling_freq, max_input_buffer_length, interp=interp)
+
+    @classmethod
+    def cascade(cls, decim1: int, taps1, center_freq: int, decim2: int, taps2, sampling_freq: int,
+                max_input_buffer_length: int, interp2: int = 1) -> "XlatingFilter":
+        """A two-stage filter (include/xlating.h, create_cascade_frequency_xlating_filter): the filter
+        (decim1, taps1, center_freq) at sampling_freq, followed by the filter (decim2, taps2, centre 0) at
+        interp2 * sampling_freq / decim1 fed its zero-stuffed outputs.  Equal, call for call, to the client of
+        Group.add_client_cascade with the same arguments.  See cascade_plan for taps."""
+        return cls(decim1, taps1, center_freq, sampling_freq, max_input_buffer_length,
+                   stage_b=(interp2, decim2, taps2))
 
     def _call(self, name: str, data: np.ndarray):
         out = C.c_void_p()

@@ -20,11 +20,21 @@
  *   dropin_fir_poly_kernel  the same for rational (L/M) filters, one polyphase branch
  *                         per output (launched only when the batch has such a request).
  *
+ * Cascade (two-stage) filters: stage A is an integer request above whose outputs go to
+ * the filter's row of the engine's cascade arena in HBM; stage B then runs the batch
+ * engine's own kernels (cascade_stage_b.cuh: ring append, integer and rational stage B)
+ * into the arena, and dropin_cascade_out_kernel copies each request's final row into
+ * its filter's pinned output buffer.
+ *
  * So a batch costs one (batched) input copy, two launches (three with rational
- * filters in it) and one stream synchronisation however many filters are in it.
+ * filters in it) and one stream synchronisation however many filters are in it; cascade
+ * filters add the append, the stage-B kernel of each kind present and the copy-out
+ * (and one launch more per further integer stage-B CTA size, which only a stage B whose
+ * window nearly fills shared memory lowers).
  */
 #pragma once
 
+#include "cascade_stage_b.cuh"
 #include "xlating_common.cuh"
 
 namespace xl {
@@ -276,6 +286,20 @@ dropin_fir_poly_kernel(const FilterDev *__restrict__ filters, const int2 *__rest
   }
   __syncthreads();
   for (int i = threadIdx.x; i < n_span; i += G_THREADS) d->out[kbase + i] = so[i];
+}
+
+// One cascade request's final row: stage B leaves it at arena[off, off + n); dst is the device address of the
+// filter's pinned output buffer.
+struct CascOut {
+  float2 *dst;
+  int off, n;
+};
+
+// grid = (ceil(max n / 256), cascade requests)
+__global__ void __launch_bounds__(256)
+dropin_cascade_out_kernel(const CascOut *__restrict__ co, const float2 *__restrict__ arena) {
+  const CascOut c = co[blockIdx.y];
+  for (int i = blockIdx.x * 256 + threadIdx.x; i < c.n; i += gridDim.x * 256) c.dst[i] = arena[c.off + i];
 }
 
 }  // namespace xl

@@ -60,6 +60,15 @@
  * filter with decimation M at L * fs fed the zero-stuffed stream, as the batch group's
  * rational clients are: history and output counts in upsampled samples, polyphase taps, no
  * Q15 path.  They share their band's group with the integer filters.
+ *
+ * Cascade filters (create_cascade_frequency_xlating_filter) are the batch group's cascade clients: stage A
+ * is an ordinary integer request whose outputs go to the filter's row of an engine-wide device arena
+ * (CascArena), stage B is walked on the host as the group walks it and runs the group's own stage-B
+ * kernels (cascade_stage_b.cuh) over a private, zeroed stage-A history ring, and a copy-out kernel moves
+ * the final rows into the filters' pinned output buffers.  They are always served by this engine: the
+ * band's group is created with XLG_TRACK_STATE, which cannot carry two stages of state, so a cascade
+ * filter never joins it and does not count towards creating it; the band's integer and rational filters
+ * form their group as before.  No Q15 path.
  */
 #include <cuda_runtime.h>
 #include <errno.h>
@@ -72,10 +81,12 @@
 #include <map>
 #include <mutex>
 #include <new>
+#include <shared_mutex>
 #include <vector>
 
 #include "block_cache.h"
 #include "call_combiner.h"
+#include "cascade_stage_b.cuh"
 #include "dropin_kernels.cuh"
 #include "stream_overlay.h"
 #include "taps_host.h"
@@ -114,6 +125,25 @@ struct Lane {
   DropinReq *h_req = nullptr;        // pinned, read by the front kernel over PCIe
   const DropinReq *d_req = nullptr;  // its device address
   int2 *d_batch = nullptr;           // (filter, q15) per request, written by the front kernel
+  // cascade requests' stage-B tables (allocated with the lane's first cascade batch): CascBlk entries (integer
+  // stage B first, by CTA size), CascPolyBlk entries of the rational ones, and their copy-out rows
+  CascBlk *h_cblk = nullptr, *d_cblk = nullptr;
+  CascPolyBlk *h_pblk = nullptr, *d_pblk = nullptr;
+  CascOut *h_cout = nullptr, *d_cout = nullptr;
+};
+
+// Cascade filters' device memory that the stage-B kernels address by int offsets from one base: per filter
+// a region [stage-B taps | stage-A row | stage-B row] (float2 units, 32-byte aligned).  It grows by moving:
+// a batch holding cascade requests keeps move_mu shared until its stream is synchronised, a move takes it
+// exclusively and repoints every cascade filter's stage-A output (FilterDev::out).
+struct CascArena {
+  std::shared_mutex move_mu;
+  std::mutex mu;                    // guards the rest (lock order: move_mu, then mu)
+  float2 *base = nullptr;
+  size_t cap = 0, top = 0;          // float2 units; regions lie below top, or in holes
+  std::map<size_t, size_t> holes;   // offset -> length of freed regions, coalesced
+  std::vector<xlating_t *> filters; // live cascade filters
+  bool ready = false;               // stage-B kernels' shared-memory limit raised on this device
 };
 
 struct Engine;
@@ -166,6 +196,7 @@ struct Engine {
     std::atomic<uint64_t> served{0}, copy_ns{0}, call_ns{0};
   };
   ServedShard served[AutoStream::kLanes];
+  CascArena casc;
 };
 constexpr size_t kPoolMaxBytes = (size_t)2 << 30;  // device + pinned bytes kept for reuse
 
@@ -231,6 +262,7 @@ struct xlating_t {
   void *h_in = nullptr;
   const void *d_in = nullptr;  // device address of h_in (zero-copy)
   float2 *h_out = nullptr;
+  float2 *d_out = nullptr;     // its device address
   short2 *h_qout = nullptr;
   float *h_phases = nullptr;  // pinned oscillator table (host-walked chain), read by the FIR kernel
   float ph_re = 1.0f, ph_im = 0.0f, inc_re = 0.0f, inc_im = 0.0f;  // host oscillator (src/xlating.c:543-544)
@@ -249,6 +281,24 @@ struct xlating_t {
                               // the first: all that the next window can reach
   float2 *d_ring = nullptr;   // the filter's private cf32 ring (inside d_mem) and its size
   size_t ring_cap = 0;
+  // --- cascade filter (create_cascade_frequency_xlating_filter): everything above describes stage A, an
+  // integer filter whose FilterDev::out is its stage-A row in the engine's CascArena
+  bool casc = false;
+  float *adopted_taps2 = nullptr;
+  uint32_t L2 = 1, D2 = 0;     // stage B's interpolation and decimation
+  long long T2 = 0;
+  int Tb2 = 0;                 // taps per polyphase branch (L2 > 1)
+  int ko2 = 0;                 // stage-B outputs per CTA: C_KO halved to fit (L2 = 1), cascade_poly_ko (L2 > 1)
+  long long hist2 = 0;         // stage B's history_offset (upsampled samples when L2 > 1)
+  long long a_pos = 0;         // stage-A outputs so far: the ring's stream position
+  int fin_cap = 0;             // stage-B outputs of one call at most
+  float2 *d_cring = nullptr;   // stage-A history ring (inside d_mem), cring_cap samples, a power of two
+  size_t cring_cap = 0;
+  size_t arena_off = 0, arena_len = 0;  // the filter's CascArena region, float2 units
+  int taps2_off = 0, a_off = 0, b_off = 0;  // stage-B taps (floats), stage-A and stage-B rows (float2) in it
+  CascBlk cblk;                // this call's stage B
+  CascPolyBlk pblk;            // (L2 > 1)
+  int req_out2 = 0;            // this call's stage-B outputs
   // the call in flight
   DropinReq req;
   int req_out = 0;
@@ -351,11 +401,93 @@ int sync_device_state(xlating *f) {
   return 0;
 }
 
+// The lane's stage-B tables, allocated with its first cascade batch (the leader owns the lane).
+cudaError_t lane_casc_tables(Lane &L) {
+  if (L.h_cblk != nullptr) return cudaSuccess;
+  const size_t hb = kMaxBatch * (sizeof(CascBlk) + sizeof(CascPolyBlk) + sizeof(CascOut));
+  char *h = nullptr, *d = nullptr;
+  cudaError_t err = cudaHostAlloc((void **)&h, hb, cudaHostAllocDefault);
+  if (err == cudaSuccess) err = cudaMalloc((void **)&d, hb);
+  if (err != cudaSuccess) {
+    if (h != nullptr) cudaFreeHost(h);
+    return err;
+  }
+  L.h_cblk = (CascBlk *)h;
+  L.d_cblk = (CascBlk *)d;
+  L.h_pblk = (CascPolyBlk *)(h + kMaxBatch * sizeof(CascBlk));
+  L.d_pblk = (CascPolyBlk *)(d + kMaxBatch * sizeof(CascBlk));
+  L.h_cout = (CascOut *)(h + kMaxBatch * (sizeof(CascBlk) + sizeof(CascPolyBlk)));
+  L.d_cout = (CascOut *)(d + kMaxBatch * (sizeof(CascBlk) + sizeof(CascPolyBlk)));
+  return cudaSuccess;
+}
+
+// Stage B of the batch's cascade requests, after their stage A on the same stream: the group's append and
+// stage-B kernels over the lane's tables, then the copy into each filter's pinned output buffer.  Integer
+// entries come first, ordered by CTA size, one launch per size; each filter keeps the CTA size it would
+// have alone in a group, so its lanes walk its taps as they would there.
+cudaError_t run_cascades(Engine *e, Lane &L, CombinerCall *const *batch, int n_req) {
+  std::vector<const xlating *> cs;
+  for (int i = 0; i < n_req; i++) {
+    const xlating *b = (const xlating *)batch[i]->user;
+    if (b->casc) cs.push_back(b);
+  }
+  std::stable_sort(cs.begin(), cs.end(), [](const xlating *x, const xlating *y) {
+    return (x->L2 == 1) != (y->L2 == 1) ? x->L2 == 1 : (x->L2 == 1 && x->ko2 > y->ko2);
+  });
+  cudaError_t err = lane_casc_tables(L);
+  if (err != cudaSuccess) return err;
+  const int n_casc = (int)cs.size();
+  int n_int = 0, n_rat = 0, max_n1 = 0, max_n2 = 0, max_rat_ctas = 0;
+  size_t poly_smem = 0;
+  for (int c = 0; c < n_casc; c++) {
+    const xlating *b = cs[c];
+    L.h_cblk[c] = b->cblk;
+    L.h_cout[c] = {b->d_out, b->b_off, b->req_out2};
+    max_n1 = std::max(max_n1, b->cblk.n1);
+    max_n2 = std::max(max_n2, b->req_out2);
+    if (b->L2 == 1) {
+      n_int++;
+    } else {
+      L.h_pblk[n_rat++] = b->pblk;
+      max_rat_ctas = std::max(max_rat_ctas, (b->pblk.n2 + b->ko2 - 1) / b->ko2);
+      poly_smem = std::max(poly_smem, cascade_poly_smem(b->ko2, (int)b->L2, (int)b->D2, b->Tb2));
+    }
+  }
+  const cudaStream_t st = L.stream;
+  err = cudaMemcpyAsync(L.d_cblk, L.h_cblk, n_casc * sizeof(CascBlk), cudaMemcpyHostToDevice, st);
+  if (err == cudaSuccess && n_rat > 0)
+    err = cudaMemcpyAsync(L.d_pblk, L.h_pblk, n_rat * sizeof(CascPolyBlk), cudaMemcpyHostToDevice, st);
+  if (err == cudaSuccess)
+    err = cudaMemcpyAsync(L.d_cout, L.h_cout, n_casc * sizeof(CascOut), cudaMemcpyHostToDevice, st);
+  if (err != cudaSuccess) return err;
+  float2 *base = e->casc.base;
+  if (max_n1 > 0) cascade_launch_append(L.d_cblk, n_casc, max_n1, base, st);
+  for (int c0 = 0; c0 < n_int;) {
+    const int ko = cs[c0]->ko2;
+    int c1 = c0, run_n2 = 0;
+    size_t smem = 0;
+    for (; c1 < n_int && cs[c1]->ko2 == ko; c1++) {
+      run_n2 = std::max(run_n2, cs[c1]->cblk.n2);
+      smem = std::max(smem, cascade_smem(ko, (int)cs[c1]->D2, (int)cs[c1]->T2));
+    }
+    if (run_n2 > 0) cascade_launch_fir(L.d_cblk + c0, c1 - c0, run_n2, ko, smem, (const float *)base, base, st);
+    c0 = c1;
+  }
+  if (max_rat_ctas > 0) cascade_launch_fir_poly(L.d_pblk, n_rat, max_rat_ctas, poly_smem, (const float *)base, base, st);
+  if (max_n2 > 0) dropin_cascade_out_kernel<<<dim3((max_n2 + 255) / 256, n_casc), 256, 0, st>>>(L.d_cout, base);
+  return cudaGetLastError();
+}
+
 // Launch one batch on lane `lane` and wait for it (CallCombiner::RunBatch; called by the
 // batch's leader thread).
 int run_batch(void *ctx, int lane, CombinerCall *const *batch, int n_req) {
   Engine *e = (Engine *)ctx;
   Lane &L = e->lanes[lane];
+  // cascade requests write and read the cascade arena: it must not move until the stream is synchronised
+  std::shared_lock<std::shared_mutex> arena_pin(e->casc.move_mu, std::defer_lock);
+  bool any_casc = false;
+  for (int i = 0; i < n_req && !any_casc; i++) any_casc = ((const xlating *)batch[i]->user)->casc;
+  if (any_casc) arena_pin.lock();
   cudaError_t err = cudaSetDevice(e->device);
   if (err == cudaSuccess) {
     int max_n = 0, max_out = 0, max_poly_ctas = 0;
@@ -393,6 +525,7 @@ int run_batch(void *ctx, int lane, CombinerCall *const *batch, int n_req) {
       if (max_poly_ctas > 0)
         dropin_fir_poly_kernel<<<dim3(max_poly_ctas, n_req), G_THREADS, 0, L.stream>>>(e->d_filters, L.d_batch);
       err = cudaGetLastError();
+      if (err == cudaSuccess && any_casc) err = run_cascades(e, L, batch, n_req);
     }
     if (err == cudaSuccess) err = cudaStreamSynchronize(L.stream);
   }
@@ -549,8 +682,141 @@ void stream_attach(xlating *f, uint32_t fs, uint32_t max_in) {
   f->sh = sh;
 }
 
+// ---- cascade filters' arena (CascArena) ----
+size_t align4(size_t v) { return (v + 3) & ~(size_t)3; }
+
+// Point filter f's stage-A output (FilterDev::out) at its row of the arena where the arena is now.
+cudaError_t casc_point(Engine *e, const xlating *f) {
+  float2 *out = e->casc.base + f->a_off;
+  return cudaMemcpy((char *)(e->d_filters + f->slot) + offsetof(FilterDev, out), &out, sizeof(out),
+                    cudaMemcpyHostToDevice);
+}
+
+// A region of len float2 from the first hole that holds it, or from the top; false when neither has room.
+// (CascArena::mu held)
+bool casc_take(CascArena &a, size_t len, size_t *off) {
+  for (auto it = a.holes.begin(); it != a.holes.end(); ++it)
+    if (it->second >= len) {
+      *off = it->first;
+      const size_t rest = it->second - len, rest_off = it->first + len;
+      a.holes.erase(it);
+      if (rest > 0) a.holes[rest_off] = rest;
+      return true;
+    }
+  if (a.top + len > a.cap) return false;
+  *off = a.top;
+  a.top += len;
+  return true;
+}
+
+// (CascArena::mu held)
+void casc_give(CascArena &a, size_t off, size_t len) {
+  auto next = a.holes.lower_bound(off);
+  if (next != a.holes.end() && off + len == next->first) {
+    len += next->second;
+    next = a.holes.erase(next);
+  }
+  if (next != a.holes.begin()) {
+    auto prev = std::prev(next);
+    if (prev->first + prev->second == off) {
+      off = prev->first;
+      len += prev->second;
+      a.holes.erase(prev);
+    }
+  }
+  if (off + len == a.top)
+    a.top = off;
+  else
+    a.holes[off] = len;
+}
+
+// Give cascade filter f (its FilterDev already in the table) its arena region: stage-B taps `taps2` (floats,
+// a multiple of 4), then its stage-A row (out_cap) and its stage-B row (fin_cap).
+int casc_attach(xlating *f, const std::vector<float> &taps2) {
+  Engine *e = f->e;
+  CascArena &a = e->casc;
+  const size_t n_taps = align4(taps2.size() / 2);
+  const size_t len = n_taps + align4((size_t)f->out_cap) + align4((size_t)f->fin_cap);
+  std::unique_lock<std::shared_mutex> moving(a.move_mu, std::defer_lock);
+  std::unique_lock<std::mutex> lk(a.mu);
+  cudaError_t err = cudaSuccess;
+  if (!a.ready) {
+    err = cascade_stage_b_init();
+    if (err != cudaSuccess) {
+      XL_LOG("cannot raise the stage-B kernels' shared memory to %d bytes: %s", kTileMaxSmem, cudaGetErrorString(err));
+      return -EIO;
+    }
+    a.ready = true;
+  }
+  size_t off = 0;
+  if (!casc_take(a, len, &off)) {
+    // the arena moves: wait until no batch with cascade requests is in flight
+    lk.unlock();
+    moving.lock();
+    lk.lock();
+    if (!casc_take(a, len, &off)) {
+      const size_t cap = std::max({2 * a.cap, a.top + len, (size_t)1 << 16});
+      float2 *nb = nullptr;
+      if (cudaMalloc(&nb, cap * sizeof(float2)) != cudaSuccess) {
+        cudaGetLastError();
+        XL_LOG("cannot grow the cascade arena to %zu bytes", cap * sizeof(float2));
+        return -ENOMEM;
+      }
+      if (a.top > 0) err = cudaMemcpy(nb, a.base, a.top * sizeof(float2), cudaMemcpyDeviceToDevice);
+      if (err != cudaSuccess) {
+        cudaFree(nb);
+        XL_LOG("cannot move the cascade arena: %s", cudaGetErrorString(err));
+        return -EIO;
+      }
+      if (a.base != nullptr) cudaFree(a.base);
+      a.base = nb;
+      a.cap = cap;
+      for (const xlating *g : a.filters)
+        if (err == cudaSuccess) err = casc_point(e, g);
+      if (err != cudaSuccess) {
+        XL_LOG("cannot repoint the cascade filters' stage A: %s", cudaGetErrorString(err));
+        return -EIO;
+      }
+      casc_take(a, len, &off);
+    }
+  }
+  if (off + len > ((size_t)1 << 30)) {  // int offsets of the stage-B kernels, taps in floats
+    casc_give(a, off, len);
+    XL_LOG("cascade filters need more than 8 GiB of device memory");
+    return -ENOMEM;
+  }
+  f->taps2_off = (int)(2 * off);
+  f->a_off = (int)(off + n_taps);
+  f->b_off = (int)(off + n_taps + align4((size_t)f->out_cap));
+  err = cudaMemcpy(a.base + off, taps2.data(), taps2.size() * sizeof(float), cudaMemcpyHostToDevice);
+  if (err == cudaSuccess) err = casc_point(e, f);
+  if (err != cudaSuccess) {
+    casc_give(a, off, len);
+    XL_LOG("cannot set up a cascade filter's stage B: %s", cudaGetErrorString(err));
+    return -EIO;
+  }
+  f->arena_off = off;
+  f->arena_len = len;
+  a.filters.push_back(f);
+  return 0;
+}
+
+void casc_detach(xlating *f) {
+  if (f->arena_len == 0) return;
+  CascArena &a = f->e->casc;
+  std::lock_guard<std::mutex> lk(a.mu);
+  casc_give(a, f->arena_off, f->arena_len);
+  for (size_t i = 0; i < a.filters.size(); i++)
+    if (a.filters[i] == f) {
+      a.filters.erase(a.filters.begin() + (long)i);
+      break;
+    }
+  f->arena_len = 0;
+}
+
 void filter_release(xlating *f) {
   stream_detach(f);
+  if (f->e != nullptr) casc_detach(f);
   if (f->e != nullptr) {
     bool pooled = false;
     {
@@ -572,24 +838,56 @@ void filter_release(xlating *f) {
   }
   if (f->group != nullptr) xlg_destroy(f->group);
   if (f->adopted_taps != nullptr) free(f->adopted_taps);
+  if (f->adopted_taps2 != nullptr) free(f->adopted_taps2);
   delete f;
+}
+
+// Stage B of a cascade filter (create_cascade_frequency_xlating_filter), its arguments already checked.
+struct CascSpec {
+  uint32_t L2, D2;
+  float *taps2;
+  size_t T2;
+};
+
+// Stage B's taps as the batch group keeps them (xlg_add_client_cascade_rational): the reference filter at
+// L2 * fs / D1 with centre 0, whose rotated taps are (h, +-0), so the real parts of the reversed taps;
+// branch-major P[r][t] = rev2[r + t * L2] when L2 > 1; zero-padded to whole 16-byte units.
+int casc_taps(const CascSpec &cs, uint32_t decim1, uint32_t sampling_freq, std::vector<float> *out) {
+  const uint64_t rate2 = (uint64_t)cs.L2 * std::max<uint32_t>(sampling_freq / decim1, 1);
+  xl_client_consts k2;
+  const int rc = xl_client_consts_build(cs.taps2, cs.T2, cs.D2, 0, (uint32_t)std::min<uint64_t>(rate2, UINT32_MAX), &k2);
+  if (rc != 0) return rc;
+  const size_t Tb2 = (cs.T2 + cs.L2 - 1) / cs.L2;
+  std::vector<float> packed(2 * (size_t)cs.L2 * Tb2);
+  xl_poly_pack(k2.rev_cf32, cs.T2, cs.L2, packed.data());  // L2 = 1: the reversed taps themselves
+  xl_client_consts_free(&k2);
+  out->assign(align4((size_t)cs.L2 * Tb2), 0.f);
+  for (size_t j = 0; j < (size_t)cs.L2 * Tb2; j++) (*out)[j] = packed[2 * j];
+  return 0;
 }
 
 // A filter with interpolation L > 1 is the filter with decimation M = `decimation` at L * fs fed the
 // zero-stuffed stream (create_rational_frequency_xlating_filter): its constants are built at L * fs, its
-// taps are kept as polyphase branches and it has no Q15 ring or taps.  L = 1 is the integer filter.
+// taps are kept as polyphase branches and it has no Q15 ring or taps.  L = 1 is the integer filter.  With
+// `cs`, the filter is stage A of a cascade filter (L = 1, no Q15 path) and gets a stage-A history ring and
+// its CascArena region.
 int filter_build(xlating *f, int device, uint32_t interp, uint32_t decimation, const float *taps, size_t taps_len,
-                 int32_t center_freq, uint32_t sampling_freq, uint32_t max_in) {
+                 int32_t center_freq, uint32_t sampling_freq, uint32_t max_in, const CascSpec *cs) {
   if (decimation == 0 || sampling_freq == 0) return -EINVAL;
   int rc = engine_get(device, &f->e);
   if (rc != 0) {
     f->e = nullptr;
     return rc;
   }
+  std::vector<float> taps2;
+  if (cs != nullptr) {
+    rc = casc_taps(*cs, decimation, sampling_freq, &taps2);
+    if (rc != 0) return rc;
+  }
   xl_client_consts k;
   rc = xl_client_consts_build(taps, taps_len, decimation, center_freq, interp * sampling_freq, &k);
   if (rc != 0) return rc;
-  const bool q15 = interp == 1;  // rational filters refuse the Q15 path
+  const bool q15 = interp == 1 && cs == nullptr;  // rational and cascade filters refuse the Q15 path
   const size_t Tb = (taps_len + interp - 1) / interp;  // taps per polyphase branch (T for L = 1)
   std::vector<float> branches;
   if (!q15) {
@@ -607,19 +905,44 @@ int filter_build(xlating *f, int device, uint32_t interp, uint32_t decimation, c
   const size_t hist_in = (taps_len - 1) / interp + 1;  // input samples the oldest window can reach
   size_t cap = 1024;
   while (cap < hist_in + max_n + 64) cap <<= 1;      // history + one block, power of two
+  size_t cring_cap = 0;
+  if (cs != nullptr) {
+    f->casc = true;
+    f->L2 = cs->L2;
+    f->D2 = cs->D2;
+    f->T2 = (long long)cs->T2;
+    f->Tb2 = (int)((cs->T2 + cs->L2 - 1) / cs->L2);
+    f->hist2 = f->T2 - 1;  // src/xlating.c:552 (upsampled samples when L2 > 1)
+    // n2 <= (L2 * n1 - 1) / D2 + 1 for any history
+    f->fin_cap = (int)((uint64_t)f->out_cap * cs->L2 / cs->D2 + 2);
+    if (cs->L2 == 1) {
+      f->ko2 = C_KO;  // what a group of this one client launches
+      while (f->ko2 > 1 && cascade_smem(f->ko2, (int)cs->D2, (int)cs->T2) > (size_t)kTileMaxSmem) f->ko2 /= 2;
+    } else {
+      f->ko2 = cascade_poly_ko((int)cs->L2, (int)cs->D2, f->Tb2);
+    }
+    // a call completes before the next one starts: the stage-B history of at most T2 - 1 upsampled samples
+    // (ceil((T2 - 1) / L2) stage-A samples, and one zero-weighted sample past the last branch) plus one
+    // call's stage-A outputs
+    const size_t back = (cs->T2 - 1 + cs->L2 - 1) / cs->L2 + 1;
+    cring_cap = 64;
+    while (cring_cap < back + (size_t)f->out_cap) cring_cap <<= 1;
+  }
+  const int host_out = cs != nullptr ? f->fin_cap : f->out_cap;  // outputs the pinned buffer receives
   FilterDev d;
   memset(&d, 0, sizeof(d));
   // device arena
   const size_t o_ring = 0;
   const size_t o_qring = align_up(o_ring + cap * sizeof(float2), 256);
-  const size_t o_taps = align_up(o_qring + (q15 ? cap * sizeof(short2) : 0), 256);
+  const size_t o_cring = align_up(o_qring + (q15 ? cap * sizeof(short2) : 0), 256);
+  const size_t o_taps = align_up(o_cring + cring_cap * sizeof(float2), 256);
   const size_t o_qtaps = align_up(o_taps + interp * Tb * sizeof(float2), 256);
   const size_t o_ph = align_up(o_qtaps + (q15 ? taps_len * sizeof(short2) : 0), 256);
   const size_t o_qph = align_up(o_ph + ((size_t)f->out_cap / 2 + 2) * sizeof(float2), 256);
   const size_t d_bytes = align_up(o_qph + (q15 ? ((size_t)f->out_cap + 2) * sizeof(short2) : 0), 256);
   // pinned host arena
   const size_t h_in_bytes = align_up((size_t)max_in * sizeof(int16_t), 256);  // cs16 is the widest input
-  const size_t h_out_bytes = align_up((size_t)f->out_cap * sizeof(float2), 256);
+  const size_t h_out_bytes = align_up((size_t)host_out * sizeof(float2), 256);
   const size_t h_qout_bytes = align_up((size_t)f->out_cap * sizeof(short2), 256);
   const size_t h_ph_bytes = align_up(((size_t)f->out_cap / 2 + 2) * sizeof(float2), 256);
   char *dm = nullptr, *hm = nullptr, *hm_dev = nullptr;
@@ -646,7 +969,9 @@ int filter_build(xlating *f, int device, uint32_t interp, uint32_t decimation, c
     f->d_bytes = d_bytes;
   }
   dm = (char *)f->d_mem;
-  CU_TRY(cudaMemset(dm, 0, o_taps));  // both rings start as the reference's zeroed working buffers (:556-565)
+  // the rings (and a cascade filter's stage-A history) start as the reference's zeroed working buffers
+  // (:556-565)
+  CU_TRY(cudaMemset(dm, 0, o_taps));
   if (q15) {
     CU_TRY(cudaMemcpy(dm + o_taps, k.rev_cf32, taps_len * sizeof(float2), cudaMemcpyHostToDevice));
     CU_TRY(cudaMemcpy(dm + o_qtaps, k.rev_q15, taps_len * sizeof(short2), cudaMemcpyHostToDevice));
@@ -662,15 +987,18 @@ int filter_build(xlating *f, int device, uint32_t interp, uint32_t decimation, c
   f->h_in = hm;
   f->d_in = hm_dev;
   f->h_out = (float2 *)(hm + h_in_bytes);
+  f->d_out = (float2 *)(hm_dev + h_in_bytes);
   f->h_qout = (short2 *)(hm + h_in_bytes + h_out_bytes);
   f->h_phases = (float *)(hm + h_in_bytes + h_out_bytes + h_qout_bytes);
   f->inc_re = k.incr_re;
   f->inc_im = k.incr_im;
   f->center_freq = center_freq;
   f->fs = sampling_freq;
-  f->tail.assign((taps_len - 1) / interp, make_float2(0.f, 0.f));  // src/xlating.c:552-565: zero history
+  if (cs == nullptr) f->tail.assign((taps_len - 1) / interp, make_float2(0.f, 0.f));  // src/xlating.c:552-565
   f->d_ring = (float2 *)(dm + o_ring);
   f->ring_cap = cap;
+  f->d_cring = cs != nullptr ? (float2 *)(dm + o_cring) : nullptr;
+  f->cring_cap = cring_cap;
   d.ring = (float2 *)(dm + o_ring);
   d.qring = q15 ? (short2 *)(dm + o_qring) : nullptr;
   d.taps = (const float2 *)(dm + o_taps);
@@ -701,10 +1029,14 @@ int filter_build(xlating *f, int device, uint32_t interp, uint32_t decimation, c
     f->e->free_slots.pop_back();
   }
   CU_TRY(cudaMemcpy(f->e->d_filters + f->slot, &d, sizeof(d), cudaMemcpyHostToDevice));
+  if (cs != nullptr) {
+    rc = casc_attach(f, taps2);  // also points d.out at the stage-A row
+    if (rc != 0) goto fail;
+  }
   f->e->live_filters++;
   f->counted = true;
   xl_client_consts_free(&k);
-  stream_attach(f, sampling_freq, max_in);
+  if (cs == nullptr) stream_attach(f, sampling_freq, max_in);  // a cascade filter never joins a band group
   return 0;
 fail:
   xl_client_consts_free(&k);
@@ -742,10 +1074,15 @@ void run_block_group(xlating *f, int fmt, const void *input, size_t input_len, u
 void run_block(xlating *f, int fmt, const void *input, size_t input_len, bool q15, void **output,
                size_t *output_len) {
   *output_len = 0;
-  if (q15 && f->L > 1) {
+  if (q15 && (f->L > 1 || f->casc)) {
     // the Q15 path serves integer filters only: refuse before anything is consumed, so that the
     // filter's cf32 stream (and its place in the band's group) carries on as if this call never happened
-    if (!f->q15_refused) XL_LOG("Q15 output is not available for a rational (L = %u) filter; use process_*_cf32", f->L);
+    if (!f->q15_refused) {
+      if (f->casc)
+        XL_LOG("Q15 output is not available for a cascade filter; use process_*_cf32");
+      else
+        XL_LOG("Q15 output is not available for a rational (L = %u) filter; use process_*_cf32", f->L);
+    }
     f->q15_refused = true;
     *output = (void *)f->h_qout;
     return;
@@ -819,6 +1156,39 @@ void run_block(xlating *f, int fmt, const void *input, size_t input_len, bool q1
   int n_out = 0;
   if (last_ok >= first) n_out = (int)((last_ok - first) / (long long)f->D) + 1;
   if (n_out > f->out_cap) n_out = f->out_cap;
+  if (f->casc) {
+    // stage B: the group's host walk over this call's n_out stage-A samples, upsampled by L2 (the
+    // zero-stuffed stream u[L2 * n] = y[n]; the same integers for L2 = 1)
+    const long long first2 = (long long)f->L2 * f->a_pos - f->hist2;
+    const int n2 = xl_walk(&f->hist2, (long long)f->L2 * n_out, (size_t)f->T2, f->D2, f->fin_cap);
+    CascBlk &cb = f->cblk;
+    cb.ring = f->d_cring;
+    cb.a_pos = f->a_pos;
+    cb.first = first2;
+    cb.mask = (unsigned)(f->cring_cap - 1);
+    cb.a_off = f->a_off;
+    cb.n1 = n_out;
+    cb.n2 = n2;
+    cb.D2 = (int)f->D2;
+    cb.T2 = (int)f->T2;
+    cb.taps_off = f->taps2_off;
+    cb.out_off = f->b_off;
+    if (f->L2 > 1) {
+      CascPolyBlk &pb = f->pblk;
+      pb.ring = f->d_cring;
+      pb.first = first2;
+      pb.mask = cb.mask;
+      pb.n2 = n2;
+      pb.L2 = (int)f->L2;
+      pb.M2 = (int)f->D2;
+      pb.Tb2 = f->Tb2;
+      pb.ko = f->ko2;
+      pb.taps_off = f->taps2_off;
+      pb.out_off = f->b_off;
+    }
+    f->a_pos += n_out;
+    f->req_out2 = n2;
+  }
   f->req.raw = slot >= 0 ? e->cache->device_ptr(slot) : f->d_in;
   f->req_slot = slot;
   f->req.S = S;
@@ -860,17 +1230,18 @@ void run_block(xlating *f, int fmt, const void *input, size_t input_len, bool q1
     XL_LOG("block dropped (%d)", rc);
     return;
   }
-  *output_len = (size_t)n_out;
+  *output_len = (size_t)(f->casc ? f->req_out2 : n_out);
 }
 
-// Both constructors after their argument checks: adopts `taps`.
+// The constructors after their argument checks: adopts `taps` (and a cascade's stage-B taps).
 int create_filter(uint32_t interp, uint32_t decimation, float *taps, size_t taps_len, int32_t center_freq,
-                  uint32_t sampling_freq, uint32_t max_input_buffer_length, xlating **filter) {
+                  uint32_t sampling_freq, uint32_t max_input_buffer_length, const CascSpec *cs, xlating **filter) {
   xlating *f = new (std::nothrow) xlating_t();
   if (f == NULL) {
     return -ENOMEM;
   }
   f->adopted_taps = taps;
+  f->adopted_taps2 = cs != nullptr ? cs->taps2 : nullptr;
   f->call.user = f;
   f->L = interp;
   int device = 0;
@@ -882,11 +1253,19 @@ int create_filter(uint32_t interp, uint32_t decimation, float *taps, size_t taps
   int rc;
   if (use_group_model()) {
     rc = xlg_create(device, sampling_freq, max_in, 0, &f->group);
-    if (rc == 0)
-      rc = interp == 1 ? xlg_add_client(f->group, decimation, taps, taps_len, center_freq, &f->client)
-                       : xlg_add_client_rational(f->group, interp, decimation, taps, taps_len, center_freq, &f->client);
+    if (rc == 0) {
+      if (cs != nullptr) {
+        f->casc = true;  // the Q15 refusal
+        rc = xlg_add_client_cascade_rational(f->group, decimation, taps, taps_len, center_freq, cs->L2, cs->D2,
+                                             cs->taps2, cs->T2, &f->client);
+      } else if (interp == 1) {
+        rc = xlg_add_client(f->group, decimation, taps, taps_len, center_freq, &f->client);
+      } else {
+        rc = xlg_add_client_rational(f->group, interp, decimation, taps, taps_len, center_freq, &f->client);
+      }
+    }
   } else {
-    rc = filter_build(f, device, interp, decimation, taps, taps_len, center_freq, sampling_freq, max_in);
+    rc = filter_build(f, device, interp, decimation, taps, taps_len, center_freq, sampling_freq, max_in, cs);
   }
   if (rc != 0) {
     filter_release(f);
@@ -910,7 +1289,8 @@ int create_frequency_xlating_filter(uint32_t decimation, float *taps, size_t tap
   if (filter == NULL || taps == NULL) {
     return -EINVAL;
   }
-  return create_filter(1, decimation, taps, taps_len, center_freq, sampling_freq, max_input_buffer_length, filter);
+  return create_filter(1, decimation, taps, taps_len, center_freq, sampling_freq, max_input_buffer_length, nullptr,
+                       filter);
 }
 
 int create_rational_frequency_xlating_filter(uint32_t interpolation, uint32_t decimation, float *taps,
@@ -937,7 +1317,42 @@ int create_rational_frequency_xlating_filter(uint32_t interpolation, uint32_t de
     return -EINVAL;
   }
   return create_filter(interpolation, decimation, taps, taps_len, center_freq, sampling_freq,
-                       max_input_buffer_length, filter);
+                       max_input_buffer_length, nullptr, filter);
+}
+
+int create_cascade_frequency_xlating_filter(uint32_t decimation1, float *taps1, size_t taps1_len, int32_t center_freq,
+                                            uint32_t interpolation2, uint32_t decimation2, float *taps2,
+                                            size_t taps2_len, uint32_t sampling_freq,
+                                            uint32_t max_input_buffer_length, xlating **filter) {
+  if (taps1_len == 0 || taps2_len == 0) {
+    return -1;  // as create_frequency_xlating_filter (neither vector adopted on this path)
+  }
+  if (filter == NULL || taps1 == NULL || taps2 == NULL) {
+    return -EINVAL;
+  }
+  // the batch group's rules (xlg_add_client_cascade_rational), checked before any CUDA call
+  const uint32_t max_in = max_input_buffer_length < 2 ? 2 : max_input_buffer_length;
+  const char *why = NULL;
+  if (decimation1 == 0 || decimation2 == 0 || interpolation2 == 0)
+    why = "decimation1, interpolation2 and decimation2 must all be at least 1";
+  else if (interpolation2 > 1 && (uint64_t)interpolation2 * (max_in / 2 / decimation1 + 2) >= (1ull << 31))
+    why = "interpolation2 x (max_input_buffer_length / 2 / decimation1 + 2) upsampled stage-A samples per call reach 2^31";
+  else if (taps2_len > (size_t)INT32_MAX ||
+           (interpolation2 == 1
+                ? cascade_smem(1, (int)decimation2, (int)taps2_len)
+                : cascade_poly_smem(1, (int)interpolation2, (int)decimation2,
+                                    (int)((taps2_len + interpolation2 - 1) / interpolation2))) > (size_t)kTileMaxSmem)
+    why = "stage B's taps and one output's window exceed the stage-B kernels' shared memory";
+  if (why != NULL) {
+    XL_LOG("cascade filter %u x %u/%u with %zu + %zu taps at %u Hz, blocks of %u: %s", decimation1, interpolation2,
+           decimation2, taps1_len, taps2_len, sampling_freq, max_in, why);
+    free(taps1);  // adopted, as on every other failure but an empty tap vector
+    free(taps2);
+    return -EINVAL;
+  }
+  const CascSpec cs = {interpolation2, decimation2, taps2, taps2_len};
+  return create_filter(1, decimation1, taps1, taps1_len, center_freq, sampling_freq, max_input_buffer_length, &cs,
+                       filter);
 }
 
 void destroy_xlating(xlating *filter) {

@@ -65,7 +65,6 @@ namespace {
 
 constexpr int kTileMinClients = 8;     // smaller aligned classes go to the generic kernel
 constexpr int kTileMinOutputs = 12;    // per block; below this even a 16-output tile is mostly idle
-constexpr int kTileMaxSmem = 200 * 1024;
 // shared memory of an SM (CTAs get kSmSmem / n - 1 KiB each at n per SM)
 constexpr int kSmSmem = 228 * 1024;
 
@@ -1762,11 +1761,7 @@ extern "C" int xlg_add_client_cascade_rational(xlg_group *g, uint32_t decim1, co
   h.hist2 = (long long)taps2_len - 1;  // src/xlating.c:552 (upsampled samples when L2 > 1)
   if (interp2 > 1) {
     h.Tb2 = (int)Tb2;
-    // about 2 * C_THREADS outputs per CTA, a whole number per branch where L2 <= C_THREADS; fewer where the
-    // window would not fit (the attach check above guarantees that one output fits)
-    int ko = interp2 <= (uint32_t)C_THREADS ? 2 * (int)interp2 * (C_THREADS / (int)interp2) : C_KO;
-    while (ko > 1 && cascade_poly_smem(ko, (int)interp2, (int)decim2, h.Tb2) > (size_t)kTileMaxSmem) ko /= 2;
-    h.ko2 = ko;
+    h.ko2 = cascade_poly_ko((int)interp2, (int)decim2, h.Tb2);
   }
   *client_id = id;
   return 0;
@@ -2650,3 +2645,29 @@ extern "C" int xlg_profile_read(xlg_group *g, xlg_profile *p, int reset) {
   }
   return 0;
 }
+
+// ---- stage-B launchers for the per-filter engine (cascade_stage_b.cuh) ----
+namespace xl {
+
+cudaError_t cascade_stage_b_init() {
+  cudaError_t err = cudaFuncSetAttribute(cascade_fir_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem);
+  if (err == cudaSuccess)
+    err = cudaFuncSetAttribute(cascade_fir_poly_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem);
+  return err;
+}
+
+void cascade_launch_append(const CascBlk *cb, int n, int max_n1, const float2 *a_rows, cudaStream_t s) {
+  cascade_append_kernel<<<dim3((max_n1 + 255) / 256, n), 256, 0, s>>>(cb, a_rows);
+}
+
+void cascade_launch_fir(const CascBlk *cb, int n, int max_n2, int ko, size_t smem, const float *taps2, float2 *out,
+                        cudaStream_t s) {
+  cascade_fir_cf32_kernel<<<dim3((max_n2 + ko - 1) / ko, n), C_THREADS, smem, s>>>(cb, taps2, out, ko);
+}
+
+void cascade_launch_fir_poly(const CascPolyBlk *pb, int n, int max_ctas, size_t smem, const float *taps2,
+                             float2 *out, cudaStream_t s) {
+  cascade_fir_poly_cf32_kernel<<<dim3(max_ctas, n), C_THREADS, smem, s>>>(pb, taps2, out);
+}
+
+}  // namespace xl

@@ -40,6 +40,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "cascade_stage_b.cuh"
 #include "xlating_common.cuh"
 
 namespace xl {
@@ -1158,25 +1159,8 @@ fir_long_reduce_kernel(const __grid_constant__ TileLaunch P, const float2 *__res
 }
 
 // ---------------------------------------------------------------------------
-// cascade clients (xlg_add_client_cascade).  Stage A is an integer client of the kernels above whose
-// outputs land in a row of the slot's arena that is never copied to the host.  Stage B is the reference
-// filter at fs / D1 with centre 0: its rotated taps are (h, +-0), its oscillator stays 1 + 0i and the
-// renormalisation divides by 1, so it is a real-tap decimator with history,
-//     z[k] = sum_{j < T2} y[first + k*D2 + j] * rev2[j]          (2 real FMAs per tap),
-// over the client's stage-A stream y, kept in a per-client power-of-two ring in HBM: y at stage-A stream
-// position p lives at ring[p & mask], and positions before the attach point read as the ring's zeros.
+// cascade clients: stage B (CascBlk, CascPolyBlk and their shared memory in cascade_stage_b.cuh)
 // ---------------------------------------------------------------------------
-struct CascBlk {
-  float2 *ring;     // the client's stage-A history ring
-  long long a_pos;  // stage-A stream position of this block's first stage-A output
-  long long first;  // stage-A stream position where this block's stage-B output 0 starts its window
-  unsigned mask;    // ring capacity - 1
-  int a_off;        // this block's stage-A outputs in the slot's output arena
-  int n1, n2;       // stage-A outputs appended / stage-B outputs computed by this block
-  int D2, T2;
-  int taps_off;     // float offset of rev2 in the real tap arena, a multiple of 4 (16-byte TMA source)
-  int out_off;      // final row in the slot's output arena
-};
 
 // companion copy: append this block's stage-A outputs to each client's ring (grid.y = client)
 __global__ void __launch_bounds__(256)
@@ -1185,14 +1169,6 @@ cascade_append_kernel(const CascBlk *__restrict__ cb, const float2 *__restrict__
   const int n1 = b.n1;
   for (int i = blockIdx.x * 256 + threadIdx.x; i < n1; i += gridDim.x * 256)
     b.ring[(unsigned)((unsigned long long)(b.a_pos + i)) & b.mask] = out[b.a_off + i];
-}
-
-constexpr int C_THREADS = 128;
-constexpr int C_R = 2;                    // outputs per thread: t and t + C_THREADS
-constexpr int C_KO = C_THREADS * C_R;     // outputs per CTA at most (the host lowers it where shared memory runs out)
-// shared memory of a CTA with ko outputs: mbarrier, taps padded to 16 bytes, the window (+1 for an odd start, even)
-__host__ __device__ constexpr size_t cascade_smem(int ko, int D2, int T2) {
-  return 16 + (size_t)((T2 + 3) & ~3) * 4 + (((size_t)(ko - 1) * D2 + T2 + 2) & ~(size_t)1) * 8;
 }
 
 // Stage B: CTA (x, c) computes outputs [x*ko, x*ko + ko) of cascade client c.  One TMA bulk copy stages the
@@ -1252,33 +1228,6 @@ cascade_fir_cf32_kernel(const CascBlk *__restrict__ cb, const float *__restrict_
 #pragma unroll
   for (int i = 0; i < C_R; i++)
     if (tid + C_THREADS * i < nk) out[b.out_off + k0 + tid + C_THREADS * i] = acc[i];
-}
-
-// ---------------------------------------------------------------------------
-// rational cascade clients (xlg_add_client_cascade_rational, interp2 = L2 > 1).  Stage B is the reference
-// filter with decimation M2 at L2 * fs / D1, centre 0, fed the zero-stuffed stage-A stream u[L2*n] = y[n]:
-// output k's upsampled window starts at w = first + k*M2, and with r = (-w) mod L2, n0 = (w + r) / L2
-// (poly_branch) only the branch r of the real reversed taps meets stage-A samples,
-//     z[k] = sum_{t < Tb2} y[n0 + t] * P[r][t],   P[r][t] = rev2[r + t*L2] (0 past T2),  Tb2 = ceil(T2 / L2).
-// The ring, its positions and its zeros before the attach are the integer cascade's (CascBlk appends them).
-// ---------------------------------------------------------------------------
-struct CascPolyBlk {
-  float2 *ring;     // the client's stage-A history ring
-  long long first;  // upsampled stream position where this block's output 0 starts its window
-  unsigned mask;    // ring capacity - 1
-  int n2;           // outputs computed by this block
-  int L2, M2, Tb2;
-  int ko;           // outputs per CTA (the host sets it per client)
-  int taps_off;     // float offset of the branch-major taps P in the real tap arena, a multiple of 4
-  int out_off;      // final row in the slot's output arena
-};
-
-// shared memory of a CTA with ko outputs: mbarrier, the L2 branches padded to 16 bytes, the window: the
-// n0 of ko consecutive outputs span at most ceil((ko - 1) * M2 / L2) samples, plus Tb2 taps (+1 for an odd
-// start, even)
-__host__ __device__ constexpr size_t cascade_poly_smem(int ko, int L2, int M2, int Tb2) {
-  return 16 + (((size_t)L2 * Tb2 + 3) & ~(size_t)3) * 4 +
-         ((((size_t)(ko - 1) * M2 + L2 - 1) / L2 + Tb2 + 2) & ~(size_t)1) * 8;
 }
 
 // Stage B of rational cascade clients: CTA (x, c) computes outputs [x*ko, x*ko + ko) of client c.  One TMA

@@ -5,11 +5,16 @@
  * batch binding.  Measures what sdr-server gets by only re-linking against
  * libxlating_b200.so (INTEGRATION.md section 1).
  *
- * usage: dropin_bench <clients> <blocks> [window [warmup_blocks [rational]]]
+ * usage: dropin_bench <clients> <blocks> [window [warmup_blocks [rational|wide|cascade]]]
  *
  * Default workload: 2.016 Msps cu8, 48/96 ksps clients mixed.  With `rational` as the fifth argument:
  * 48 ksps clients of a 2.048 Msps cu8 stream, each a rational 3/128 filter
  * (create_rational_frequency_xlating_filter) with taps designed at 3 x 2.048 MHz with gain 3.
+ * `wide` and `cascade`: 48 ksps clients of a 61.44 Msps cu8 stream, the same channel two ways: `wide` a
+ * single-stage filter with D = 1280 and the server's own taps (cutoff rate / 2, transition rate / 5), `cascade`
+ * a 32 x 40 cascade filter (create_cascade_frequency_xlating_filter) with cascade_plan's taps: stage A passes
+ * to 3/5 of the rate and stops from 1.92 MHz - 6/5 of the rate, stage B is the server's design at 1.92 Msps.
+ * Both print the tap lengths they designed.
  *
  * The timed region starts after `warmup_blocks` (default 16) blocks have gone through the same
  * threads: a server's one-time start-up work -- the first CUDA call of every dsp thread, the
@@ -95,6 +100,8 @@ int main(int argc, char **argv) {
   g_warmup = argc > 4 ? atoi(argv[4]) : 16;
   if (g_warmup < 1) g_warmup = 1;
   const int rational = argc > 5 && strcmp(argv[5], "rational") == 0;
+  const int wide = argc > 5 && strcmp(argv[5], "wide") == 0;
+  const int cascade = argc > 5 && strcmp(argv[5], "cascade") == 0;
   g_clients = n_clients;
   g_blocks = n_blocks + g_warmup; /* warm-up blocks first, then the timed ones */
   pthread_barrier_init(&g_warm_barrier, NULL, (unsigned)n_clients + 1);
@@ -102,8 +109,9 @@ int main(int argc, char **argv) {
   g_queue = (sem_t *)calloc((size_t)n_clients, sizeof(sem_t));
   for (int c = 0; c < n_clients; c++) sem_init(&g_queue[c], 0, 0);
   sem_init(&g_sdr, 0, 0);
-  const uint32_t fs = rational ? 2048000 : 2016000;
+  const uint32_t fs = (wide || cascade) ? 61440000 : rational ? 2048000 : 2016000;
   const uint32_t interp = 3, decim = 128; /* rational: 2.048 MHz * 3 / 128 = 48 kHz */
+  const uint32_t d1 = 32, d2 = 40;        /* cascade: 61.44 MHz / 32 / 40 = 48 kHz */
   uint8_t *master[4];
   uint64_t s = 0x9E3779B97F4A7C15ull;
   for (int i = 0; i < 4; i++) {
@@ -117,7 +125,7 @@ int main(int argc, char **argv) {
   }
   client_t *clients = (client_t *)calloc((size_t)n_clients, sizeof(client_t));
   for (int c = 0; c < n_clients; c++) {
-    const uint32_t rate = (rational || c % 2 == 0) ? 48000 : 96000;
+    const uint32_t rate = (rational || wide || cascade || c % 2 == 0) ? 48000 : 96000;
     float *taps = NULL;
     size_t len = 0;
     const int32_t center = (int32_t)(-(int32_t)fs / 2 + (int32_t)rate / 2 +
@@ -126,8 +134,19 @@ int main(int argc, char **argv) {
     if (rational) {
       if (create_low_pass_filter((float)interp, interp * fs, rate / 2, rate / 5, &taps, &len) != 0) return 1;
       rc = create_rational_frequency_xlating_filter(interp, decim, taps, len, center, fs, BLOCK, &clients[c].filter);
+    } else if (cascade) {
+      const uint32_t fs1 = fs / d1, e = 3 * rate / 5;
+      float *taps2 = NULL;
+      size_t len2 = 0;
+      if (create_low_pass_filter(1.0f, fs, fs1 / 2, fs1 - 2 * e, &taps, &len) != 0 ||
+          create_low_pass_filter(1.0f, fs1, rate / 2, rate / 5, &taps2, &len2) != 0)
+        return 1;
+      if (c == 0) fprintf(stderr, "cascade %u x %u: taps %zu %zu\n", d1, d2, len, len2);
+      rc = create_cascade_frequency_xlating_filter(d1, taps, len, center, 1, d2, taps2, len2, fs, BLOCK,
+                                                   &clients[c].filter);
     } else {
       if (create_low_pass_filter(1.0f, fs, rate / 2, rate / 5, &taps, &len) != 0) return 1;
+      if (wide && c == 0) fprintf(stderr, "wide D = %u: taps %zu\n", fs / rate, len);
       rc = create_frequency_xlating_filter(fs / rate, taps, len, center, fs, BLOCK, &clients[c].filter);
     }
     if (rc != 0) {
@@ -186,7 +205,8 @@ int main(int argc, char **argv) {
          "\"outputs\": %llu, \"launch_batches\": %llu, \"engine_calls\": %llu, \"shared_inputs\": %llu, "
          "\"stream_served\": %llu, \"stream_blocks\": %llu, \"stream_hits\": %llu, \"stream_desyncs\": %llu, "
          "\"stream_joins\": %llu, \"stream_members\": %llu}\n",
-         rational ? "rational_3_128_of_2048k" : "integer_48k_96k_of_2016k", SIMD_STATUS, n_clients, n_blocks, g_window, dt, n_blocks * (BLOCK / 2) / dt / 1e6, (double)n_clients * n_blocks / dt,
+         rational ? "rational_3_128_of_2048k" : wide ? "wide_1280_of_61440k" : cascade ? "cascade_32x40_of_61440k"
+                  : "integer_48k_96k_of_2016k", SIMD_STATUS, n_clients, n_blocks, g_window, dt, n_blocks * (BLOCK / 2) / dt / 1e6, (double)n_clients * n_blocks / dt,
          dt / n_blocks * 1e6, (unsigned long long)outputs, (unsigned long long)batches, (unsigned long long)calls,
          (unsigned long long)shared, (unsigned long long)st[0], (unsigned long long)st[1], (unsigned long long)st[2],
          (unsigned long long)st[3], (unsigned long long)st[4], (unsigned long long)st[6]);
