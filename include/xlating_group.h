@@ -151,11 +151,40 @@ int xlg_add_client_cascade_rational(xlg_group *g, uint32_t decim1, const float *
                                     int32_t center_freq, uint32_t interp2, uint32_t decim2,
                                     const float *taps2, size_t taps2_len, int *client_id);
 int xlg_remove_client(xlg_group *g, int client_id);
+/* Extension: sub-band clients (DESIGN.md section 5, "Sub-band clients").  Many narrow clients near each other
+ * share one first stage instead of each running its own (a cascade client's stage A).
+ *   A SUB-BAND is create_frequency_xlating_filter(decim1, taps1, taps1_len, center_freq, fs, ...), fed the
+ *   group's blocks exactly as an xlg_add_client client is (same history, zero history before its attach
+ *   point, oscillator, renormalisation; XLG_NO_RENORM applies).  It has no host-visible output, its id comes
+ *   from a small-integer space of its own, and xlg_client_count does not count it.  Taps are copied.
+ *   -EINVAL (logged) for decim1 or taps1_len of 0, or fs % decim1 != 0 (a member's centre is in Hz at the
+ *   integer rate fs / decim1); -ENOTSUP (logged) on an XLG_TRACK_STATE group.  A group with a sub-band refuses
+ *   XLG_PATH_Q15 submits (-ENOTSUP, logged, nothing enqueued). */
+int xlg_add_subband(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, int32_t center_freq,
+                    int *subband_id);
+/* -EBUSY (logged) while the sub-band still has members; -EINVAL for an unknown id. */
+int xlg_remove_subband(xlg_group *g, int subband_id);
+/* A MEMBER of a sub-band is the float path (src/xlating.c:52-83) of create_frequency_xlating_filter(decim2,
+ * taps2, taps2_len, center_offset, fs / decim1, ...), fed the sub-band's cf32 outputs block by block, with
+ * taps2_len - 1 zeros of history at the block it is attached before (sub-band samples from before that block
+ * read as zero).  center_offset is its centre relative to the sub-band's, in Hz at fs / decim1; the group's
+ * XLG_NO_RENORM applies to it as well.  Its output per block is what xlg_output returns for its client id,
+ * and *out_len is known when xlg_submit returns.  *client_id is an ordinary client id: xlg_output,
+ * xlg_read_output, xlg_copy_output and xlg_remove_client work on it; xlg_client_info reports kind 6.  Taps
+ * are copied.  -EINVAL (logged) for decim2 or taps2_len of 0, an unknown sub-band, or taps and a window too
+ * long for the member kernel's shared memory (17 * taps2_len + 63 * decim2 <= about 25600). */
+int xlg_add_client_subband(xlg_group *g, int subband_id, uint32_t decim2, const float *taps2, size_t taps2_len,
+                           int32_t center_offset, int *client_id);
+/* A member's sub-band, the kind (0, 1 or 2, as xlg_client_info) of the kernel serving the sub-band, and the
+ * member's history_offset in sub-band samples.  -EINVAL for any client that is not a member. */
+int xlg_subband_info(const xlg_group *g, int client_id, int *subband_id, int *stage_a_kind, size_t *member_history);
 /* Size the per-ticket result arenas (device and pinned host) for `output_samples_per_block` complex output
  * samples per block summed over all clients (a client at decimation D produces about max_input_len/2/D + 2).
  * A cascade client counts two rows, each rounded up to a multiple of 4 samples: its stage-A row of
  * n1 = max_input_len/2/decim1 + 2 samples, which stays on the device, and its final row of
- * floor(n1 * interp2 / decim2) + 2 (interp2 = 1 for xlg_add_client_cascade).
+ * floor(n1 * interp2 / decim2) + 2 (interp2 = 1 for xlg_add_client_cascade).  A sub-band counts one row of
+ * n1 = max_input_len/2/decim1 + 2 samples, rounded up to 4, which stays on the device; a member counts its
+ * final row of floor(n1 / decim2) + 2, rounded up to 4.
  * Optional: the arenas grow on demand when clients are added, but a growth re-allocates every ring entry and
  * the results still waiting in the ring are lost (-ESTALE for consumers that had not read them yet, like a
  * block overwritten in the reference's queue).  A server that knows its client limit reserves once, up front. */
@@ -255,11 +284,21 @@ typedef struct {
 } xlg_cascade_profile;
 int xlg_cascade_profile_read(xlg_group *g, xlg_cascade_profile *p, int reset);
 
+/* Sub-band members (xlg_add_client_subband), counted like xlg_profile's while profiling is enabled.
+ * xlg_profile counts each sub-band's first stage once, as the integer client it is. */
+typedef struct {
+  double member_ms;          /* the sub-band ring appends, the member oscillators and the member kernel */
+  uint64_t member_launches;
+  uint64_t member_macs;      /* complex MACs of the members: sum n2 * taps2_len */
+  uint64_t row_samples;      /* sub-band samples produced (and appended to the rings) */
+} xlg_subband_profile;
+int xlg_subband_profile_read(xlg_group *g, xlg_subband_profile *p, int reset);
+
 /* Introspection for tests: history length (src/xlating.c:29 history_offset; upsampled samples for a
  * rational client, stage A's for a cascade client) and which kernel currently serves the client
  * (0 = generic, 1 = tiled, 2 = long-filter split-K, 3 = rational, polyphase generic, 4 = rational, tiled: at
  * least 8 clients with identical (interp, decim, taps_len, window alignment), gcd(interp, decim) = 1, whose
- * branches fit the tiled kernel's shared memory, 5 = cascade). */
+ * branches fit the tiled kernel's shared memory, 5 = cascade, 6 = sub-band member). */
 int xlg_client_info(const xlg_group *g, int client_id, size_t *history, int *kernel_kind);
 /* A cascade client's stages: the kind (0, 1 or 2, as xlg_client_info) of the kernel serving stage A, and the
  * history_offset of each stage (stage B's in stage-A samples, upsampled by interp2 for a rational cascade

@@ -55,7 +55,7 @@ DROPIN_EXTENSION_SYMBOLS = ["create_rational_frequency_xlating_filter", "create_
 GROUP_SYMBOLS = [
     "xlg_create", "xlg_create_ex", "xlg_destroy", "xlg_add_client", "xlg_add_client_ex", "xlg_add_client_rational_ex", "xlg_remove_client", "xlg_reserve", "xlg_client_count", "xlg_submit",
     "xlg_wait", "xlg_input_consumed", "xlg_output", "xlg_read_output", "xlg_copy_output", "xlg_alloc_pinned", "xlg_free_pinned", "xlg_wait_stream", "xlg_partition_active", "xlg_timer_start",
-    "xlg_timer_stop", "xlg_profile_enable", "xlg_profile_read", "xlg_client_info", "xlg_add_client_rational", "xlg_poly_profile_read", "xlg_add_client_cascade", "xlg_add_client_cascade_rational", "xlg_cascade_info", "xlg_cascade_profile_read", "xlg_dropin_stats", "xlg_dropin_stream_stats", "xlg_dropin_stream_times",
+    "xlg_timer_stop", "xlg_profile_enable", "xlg_profile_read", "xlg_client_info", "xlg_add_client_rational", "xlg_poly_profile_read", "xlg_add_client_cascade", "xlg_add_client_cascade_rational", "xlg_cascade_info", "xlg_cascade_profile_read", "xlg_add_subband", "xlg_remove_subband", "xlg_add_client_subband", "xlg_subband_info", "xlg_subband_profile_read", "xlg_dropin_stats", "xlg_dropin_stream_stats", "xlg_dropin_stream_times",
 ]
 
 
@@ -83,6 +83,11 @@ class XlgPolyProfile(C.Structure):
 class XlgCascadeProfile(C.Structure):
     _fields_ = [("stage_b_ms", C.c_double), ("stage_b_launches", C.c_uint64), ("stage_b_macs", C.c_uint64),
                 ("d2h_bytes", C.c_uint64)]
+
+
+class XlgSubbandProfile(C.Structure):
+    _fields_ = [("member_ms", C.c_double), ("member_launches", C.c_uint64), ("member_macs", C.c_uint64),
+                ("row_samples", C.c_uint64)]
 
 
 def build(verbose: bool = False) -> None:
@@ -147,6 +152,16 @@ def lib() -> C.CDLL:
     L.xlg_cascade_info.restype = C.c_int
     L.xlg_cascade_profile_read.argtypes = [vp, C.POINTER(XlgCascadeProfile), C.c_int]
     L.xlg_cascade_profile_read.restype = C.c_int
+    L.xlg_add_subband.argtypes = [vp, u32, fp, sz, i32, C.POINTER(C.c_int)]
+    L.xlg_add_subband.restype = C.c_int
+    L.xlg_remove_subband.argtypes = [vp, C.c_int]
+    L.xlg_remove_subband.restype = C.c_int
+    L.xlg_add_client_subband.argtypes = [vp, C.c_int, u32, fp, sz, i32, C.POINTER(C.c_int)]
+    L.xlg_add_client_subband.restype = C.c_int
+    L.xlg_subband_info.argtypes = [vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(sz)]
+    L.xlg_subband_info.restype = C.c_int
+    L.xlg_subband_profile_read.argtypes = [vp, C.POINTER(XlgSubbandProfile), C.c_int]
+    L.xlg_subband_profile_read.restype = C.c_int
     L.xl_poly_pack.argtypes = [C.POINTER(C.c_float), sz, u32, C.POINTER(C.c_float)]
     L.xl_poly_pack.restype = None
     L.xlg_reserve.argtypes = [vp, sz]
@@ -396,6 +411,41 @@ class Group:
             raise ValueError(code)
         return kind.value, h1.value, h2.value
 
+    def add_subband(self, decim1: int, taps1, center_freq: int) -> int:
+        """A sub-band (include/xlating_group.h, xlg_add_subband): the reference filter (decim1, taps1,
+        center_freq) at fs, shared by its members and invisible to the caller.  Returns a sub-band id."""
+        t1 = np.ascontiguousarray(taps1, dtype=np.float32)
+        sid = C.c_int(-1)
+        code = self._L.xlg_add_subband(self._h, decim1, t1.ctypes.data_as(C.POINTER(C.c_float)), len(t1),
+                                       center_freq, C.byref(sid))
+        if code != 0:
+            raise ValueError(code)
+        return sid.value
+
+    def remove_subband(self, sid: int) -> None:
+        code = self._L.xlg_remove_subband(self._h, sid)
+        if code != 0:
+            raise ValueError(code)
+
+    def add_client_subband(self, sid: int, decim2: int, taps2, center_offset: int) -> int:
+        """A member of sub-band `sid` (xlg_add_client_subband): the reference's float path (decim2, taps2,
+        center_offset) at fs / decim1 fed the sub-band's outputs.  Returns an ordinary client id."""
+        t2 = np.ascontiguousarray(taps2, dtype=np.float32)
+        cid = C.c_int(-1)
+        code = self._L.xlg_add_client_subband(self._h, sid, decim2, t2.ctypes.data_as(C.POINTER(C.c_float)),
+                                              len(t2), center_offset, C.byref(cid))
+        if code != 0:
+            raise ValueError(code)
+        return cid.value
+
+    def subband_info(self, cid: int):
+        """(sub-band id, kind of the kernel serving the sub-band, member history in sub-band samples)."""
+        sid, kind, h = C.c_int(0), C.c_int(0), C.c_size_t(0)
+        code = self._L.xlg_subband_info(self._h, cid, C.byref(sid), C.byref(kind), C.byref(h))
+        if code != 0:
+            raise ValueError(code)
+        return sid.value, kind.value, h.value
+
     def remove_client(self, cid: int) -> None:
         code = self._L.xlg_remove_client(self._h, cid)
         if code != 0:
@@ -525,6 +575,11 @@ class Group:
         p = XlgCascadeProfile()
         self._L.xlg_cascade_profile_read(self._h, C.byref(p), 1 if reset else 0)
         return {k: getattr(p, k) for k, _ in XlgCascadeProfile._fields_}
+
+    def subband_profile_read(self, reset: bool = True) -> dict:
+        p = XlgSubbandProfile()
+        self._L.xlg_subband_profile_read(self._h, C.byref(p), 1 if reset else 0)
+        return {k: getattr(p, k) for k, _ in XlgSubbandProfile._fields_}
 
     def close(self):
         if self._h:
@@ -659,6 +714,53 @@ def cascade_plan(fs: int, rates):
         plan.append({"rate": rate, "d1": d1, "interp2": L2, "d2": M2, "center": p["center"], "taps1": t1,
                      "taps2": t2, "fmas": cost})
     return plan
+
+
+def subband_fmas(fs: int, d1: int, t1: int, n_subbands: int, members) -> float:
+    """Algorithmic real FMAs per input sample of a sub-band plan: 4 per complex tap of each sub-band at
+    fs / d1, and 4 per complex tap of each member at its own rate.  members: (rate, t2) pairs."""
+    return 4.0 * n_subbands * t1 / d1 + sum(4.0 * t2 * rate / fs for rate, t2 in members)
+
+
+def subband_plan(fs: int, clients):
+    """Sub-band clients for `clients`, a list of (center, rate).  For every D1 >= 2 that divides fs with
+    fs1 = fs / D1 even, fs1 > 2 * max rate and every rate dividing fs1: sub-band centres fs1 / 2 apart from
+    the lowest client centre up across the occupied span, each client assigned to the nearest one (so its
+    offset |c2| <= fs1 / 4), the sub-bands designed with create_low_pass_filter(1, fs, fs1 / 2, fs1 - 2e),
+    e = fs1 / 4 + max rate / 2 (it passes everything a member reads, and everything it aliases lands outside
+    [-e, e]), the members with the server's own taps at fs1 (cutoff rate / 2, transition rate / 5).  Of
+    these, the D1 with the fewest FMAs per input sample (subband_fmas, counting only sub-bands with members;
+    ties go to the smaller D1).  Returns {"d1", "taps1", "e", "subbands": [{"center"}], "members": [{"subband",
+    "center", "rate", "d2", "offset", "taps2"}] in the order of `clients`, "fmas"}."""
+    centers = [int(c) for c, _ in clients]
+    rates = [int(r) for _, r in clients]
+    rmax = max(rates)
+    lo, hi = min(centers), max(centers)
+    best = None
+    for d1 in range(2, fs // (2 * rmax) + 1):
+        if fs % d1:
+            continue
+        fs1 = fs // d1
+        if fs1 % 2 or fs1 <= 2 * rmax or any(fs1 % r for r in rates):
+            continue
+        half = fs1 // 2
+        n_cent = (hi - lo + half - 1) // half + 1
+        assign = [min(range(n_cent), key=lambda k: abs(c - (lo + k * half))) for c in centers]
+        used = sorted(set(assign))
+        e = fs1 // 4 + rmax // 2
+        t1 = create_low_pass_filter(1.0, fs, fs1 // 2, fs1 - 2 * e)
+        designs = {r: create_low_pass_filter(1.0, fs1, r // 2, r // 5) for r in set(rates)}
+        cost = subband_fmas(fs, d1, t1.size, len(used), [(r, designs[r].size) for r in rates])
+        if best is None or cost < best[0]:
+            best = (cost, d1, fs1, half, e, t1, designs, used, assign)
+    if best is None:
+        raise ValueError(f"{fs} has no divisor D1 >= 2 whose sub-band rate serves the rates {sorted(set(rates))}")
+    cost, d1, fs1, half, e, t1, designs, used, assign = best
+    index = {k: i for i, k in enumerate(used)}
+    subbands = [{"center": lo + k * half} for k in used]
+    members = [{"subband": index[k], "center": c, "rate": r, "d2": fs1 // r, "offset": c - (lo + k * half),
+                "taps2": designs[r]} for c, r, k in zip(centers, rates, assign)]
+    return {"d1": d1, "fs1": fs1, "taps1": t1, "e": e, "subbands": subbands, "members": members, "fmas": cost}
 
 
 # ---------------------------------------------------------------------------

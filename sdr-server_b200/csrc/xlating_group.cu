@@ -16,6 +16,9 @@
  *                    oscillator table, output arena (+ pinned host mirrors)
  *   cascade clients  a stage-A history ring each (HostClient::d_cring), their stage-B taps
  *                    (d_taps2); stage-A rows follow the host-visible rows of the arena
+ *   sub-bands        a history ring each (HostClient::d_cring), rows after the host-visible ones;
+ *                    their members' taps packed per group of SB_MG (d_sbtaps, SbGroup), and per
+ *                    slot the members' oscillator table (d_sbph)
  *
  * Streams: s_in (H2D), s_ph (oscillator pre-pass chain), s_cs[0..n_cs) (convert + FIR,
  * round-robin by block; 3 by default, XLATING_B200_CSTREAMS=1..4), s_out (D2H); events order them per block so block b+1's
@@ -28,6 +31,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <errno.h>
+#include <limits.h>
 #include <sched.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -126,6 +130,25 @@ struct HostClient {
   int fin_off = 0, fin_cap = 0;  // final row of the slot's output arena
   int taps2_off = 0;             // rev2 in the real tap arena
   int last_n2 = 0;               // stage-B outputs of the block being submitted
+  // sub-band (xlg_add_subband): an integer client, not visible to the caller, whose row lies after every
+  // host-visible row; d_cring, cring_cap and a_pos above are its history ring
+  bool sb = false;
+  int sb_id = -1;
+  // sub-band member (xlg_add_client_subband): not an integer client -- its ClientDev only carries its
+  // oscillator; D2, T2, hist2 (in sub-band samples) and last_n2 above are its own, rev2 holds its rotated
+  // reversed taps (2 * T2 floats), out_off / out_cap its final row
+  bool mem = false;
+  int sb_cid = -1;               // its sub-band's client index
+  long long zb2 = 0;             // sub-band position of its attach point: earlier samples read as zero
+  int ph_row = 0;                // its rows of the slot's member oscillator table
+};
+
+// members of one sub-band that read the same windows: equal (D2, T2, hist2) and, until their windows have
+// passed it, the same attach point
+struct SbClassHost {
+  int sb_cid;
+  std::vector<int> members;
+  long long zb;  // the largest attach point of its members
 };
 
 struct Slot {
@@ -155,6 +178,14 @@ struct Slot {
   cudaEvent_t pf_casc[2] = {nullptr, nullptr};
   bool pf_cb = false;
   uint64_t casc_macs = 0, d2h_bytes = 0;
+  CascBlk *d_sbcb = nullptr, *h_sbcb = nullptr;  // sub-bands: this block's ring appends
+  size_t sbcb_cap = 0;
+  SbBlk *d_sbblk = nullptr, *h_sbblk = nullptr;  // member classes: this block's windows and counts
+  size_t sbblk_cap = 0;
+  float2 *d_sbph = nullptr;                      // member oscillator table (HostClient::ph_row)
+  cudaEvent_t pf_sb[2] = {nullptr, nullptr};
+  bool pf_sbk = false;
+  uint64_t sb_macs = 0, sb_rows = 0;
   std::atomic<int64_t> ticket{-1};
   bool q15 = false;
   bool harvested = true;
@@ -351,8 +382,17 @@ struct xlg_group {
   int n_casc = 0;                           // active cascade clients
   int n_casc_int = 0;                       // of which integer stage B (their CascBlk entries come first)
   std::vector<float2 *> dead_rings;         // rings of removed cascade clients, freed once the pipeline is drained
-  cudaEvent_t ev_last_casc = nullptr;       // ev_casc of the last block with cascade clients
+  cudaEvent_t ev_last_casc = nullptr;       // ev_casc of the last block with cascade clients or sub-bands
   bool have_last_casc = false;
+  std::vector<int> subbands;                // sub-band id -> client index (-1 = free)
+  std::vector<int> sb_list;                 // active sub-bands' client indices (their appends, in this order)
+  std::vector<SbClassHost> sb_classes;
+  int n_sb_mem = 0, n_sb_groups = 0;
+  SbGroup *d_sbgrp = nullptr;
+  SbMem *d_sbmem = nullptr;
+  float2 *d_sbtaps = nullptr;
+  size_t cap_sbgrp = 0, cap_sbmem = 0, cap_sbtaps = 0, sbph_cap = 0;
+  xlg_subband_profile sb_prof;
   int n_generic = 0;
   int max_client = 0;     // highest active id + 1
   bool dirty = true;
@@ -418,6 +458,15 @@ static void slot_free(Slot &s) {
   if (s.h_pblk) cudaFreeHost(s.h_pblk);
   s.d_pblk = s.h_pblk = nullptr;
   s.pblk_cap = 0;
+  if (s.d_sbcb) cudaFree(s.d_sbcb);
+  if (s.h_sbcb) cudaFreeHost(s.h_sbcb);
+  if (s.d_sbblk) cudaFree(s.d_sbblk);
+  if (s.h_sbblk) cudaFreeHost(s.h_sbblk);
+  if (s.d_sbph) cudaFree(s.d_sbph);
+  s.d_sbcb = s.h_sbcb = nullptr;
+  s.d_sbblk = s.h_sbblk = nullptr;
+  s.d_sbph = nullptr;
+  s.sbcb_cap = s.sbblk_cap = 0;
   s.d_pscratch = nullptr;
   s.d_vblk = s.h_vblk = nullptr;
   s.d_endph = nullptr;
@@ -493,6 +542,12 @@ static void harvest_locked(xlg_group *g, Slot &s) {
   }
   g->casc_prof.stage_b_macs += s.casc_macs;
   g->casc_prof.d2h_bytes += s.d2h_bytes;
+  if (s.pf_sbk && cudaEventElapsedTime(&ms, s.pf_sb[0], s.pf_sb[1]) == cudaSuccess) {
+    g->sb_prof.member_ms += ms;
+    g->sb_prof.member_launches++;
+  }
+  g->sb_prof.member_macs += s.sb_macs;
+  g->sb_prof.row_samples += s.sb_rows;
   g->prof.blocks++;
   g->prof.out_samples += s.out_samples;
   g->prof.in_samples += s.in_samples;
@@ -626,6 +681,141 @@ static long long first_input(const HostClient &h, long long S) {
 static bool poly_settled(const xlg_group *g, const HostClient &h) {
   return (h.zero_before == 0 && g->S < (long long)g->ring_cap / 2) || h.zero_before <= first_input(h, g->S);
 }
+// Sub-bands and their members (the pipeline is drained): sub-band rows after every host-visible row (the
+// D2H copy ends before them), one zeroed history ring per sub-band, grown when a longer member attaches,
+// the member classes, their groups of SB_MG members with packed taps, and the per-slot tables.
+static int rebuild_subbands(xlg_group *g, size_t &out_total) {
+  g->sb_list.clear();
+  g->sb_classes.clear();
+  g->n_sb_mem = g->n_sb_groups = 0;
+  const int nc = (int)g->clients.size();
+  for (int i = 0; i < nc; i++)
+    if (g->clients[i].active && g->clients[i].sb) g->sb_list.push_back(i);
+  if (g->sb_list.empty()) return 0;
+  CU_OK(cudaFuncSetAttribute(subband_fir_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem));
+  std::vector<size_t> back(nc, 0);  // longest member history per sub-band
+  std::map<std::tuple<int, uint32_t, size_t, long long, long long>, std::vector<int>> keyed;
+  for (int i = 0; i < nc; i++) {
+    const HostClient &h = g->clients[i];
+    if (!h.active || !h.mem) continue;
+    back[h.sb_cid] = std::max(back[h.sb_cid], h.T2 - 1);
+    // its window has passed its attach point: it reads what every settled member of the class reads
+    const bool settled = h.zb2 <= g->clients[h.sb_cid].a_pos - h.hist2;
+    keyed[std::make_tuple(h.sb_cid, h.D2, h.T2, h.hist2, settled ? LLONG_MIN : h.zb2)].push_back(i);
+  }
+  for (int i : g->sb_list) {
+    HostClient &h = g->clients[i];
+    h.out_off = (int)out_total;
+    out_total += (size_t)h.out_cap;
+    out_total = (out_total + 3) & ~(size_t)3;
+    // a member of block b reads sub-band samples of earlier blocks; the submit of block b + XLG_SLOTS waits
+    // for ticket b, so T2 - 1 + (XLG_SLOTS + 1) * max n1 samples are never overwritten while still needed
+    const size_t cap = next_pow2(back[i] + (size_t)(XLG_SLOTS + 1) * (size_t)h.out_cap);
+    if (h.d_cring != nullptr && cap <= h.cring_cap) continue;
+    float2 *ring = nullptr;
+    CU_OK(cudaMalloc(&ring, cap * sizeof(float2)));
+    std::vector<float2> fresh(cap, make_float2(0.f, 0.f));
+    if (h.d_cring != nullptr) {
+      // grow: the last cring_cap positions keep their samples at their new places
+      std::vector<float2> old(h.cring_cap);
+      CU_OK(cudaMemcpy(old.data(), h.d_cring, h.cring_cap * sizeof(float2), cudaMemcpyDeviceToHost));
+      for (size_t k = 1; k <= h.cring_cap; k++) {
+        const unsigned long long p = (unsigned long long)(h.a_pos - (long long)k);
+        fresh[p & (cap - 1)] = old[p & (h.cring_cap - 1)];
+      }
+      cudaFree(h.d_cring);
+    }
+    CU_OK(cudaMemcpy(ring, fresh.data(), cap * sizeof(float2), cudaMemcpyHostToDevice));
+    h.d_cring = ring;
+    h.cring_cap = cap;
+  }
+  std::vector<SbGroup> groups;
+  std::vector<SbMem> mems;
+  std::vector<float2> taps;
+  for (auto &kv : keyed) {
+    const int cls = (int)g->sb_classes.size();
+    SbClassHost ch;
+    ch.sb_cid = std::get<0>(kv.first);
+    ch.members = kv.second;
+    ch.zb = LLONG_MIN;
+    const int T2 = (int)std::get<2>(kv.first), tpad = sb_tpad(T2);
+    for (size_t m0 = 0; m0 < ch.members.size(); m0 += SB_MG) {
+      SbGroup gp;
+      memset(&gp, 0, sizeof(gp));
+      gp.cls = cls;
+      gp.n_mem = (int)std::min<size_t>(SB_MG, ch.members.size() - m0);
+      gp.taps_off = (int)taps.size();
+      taps.resize(taps.size() + (size_t)SB_MG * tpad, make_float2(0.f, 0.f));
+      for (int m = 0; m < gp.n_mem; m++) {
+        HostClient &h = g->clients[ch.members[m0 + m]];
+        memcpy(&taps[gp.taps_off + (size_t)m * tpad], h.rev2.data(), h.rev2.size() * sizeof(float));
+        mems.push_back(SbMem{ch.members[m0 + m], cls, 0});
+        ch.zb = std::max(ch.zb, h.zb2);
+      }
+      groups.push_back(gp);
+    }
+    g->sb_classes.push_back(ch);
+  }
+  // oscillator table: groups of 32 members in SbMem order, phase of even output k of slot l at
+  // base + 32 * (k / 2) + l
+  size_t rows = 0;
+  for (size_t base = 0; base < mems.size(); base += 32) {
+    int cap = 0;
+    for (size_t i = base; i < std::min(base + 32, mems.size()); i++) cap = std::max(cap, g->clients[mems[i].cid].out_cap);
+    for (size_t i = base; i < std::min(base + 32, mems.size()); i++) {
+      mems[i].ph_off = (int)(rows + (i - base));
+      g->clients[mems[i].cid].ph_row = mems[i].ph_off;
+    }
+    rows += (size_t)(cap / 2 + 1) * 32;
+  }
+  {
+    size_t i = 0;
+    for (SbGroup &gp : groups)
+      for (int m = 0; m < gp.n_mem; m++, i++) {
+        const HostClient &h = g->clients[mems[i].cid];
+        gp.out_off[m] = h.out_off;
+        gp.ph_off[m] = h.ph_row;
+        gp.incr[m] = make_float2(h.incr_re, h.incr_im);
+      }
+  }
+  g->n_sb_mem = (int)mems.size();
+  while (mems.size() % 32 != 0) mems.push_back(SbMem{-1, 0, 0});
+  g->n_sb_groups = (int)groups.size();
+  if (dev_assign(&g->d_sbgrp, &g->cap_sbgrp, groups.data(), groups.size() * sizeof(SbGroup)) ||
+      dev_assign(&g->d_sbmem, &g->cap_sbmem, mems.data(), mems.size() * sizeof(SbMem)) ||
+      dev_assign(&g->d_sbtaps, &g->cap_sbtaps, taps.data(), taps.size() * sizeof(float2)))
+    return -EIO;
+  const size_t n_sb = g->sb_list.size(), n_cls = g->sb_classes.size();
+  const bool grow_ph = rows > g->sbph_cap;
+  if (grow_ph) g->sbph_cap = rows + rows / 4 + 1024;
+  for (Slot &s : g->slots) {
+    if (s.pf_sb[0] == nullptr)
+      for (cudaEvent_t &ev : s.pf_sb) CU_OK(cudaEventCreate(&ev));
+    if (s.sbcb_cap < n_sb) {
+      if (s.d_sbcb) cudaFree(s.d_sbcb);
+      if (s.h_sbcb) cudaFreeHost(s.h_sbcb);
+      s.d_sbcb = s.h_sbcb = nullptr;
+      s.sbcb_cap = std::max<size_t>(n_sb * 2, 16);
+      CU_OK(cudaMalloc(&s.d_sbcb, s.sbcb_cap * sizeof(CascBlk)));
+      CU_OK(cudaHostAlloc(&s.h_sbcb, s.sbcb_cap * sizeof(CascBlk), cudaHostAllocDefault));
+    }
+    if (s.sbblk_cap < n_cls) {
+      if (s.d_sbblk) cudaFree(s.d_sbblk);
+      if (s.h_sbblk) cudaFreeHost(s.h_sbblk);
+      s.d_sbblk = s.h_sbblk = nullptr;
+      s.sbblk_cap = std::max<size_t>(n_cls * 2, 16);
+      CU_OK(cudaMalloc(&s.d_sbblk, s.sbblk_cap * sizeof(SbBlk)));
+      CU_OK(cudaHostAlloc(&s.h_sbblk, s.sbblk_cap * sizeof(SbBlk), cudaHostAllocDefault));
+    }
+    if ((grow_ph || s.d_sbph == nullptr) && g->sbph_cap > 0) {
+      if (s.d_sbph) cudaFree(s.d_sbph);
+      s.d_sbph = nullptr;
+      CU_OK(cudaMalloc(&s.d_sbph, g->sbph_cap * sizeof(float2)));
+    }
+  }
+  return 0;
+}
+
 static int rebuild_layout(xlg_group *g) {
   // XLATING_B200_REBUILD_TIMING=1: where a re-layout spends its time (logged per call)
   static const bool timing = getenv("XLATING_B200_REBUILD_TIMING") != nullptr;
@@ -658,13 +848,21 @@ static int rebuild_layout(xlg_group *g) {
   for (int i = 0; i < nc; i++) {
     HostClient &h = g->clients[i];
     if (!h.active) continue;
+    if (h.mem) {
+      // n2 <= (n1 - 1) / D2 + 1 for any history, n1 at most its sub-band's row
+      h.out_cap = (int)(((uint64_t)g->max_input_len / 2 / g->clients[h.sb_cid].D + 2) / h.D2 + 2);
+      h.out_off = (int)out_total;
+      out_total += (size_t)h.out_cap;
+      out_total = (out_total + 3) & ~(size_t)3;
+      continue;
+    }
     h.out_cap = (int)((uint64_t)g->max_input_len / 2 * h.L / h.D + 2);
     if (h.casc) {
       // n2 <= (L2 * n1 - 1) / D2 + 1 for any history
       h.fin_cap = (int)((uint64_t)h.out_cap * h.L2 / h.D2 + 2);
       h.fin_off = (int)out_total;
       out_total += (size_t)h.fin_cap;
-    } else {
+    } else if (!h.sb) {
       h.out_off = (int)out_total;
       out_total += (size_t)h.out_cap;
     }
@@ -724,6 +922,7 @@ static int rebuild_layout(xlg_group *g) {
       CU_OK(cudaHostAlloc(&s.h_pblk, s.pblk_cap * sizeof(CascPolyBlk), cudaHostAllocDefault));
     }
   }
+  if (rebuild_subbands(g, out_total)) return -EIO;
   if (ensure_ring(g, max_hist, g->qring != nullptr)) return -EIO;
   if (ensure_arenas(g, out_total, g->q_alloc)) return -EIO;
 
@@ -785,6 +984,10 @@ static int rebuild_layout(xlg_group *g) {
   for (int i = 0; i < nc; i++) {
     HostClient &h = g->clients[i];
     if (!h.active) continue;
+    if (h.mem) {
+      h.kind = 6;  // served by subband_fir_cf32_kernel
+      continue;
+    }
     h.kind = h.L > 1 ? 3 : 0;
     h.tile_ineligible = false;
     h.pending_settle = false;
@@ -1051,7 +1254,8 @@ static int rebuild_layout(xlg_group *g) {
     }
     std::vector<int> loose;
     for (int i = 0; i < nc; i++)
-      if (g->clients[i].active && (g->clients[i].kind == 0 || g->clients[i].kind >= 3)) loose.push_back(i);
+      if (g->clients[i].active && !g->clients[i].mem && (g->clients[i].kind == 0 || g->clients[i].kind >= 3))
+        loose.push_back(i);
     for (size_t base = 0; base < loose.size(); base += 32) {
       int cap = 0;
       for (size_t m = base; m < std::min(base + 32, loose.size()); m++) cap = std::max(cap, g->clients[loose[m]].out_cap);
@@ -1149,7 +1353,7 @@ static int rebuild_layout(xlg_group *g) {
     d.qtaps_off = h.taps_off;
     d.out_off = h.out_off;
     d.out_cap = h.out_cap;
-    d.active = 1;
+    d.active = h.mem ? 0 : 1;  // a member's entry only carries its oscillator (subband_phase_kernel)
     d.kind = h.kind;
     d.renorm = (g->flags & XLG_NO_RENORM) ? 0 : 1;
     d.ph_off = h.ph_off;
@@ -1236,7 +1440,7 @@ static void choose_partition(xlg_group *g) {
     const double n = (double)(g->max_input_len / 2);
     double steps = 0, fma = 0;
     for (const HostClient &h : g->clients) {
-      if (!h.active) continue;
+      if (!h.active || h.mem) continue;
       const double n_out = n * h.L / (double)h.D;
       steps = std::max(steps, n_out);
       fma += 4.0 * n_out * (double)((h.T + h.L - 1) / h.L);
@@ -1366,6 +1570,7 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
   memset(&g->prof, 0, sizeof(g->prof));
   memset(&g->poly_prof, 0, sizeof(g->poly_prof));
   memset(&g->casc_prof, 0, sizeof(g->casc_prof));
+  memset(&g->sb_prof, 0, sizeof(g->sb_prof));
   g->device = device;
   g->fs = sampling_freq;
   g->max_input_len = max_input_len;
@@ -1547,6 +1752,8 @@ extern "C" void xlg_destroy(xlg_group *g) {
     for (cudaEvent_t ev : s.pf_casc)
       if (ev) cudaEventDestroy(ev);
     if (s.ev_casc) cudaEventDestroy(s.ev_casc);
+    for (cudaEvent_t ev : s.pf_sb)
+      if (ev) cudaEventDestroy(ev);
   }
   for (HostOut &h : g->ring_out) {
     if (h.h_out) cudaFreeHost(h.h_out);
@@ -1576,6 +1783,9 @@ extern "C" void xlg_destroy(xlg_group *g) {
   if (g->d_poly4) cudaFree(g->d_poly4);
   if (g->d_ones) cudaFree(g->d_ones);
   if (g->d_taps2) cudaFree(g->d_taps2);
+  if (g->d_sbgrp) cudaFree(g->d_sbgrp);
+  if (g->d_sbmem) cudaFree(g->d_sbmem);
+  if (g->d_sbtaps) cudaFree(g->d_sbtaps);
   for (HostClient &h : g->clients)
     if (h.d_cring) cudaFree(h.d_cring);
   for (float2 *p : g->dead_rings) cudaFree(p);
@@ -1777,7 +1987,8 @@ extern "C" int xlg_reserve(xlg_group *g, size_t output_samples_per_block) {
 }
 
 extern "C" int xlg_remove_client(xlg_group *g, int client_id) {
-  if (g == nullptr || client_id < 0 || client_id >= (int)g->clients.size() || !g->clients[client_id].active)
+  if (g == nullptr || client_id < 0 || client_id >= (int)g->clients.size() || !g->clients[client_id].active ||
+      g->clients[client_id].sb)
     return -EINVAL;
   g->clients[client_id].active = false;
   if (g->clients[client_id].d_cring) g->dead_rings.push_back(g->clients[client_id].d_cring);  // in-flight tickets read it
@@ -1792,14 +2003,15 @@ extern "C" int xlg_remove_client(xlg_group *g, int client_id) {
 extern "C" int xlg_client_count(const xlg_group *g) {
   if (g == nullptr) return -EINVAL;
   int n = 0;
-  for (const HostClient &h : g->clients) n += h.active ? 1 : 0;
+  for (const HostClient &h : g->clients) n += h.active && !h.sb ? 1 : 0;
   return n;
 }
 
 extern "C" int xlg_client_info(const xlg_group *g, int client_id, size_t *history, int *kernel_kind) {
-  if (g == nullptr || client_id < 0 || client_id >= (int)g->clients.size() || !g->clients[client_id].active)
+  if (g == nullptr || client_id < 0 || client_id >= (int)g->clients.size() || !g->clients[client_id].active ||
+      g->clients[client_id].sb)
     return -EINVAL;
-  if (history) *history = (size_t)g->clients[client_id].hist;
+  if (history) *history = (size_t)(g->clients[client_id].mem ? g->clients[client_id].hist2 : g->clients[client_id].hist);
   if (kernel_kind) *kernel_kind = g->clients[client_id].casc ? 5 : g->clients[client_id].kind;
   return 0;
 }
@@ -1813,6 +2025,122 @@ extern "C" int xlg_cascade_info(const xlg_group *g, int client_id, int *stage_a_
   if (stage_a_kind) *stage_a_kind = h.kind;
   if (stage_a_history) *stage_a_history = (size_t)h.hist;
   if (stage_b_history) *stage_b_history = (size_t)h.hist2;
+  return 0;
+}
+
+extern "C" int xlg_add_subband(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len,
+                               int32_t center_freq, int *subband_id) {
+  if (g == nullptr || subband_id == nullptr) return -EINVAL;
+  if (decim1 == 0 || taps1_len == 0 || taps1 == nullptr) {
+    XL_LOG("sub-band: decimation %u and tap count %zu must both be at least 1", decim1, taps1_len);
+    return -EINVAL;
+  }
+  if (g->fs % decim1 != 0) {
+    XL_LOG("sub-band: decimation %u does not divide the band rate %u (members are centred in Hz at fs / decim1)",
+           decim1, g->fs);
+    return -EINVAL;
+  }
+  if (g->flags & XLG_TRACK_STATE) {
+    XL_LOG("sub-band: an XLG_TRACK_STATE group cannot carry the state of two stages");
+    return -ENOTSUP;
+  }
+  int cid = -1;
+  const int rc = attach_client(g, 1, decim1, g->fs, taps1, taps1_len, center_freq, nullptr, &cid);
+  if (rc) return rc;
+  int id = 0;
+  while (id < (int)g->subbands.size() && g->subbands[id] >= 0) id++;
+  if (id == (int)g->subbands.size()) g->subbands.push_back(-1);
+  g->subbands[id] = cid;
+  g->clients[cid].sb = true;
+  g->clients[cid].sb_id = id;
+  *subband_id = id;
+  return 0;
+}
+
+static int subband_client(const xlg_group *g, int subband_id) {
+  if (subband_id < 0 || subband_id >= (int)g->subbands.size()) return -1;
+  return g->subbands[subband_id];
+}
+
+extern "C" int xlg_remove_subband(xlg_group *g, int subband_id) {
+  if (g == nullptr) return -EINVAL;
+  const int cid = subband_client(g, subband_id);
+  if (cid < 0) {
+    XL_LOG("sub-band %d does not exist", subband_id);
+    return -EINVAL;
+  }
+  int members = 0;
+  for (const HostClient &h : g->clients) members += h.active && h.mem && h.sb_cid == cid ? 1 : 0;
+  if (members > 0) {
+    XL_LOG("sub-band %d still has %d members; remove them first", subband_id, members);
+    return -EBUSY;
+  }
+  g->clients[cid].sb = false;
+  g->subbands[subband_id] = -1;
+  return xlg_remove_client(g, cid);
+}
+
+extern "C" int xlg_add_client_subband(xlg_group *g, int subband_id, uint32_t decim2, const float *taps2,
+                                      size_t taps2_len, int32_t center_offset, int *client_id) {
+  if (g == nullptr || client_id == nullptr) return -EINVAL;
+  const int sb = subband_client(g, subband_id);
+  if (sb < 0) {
+    XL_LOG("sub-band member: sub-band %d does not exist", subband_id);
+    return -EINVAL;
+  }
+  if (decim2 == 0 || taps2_len == 0 || taps2 == nullptr) {
+    XL_LOG("sub-band member: decimation %u and tap count %zu must both be at least 1", decim2, taps2_len);
+    return -EINVAL;
+  }
+  if (taps2_len > (size_t)INT32_MAX || decim2 > (uint32_t)INT32_MAX ||
+      subband_smem((int)decim2, (int)taps2_len) > (size_t)kTileMaxSmem) {
+    XL_LOG("sub-band member: %zu taps at decimation %u exceed the member kernel's shared memory", taps2_len, decim2);
+    return -EINVAL;
+  }
+  // the reference filter at fs / D1 centred center_offset from the sub-band: rotated reversed taps (the
+  // even-length reversal quirk included) and oscillator step
+  xl_client_consts k;
+  int rc = xl_client_consts_build(taps2, taps2_len, decim2, center_offset, g->fs / g->clients[sb].D, &k);
+  if (rc) return rc;
+  int id = -1;
+  for (size_t i = 0; i < g->clients.size(); i++)
+    if (!g->clients[i].active) {
+      id = (int)i;
+      break;
+    }
+  if (id < 0) {
+    g->clients.emplace_back();
+    id = (int)g->clients.size() - 1;
+  }
+  HostClient &h = g->clients[id];
+  h = HostClient();
+  h.active = true;
+  h.mem = true;
+  h.sb_cid = sb;
+  h.D = 0;
+  h.D2 = decim2;
+  h.T2 = taps2_len;
+  h.rev2.assign(k.rev_cf32, k.rev_cf32 + 2 * taps2_len);
+  h.incr_re = k.incr_re;
+  h.incr_im = k.incr_im;
+  h.hist2 = (long long)taps2_len - 1;  // src/xlating.c:552
+  h.zb2 = g->clients[sb].a_pos;
+  h.is_new = true;
+  xl_client_consts_free(&k);
+  g->dirty = true;
+  *client_id = id;
+  return 0;
+}
+
+extern "C" int xlg_subband_info(const xlg_group *g, int client_id, int *subband_id, int *stage_a_kind,
+                                size_t *member_history) {
+  if (g == nullptr || client_id < 0 || client_id >= (int)g->clients.size() || !g->clients[client_id].active ||
+      !g->clients[client_id].mem)
+    return -EINVAL;
+  const HostClient &h = g->clients[client_id];
+  if (subband_id) *subband_id = g->clients[h.sb_cid].sb_id;
+  if (stage_a_kind) *stage_a_kind = g->clients[h.sb_cid].kind;
+  if (member_history) *member_history = (size_t)h.hist2;
   return 0;
 }
 
@@ -1843,6 +2171,9 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     for (const HostClient &h : g->clients)
       if (h.active && (h.L > 1 || h.casc)) {
         XL_LOG("the Q15 path does not serve rational or cascade clients; submit without XLG_PATH_Q15");
+        return -ENOTSUP;
+      } else if (h.active && h.sb) {
+        XL_LOG("the Q15 path does not serve sub-bands; submit without XLG_PATH_Q15");
         return -ENOTSUP;
       }
   CU_OK(cudaSetDevice(g->device));
@@ -1918,7 +2249,7 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
   size_t casc_smem = 0, casc_poly_smem = 0;
   for (size_t i = 0; i < g->clients.size(); i++) {
     HostClient &h = g->clients[i];
-    if (!h.active) continue;
+    if (!h.active || h.mem) continue;
     // upsampled coordinates (the same integers for L = 1)
     const long long Su = S * h.L, Eu = (S + n) * h.L;
     const long long first = Su - h.hist;
@@ -1983,6 +2314,54 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       h.a_pos += n_out;
       h.last_n2 = n2;
       max_n1 = std::max(max_n1, n_out);
+    }
+  }
+
+  // sub-band members: each class walks its sub-band's n1 new samples with the reference's count formula, in
+  // sub-band coordinates (the sub-band's a_pos before this block's samples)
+  const int n_sb = (int)g->sb_list.size();
+  int max_sb_n1 = 0, max_sb_n2 = 0;
+  size_t sb_smem = 0;
+  s.sb_macs = s.sb_rows = 0;
+  if (n_sb > 0) {
+    for (size_t c = 0; c < g->sb_classes.size(); c++) {
+      const SbClassHost &ch = g->sb_classes[c];
+      const HostClient &a = g->clients[ch.sb_cid];
+      const HostClient &m0 = g->clients[ch.members[0]];
+      long long hist2 = m0.hist2;
+      const long long first2 = a.a_pos - hist2;
+      const int n2 = xl_walk(&hist2, ho.n_out[ch.sb_cid], m0.T2, m0.D2, m0.out_cap);
+      SbBlk &b = s.h_sbblk[c];
+      b.ring = a.d_cring;
+      b.first = first2;
+      b.zb = ch.zb;
+      b.mask = (unsigned)(a.cring_cap - 1);
+      b.n2 = n2;
+      b.D2 = (int)m0.D2;
+      b.T2 = (int)m0.T2;
+      for (int id : ch.members) {
+        g->clients[id].hist2 = hist2;
+        ho.n_out[id] = n2;
+        ho.out_off[id] = g->clients[id].out_off;
+      }
+      s.sb_macs += (uint64_t)n2 * m0.T2 * ch.members.size();
+      max_sb_n2 = std::max(max_sb_n2, n2);
+      sb_smem = std::max(sb_smem, subband_smem(b.D2, b.T2));
+    }
+    for (int k = 0; k < n_sb; k++) {
+      const int i = g->sb_list[k];
+      HostClient &a = g->clients[i];
+      const int n1 = ho.n_out[i];
+      CascBlk &cb = s.h_sbcb[k];
+      memset(&cb, 0, sizeof(cb));
+      cb.ring = a.d_cring;
+      cb.a_pos = a.a_pos;
+      cb.mask = (unsigned)(a.cring_cap - 1);
+      cb.a_off = a.out_off;
+      cb.n1 = n1;
+      a.a_pos += n1;
+      s.sb_rows += (uint64_t)n1;
+      max_sb_n1 = std::max(max_sb_n1, n1);
     }
   }
 
@@ -2386,6 +2765,34 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
         ho.out_off[i] = g->clients[i].fin_off;
       }
   }
+  // ---- sub-bands: append their outputs to their rings, then the members' oscillators and FIR ----
+  s.pf_sbk = false;
+  if (n_sb > 0) {
+    // the rings are appended in block order (the cascades' event orders both)
+    if (g->have_last_casc) CU_OK(cudaStreamWaitEvent(cs, g->ev_last_casc, 0));
+    if (g->profiling) {
+      CU_OK(cudaEventRecord(s.pf_sb[0], cs));
+      s.pf_sbk = true;
+    }
+    CU_OK(cudaMemcpyAsync(s.d_sbcb, s.h_sbcb, (size_t)n_sb * sizeof(CascBlk), cudaMemcpyHostToDevice, cs));
+    if (max_sb_n1 > 0) cascade_append_kernel<<<dim3((max_sb_n1 + 255) / 256, n_sb), 256, 0, cs>>>(s.d_sbcb, s.d_out);
+    if (max_sb_n2 > 0) {
+      CU_OK(cudaMemcpyAsync(s.d_sbblk, s.h_sbblk, g->sb_classes.size() * sizeof(SbBlk), cudaMemcpyHostToDevice, cs));
+      subband_phase_kernel<<<(g->n_sb_mem + 31) / 32, 32, 0, cs>>>(g->d_clients, g->d_sbmem, s.d_sbblk, s.d_sbph);
+      subband_fir_cf32_kernel<<<dim3((max_sb_n2 + SB_KO - 1) / SB_KO, g->n_sb_groups), SB_THREADS, sb_smem, cs>>>(
+          s.d_sbblk, g->d_sbgrp, g->d_sbtaps, s.d_sbph, s.d_out);
+    }
+    if (g->profiling) CU_OK(cudaEventRecord(s.pf_sb[1], cs));
+    CU_OK(cudaEventRecord(s.ev_casc, cs));
+    g->ev_last_casc = s.ev_casc;
+    g->have_last_casc = true;
+    // (the FIR launches above sized themselves by these counts) a sub-band is not a client: nothing to
+    // read, and the D2H copy ends before its row
+    for (int i : g->sb_list) {
+      ho.n_out[i] = 0;
+      ho.out_off[i] = 0;
+    }
+  }
   CU_OK(cudaGetLastError());
   CU_OK(cudaEventRecord(s.ev_fir, cs));
 
@@ -2628,6 +3035,14 @@ extern "C" int xlg_cascade_profile_read(xlg_group *g, xlg_cascade_profile *p, in
   std::lock_guard<std::mutex> lk(g->mu);
   *p = g->casc_prof;
   if (reset) memset(&g->casc_prof, 0, sizeof(g->casc_prof));
+  return 0;
+}
+
+extern "C" int xlg_subband_profile_read(xlg_group *g, xlg_subband_profile *p, int reset) {
+  if (g == nullptr || p == nullptr) return -EINVAL;
+  std::lock_guard<std::mutex> lk(g->mu);
+  *p = g->sb_prof;
+  if (reset) memset(&g->sb_prof, 0, sizeof(g->sb_prof));
   return 0;
 }
 

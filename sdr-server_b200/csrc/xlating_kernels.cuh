@@ -1301,4 +1301,154 @@ cascade_fir_poly_cf32_kernel(const CascPolyBlk *__restrict__ pb, const float *__
   }
 }
 
+// ---------------------------------------------------------------------------
+// sub-band members (xlg_add_client_subband).  A sub-band is an integer client whose outputs are appended to
+// a history ring (cascade_append_kernel, as a cascade's stage A).  A member is the reference's float path at
+// fs / D1 with its own centre, fed that ring:
+//     z[k] = phase_k * sum_{j < T2} y[first + k*D2 + j] * rev2[j]          (complex taps, 4 real FMAs each)
+// Members of one sub-band with equal (D2, T2, window alignment, first valid position) form a class: they
+// read the same windows, so a CTA stages the windows of a span of outputs once and every staged sample
+// feeds SB_MG members.
+// ---------------------------------------------------------------------------
+constexpr int SB_WARPS = 4;                  // warps of a CTA; warp w serves members [w*SB_RM, (w+1)*SB_RM)
+constexpr int SB_THREADS = 32 * SB_WARPS;
+constexpr int SB_RM = 4;                     // members per thread
+constexpr int SB_RO = 2;                     // outputs per thread: lane and lane + 32
+constexpr int SB_MG = SB_WARPS * SB_RM;      // members per CTA (a group)
+constexpr int SB_KO = 32 * SB_RO;            // outputs per CTA
+
+struct SbBlk {          // one class, this block
+  const float2 *ring;   // its sub-band's history ring
+  long long first;      // ring position where output 0's window starts
+  long long zb;         // ring positions before this read as zero (its members' attach point)
+  unsigned mask;        // ring capacity - 1
+  int n2, D2, T2;
+};
+
+struct SbGroup {        // up to SB_MG members of one class (the layout's)
+  int cls, n_mem;
+  int taps_off;         // float2 offset of the [SB_MG][sb_tpad(T2)] rotated reversed taps, zero rows for padding
+  int pad_;
+  int out_off[SB_MG];   // final rows in the slot's output arena
+  int ph_off[SB_MG];    // oscillator table: phase of EVEN output k at ph[ph_off + 32 * (k / 2)]
+  float2 incr[SB_MG];
+};
+
+struct SbMem {          // the member oscillator pre-pass: one entry per member, 32 per table group
+  int cid;              // its ClientDev (phase, incr, renorm; inactive for the other kernels), -1 = padding
+  int cls;
+  int ph_off;
+};
+
+__host__ __device__ constexpr int sb_tpad(int T2) { return (T2 + 1) & ~1; }  // 16-byte rows
+// shared memory of a CTA: mbarrier, SB_MG tap rows, the window of SB_KO outputs (+1 for an odd start, even)
+__host__ __device__ constexpr size_t subband_smem(int D2, int T2) {
+  return 16 + (size_t)SB_MG * sb_tpad(T2) * 8 + (((size_t)(SB_KO - 1) * D2 + T2 + 2) & ~(size_t)1) * 8;
+}
+
+// The members' oscillators: their output counts are known on the host, so one lane per member replays the
+// group's recursion (osc_chain_cf32) on this block's count.  As in phase_cf32_kernel, a warp owns a table
+// group of 32 members and stores the even phases interleaved, one coalesced line per step.
+__global__ void __launch_bounds__(32)
+subband_phase_kernel(ClientDev *__restrict__ cl, const SbMem *__restrict__ mem, const SbBlk *__restrict__ blk,
+                     float2 *__restrict__ ph) {
+  const SbMem m = mem[blockIdx.x * 32 + threadIdx.x];
+  if (m.cid < 0) return;
+  ClientDev *d = cl + m.cid;
+  d->phase = osc_chain_cf32<32>(d->phase, d->incr, ph + m.ph_off, blk[m.cls].n2, d->renorm);
+}
+
+// CTA (x, g) computes outputs [x*SB_KO, x*SB_KO + SB_KO) of the members of group g.  One TMA bulk copy
+// stages the group's taps, one or two (the ring wraps) the window; an odd window start is fetched from one
+// sample earlier.  Lane l holds outputs l and l + 32 of SB_RM members in registers, so each sample it loads
+// feeds SB_RM members and each tap SB_RO outputs.  With even D2 lane l walks the taps from j = l (mod T2):
+// its window reads then lie D2 + 1 samples apart, an odd stride, and its tap reads are consecutive, so
+// neither has bank conflicts (with odd D2 every lane starts at j = 0 and the tap read is a broadcast).
+__global__ void __launch_bounds__(SB_THREADS)
+subband_fir_cf32_kernel(const SbBlk *__restrict__ blk, const SbGroup *__restrict__ grp,
+                        const float2 *__restrict__ taps, const float2 *__restrict__ ph, float2 *__restrict__ out) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  uint64_t *bar = reinterpret_cast<uint64_t *>(smem);
+  const SbGroup &gp = grp[blockIdx.y];
+  const SbBlk b = blk[gp.cls];
+  const int k0 = blockIdx.x * SB_KO;
+  if (k0 >= b.n2) return;
+  const int D2 = b.D2, T2 = b.T2, tpad = sb_tpad(T2);
+  const int nk = min(SB_KO, b.n2 - k0);
+  float2 *ts = reinterpret_cast<float2 *>(smem + 16);
+  float2 *xs = ts + (size_t)SB_MG * tpad;
+  const long long w0 = b.first + (long long)k0 * D2;
+  const unsigned idx = (unsigned)((unsigned long long)w0) & b.mask;
+  const unsigned shift = idx & 1u;
+  const unsigned need = ((unsigned)((nk - 1) * D2 + T2) + shift + 1u) & ~1u;
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    mbar_init(bar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  __syncthreads();
+  if (tid == 0) {
+    const unsigned tbytes = (unsigned)(SB_MG * tpad) * 8u;
+    const unsigned p1 = min(need, b.mask + 1u - (idx - shift));
+    mbar_expect_tx(bar, tbytes + need * 8u);
+    tma_bulk_g2s(ts, taps + gp.taps_off, tbytes, bar);
+    tma_bulk_g2s(xs, b.ring + (idx - shift), p1 * 8u, bar);
+    if (p1 < need) tma_bulk_g2s(xs + p1, b.ring, (need - p1) * 8u, bar);
+  }
+  mbar_wait(bar, 0);
+  const long long base = w0 - (long long)shift;
+  if (b.zb > base) {  // a class attached mid-stream: its members read zeros before their attach point
+    for (unsigned i = tid; i < need; i += SB_THREADS)
+      if (base + (long long)i < b.zb) xs[i] = make_float2(0.f, 0.f);
+    __syncthreads();
+  }
+  const int warp = tid >> 5, lane = tid & 31;
+  const int m0 = warp * SB_RM;
+  if (m0 >= gp.n_mem) return;
+  const float2 *x[SB_RO];
+#pragma unroll
+  for (int i = 0; i < SB_RO; i++) x[i] = xs + shift + (size_t)min(lane + 32 * i, nk - 1) * D2;
+  const float2 *t[SB_RM];
+#pragma unroll
+  for (int r = 0; r < SB_RM; r++) t[r] = ts + (size_t)(m0 + r) * tpad;
+  float2 acc[SB_RO][SB_RM];
+#pragma unroll
+  for (int i = 0; i < SB_RO; i++)
+#pragma unroll
+    for (int r = 0; r < SB_RM; r++) acc[i][r] = make_float2(0.f, 0.f);
+  int j = (D2 & 1) ? 0 : lane % T2;
+#pragma unroll 2
+  for (int s = 0; s < T2; s++) {
+    float2 v[SB_RO], h[SB_RM];
+#pragma unroll
+    for (int i = 0; i < SB_RO; i++) v[i] = x[i][j];
+#pragma unroll
+    for (int r = 0; r < SB_RM; r++) h[r] = t[r][j];
+#pragma unroll
+    for (int i = 0; i < SB_RO; i++)
+#pragma unroll
+      for (int r = 0; r < SB_RM; r++) {
+        acc[i][r].x = fmaf(v[i].x, h[r].x, acc[i][r].x);
+        acc[i][r].x = fmaf(-v[i].y, h[r].y, acc[i][r].x);
+        acc[i][r].y = fmaf(v[i].x, h[r].y, acc[i][r].y);
+        acc[i][r].y = fmaf(v[i].y, h[r].x, acc[i][r].y);
+      }
+    if (++j == T2) j = 0;
+  }
+#pragma unroll
+  for (int r = 0; r < SB_RM; r++) {
+    const int m = m0 + r;
+    if (m >= gp.n_mem) break;
+#pragma unroll
+    for (int i = 0; i < SB_RO; i++) {
+      const int k = k0 + lane + 32 * i;
+      if (lane + 32 * i >= nk) continue;
+      float2 p = ph[gp.ph_off[m] + 32 * (k >> 1)];
+      if (k & 1) p = cmul_unfused(p, gp.incr[m]);     // odd outputs: one step from the stored even phase
+      out[gp.out_off[m] + k] = cmul_unfused(acc[i][r], p);  // src/xlating.c:70
+    }
+  }
+}
+
 }  // namespace xl
