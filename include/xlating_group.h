@@ -175,8 +175,22 @@ int xlg_remove_subband(xlg_group *g, int subband_id);
  * long for the member kernel's shared memory (17 * taps2_len + 63 * decim2 <= about 25600). */
 int xlg_add_client_subband(xlg_group *g, int subband_id, uint32_t decim2, const float *taps2, size_t taps2_len,
                            int32_t center_offset, int *client_id);
+/* Extension: rational members (DESIGN.md section 5, "Rational sub-band members"), for client rates that do not
+ * divide fs / decim1.  A rational member is the float path of create_frequency_xlating_filter(decim2, taps2,
+ * taps2_len, center_offset, interp2 * fs / decim1, ...), fed the zero-stuffed sub-band stream
+ * (u[interp2 * n] = y[n], 0 elsewhere) from the block it is attached before, with taps2_len - 1 upsampled
+ * zeros of history.  Every output sums only the ceil(taps2_len / interp2) taps of one polyphase branch, and
+ * the output rate is fs * interp2 / (decim1 * decim2); design the taps at interp2 * fs / decim1 with gain
+ * interp2.  xlg_add_client_subband is its interp2 = 1 case.  Kind 6 in xlg_client_info; xlg_subband_info's
+ * member history is in upsampled samples.  -EINVAL (logged) for interp2 = 0, interp2 * fs / decim1 above
+ * UINT32_MAX, interp2 * (max_input_len / 2 / decim1 + 2) >= 2^31, one branch and a window too long for the
+ * member kernel's shared memory (17 * ceil(taps2_len / interp2) + 63 * decim2 <= about 25600), and every
+ * refusal of xlg_add_client_subband. */
+int xlg_add_client_subband_rational(xlg_group *g, int subband_id, uint32_t interp2, uint32_t decim2,
+                                    const float *taps2, size_t taps2_len, int32_t center_offset, int *client_id);
 /* A member's sub-band, the kind (0, 1 or 2, as xlg_client_info) of the kernel serving the sub-band, and the
- * member's history_offset in sub-band samples.  -EINVAL for any client that is not a member. */
+ * member's history_offset in sub-band samples (upsampled samples for a rational member).  -EINVAL for any
+ * client that is not a member. */
 int xlg_subband_info(const xlg_group *g, int client_id, int *subband_id, int *stage_a_kind, size_t *member_history);
 /* Size the per-ticket result arenas (device and pinned host) for `output_samples_per_block` complex output
  * samples per block summed over all clients (a client at decimation D produces about max_input_len/2/D + 2).
@@ -184,7 +198,7 @@ int xlg_subband_info(const xlg_group *g, int client_id, int *subband_id, int *st
  * n1 = max_input_len/2/decim1 + 2 samples, which stays on the device, and its final row of
  * floor(n1 * interp2 / decim2) + 2 (interp2 = 1 for xlg_add_client_cascade).  A sub-band counts one row of
  * n1 = max_input_len/2/decim1 + 2 samples, rounded up to 4, which stays on the device; a member counts its
- * final row of floor(n1 / decim2) + 2, rounded up to 4.
+ * final row of floor(n1 * interp2 / decim2) + 2, rounded up to 4 (interp2 = 1 for xlg_add_client_subband).
  * Optional: the arenas grow on demand when clients are added, but a growth re-allocates every ring entry and
  * the results still waiting in the ring are lost (-ESTALE for consumers that had not read them yet, like a
  * block overwritten in the reference's queue).  A server that knows its client limit reserves once, up front. */
@@ -289,7 +303,7 @@ int xlg_cascade_profile_read(xlg_group *g, xlg_cascade_profile *p, int reset);
 typedef struct {
   double member_ms;          /* the sub-band ring appends, the member oscillators and the member kernel */
   uint64_t member_launches;
-  uint64_t member_macs;      /* complex MACs of the members: sum n2 * taps2_len */
+  uint64_t member_macs;      /* complex MACs of the members: sum n2 * ceil(taps2_len / interp2) */
   uint64_t row_samples;      /* sub-band samples produced (and appended to the rings) */
 } xlg_subband_profile;
 int xlg_subband_profile_read(xlg_group *g, xlg_subband_profile *p, int reset);

@@ -55,7 +55,7 @@ DROPIN_EXTENSION_SYMBOLS = ["create_rational_frequency_xlating_filter", "create_
 GROUP_SYMBOLS = [
     "xlg_create", "xlg_create_ex", "xlg_destroy", "xlg_add_client", "xlg_add_client_ex", "xlg_add_client_rational_ex", "xlg_remove_client", "xlg_reserve", "xlg_client_count", "xlg_submit",
     "xlg_wait", "xlg_input_consumed", "xlg_output", "xlg_read_output", "xlg_copy_output", "xlg_alloc_pinned", "xlg_free_pinned", "xlg_wait_stream", "xlg_partition_active", "xlg_timer_start",
-    "xlg_timer_stop", "xlg_profile_enable", "xlg_profile_read", "xlg_client_info", "xlg_add_client_rational", "xlg_poly_profile_read", "xlg_add_client_cascade", "xlg_add_client_cascade_rational", "xlg_cascade_info", "xlg_cascade_profile_read", "xlg_add_subband", "xlg_remove_subband", "xlg_add_client_subband", "xlg_subband_info", "xlg_subband_profile_read", "xlg_dropin_stats", "xlg_dropin_stream_stats", "xlg_dropin_stream_times",
+    "xlg_timer_stop", "xlg_profile_enable", "xlg_profile_read", "xlg_client_info", "xlg_add_client_rational", "xlg_poly_profile_read", "xlg_add_client_cascade", "xlg_add_client_cascade_rational", "xlg_cascade_info", "xlg_cascade_profile_read", "xlg_add_subband", "xlg_remove_subband", "xlg_add_client_subband", "xlg_add_client_subband_rational", "xlg_subband_info", "xlg_subband_profile_read", "xlg_dropin_stats", "xlg_dropin_stream_stats", "xlg_dropin_stream_times",
 ]
 
 
@@ -158,6 +158,8 @@ def lib() -> C.CDLL:
     L.xlg_remove_subband.restype = C.c_int
     L.xlg_add_client_subband.argtypes = [vp, C.c_int, u32, fp, sz, i32, C.POINTER(C.c_int)]
     L.xlg_add_client_subband.restype = C.c_int
+    L.xlg_add_client_subband_rational.argtypes = [vp, C.c_int, u32, u32, fp, sz, i32, C.POINTER(C.c_int)]
+    L.xlg_add_client_subband_rational.restype = C.c_int
     L.xlg_subband_info.argtypes = [vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(sz)]
     L.xlg_subband_info.restype = C.c_int
     L.xlg_subband_profile_read.argtypes = [vp, C.POINTER(XlgSubbandProfile), C.c_int]
@@ -427,13 +429,15 @@ class Group:
         if code != 0:
             raise ValueError(code)
 
-    def add_client_subband(self, sid: int, decim2: int, taps2, center_offset: int) -> int:
-        """A member of sub-band `sid` (xlg_add_client_subband): the reference's float path (decim2, taps2,
-        center_offset) at fs / decim1 fed the sub-band's outputs.  Returns an ordinary client id."""
+    def add_client_subband(self, sid: int, decim2: int, taps2, center_offset: int, interp2: int = 1) -> int:
+        """A member of sub-band `sid` (xlg_add_client_subband_rational): the reference's float path (decim2,
+        taps2, center_offset) at interp2 * fs / decim1 fed the sub-band's zero-stuffed outputs (interp2 = 1:
+        xlg_add_client_subband).  Returns an ordinary client id.  See subband_plan for taps."""
         t2 = np.ascontiguousarray(taps2, dtype=np.float32)
         cid = C.c_int(-1)
-        code = self._L.xlg_add_client_subband(self._h, sid, decim2, t2.ctypes.data_as(C.POINTER(C.c_float)),
-                                              len(t2), center_offset, C.byref(cid))
+        code = self._L.xlg_add_client_subband_rational(self._h, sid, interp2, decim2,
+                                                       t2.ctypes.data_as(C.POINTER(C.c_float)), len(t2),
+                                                       center_offset, C.byref(cid))
         if code != 0:
             raise ValueError(code)
         return cid.value
@@ -718,8 +722,18 @@ def cascade_plan(fs: int, rates):
 
 def subband_fmas(fs: int, d1: int, t1: int, n_subbands: int, members) -> float:
     """Algorithmic real FMAs per input sample of a sub-band plan: 4 per complex tap of each sub-band at
-    fs / d1, and 4 per complex tap of each member at its own rate.  members: (rate, t2) pairs."""
-    return 4.0 * n_subbands * t1 / d1 + sum(4.0 * t2 * rate / fs for rate, t2 in members)
+    fs / d1, and 4 per complex tap of each member's polyphase branch (ceil(t2 / interp2) taps) at its own rate.
+    members: (rate, t2) or (rate, t2, interp2) tuples."""
+    return 4.0 * n_subbands * t1 / d1 + sum(4.0 * -(-m[1] // (m[2] if len(m) > 2 else 1)) * m[0] / fs
+                                           for m in members)
+
+
+def subband_member_fits(interp2: int, decim2: int, t2: int) -> bool:
+    """Whether the member kernel's shared memory holds a member (xlg_add_client_subband_rational refuses the
+    others): 16 members' taps of one branch and the window of 64 outputs, subband_smem in csrc/xlating_kernels.cuh
+    against the 200 KiB the kernel is given."""
+    return (16 + 16 * 8 * ((-(-t2 // interp2) + 1) & ~1) + 8 * ((63 * decim2 - (-t2 // interp2) + 2) & ~1)
+            <= 200 * 1024)
 
 
 def subband_plan(fs: int, clients):
@@ -730,36 +744,49 @@ def subband_plan(fs: int, clients):
     e = fs1 / 4 + max rate / 2 (it passes everything a member reads, and everything it aliases lands outside
     [-e, e]), the members with the server's own taps at fs1 (cutoff rate / 2, transition rate / 5).  Of
     these, the D1 with the fewest FMAs per input sample (subband_fmas, counting only sub-bands with members;
-    ties go to the smaller D1).  Returns {"d1", "taps1", "e", "subbands": [{"center"}], "members": [{"subband",
-    "center", "rate", "d2", "offset", "taps2"}] in the order of `clients`, "fmas"}."""
+    ties go to the smaller D1).  Only where no D1 lets every rate divide fs1, every D1 with fs1 even and
+    fs1 > 2 * max rate is a candidate: each member then resamples by interp2 / d2 = rate / fs1 (reduced;
+    interp2 = 1 where the rate divides fs1) with taps create_low_pass_filter(interp2, interp2 * fs1, rate / 2,
+    rate / 5), and a D1 with a member the kernel would refuse (subband_member_fits) is skipped.  Returns
+    {"d1", "taps1", "e", "subbands": [{"center"}], "members": [{"subband", "center", "rate", "interp2", "d2",
+    "offset", "taps2"}] in the order of `clients`, "fmas"}."""
     centers = [int(c) for c, _ in clients]
     rates = [int(r) for _, r in clients]
     rmax = max(rates)
     lo, hi = min(centers), max(centers)
     best = None
-    for d1 in range(2, fs // (2 * rmax) + 1):
-        if fs % d1:
-            continue
-        fs1 = fs // d1
-        if fs1 % 2 or fs1 <= 2 * rmax or any(fs1 % r for r in rates):
-            continue
-        half = fs1 // 2
-        n_cent = (hi - lo + half - 1) // half + 1
-        assign = [min(range(n_cent), key=lambda k: abs(c - (lo + k * half))) for c in centers]
-        used = sorted(set(assign))
-        e = fs1 // 4 + rmax // 2
-        t1 = create_low_pass_filter(1.0, fs, fs1 // 2, fs1 - 2 * e)
-        designs = {r: create_low_pass_filter(1.0, fs1, r // 2, r // 5) for r in set(rates)}
-        cost = subband_fmas(fs, d1, t1.size, len(used), [(r, designs[r].size) for r in rates])
-        if best is None or cost < best[0]:
-            best = (cost, d1, fs1, half, e, t1, designs, used, assign)
+    for rational in (False, True):
+        for d1 in range(2, fs // (2 * rmax) + 1):
+            if fs % d1:
+                continue
+            fs1 = fs // d1
+            if fs1 % 2 or fs1 <= 2 * rmax or (not rational and any(fs1 % r for r in rates)):
+                continue
+            shapes = {}  # rate -> (interp2, d2, taps2)
+            for r in set(rates):
+                g = math.gcd(r, fs1)
+                L2, M2 = r // g, fs1 // g
+                shapes[r] = (L2, M2, create_low_pass_filter(float(L2), L2 * fs1, r // 2, r // 5))
+            if rational and not all(subband_member_fits(L2, M2, t.size) for L2, M2, t in shapes.values()):
+                continue
+            half = fs1 // 2
+            n_cent = (hi - lo + half - 1) // half + 1
+            assign = [min(range(n_cent), key=lambda k: abs(c - (lo + k * half))) for c in centers]
+            used = sorted(set(assign))
+            e = fs1 // 4 + rmax // 2
+            t1 = create_low_pass_filter(1.0, fs, fs1 // 2, fs1 - 2 * e)
+            cost = subband_fmas(fs, d1, t1.size, len(used), [(r, shapes[r][2].size, shapes[r][0]) for r in rates])
+            if best is None or cost < best[0]:
+                best = (cost, d1, fs1, half, e, t1, shapes, used, assign)
+        if best is not None:
+            break
     if best is None:
         raise ValueError(f"{fs} has no divisor D1 >= 2 whose sub-band rate serves the rates {sorted(set(rates))}")
-    cost, d1, fs1, half, e, t1, designs, used, assign = best
+    cost, d1, fs1, half, e, t1, shapes, used, assign = best
     index = {k: i for i, k in enumerate(used)}
     subbands = [{"center": lo + k * half} for k in used]
-    members = [{"subband": index[k], "center": c, "rate": r, "d2": fs1 // r, "offset": c - (lo + k * half),
-                "taps2": designs[r]} for c, r, k in zip(centers, rates, assign)]
+    members = [{"subband": index[k], "center": c, "rate": r, "interp2": shapes[r][0], "d2": shapes[r][1],
+                "offset": c - (lo + k * half), "taps2": shapes[r][2]} for c, r, k in zip(centers, rates, assign)]
     return {"d1": d1, "fs1": fs1, "taps1": t1, "e": e, "subbands": subbands, "members": members, "fmas": cost}
 
 

@@ -17,8 +17,8 @@
  *   cascade clients  a stage-A history ring each (HostClient::d_cring), their stage-B taps
  *                    (d_taps2); stage-A rows follow the host-visible rows of the arena
  *   sub-bands        a history ring each (HostClient::d_cring), rows after the host-visible ones;
- *                    their members' taps packed per group of SB_MG (d_sbtaps, SbGroup), and per
- *                    slot the members' oscillator table (d_sbph)
+ *                    their members' taps packed per group of SB_MG (d_sbtaps, SbGroup; branch-major
+ *                    for rational members), and per slot the members' oscillator table (d_sbph)
  *
  * Streams: s_in (H2D), s_ph (oscillator pre-pass chain), s_cs[0..n_cs) (convert + FIR,
  * round-robin by block; 3 by default, XLATING_B200_CSTREAMS=1..4), s_out (D2H); events order them per block so block b+1's
@@ -134,19 +134,21 @@ struct HostClient {
   // host-visible row; d_cring, cring_cap and a_pos above are its history ring
   bool sb = false;
   int sb_id = -1;
-  // sub-band member (xlg_add_client_subband): not an integer client -- its ClientDev only carries its
-  // oscillator; D2, T2, hist2 (in sub-band samples) and last_n2 above are its own, rev2 holds its rotated
-  // reversed taps (2 * T2 floats), out_off / out_cap its final row
+  // sub-band member (xlg_add_client_subband[_rational]): not an integer client -- its ClientDev only carries
+  // its oscillator; L2, D2, T2, Tb2, hist2 (in sub-band samples, upsampled when L2 > 1) and last_n2 above are
+  // its own, rev2 holds its rotated reversed taps (2 * T2 floats; branch-major, 2 * L2 * Tb2, when L2 > 1),
+  // out_off / out_cap its final row
   bool mem = false;
   int sb_cid = -1;               // its sub-band's client index
   long long zb2 = 0;             // sub-band position of its attach point: earlier samples read as zero
   int ph_row = 0;                // its rows of the slot's member oscillator table
 };
 
-// members of one sub-band that read the same windows: equal (D2, T2, hist2) and, until their windows have
+// members of one sub-band that read the same windows: equal (L2, D2, T2, hist2) and, until their windows have
 // passed it, the same attach point
 struct SbClassHost {
   int sb_cid;
+  int L2, Tb;    // Tb: taps per branch (T2 when L2 = 1)
   std::vector<int> members;
   long long zb;  // the largest attach point of its members
 };
@@ -388,6 +390,7 @@ struct xlg_group {
   std::vector<int> sb_list;                 // active sub-bands' client indices (their appends, in this order)
   std::vector<SbClassHost> sb_classes;
   int n_sb_mem = 0, n_sb_groups = 0;
+  int n_sb_groups_int = 0;                  // of which integer classes' (their SbGroup entries come first)
   SbGroup *d_sbgrp = nullptr;
   SbMem *d_sbmem = nullptr;
   float2 *d_sbtaps = nullptr;
@@ -687,29 +690,43 @@ static bool poly_settled(const xlg_group *g, const HostClient &h) {
 static int rebuild_subbands(xlg_group *g, size_t &out_total) {
   g->sb_list.clear();
   g->sb_classes.clear();
-  g->n_sb_mem = g->n_sb_groups = 0;
+  g->n_sb_mem = g->n_sb_groups = g->n_sb_groups_int = 0;
   const int nc = (int)g->clients.size();
   for (int i = 0; i < nc; i++)
     if (g->clients[i].active && g->clients[i].sb) g->sb_list.push_back(i);
   if (g->sb_list.empty()) return 0;
   CU_OK(cudaFuncSetAttribute(subband_fir_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem));
   std::vector<size_t> back(nc, 0);  // longest member history per sub-band
+  // integer classes (L2 = 1) and rational ones apart: the integer classes' groups come first
   std::map<std::tuple<int, uint32_t, size_t, long long, long long>, std::vector<int>> keyed;
+  std::map<std::tuple<int, uint32_t, uint32_t, size_t, long long, long long>, std::vector<int>> keyed_rat;
+  bool any_rat = false;
   for (int i = 0; i < nc; i++) {
     const HostClient &h = g->clients[i];
     if (!h.active || !h.mem) continue;
-    back[h.sb_cid] = std::max(back[h.sb_cid], h.T2 - 1);
+    // a rational member's history of at most T2 - 1 upsampled samples reaches back ceil((T2 - 1) / L2)
+    // sub-band samples, and its last branch may read one zero-weighted sample past the block
+    back[h.sb_cid] = std::max(back[h.sb_cid], h.L2 == 1 ? h.T2 - 1 : (h.T2 - 1 + h.L2 - 1) / h.L2 + 1);
     // its window has passed its attach point: it reads what every settled member of the class reads
-    const bool settled = h.zb2 <= g->clients[h.sb_cid].a_pos - h.hist2;
-    keyed[std::make_tuple(h.sb_cid, h.D2, h.T2, h.hist2, settled ? LLONG_MIN : h.zb2)].push_back(i);
+    const bool settled = h.zb2 * (long long)h.L2 <= (long long)h.L2 * g->clients[h.sb_cid].a_pos - h.hist2;
+    if (h.L2 == 1) {
+      keyed[std::make_tuple(h.sb_cid, h.D2, h.T2, h.hist2, settled ? LLONG_MIN : h.zb2)].push_back(i);
+    } else {
+      keyed_rat[std::make_tuple(h.sb_cid, h.L2, h.D2, h.T2, h.hist2, settled ? LLONG_MIN : h.zb2)].push_back(i);
+      any_rat = true;
+    }
   }
+  if (any_rat)
+    CU_OK(cudaFuncSetAttribute(subband_fir_poly_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               kTileMaxSmem));
   for (int i : g->sb_list) {
     HostClient &h = g->clients[i];
     h.out_off = (int)out_total;
     out_total += (size_t)h.out_cap;
     out_total = (out_total + 3) & ~(size_t)3;
     // a member of block b reads sub-band samples of earlier blocks; the submit of block b + XLG_SLOTS waits
-    // for ticket b, so T2 - 1 + (XLG_SLOTS + 1) * max n1 samples are never overwritten while still needed
+    // for ticket b, so its history (above) + (XLG_SLOTS + 1) * max n1 samples are never overwritten while
+    // still needed
     const size_t cap = next_pow2(back[i] + (size_t)(XLG_SLOTS + 1) * (size_t)h.out_cap);
     if (h.d_cring != nullptr && cap <= h.cring_cap) continue;
     float2 *ring = nullptr;
@@ -732,30 +749,41 @@ static int rebuild_subbands(xlg_group *g, size_t &out_total) {
   std::vector<SbGroup> groups;
   std::vector<SbMem> mems;
   std::vector<float2> taps;
-  for (auto &kv : keyed) {
+  // one class: its groups of SB_MG members, taps [branch][SB_MG][tpad] per group, so that one bulk copy
+  // stages one branch for the group (a single branch, the reversed taps themselves, when L2 = 1)
+  auto add_class = [&](int sb_cid, const std::vector<int> &members) {
     const int cls = (int)g->sb_classes.size();
     SbClassHost ch;
-    ch.sb_cid = std::get<0>(kv.first);
-    ch.members = kv.second;
+    ch.sb_cid = sb_cid;
+    ch.members = members;
     ch.zb = LLONG_MIN;
-    const int T2 = (int)std::get<2>(kv.first), tpad = sb_tpad(T2);
+    const HostClient &h0 = g->clients[members[0]];
+    ch.L2 = (int)h0.L2;
+    ch.Tb = h0.L2 == 1 ? (int)h0.T2 : h0.Tb2;
+    const int tpad = sb_tpad(ch.Tb);
     for (size_t m0 = 0; m0 < ch.members.size(); m0 += SB_MG) {
       SbGroup gp;
       memset(&gp, 0, sizeof(gp));
       gp.cls = cls;
       gp.n_mem = (int)std::min<size_t>(SB_MG, ch.members.size() - m0);
       gp.taps_off = (int)taps.size();
-      taps.resize(taps.size() + (size_t)SB_MG * tpad, make_float2(0.f, 0.f));
+      gp.l2 = ch.L2;
+      taps.resize(taps.size() + (size_t)ch.L2 * SB_MG * tpad, make_float2(0.f, 0.f));
       for (int m = 0; m < gp.n_mem; m++) {
         HostClient &h = g->clients[ch.members[m0 + m]];
-        memcpy(&taps[gp.taps_off + (size_t)m * tpad], h.rev2.data(), h.rev2.size() * sizeof(float));
+        for (int r = 0; r < ch.L2; r++)
+          memcpy(&taps[gp.taps_off + ((size_t)r * SB_MG + m) * tpad], h.rev2.data() + 2 * (size_t)r * ch.Tb,
+                 2 * (size_t)ch.Tb * sizeof(float));
         mems.push_back(SbMem{ch.members[m0 + m], cls, 0});
         ch.zb = std::max(ch.zb, h.zb2);
       }
       groups.push_back(gp);
     }
     g->sb_classes.push_back(ch);
-  }
+  };
+  for (auto &kv : keyed) add_class(std::get<0>(kv.first), kv.second);
+  g->n_sb_groups_int = (int)groups.size();
+  for (auto &kv : keyed_rat) add_class(std::get<0>(kv.first), kv.second);
   // oscillator table: groups of 32 members in SbMem order, phase of even output k of slot l at
   // base + 32 * (k / 2) + l
   size_t rows = 0;
@@ -849,8 +877,8 @@ static int rebuild_layout(xlg_group *g) {
     HostClient &h = g->clients[i];
     if (!h.active) continue;
     if (h.mem) {
-      // n2 <= (n1 - 1) / D2 + 1 for any history, n1 at most its sub-band's row
-      h.out_cap = (int)(((uint64_t)g->max_input_len / 2 / g->clients[h.sb_cid].D + 2) / h.D2 + 2);
+      // n2 <= (L2 * n1 - 1) / D2 + 1 for any history, n1 at most its sub-band's row
+      h.out_cap = (int)(((uint64_t)g->max_input_len / 2 / g->clients[h.sb_cid].D + 2) * h.L2 / h.D2 + 2);
       h.out_off = (int)out_total;
       out_total += (size_t)h.out_cap;
       out_total = (out_total + 3) & ~(size_t)3;
@@ -985,7 +1013,7 @@ static int rebuild_layout(xlg_group *g) {
     HostClient &h = g->clients[i];
     if (!h.active) continue;
     if (h.mem) {
-      h.kind = 6;  // served by subband_fir_cf32_kernel
+      h.kind = 6;  // served by subband_fir_cf32_kernel (subband_fir_poly_cf32_kernel when L2 > 1)
       continue;
     }
     h.kind = h.L > 1 ? 3 : 0;
@@ -2082,6 +2110,12 @@ extern "C" int xlg_remove_subband(xlg_group *g, int subband_id) {
 
 extern "C" int xlg_add_client_subband(xlg_group *g, int subband_id, uint32_t decim2, const float *taps2,
                                       size_t taps2_len, int32_t center_offset, int *client_id) {
+  return xlg_add_client_subband_rational(g, subband_id, 1, decim2, taps2, taps2_len, center_offset, client_id);
+}
+
+extern "C" int xlg_add_client_subband_rational(xlg_group *g, int subband_id, uint32_t interp2, uint32_t decim2,
+                                               const float *taps2, size_t taps2_len, int32_t center_offset,
+                                               int *client_id) {
   if (g == nullptr || client_id == nullptr) return -EINVAL;
   const int sb = subband_client(g, subband_id);
   if (sb < 0) {
@@ -2092,15 +2126,32 @@ extern "C" int xlg_add_client_subband(xlg_group *g, int subband_id, uint32_t dec
     XL_LOG("sub-band member: decimation %u and tap count %zu must both be at least 1", decim2, taps2_len);
     return -EINVAL;
   }
-  if (taps2_len > (size_t)INT32_MAX || decim2 > (uint32_t)INT32_MAX ||
-      subband_smem((int)decim2, (int)taps2_len) > (size_t)kTileMaxSmem) {
-    XL_LOG("sub-band member: %zu taps at decimation %u exceed the member kernel's shared memory", taps2_len, decim2);
+  if (interp2 == 0) {
+    XL_LOG("sub-band member: interpolation must be at least 1");
     return -EINVAL;
   }
-  // the reference filter at fs / D1 centred center_offset from the sub-band: rotated reversed taps (the
-  // even-length reversal quirk included) and oscillator step
+  const uint32_t decim1 = g->clients[sb].D;
+  if ((uint64_t)interp2 * (g->fs / decim1) > UINT32_MAX) {
+    XL_LOG("sub-band member: %u x %u Hz upsampled rate exceeds UINT32_MAX", interp2, g->fs / decim1);
+    return -EINVAL;
+  }
+  if ((uint64_t)interp2 * ((uint64_t)g->max_input_len / 2 / decim1 + 2) >= (1ull << 31)) {
+    XL_LOG("sub-band member: %u x %u sub-band samples per block upsampled exceed 2^31", interp2,
+           g->max_input_len / 2 / decim1 + 2);
+    return -EINVAL;
+  }
+  // one branch's taps for a group and the window of SB_KO outputs (of one residue) in shared memory
+  const size_t Tb2 = (taps2_len + interp2 - 1) / interp2;
+  if (taps2_len > (size_t)INT32_MAX || decim2 > (uint32_t)INT32_MAX ||
+      subband_smem((int)decim2, (int)Tb2) > (size_t)kTileMaxSmem) {
+    XL_LOG("sub-band member: %zu taps at interpolation %u, decimation %u exceed the member kernel's shared memory",
+           taps2_len, interp2, decim2);
+    return -EINVAL;
+  }
+  // the reference filter at interp2 * fs / D1 centred center_offset from the sub-band: rotated reversed taps
+  // (the even-length reversal quirk included) and oscillator step
   xl_client_consts k;
-  int rc = xl_client_consts_build(taps2, taps2_len, decim2, center_offset, g->fs / g->clients[sb].D, &k);
+  int rc = xl_client_consts_build(taps2, taps2_len, decim2, center_offset, interp2 * (g->fs / decim1), &k);
   if (rc) return rc;
   int id = -1;
   for (size_t i = 0; i < g->clients.size(); i++)
@@ -2118,12 +2169,19 @@ extern "C" int xlg_add_client_subband(xlg_group *g, int subband_id, uint32_t dec
   h.mem = true;
   h.sb_cid = sb;
   h.D = 0;
+  h.L2 = interp2;
   h.D2 = decim2;
   h.T2 = taps2_len;
-  h.rev2.assign(k.rev_cf32, k.rev_cf32 + 2 * taps2_len);
+  h.Tb2 = (int)Tb2;
+  if (interp2 == 1) {
+    h.rev2.assign(k.rev_cf32, k.rev_cf32 + 2 * taps2_len);
+  } else {
+    h.rev2.resize(2 * (size_t)interp2 * Tb2);  // branch-major P[r][t] = rev[r + t * L2], zero-padded
+    xl_poly_pack(k.rev_cf32, taps2_len, interp2, h.rev2.data());
+  }
   h.incr_re = k.incr_re;
   h.incr_im = k.incr_im;
-  h.hist2 = (long long)taps2_len - 1;  // src/xlating.c:552
+  h.hist2 = (long long)taps2_len - 1;  // src/xlating.c:552 (upsampled samples when L2 > 1)
   h.zb2 = g->clients[sb].a_pos;
   h.is_new = true;
   xl_client_consts_free(&k);
@@ -2318,10 +2376,12 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
   }
 
   // sub-band members: each class walks its sub-band's n1 new samples with the reference's count formula, in
-  // sub-band coordinates (the sub-band's a_pos before this block's samples)
+  // sub-band coordinates (the sub-band's a_pos before this block's samples), upsampled by L2 for a rational
+  // class
   const int n_sb = (int)g->sb_list.size();
   int max_sb_n1 = 0, max_sb_n2 = 0;
-  size_t sb_smem = 0;
+  int max_sbr_ctas = 0, max_sbr_l2 = 0;  // rational classes: output tiles of the longest residue, largest L2
+  size_t sb_smem = 0, sbr_smem = 0;
   s.sb_macs = s.sb_rows = 0;
   if (n_sb > 0) {
     for (size_t c = 0; c < g->sb_classes.size(); c++) {
@@ -2329,8 +2389,8 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       const HostClient &a = g->clients[ch.sb_cid];
       const HostClient &m0 = g->clients[ch.members[0]];
       long long hist2 = m0.hist2;
-      const long long first2 = a.a_pos - hist2;
-      const int n2 = xl_walk(&hist2, ho.n_out[ch.sb_cid], m0.T2, m0.D2, m0.out_cap);
+      const long long first2 = (long long)ch.L2 * a.a_pos - hist2;
+      const int n2 = xl_walk(&hist2, (long long)ch.L2 * ho.n_out[ch.sb_cid], m0.T2, m0.D2, m0.out_cap);
       SbBlk &b = s.h_sbblk[c];
       b.ring = a.d_cring;
       b.first = first2;
@@ -2338,15 +2398,21 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       b.mask = (unsigned)(a.cring_cap - 1);
       b.n2 = n2;
       b.D2 = (int)m0.D2;
-      b.T2 = (int)m0.T2;
+      b.T2 = ch.Tb;
       for (int id : ch.members) {
         g->clients[id].hist2 = hist2;
         ho.n_out[id] = n2;
         ho.out_off[id] = g->clients[id].out_off;
       }
-      s.sb_macs += (uint64_t)n2 * m0.T2 * ch.members.size();
-      max_sb_n2 = std::max(max_sb_n2, n2);
-      sb_smem = std::max(sb_smem, subband_smem(b.D2, b.T2));
+      s.sb_macs += (uint64_t)n2 * ch.Tb * ch.members.size();
+      if (ch.L2 == 1) {
+        max_sb_n2 = std::max(max_sb_n2, n2);
+        sb_smem = std::max(sb_smem, subband_smem(b.D2, b.T2));
+      } else if (n2 > 0) {
+        max_sbr_ctas = std::max(max_sbr_ctas, ((n2 + ch.L2 - 1) / ch.L2 + SB_KO - 1) / SB_KO);
+        max_sbr_l2 = std::max(max_sbr_l2, ch.L2);
+        sbr_smem = std::max(sbr_smem, subband_smem(b.D2, b.T2));
+      }
     }
     for (int k = 0; k < n_sb; k++) {
       const int i = g->sb_list[k];
@@ -2776,11 +2842,17 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     }
     CU_OK(cudaMemcpyAsync(s.d_sbcb, s.h_sbcb, (size_t)n_sb * sizeof(CascBlk), cudaMemcpyHostToDevice, cs));
     if (max_sb_n1 > 0) cascade_append_kernel<<<dim3((max_sb_n1 + 255) / 256, n_sb), 256, 0, cs>>>(s.d_sbcb, s.d_out);
-    if (max_sb_n2 > 0) {
+    if (max_sb_n2 > 0 || max_sbr_ctas > 0) {
       CU_OK(cudaMemcpyAsync(s.d_sbblk, s.h_sbblk, g->sb_classes.size() * sizeof(SbBlk), cudaMemcpyHostToDevice, cs));
       subband_phase_kernel<<<(g->n_sb_mem + 31) / 32, 32, 0, cs>>>(g->d_clients, g->d_sbmem, s.d_sbblk, s.d_sbph);
-      subband_fir_cf32_kernel<<<dim3((max_sb_n2 + SB_KO - 1) / SB_KO, g->n_sb_groups), SB_THREADS, sb_smem, cs>>>(
-          s.d_sbblk, g->d_sbgrp, g->d_sbtaps, s.d_sbph, s.d_out);
+      if (max_sb_n2 > 0)
+        subband_fir_cf32_kernel<<<dim3((max_sb_n2 + SB_KO - 1) / SB_KO, g->n_sb_groups_int), SB_THREADS, sb_smem,
+                                  cs>>>(s.d_sbblk, g->d_sbgrp, g->d_sbtaps, s.d_sbph, s.d_out);
+      // rational classes: their groups follow the integer ones, one CTA layer per residue
+      if (max_sbr_ctas > 0)
+        subband_fir_poly_cf32_kernel<<<dim3(max_sbr_ctas, g->n_sb_groups - g->n_sb_groups_int, max_sbr_l2), SB_THREADS,
+                                       sbr_smem, cs>>>(s.d_sbblk, g->d_sbgrp + g->n_sb_groups_int, g->d_sbtaps,
+                                                       s.d_sbph, s.d_out);
     }
     if (g->profiling) CU_OK(cudaEventRecord(s.pf_sb[1], cs));
     CU_OK(cudaEventRecord(s.ev_casc, cs));

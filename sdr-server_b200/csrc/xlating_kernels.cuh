@@ -1309,6 +1309,13 @@ cascade_fir_poly_cf32_kernel(const CascPolyBlk *__restrict__ pb, const float *__
 // Members of one sub-band with equal (D2, T2, window alignment, first valid position) form a class: they
 // read the same windows, so a CTA stages the windows of a span of outputs once and every staged sample
 // feeds SB_MG members.
+// A rational member (xlg_add_client_subband_rational, L2 > 1) is the reference's float path with decimation
+// M2 at L2 * fs / D1, fed the zero-stuffed ring u[L2*n] = y[n]: output k's upsampled window starts at
+// w = first + k*M2, and with r = (-w) mod L2, n0 = (w + r) / L2 (poly_branch) only branch r of its taps meets
+// sub-band samples,
+//     z[k] = phase_k * sum_{t < Tb2} y[n0 + t] * P[r][t],   P[r][t] = rev2[r + t*L2] (0 past T2).
+// Outputs k and k + L2 share r and their n0 lie M2 apart, so the outputs of one residue rho = k mod L2 are an
+// integer class with decimation M2 and Tb2 taps, strided by L2.
 // ---------------------------------------------------------------------------
 constexpr int SB_WARPS = 4;                  // warps of a CTA; warp w serves members [w*SB_RM, (w+1)*SB_RM)
 constexpr int SB_THREADS = 32 * SB_WARPS;
@@ -1319,16 +1326,17 @@ constexpr int SB_KO = 32 * SB_RO;            // outputs per CTA
 
 struct SbBlk {          // one class, this block
   const float2 *ring;   // its sub-band's history ring
-  long long first;      // ring position where output 0's window starts
+  long long first;      // ring position where output 0's window starts (upsampled position when L2 > 1)
   long long zb;         // ring positions before this read as zero (its members' attach point)
   unsigned mask;        // ring capacity - 1
-  int n2, D2, T2;
+  int n2, D2, T2;       // L2 > 1: D2 = M2 and T2 = Tb2, the taps per branch
 };
 
 struct SbGroup {        // up to SB_MG members of one class (the layout's)
   int cls, n_mem;
-  int taps_off;         // float2 offset of the [SB_MG][sb_tpad(T2)] rotated reversed taps, zero rows for padding
-  int pad_;
+  int taps_off;         // float2 offset of the [L2][SB_MG][sb_tpad(T2)] rotated reversed taps (branch-major
+                        // when L2 > 1), zero rows for padding
+  int l2;               // its class's L2 (1: an integer class)
   int out_off[SB_MG];   // final rows in the slot's output arena
   int ph_off[SB_MG];    // oscillator table: phase of EVEN output k at ph[ph_off + 32 * (k / 2)]
   float2 incr[SB_MG];
@@ -1444,6 +1452,103 @@ subband_fir_cf32_kernel(const SbBlk *__restrict__ blk, const SbGroup *__restrict
     for (int i = 0; i < SB_RO; i++) {
       const int k = k0 + lane + 32 * i;
       if (lane + 32 * i >= nk) continue;
+      float2 p = ph[gp.ph_off[m] + 32 * (k >> 1)];
+      if (k & 1) p = cmul_unfused(p, gp.incr[m]);     // odd outputs: one step from the stored even phase
+      out[gp.out_off[m] + k] = cmul_unfused(acc[i][r], p);  // src/xlating.c:70
+    }
+  }
+}
+
+// Rational classes (SbGroup::l2 > 1), grid (output tiles of the longest residue, groups, largest L2): CTA
+// (x, g, rho) computes outputs rho + L2*q, q in [x*SB_KO, x*SB_KO + SB_KO), of the members of group g -- the
+// integer class of residue rho: its window from n0 of output rho, decimation M2, and branch r(rho)'s taps,
+// staged, walked and rotated as subband_fir_cf32_kernel does.
+__global__ void __launch_bounds__(SB_THREADS)
+subband_fir_poly_cf32_kernel(const SbBlk *__restrict__ blk, const SbGroup *__restrict__ grp,
+                             const float2 *__restrict__ taps, const float2 *__restrict__ ph,
+                             float2 *__restrict__ out) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  uint64_t *bar = reinterpret_cast<uint64_t *>(smem);
+  const SbGroup &gp = grp[blockIdx.y];
+  const SbBlk b = blk[gp.cls];
+  const int L2 = gp.l2, rho = blockIdx.z;
+  if (rho >= min(L2, b.n2)) return;
+  long long first;  // n0 of output rho: the residue's outputs rho + L2*q start their windows at first + q*M2
+  const int br = poly_branch(b.first + (long long)rho * b.D2, L2, &first);
+  const int n2 = (b.n2 - rho + L2 - 1) / L2;
+  const int k0 = blockIdx.x * SB_KO;
+  if (k0 >= n2) return;
+  const int D2 = b.D2, T2 = b.T2, tpad = sb_tpad(T2);
+  const int nk = min(SB_KO, n2 - k0);
+  float2 *ts = reinterpret_cast<float2 *>(smem + 16);
+  float2 *xs = ts + (size_t)SB_MG * tpad;
+  const long long w0 = first + (long long)k0 * D2;
+  const unsigned idx = (unsigned)((unsigned long long)w0) & b.mask;
+  const unsigned shift = idx & 1u;
+  const unsigned need = ((unsigned)((nk - 1) * D2 + T2) + shift + 1u) & ~1u;
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    mbar_init(bar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  __syncthreads();
+  if (tid == 0) {
+    const unsigned tbytes = (unsigned)(SB_MG * tpad) * 8u;
+    const unsigned p1 = min(need, b.mask + 1u - (idx - shift));
+    mbar_expect_tx(bar, tbytes + need * 8u);
+    tma_bulk_g2s(ts, taps + gp.taps_off + (size_t)br * SB_MG * tpad, tbytes, bar);  // branch br's rows
+    tma_bulk_g2s(xs, b.ring + (idx - shift), p1 * 8u, bar);
+    if (p1 < need) tma_bulk_g2s(xs + p1, b.ring, (need - p1) * 8u, bar);
+  }
+  mbar_wait(bar, 0);
+  const long long base = w0 - (long long)shift;
+  if (b.zb > base) {  // a class attached mid-stream: its members read zeros before their attach point
+    for (unsigned i = tid; i < need; i += SB_THREADS)
+      if (base + (long long)i < b.zb) xs[i] = make_float2(0.f, 0.f);
+    __syncthreads();
+  }
+  const int warp = tid >> 5, lane = tid & 31;
+  const int m0 = warp * SB_RM;
+  if (m0 >= gp.n_mem) return;
+  const float2 *x[SB_RO];
+#pragma unroll
+  for (int i = 0; i < SB_RO; i++) x[i] = xs + shift + (size_t)min(lane + 32 * i, nk - 1) * D2;
+  const float2 *t[SB_RM];
+#pragma unroll
+  for (int r = 0; r < SB_RM; r++) t[r] = ts + (size_t)(m0 + r) * tpad;
+  float2 acc[SB_RO][SB_RM];
+#pragma unroll
+  for (int i = 0; i < SB_RO; i++)
+#pragma unroll
+    for (int r = 0; r < SB_RM; r++) acc[i][r] = make_float2(0.f, 0.f);
+  int j = (D2 & 1) ? 0 : lane % T2;
+#pragma unroll 2
+  for (int s = 0; s < T2; s++) {
+    float2 v[SB_RO], h[SB_RM];
+#pragma unroll
+    for (int i = 0; i < SB_RO; i++) v[i] = x[i][j];
+#pragma unroll
+    for (int r = 0; r < SB_RM; r++) h[r] = t[r][j];
+#pragma unroll
+    for (int i = 0; i < SB_RO; i++)
+#pragma unroll
+      for (int r = 0; r < SB_RM; r++) {
+        acc[i][r].x = fmaf(v[i].x, h[r].x, acc[i][r].x);
+        acc[i][r].x = fmaf(-v[i].y, h[r].y, acc[i][r].x);
+        acc[i][r].y = fmaf(v[i].x, h[r].y, acc[i][r].y);
+        acc[i][r].y = fmaf(v[i].y, h[r].x, acc[i][r].y);
+      }
+    if (++j == T2) j = 0;
+  }
+#pragma unroll
+  for (int r = 0; r < SB_RM; r++) {
+    const int m = m0 + r;
+    if (m >= gp.n_mem) break;
+#pragma unroll
+    for (int i = 0; i < SB_RO; i++) {
+      if (lane + 32 * i >= nk) continue;
+      const int k = rho + L2 * (k0 + lane + 32 * i);  // the member's output
       float2 p = ph[gp.ph_off[m] + 32 * (k >> 1)];
       if (k & 1) p = cmul_unfused(p, gp.incr[m]);     // odd outputs: one step from the stored even phase
       out[gp.out_off[m] + k] = cmul_unfused(acc[i][r], p);  // src/xlating.c:70

@@ -7,8 +7,12 @@ Workloads (centres drawn uniformly across the band from a fixed seed):
   61M_1024   1024 clients at 48 kHz on a 61.44 Msps cs16 stream
   61M_4096   4096 clients at 48 kHz on a 61.44 Msps cs16 stream
   2M_256     256 clients on a 2.016 Msps cu8 stream, 48 and 96 kHz alternating
-Plans, alternated within every round: "single" (client_plan's taps, one integer client each), "cascade"
-(cascade_plan) and "subband" (subband_plan).
+  2048k_256  256 clients at 48 kHz on a 2.048 Msps cu8 stream (RTL-SDR)
+  10M_256    256 clients at 48 kHz on a 10 Msps cs16 stream (Airspy)
+  20M_256    256 clients at 48 kHz on a 20 Msps cs8 stream (HackRF)
+Plans, alternated within every round: "single" (one client each: client_plan's taps as an integer client, or
+rational_plan's as a rational client where the rate does not divide fs), "cascade" (cascade_plan) and
+"subband" (subband_plan; at the last three rates its members resample by a rational L2 / M2).
 
 Per workload and plan (one JSON line each): input MS/s and step time over K pipelined blocks (CUDA events,
 xlg_timer_*), algorithmic real FMAs per input sample from the shapes, and from a profiled run of its own (one
@@ -37,6 +41,9 @@ WORKLOADS = {  # fs, format, clients, rates
     "61M_1024": (61440000, "cs16", 1024, (48000,)),
     "61M_4096": (61440000, "cs16", 4096, (48000,)),
     "2M_256": (2016000, "cu8", 256, (48000, 96000)),
+    "2048k_256": (2048000, "cu8", 256, (48000,)),
+    "10M_256": (10000000, "cs16", 256, (48000,)),
+    "20M_256": (20000000, "cs8", 256, (48000,)),
 }
 PLANS = ("single", "cascade", "subband")
 SAMPLED = 3
@@ -54,14 +61,24 @@ def build(name, plan, profile):
     """The group of one plan, its client ids, FMAs per input sample, and oracles of SAMPLED clients
     (callables block -> cf32 outputs)."""
     from cascade import cascade_oracle
+    from cascade_rational import RationalCascadeOracle
     from oracle import pyoracle as po
-    from subband import SubbandOracle
+    from rational import oracle_filter, stuff
+    from subband_rational import RationalSubbandOracle
     fs, fmt, n, _ = WORKLOADS[name]
     clients = workload_clients(name)
     g = pkg.Group(fs, BLOCK)
     picks = [0, n // 2, n - 1]
     oracles = []
-    if plan == "single":
+    if plan == "single" and any(fs % r for _, r in clients):
+        rp = pkg.rational_plan(fs, [r for _, r in clients])
+        ids = [g.add_client_rational(q["interp"], q["decim"], q["taps"], c) for q, (c, _) in zip(rp, clients)]
+        fmas = sum(4.0 * -(-q["taps"].size // q["interp"]) * q["rate"] / fs for q in rp)
+        for k in picks:
+            q, (c, _) = rp[k], clients[k]
+            o = oracle_filter(po, q["interp"], q["decim"], q["taps"], c, fs, BLOCK)
+            oracles.append((ids[k], lambda x, o=o, L=q["interp"]: o.process_cf32("cs16", stuff(fmt, x, L))))
+    elif plan == "single":
         taps = {r: pkg.create_low_pass_filter(1.0, fs, r // 2, r // 5) for _, r in clients}
         ids = [g.add_client(fs // r, taps[r], c) for c, r in clients]
         fmas = sum(4.0 * taps[r].size / (fs // r) for _, r in clients)
@@ -77,17 +94,19 @@ def build(name, plan, profile):
         for k in picks:
             c, r = clients[k]
             p = plans[r]
-            o = cascade_oracle(p["d1"], p["taps1"], c, p["d2"], p["taps2"], fs, BLOCK)
+            o = (RationalCascadeOracle(p["d1"], p["taps1"], c, p["interp2"], p["d2"], p["taps2"], fs, BLOCK)
+                 if p["interp2"] > 1 else cascade_oracle(p["d1"], p["taps1"], c, p["d2"], p["taps2"], fs, BLOCK))
             oracles.append((ids[k], lambda x, o=o: o.process_cf32(fmt, x)))
     else:
         p = pkg.subband_plan(fs, clients)
         sids = [g.add_subband(p["d1"], p["taps1"], sb["center"]) for sb in p["subbands"]]
-        ids = [g.add_client_subband(sids[m["subband"]], m["d2"], m["taps2"], m["offset"]) for m in p["members"]]
+        ids = [g.add_client_subband(sids[m["subband"]], m["d2"], m["taps2"], m["offset"], m["interp2"])
+               for m in p["members"]]
         fmas = p["fmas"]
         for k in picks:
             m = p["members"][k]
-            o = SubbandOracle(p["d1"], p["taps1"], p["subbands"][m["subband"]]["center"], fs, BLOCK)
-            o.add_member(0, m["d2"], m["taps2"], m["offset"])
+            o = RationalSubbandOracle(p["d1"], p["taps1"], p["subbands"][m["subband"]]["center"], fs, BLOCK)
+            o.add_member(0, m["d2"], m["taps2"], m["offset"], m["interp2"])
             oracles.append((ids[k], lambda x, o=o: o.process_cf32(fmt, x)[0]))
     if profile:
         g.profile_enable(True)
