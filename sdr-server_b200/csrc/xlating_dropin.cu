@@ -285,17 +285,9 @@ struct xlating_t {
   // integer filter whose FilterDev::out is its stage-A row in the engine's CascArena
   bool casc = false;
   float *adopted_taps2 = nullptr;
-  uint32_t L2 = 1, D2 = 0;     // stage B's interpolation and decimation
-  long long T2 = 0;
-  int Tb2 = 0;                 // taps per polyphase branch (L2 > 1)
-  int ko2 = 0;                 // stage-B outputs per CTA: C_KO halved to fit (L2 = 1), cascade_poly_ko (L2 > 1)
-  long long hist2 = 0;         // stage B's history_offset (upsampled samples when L2 > 1)
-  long long a_pos = 0;         // stage-A outputs so far: the ring's stream position
-  int fin_cap = 0;             // stage-B outputs of one call at most
-  float2 *d_cring = nullptr;   // stage-A history ring (inside d_mem), cring_cap samples, a power of two
-  size_t cring_cap = 0;
+  StageB b2;                   // its ring lies inside d_mem; taps_off (floats) and fin_off (float2) in the region
   size_t arena_off = 0, arena_len = 0;  // the filter's CascArena region, float2 units
-  int taps2_off = 0, a_off = 0, b_off = 0;  // stage-B taps (floats), stage-A and stage-B rows (float2) in it
+  int a_off = 0;               // stage-A row (float2) in it
   CascBlk cblk;                // this call's stage B
   CascPolyBlk pblk;            // (L2 > 1)
   int req_out2 = 0;            // this call's stage-B outputs
@@ -432,7 +424,8 @@ cudaError_t run_cascades(Engine *e, Lane &L, CombinerCall *const *batch, int n_r
     if (b->casc) cs.push_back(b);
   }
   std::stable_sort(cs.begin(), cs.end(), [](const xlating *x, const xlating *y) {
-    return (x->L2 == 1) != (y->L2 == 1) ? x->L2 == 1 : (x->L2 == 1 && x->ko2 > y->ko2);
+    const bool xi = x->b2.geo.L2 == 1, yi = y->b2.geo.L2 == 1;
+    return xi != yi ? xi : (xi && x->b2.ko > y->b2.ko);
   });
   cudaError_t err = lane_casc_tables(L);
   if (err != cudaSuccess) return err;
@@ -442,15 +435,15 @@ cudaError_t run_cascades(Engine *e, Lane &L, CombinerCall *const *batch, int n_r
   for (int c = 0; c < n_casc; c++) {
     const xlating *b = cs[c];
     L.h_cblk[c] = b->cblk;
-    L.h_cout[c] = {b->d_out, b->b_off, b->req_out2};
+    L.h_cout[c] = {b->d_out, b->b2.fin_off, b->req_out2};
     max_n1 = std::max(max_n1, b->cblk.n1);
     max_n2 = std::max(max_n2, b->req_out2);
-    if (b->L2 == 1) {
+    if (b->b2.geo.L2 == 1) {
       n_int++;
     } else {
       L.h_pblk[n_rat++] = b->pblk;
-      max_rat_ctas = std::max(max_rat_ctas, (b->pblk.n2 + b->ko2 - 1) / b->ko2);
-      poly_smem = std::max(poly_smem, cascade_poly_smem(b->ko2, (int)b->L2, (int)b->D2, b->Tb2));
+      max_rat_ctas = std::max(max_rat_ctas, (b->pblk.n2 + b->b2.ko - 1) / b->b2.ko);
+      poly_smem = std::max(poly_smem, cascade_poly_smem(b->b2.ko, (int)b->b2.geo.L2, (int)b->b2.geo.D2, b->b2.geo.Tb2));
     }
   }
   const cudaStream_t st = L.stream;
@@ -463,12 +456,12 @@ cudaError_t run_cascades(Engine *e, Lane &L, CombinerCall *const *batch, int n_r
   float2 *base = e->casc.base;
   if (max_n1 > 0) cascade_launch_append(L.d_cblk, n_casc, max_n1, base, st);
   for (int c0 = 0; c0 < n_int;) {
-    const int ko = cs[c0]->ko2;
+    const int ko = cs[c0]->b2.ko;
     int c1 = c0, run_n2 = 0;
     size_t smem = 0;
-    for (; c1 < n_int && cs[c1]->ko2 == ko; c1++) {
+    for (; c1 < n_int && cs[c1]->b2.ko == ko; c1++) {
       run_n2 = std::max(run_n2, cs[c1]->cblk.n2);
-      smem = std::max(smem, cascade_smem(ko, (int)cs[c1]->D2, (int)cs[c1]->T2));
+      smem = std::max(smem, cascade_smem(ko, cs[c1]->cblk.D2, cs[c1]->cblk.T2));
     }
     if (run_n2 > 0) cascade_launch_fir(L.d_cblk + c0, c1 - c0, run_n2, ko, smem, (const float *)base, base, st);
     c0 = c1;
@@ -730,13 +723,14 @@ void casc_give(CascArena &a, size_t off, size_t len) {
     a.holes[off] = len;
 }
 
-// Give cascade filter f (its FilterDev already in the table) its arena region: stage-B taps `taps2` (floats,
-// a multiple of 4), then its stage-A row (out_cap) and its stage-B row (fin_cap).
-int casc_attach(xlating *f, const std::vector<float> &taps2) {
+// Give cascade filter f (its FilterDev already in the table) its arena region: its stage-B taps (floats, a
+// multiple of 4), then its stage-A row (out_cap) and its stage-B row (fin_cap).
+int casc_attach(xlating *f) {
   Engine *e = f->e;
   CascArena &a = e->casc;
+  const std::vector<float> &taps2 = f->b2.taps;
   const size_t n_taps = align4(taps2.size() / 2);
-  const size_t len = n_taps + align4((size_t)f->out_cap) + align4((size_t)f->fin_cap);
+  const size_t len = n_taps + align4((size_t)f->out_cap) + align4((size_t)f->b2.fin_cap);
   std::unique_lock<std::shared_mutex> moving(a.move_mu, std::defer_lock);
   std::unique_lock<std::mutex> lk(a.mu);
   cudaError_t err = cudaSuccess;
@@ -785,9 +779,9 @@ int casc_attach(xlating *f, const std::vector<float> &taps2) {
     XL_LOG("cascade filters need more than 8 GiB of device memory");
     return -ENOMEM;
   }
-  f->taps2_off = (int)(2 * off);
+  f->b2.taps_off = (int)(2 * off);
   f->a_off = (int)(off + n_taps);
-  f->b_off = (int)(off + n_taps + align4((size_t)f->out_cap));
+  f->b2.fin_off = (int)(off + n_taps + align4((size_t)f->out_cap));
   err = cudaMemcpy(a.base + off, taps2.data(), taps2.size() * sizeof(float), cudaMemcpyHostToDevice);
   if (err == cudaSuccess) err = casc_point(e, f);
   if (err != cudaSuccess) {
@@ -849,23 +843,6 @@ struct CascSpec {
   size_t T2;
 };
 
-// Stage B's taps as the batch group keeps them (xlg_add_client_cascade_rational): the reference filter at
-// L2 * fs / D1 with centre 0, whose rotated taps are (h, +-0), so the real parts of the reversed taps;
-// branch-major P[r][t] = rev2[r + t * L2] when L2 > 1; zero-padded to whole 16-byte units.
-int casc_taps(const CascSpec &cs, uint32_t decim1, uint32_t sampling_freq, std::vector<float> *out) {
-  const uint64_t rate2 = (uint64_t)cs.L2 * std::max<uint32_t>(sampling_freq / decim1, 1);
-  xl_client_consts k2;
-  const int rc = xl_client_consts_build(cs.taps2, cs.T2, cs.D2, 0, (uint32_t)std::min<uint64_t>(rate2, UINT32_MAX), &k2);
-  if (rc != 0) return rc;
-  const size_t Tb2 = (cs.T2 + cs.L2 - 1) / cs.L2;
-  std::vector<float> packed(2 * (size_t)cs.L2 * Tb2);
-  xl_poly_pack(k2.rev_cf32, cs.T2, cs.L2, packed.data());  // L2 = 1: the reversed taps themselves
-  xl_client_consts_free(&k2);
-  out->assign(align4((size_t)cs.L2 * Tb2), 0.f);
-  for (size_t j = 0; j < (size_t)cs.L2 * Tb2; j++) (*out)[j] = packed[2 * j];
-  return 0;
-}
-
 // A filter with interpolation L > 1 is the filter with decimation M = `decimation` at L * fs fed the
 // zero-stuffed stream (create_rational_frequency_xlating_filter): its constants are built at L * fs, its
 // taps are kept as polyphase branches and it has no Q15 ring or taps.  L = 1 is the integer filter.  With
@@ -879,9 +856,9 @@ int filter_build(xlating *f, int device, uint32_t interp, uint32_t decimation, c
     f->e = nullptr;
     return rc;
   }
-  std::vector<float> taps2;
   if (cs != nullptr) {
-    rc = casc_taps(*cs, decimation, sampling_freq, &taps2);
+    // the batch group's stage B (xlg_add_client_cascade_rational), ko included
+    rc = stage_b_init(&f->b2, cs->taps2, cs->T2, cs->L2, cs->D2, sampling_freq / decimation);
     if (rc != 0) return rc;
   }
   xl_client_consts k;
@@ -908,27 +885,12 @@ int filter_build(xlating *f, int device, uint32_t interp, uint32_t decimation, c
   size_t cring_cap = 0;
   if (cs != nullptr) {
     f->casc = true;
-    f->L2 = cs->L2;
-    f->D2 = cs->D2;
-    f->T2 = (long long)cs->T2;
-    f->Tb2 = (int)((cs->T2 + cs->L2 - 1) / cs->L2);
-    f->hist2 = f->T2 - 1;  // src/xlating.c:552 (upsampled samples when L2 > 1)
-    // n2 <= (L2 * n1 - 1) / D2 + 1 for any history
-    f->fin_cap = (int)((uint64_t)f->out_cap * cs->L2 / cs->D2 + 2);
-    if (cs->L2 == 1) {
-      f->ko2 = C_KO;  // what a group of this one client launches
-      while (f->ko2 > 1 && cascade_smem(f->ko2, (int)cs->D2, (int)cs->T2) > (size_t)kTileMaxSmem) f->ko2 /= 2;
-    } else {
-      f->ko2 = cascade_poly_ko((int)cs->L2, (int)cs->D2, f->Tb2);
-    }
-    // a call completes before the next one starts: the stage-B history of at most T2 - 1 upsampled samples
-    // (ceil((T2 - 1) / L2) stage-A samples, and one zero-weighted sample past the last branch) plus one
-    // call's stage-A outputs
-    const size_t back = (cs->T2 - 1 + cs->L2 - 1) / cs->L2 + 1;
+    f->b2.fin_cap = stage_b_rows((uint64_t)f->out_cap, cs->L2, cs->D2);
+    // a call completes before the next one starts: stage B's history plus one call's stage-A outputs
     cring_cap = 64;
-    while (cring_cap < back + (size_t)f->out_cap) cring_cap <<= 1;
+    while (cring_cap < history_reach(cs->T2, cs->L2) + (size_t)f->out_cap) cring_cap <<= 1;
   }
-  const int host_out = cs != nullptr ? f->fin_cap : f->out_cap;  // outputs the pinned buffer receives
+  const int host_out = cs != nullptr ? f->b2.fin_cap : f->out_cap;  // outputs the pinned buffer receives
   FilterDev d;
   memset(&d, 0, sizeof(d));
   // device arena
@@ -997,8 +959,10 @@ int filter_build(xlating *f, int device, uint32_t interp, uint32_t decimation, c
   if (cs == nullptr) f->tail.assign((taps_len - 1) / interp, make_float2(0.f, 0.f));  // src/xlating.c:552-565
   f->d_ring = (float2 *)(dm + o_ring);
   f->ring_cap = cap;
-  f->d_cring = cs != nullptr ? (float2 *)(dm + o_cring) : nullptr;
-  f->cring_cap = cring_cap;
+  if (cs != nullptr) {
+    f->b2.ring.p = (float2 *)(dm + o_cring);
+    f->b2.ring.cap = cring_cap;
+  }
   d.ring = (float2 *)(dm + o_ring);
   d.qring = q15 ? (short2 *)(dm + o_qring) : nullptr;
   d.taps = (const float2 *)(dm + o_taps);
@@ -1030,7 +994,7 @@ int filter_build(xlating *f, int device, uint32_t interp, uint32_t decimation, c
   }
   CU_TRY(cudaMemcpy(f->e->d_filters + f->slot, &d, sizeof(d), cudaMemcpyHostToDevice));
   if (cs != nullptr) {
-    rc = casc_attach(f, taps2);  // also points d.out at the stage-A row
+    rc = casc_attach(f);  // also points d.out at the stage-A row
     if (rc != 0) goto fail;
   }
   f->e->live_filters++;
@@ -1157,37 +1121,11 @@ void run_block(xlating *f, int fmt, const void *input, size_t input_len, bool q1
   if (last_ok >= first) n_out = (int)((last_ok - first) / (long long)f->D) + 1;
   if (n_out > f->out_cap) n_out = f->out_cap;
   if (f->casc) {
-    // stage B: the group's host walk over this call's n_out stage-A samples, upsampled by L2 (the
-    // zero-stuffed stream u[L2 * n] = y[n]; the same integers for L2 = 1)
-    const long long first2 = (long long)f->L2 * f->a_pos - f->hist2;
-    const int n2 = xl_walk(&f->hist2, (long long)f->L2 * n_out, (size_t)f->T2, f->D2, f->fin_cap);
-    CascBlk &cb = f->cblk;
-    cb.ring = f->d_cring;
-    cb.a_pos = f->a_pos;
-    cb.first = first2;
-    cb.mask = (unsigned)(f->cring_cap - 1);
-    cb.a_off = f->a_off;
-    cb.n1 = n_out;
-    cb.n2 = n2;
-    cb.D2 = (int)f->D2;
-    cb.T2 = (int)f->T2;
-    cb.taps_off = f->taps2_off;
-    cb.out_off = f->b_off;
-    if (f->L2 > 1) {
-      CascPolyBlk &pb = f->pblk;
-      pb.ring = f->d_cring;
-      pb.first = first2;
-      pb.mask = cb.mask;
-      pb.n2 = n2;
-      pb.L2 = (int)f->L2;
-      pb.M2 = (int)f->D2;
-      pb.Tb2 = f->Tb2;
-      pb.ko = f->ko2;
-      pb.taps_off = f->taps2_off;
-      pb.out_off = f->b_off;
-    }
-    f->a_pos += n_out;
-    f->req_out2 = n2;
+    // stage B: the group's host walk and tables over this call's n_out stage-A samples
+    const StageBStep w = stage_b_walk(f->b2.geo, f->b2.ring.pos, n_out, f->b2.fin_cap);
+    stage_b_fill(f->b2, w, n_out, f->a_off, &f->cblk, &f->pblk);
+    f->b2.ring.pos += n_out;
+    f->req_out2 = w.n2;
   }
   f->req.raw = slot >= 0 ? e->cache->device_ptr(slot) : f->d_in;
   f->req_slot = slot;
@@ -1304,13 +1242,7 @@ int create_rational_frequency_xlating_filter(uint32_t interpolation, uint32_t de
   }
   // the batch group's rules (xlg_add_client_rational), checked before any CUDA call
   const uint32_t max_in = max_input_buffer_length < 2 ? 2 : max_input_buffer_length;
-  const char *why = NULL;
-  if (interpolation == 0 || decimation == 0)
-    why = "interpolation and decimation must both be at least 1";
-  else if ((uint64_t)interpolation * sampling_freq > UINT32_MAX)
-    why = "the upsampled rate interpolation x sampling_freq exceeds UINT32_MAX";
-  else if ((uint64_t)interpolation * (max_in / 2) >= (1ull << 31))
-    why = "interpolation x max_input_buffer_length / 2 upsampled samples per call reach 2^31";
+  const char *why = rational_refusal(sampling_freq, max_in, interpolation, decimation);
   if (why != NULL) {
     XL_LOG("rational filter %u/%u at %u Hz, blocks of %u: %s", interpolation, decimation, sampling_freq, max_in, why);
     free(taps);  // adopted, as on every other failure but taps_len == 0
@@ -1332,17 +1264,7 @@ int create_cascade_frequency_xlating_filter(uint32_t decimation1, float *taps1, 
   }
   // the batch group's rules (xlg_add_client_cascade_rational), checked before any CUDA call
   const uint32_t max_in = max_input_buffer_length < 2 ? 2 : max_input_buffer_length;
-  const char *why = NULL;
-  if (decimation1 == 0 || decimation2 == 0 || interpolation2 == 0)
-    why = "decimation1, interpolation2 and decimation2 must all be at least 1";
-  else if (interpolation2 > 1 && (uint64_t)interpolation2 * (max_in / 2 / decimation1 + 2) >= (1ull << 31))
-    why = "interpolation2 x (max_input_buffer_length / 2 / decimation1 + 2) upsampled stage-A samples per call reach 2^31";
-  else if (taps2_len > (size_t)INT32_MAX ||
-           (interpolation2 == 1
-                ? cascade_smem(1, (int)decimation2, (int)taps2_len)
-                : cascade_poly_smem(1, (int)interpolation2, (int)decimation2,
-                                    (int)((taps2_len + interpolation2 - 1) / interpolation2))) > (size_t)kTileMaxSmem)
-    why = "stage B's taps and one output's window exceed the stage-B kernels' shared memory";
+  const char *why = cascade_refusal(max_in, decimation1, interpolation2, decimation2, taps2_len);
   if (why != NULL) {
     XL_LOG("cascade filter %u x %u/%u with %zu + %zu taps at %u Hz, blocks of %u: %s", decimation1, interpolation2,
            decimation2, taps1_len, taps2_len, sampling_freq, max_in, why);

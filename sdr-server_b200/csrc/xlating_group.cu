@@ -14,9 +14,9 @@
  *                    for the tiled kernel's TMA chunks
  *   per slot (XLG_SLOTS in flight): raw input staging, BlkInfo, per-output
  *                    oscillator table, output arena (+ pinned host mirrors)
- *   cascade clients  a stage-A history ring each (HostClient::d_cring), their stage-B taps
+ *   cascade clients  a stage-A history ring each (HostClient::b2.ring), their stage-B taps
  *                    (d_taps2); stage-A rows follow the host-visible rows of the arena
- *   sub-bands        a history ring each (HostClient::d_cring), rows after the host-visible ones;
+ *   sub-bands        a history ring each (HostClient::b2.ring), rows after the host-visible ones;
  *                    their members' taps packed per group of SB_MG (d_sbtaps, SbGroup; branch-major
  *                    for rational members), and per slot the members' oscillator table (d_sbph)
  *
@@ -116,29 +116,19 @@ struct HostClient {
   bool pending_settle = false;   // still inside its zero-history window at the last layout rebuild
   int poly_off = 0, poly_rowcap = 0;  // kind 4: its branches' rows in the slot's polyphase scratch
   // cascade client (xlg_add_client_cascade): everything above describes its stage A, an integer client
-  // whose out_off row lies after every host-visible row; stage B is described here
+  // whose out_off row lies after every host-visible row; stage B is described in b2
   bool casc = false;
-  uint32_t L2 = 1, D2 = 0;       // stage B's interpolation (> 1: xlg_add_client_cascade_rational) and decimation
-  size_t T2 = 0;
-  int Tb2 = 0, ko2 = 0;          // L2 > 1: taps per branch, outputs per CTA of cascade_fir_poly_cf32_kernel
-  std::vector<float> rev2;       // stage B's reversed taps (the real parts of its rotated taps at centre 0),
-                                 // packed branch-major (xl_poly_pack) when L2 > 1
-  long long hist2 = 0;           // stage B's history_offset, in stage-A samples (upsampled when L2 > 1)
-  long long a_pos = 0;           // stage-A outputs produced since the attach: the ring's stream position
-  float2 *d_cring = nullptr;     // stage-A history ring, cring_cap samples (a power of two)
-  size_t cring_cap = 0;
-  int fin_off = 0, fin_cap = 0;  // final row of the slot's output arena
-  int taps2_off = 0;             // rev2 in the real tap arena
+  StageB b2;                     // (its fin_off / fin_cap: the final row of the slot's output arena)
   int last_n2 = 0;               // stage-B outputs of the block being submitted
   // sub-band (xlg_add_subband): an integer client, not visible to the caller, whose row lies after every
-  // host-visible row; d_cring, cring_cap and a_pos above are its history ring
+  // host-visible row; b2.ring is its history ring
   bool sb = false;
   int sb_id = -1;
   // sub-band member (xlg_add_client_subband[_rational]): not an integer client -- its ClientDev only carries
-  // its oscillator; L2, D2, T2, Tb2, hist2 (in sub-band samples, upsampled when L2 > 1) and last_n2 above are
-  // its own, rev2 holds its rotated reversed taps (2 * T2 floats; branch-major, 2 * L2 * Tb2, when L2 > 1),
-  // out_off / out_cap its final row
+  // its oscillator; b2.geo is its filter (in sub-band samples), mtaps its rotated reversed taps (2 * T2 floats;
+  // branch-major, 2 * L2 * Tb2, when L2 > 1), out_off / out_cap its final row
   bool mem = false;
+  std::vector<float> mtaps;
   int sb_cid = -1;               // its sub-band's client index
   long long zb2 = 0;             // sub-band position of its attach point: earlier samples read as zero
   int ph_row = 0;                // its rows of the slot's member oscillator table
@@ -151,6 +141,32 @@ struct SbClassHost {
   int L2, Tb;    // Tb: taps per branch (T2 when L2 = 1)
   std::vector<int> members;
   long long zb;  // the largest attach point of its members
+};
+
+// A per-slot table the host fills each block and the kernels read: pinned entries and their device copy.
+template <typename T>
+struct BlkTable {
+  T *h = nullptr, *d = nullptr;
+  size_t cap = 0;
+  // room for n entries (the pipeline is drained); a table grows to max(2n, 16)
+  int reserve(size_t n) {
+    if (cap >= n) return 0;
+    release();
+    const size_t want = std::max<size_t>(n * 2, 16);
+    CU_OK(cudaMalloc(&d, want * sizeof(T)));
+    CU_OK(cudaHostAlloc(&h, want * sizeof(T), cudaHostAllocDefault));
+    cap = want;
+    return 0;
+  }
+  cudaError_t upload(size_t n, cudaStream_t s) const {
+    return cudaMemcpyAsync(d, h, n * sizeof(T), cudaMemcpyHostToDevice, s);
+  }
+  void release() {
+    if (d) cudaFree(d);
+    if (h) cudaFreeHost(h);
+    d = h = nullptr;
+    cap = 0;
+  }
 };
 
 struct Slot {
@@ -172,18 +188,15 @@ struct Slot {
   float2 *d_pscratch = nullptr;  // kind 4: unrotated outputs per branch (ClientDev::poly_off)
   BlkInfo *d_vblk = nullptr, *h_vblk = nullptr;  // kind 4: per branch class, this block's window start and count
   uint64_t poly_macs = 0;
-  CascBlk *d_cblk = nullptr, *h_cblk = nullptr;  // cascade clients: this block's ring positions, windows and counts
-  size_t cblk_cap = 0;                           // (integer stage B first, then the rational ones)
-  CascPolyBlk *d_pblk = nullptr, *h_pblk = nullptr;  // rational cascade clients: this block's stage B
-  size_t pblk_cap = 0;
+  BlkTable<CascBlk> cblk;        // cascade clients: this block's ring positions, windows and counts
+                                 // (integer stage B first, then the rational ones)
+  BlkTable<CascPolyBlk> pblk;    // rational cascade clients: this block's stage B
   cudaEvent_t ev_casc = nullptr;                 // stage B of this block done (its rings' appends are ordered on it)
   cudaEvent_t pf_casc[2] = {nullptr, nullptr};
   bool pf_cb = false;
   uint64_t casc_macs = 0, d2h_bytes = 0;
-  CascBlk *d_sbcb = nullptr, *h_sbcb = nullptr;  // sub-bands: this block's ring appends
-  size_t sbcb_cap = 0;
-  SbBlk *d_sbblk = nullptr, *h_sbblk = nullptr;  // member classes: this block's windows and counts
-  size_t sbblk_cap = 0;
+  BlkTable<CascBlk> sbcb;        // sub-bands: this block's ring appends
+  BlkTable<SbBlk> sbblk;         // member classes: this block's windows and counts
   float2 *d_sbph = nullptr;                      // member oscillator table (HostClient::ph_row)
   cudaEvent_t pf_sb[2] = {nullptr, nullptr};
   bool pf_sbk = false;
@@ -453,23 +466,12 @@ static void slot_free(Slot &s) {
   if (s.d_pscratch) cudaFree(s.d_pscratch);
   if (s.d_vblk) cudaFree(s.d_vblk);
   if (s.h_vblk) cudaFreeHost(s.h_vblk);
-  if (s.d_cblk) cudaFree(s.d_cblk);
-  if (s.h_cblk) cudaFreeHost(s.h_cblk);
-  s.d_cblk = s.h_cblk = nullptr;
-  s.cblk_cap = 0;
-  if (s.d_pblk) cudaFree(s.d_pblk);
-  if (s.h_pblk) cudaFreeHost(s.h_pblk);
-  s.d_pblk = s.h_pblk = nullptr;
-  s.pblk_cap = 0;
-  if (s.d_sbcb) cudaFree(s.d_sbcb);
-  if (s.h_sbcb) cudaFreeHost(s.h_sbcb);
-  if (s.d_sbblk) cudaFree(s.d_sbblk);
-  if (s.h_sbblk) cudaFreeHost(s.h_sbblk);
+  s.cblk.release();
+  s.pblk.release();
+  s.sbcb.release();
+  s.sbblk.release();
   if (s.d_sbph) cudaFree(s.d_sbph);
-  s.d_sbcb = s.h_sbcb = nullptr;
-  s.d_sbblk = s.h_sbblk = nullptr;
   s.d_sbph = nullptr;
-  s.sbcb_cap = s.sbblk_cap = 0;
   s.d_pscratch = nullptr;
   s.d_vblk = s.h_vblk = nullptr;
   s.d_endph = nullptr;
@@ -675,6 +677,29 @@ static int dev_assign(T **dptr, size_t *cap_bytes, const void *src, size_t bytes
   CU_OK(cudaMemcpy(*dptr, src, bytes, cudaMemcpyHostToDevice));
   return 0;
 }
+// Give a cascade's or a sub-band's history ring room for cap samples (a power of two; the pipeline is drained):
+// a new ring is zero, which its positions before the attach read, and a grown one keeps its last samples at
+// their new places.
+static int ring_ensure(HistRing &r, size_t cap) {
+  if (r.p != nullptr && cap <= r.cap) return 0;
+  float2 *ring = nullptr;
+  CU_OK(cudaMalloc(&ring, cap * sizeof(float2)));
+  if (r.p == nullptr) {
+    CU_OK(cudaMemset(ring, 0, cap * sizeof(float2)));
+  } else {
+    std::vector<float2> old(r.cap), fresh(cap, make_float2(0.f, 0.f));
+    CU_OK(cudaMemcpy(old.data(), r.p, r.cap * sizeof(float2), cudaMemcpyDeviceToHost));
+    for (size_t k = 1; k <= r.cap; k++) {
+      const unsigned long long p = (unsigned long long)(r.pos - (long long)k);
+      fresh[p & (cap - 1)] = old[p & (r.cap - 1)];
+    }
+    CU_OK(cudaMemcpy(ring, fresh.data(), cap * sizeof(float2), cudaMemcpyHostToDevice));
+    cudaFree(r.p);
+  }
+  r.p = ring;
+  r.cap = cap;
+  return 0;
+}
 // first input sample a client's next window reads: floor((L*S - hist) / L)  (S - hist for integer clients)
 static long long first_input(const HostClient &h, long long S) {
   const long long fu = S * h.L - h.hist;
@@ -704,15 +729,14 @@ static int rebuild_subbands(xlg_group *g, size_t &out_total) {
   for (int i = 0; i < nc; i++) {
     const HostClient &h = g->clients[i];
     if (!h.active || !h.mem) continue;
-    // a rational member's history of at most T2 - 1 upsampled samples reaches back ceil((T2 - 1) / L2)
-    // sub-band samples, and its last branch may read one zero-weighted sample past the block
-    back[h.sb_cid] = std::max(back[h.sb_cid], h.L2 == 1 ? h.T2 - 1 : (h.T2 - 1 + h.L2 - 1) / h.L2 + 1);
+    const StageBGeom &b = h.b2.geo;
+    back[h.sb_cid] = std::max(back[h.sb_cid], history_reach(b.T2, b.L2));
     // its window has passed its attach point: it reads what every settled member of the class reads
-    const bool settled = h.zb2 * (long long)h.L2 <= (long long)h.L2 * g->clients[h.sb_cid].a_pos - h.hist2;
-    if (h.L2 == 1) {
-      keyed[std::make_tuple(h.sb_cid, h.D2, h.T2, h.hist2, settled ? LLONG_MIN : h.zb2)].push_back(i);
+    const bool settled = h.zb2 * (long long)b.L2 <= (long long)b.L2 * g->clients[h.sb_cid].b2.ring.pos - b.hist2;
+    if (b.L2 == 1) {
+      keyed[std::make_tuple(h.sb_cid, b.D2, b.T2, b.hist2, settled ? LLONG_MIN : h.zb2)].push_back(i);
     } else {
-      keyed_rat[std::make_tuple(h.sb_cid, h.L2, h.D2, h.T2, h.hist2, settled ? LLONG_MIN : h.zb2)].push_back(i);
+      keyed_rat[std::make_tuple(h.sb_cid, b.L2, b.D2, b.T2, b.hist2, settled ? LLONG_MIN : h.zb2)].push_back(i);
       any_rat = true;
     }
   }
@@ -727,24 +751,7 @@ static int rebuild_subbands(xlg_group *g, size_t &out_total) {
     // a member of block b reads sub-band samples of earlier blocks; the submit of block b + XLG_SLOTS waits
     // for ticket b, so its history (above) + (XLG_SLOTS + 1) * max n1 samples are never overwritten while
     // still needed
-    const size_t cap = next_pow2(back[i] + (size_t)(XLG_SLOTS + 1) * (size_t)h.out_cap);
-    if (h.d_cring != nullptr && cap <= h.cring_cap) continue;
-    float2 *ring = nullptr;
-    CU_OK(cudaMalloc(&ring, cap * sizeof(float2)));
-    std::vector<float2> fresh(cap, make_float2(0.f, 0.f));
-    if (h.d_cring != nullptr) {
-      // grow: the last cring_cap positions keep their samples at their new places
-      std::vector<float2> old(h.cring_cap);
-      CU_OK(cudaMemcpy(old.data(), h.d_cring, h.cring_cap * sizeof(float2), cudaMemcpyDeviceToHost));
-      for (size_t k = 1; k <= h.cring_cap; k++) {
-        const unsigned long long p = (unsigned long long)(h.a_pos - (long long)k);
-        fresh[p & (cap - 1)] = old[p & (h.cring_cap - 1)];
-      }
-      cudaFree(h.d_cring);
-    }
-    CU_OK(cudaMemcpy(ring, fresh.data(), cap * sizeof(float2), cudaMemcpyHostToDevice));
-    h.d_cring = ring;
-    h.cring_cap = cap;
+    if (ring_ensure(h.b2.ring, next_pow2(back[i] + (size_t)(XLG_SLOTS + 1) * (size_t)h.out_cap))) return -EIO;
   }
   std::vector<SbGroup> groups;
   std::vector<SbMem> mems;
@@ -758,8 +765,8 @@ static int rebuild_subbands(xlg_group *g, size_t &out_total) {
     ch.members = members;
     ch.zb = LLONG_MIN;
     const HostClient &h0 = g->clients[members[0]];
-    ch.L2 = (int)h0.L2;
-    ch.Tb = h0.L2 == 1 ? (int)h0.T2 : h0.Tb2;
+    ch.L2 = (int)h0.b2.geo.L2;
+    ch.Tb = h0.b2.geo.Tb2;
     const int tpad = sb_tpad(ch.Tb);
     for (size_t m0 = 0; m0 < ch.members.size(); m0 += SB_MG) {
       SbGroup gp;
@@ -772,7 +779,7 @@ static int rebuild_subbands(xlg_group *g, size_t &out_total) {
       for (int m = 0; m < gp.n_mem; m++) {
         HostClient &h = g->clients[ch.members[m0 + m]];
         for (int r = 0; r < ch.L2; r++)
-          memcpy(&taps[gp.taps_off + ((size_t)r * SB_MG + m) * tpad], h.rev2.data() + 2 * (size_t)r * ch.Tb,
+          memcpy(&taps[gp.taps_off + ((size_t)r * SB_MG + m) * tpad], h.mtaps.data() + 2 * (size_t)r * ch.Tb,
                  2 * (size_t)ch.Tb * sizeof(float));
         mems.push_back(SbMem{ch.members[m0 + m], cls, 0});
         ch.zb = std::max(ch.zb, h.zb2);
@@ -819,22 +826,7 @@ static int rebuild_subbands(xlg_group *g, size_t &out_total) {
   for (Slot &s : g->slots) {
     if (s.pf_sb[0] == nullptr)
       for (cudaEvent_t &ev : s.pf_sb) CU_OK(cudaEventCreate(&ev));
-    if (s.sbcb_cap < n_sb) {
-      if (s.d_sbcb) cudaFree(s.d_sbcb);
-      if (s.h_sbcb) cudaFreeHost(s.h_sbcb);
-      s.d_sbcb = s.h_sbcb = nullptr;
-      s.sbcb_cap = std::max<size_t>(n_sb * 2, 16);
-      CU_OK(cudaMalloc(&s.d_sbcb, s.sbcb_cap * sizeof(CascBlk)));
-      CU_OK(cudaHostAlloc(&s.h_sbcb, s.sbcb_cap * sizeof(CascBlk), cudaHostAllocDefault));
-    }
-    if (s.sbblk_cap < n_cls) {
-      if (s.d_sbblk) cudaFree(s.d_sbblk);
-      if (s.h_sbblk) cudaFreeHost(s.h_sbblk);
-      s.d_sbblk = s.h_sbblk = nullptr;
-      s.sbblk_cap = std::max<size_t>(n_cls * 2, 16);
-      CU_OK(cudaMalloc(&s.d_sbblk, s.sbblk_cap * sizeof(SbBlk)));
-      CU_OK(cudaHostAlloc(&s.h_sbblk, s.sbblk_cap * sizeof(SbBlk), cudaHostAllocDefault));
-    }
+    if (s.sbcb.reserve(n_sb) || s.sbblk.reserve(n_cls)) return -EIO;
     if ((grow_ph || s.d_sbph == nullptr) && g->sbph_cap > 0) {
       if (s.d_sbph) cudaFree(s.d_sbph);
       s.d_sbph = nullptr;
@@ -877,8 +869,8 @@ static int rebuild_layout(xlg_group *g) {
     HostClient &h = g->clients[i];
     if (!h.active) continue;
     if (h.mem) {
-      // n2 <= (L2 * n1 - 1) / D2 + 1 for any history, n1 at most its sub-band's row
-      h.out_cap = (int)(((uint64_t)g->max_input_len / 2 / g->clients[h.sb_cid].D + 2) * h.L2 / h.D2 + 2);
+      // n1 at most its sub-band's row
+      h.out_cap = stage_b_rows((uint64_t)g->max_input_len / 2 / g->clients[h.sb_cid].D + 2, h.b2.geo.L2, h.b2.geo.D2);
       h.out_off = (int)out_total;
       out_total += (size_t)h.out_cap;
       out_total = (out_total + 3) & ~(size_t)3;
@@ -886,10 +878,9 @@ static int rebuild_layout(xlg_group *g) {
     }
     h.out_cap = (int)((uint64_t)g->max_input_len / 2 * h.L / h.D + 2);
     if (h.casc) {
-      // n2 <= (L2 * n1 - 1) / D2 + 1 for any history
-      h.fin_cap = (int)((uint64_t)h.out_cap * h.L2 / h.D2 + 2);
-      h.fin_off = (int)out_total;
-      out_total += (size_t)h.fin_cap;
+      h.b2.fin_cap = stage_b_rows((uint64_t)h.out_cap, h.b2.geo.L2, h.b2.geo.D2);
+      h.b2.fin_off = (int)out_total;
+      out_total += (size_t)h.b2.fin_cap;
     } else if (!h.sb) {
       h.out_off = (int)out_total;
       out_total += (size_t)h.out_cap;
@@ -897,8 +888,7 @@ static int rebuild_layout(xlg_group *g) {
     out_total = (out_total + 3) & ~(size_t)3;  // keep rows 32-byte aligned
     h.taps_off = (int)taps_total;
     taps_total += h.rev.size() / 2;
-    // a rational client's history of at most T - 1 upsampled samples reaches back ceil((T-1)/L) + 1 inputs
-    max_hist = std::max(max_hist, h.L == 1 ? h.T - 1 : (h.T - 1 + h.L - 1) / h.L + 1);
+    max_hist = std::max(max_hist, history_reach(h.T, h.L));
   }
   // cascade clients: stage-A rows after every host-visible row (the D2H copy ends before them), stage-B taps,
   // and a zeroed history ring for each new client (its positions before the attach read as zero)
@@ -911,44 +901,21 @@ static int rebuild_layout(xlg_group *g) {
       h.out_off = (int)out_total;
       out_total += (size_t)h.out_cap;
       out_total = (out_total + 3) & ~(size_t)3;
-      h.taps2_off = (int)taps2.size();
-      taps2.insert(taps2.end(), h.rev2.begin(), h.rev2.end());
-      taps2.resize((taps2.size() + 3) & ~(size_t)3, 0.f);  // 16-byte aligned bulk copies of whole float4s
-      if (h.d_cring == nullptr) {
-        // stage B of block b reads stage-A outputs of earlier blocks; the submit of block b + XLG_SLOTS waits
-        // for ticket b, so T2 - 1 + (XLG_SLOTS + 1) * max n1 samples are never overwritten while still needed;
-        // a rational stage B's history of at most T2 - 1 upsampled samples reaches back ceil((T2 - 1) / L2)
-        // stage-A samples, and its last branch may read one zero-weighted sample past the block
-        const size_t back = h.L2 == 1 ? h.T2 - 1 : (h.T2 - 1 + h.L2 - 1) / h.L2 + 1;
-        h.cring_cap = next_pow2(back + (size_t)(XLG_SLOTS + 1) * (size_t)h.out_cap);
-        CU_OK(cudaMalloc(&h.d_cring, h.cring_cap * sizeof(float2)));
-        CU_OK(cudaMemset(h.d_cring, 0, h.cring_cap * sizeof(float2)));
-      }
+      h.b2.taps_off = (int)taps2.size();
+      taps2.insert(taps2.end(), h.b2.taps.begin(), h.b2.taps.end());
+      // stage B of block b reads stage-A outputs of earlier blocks; the submit of block b + XLG_SLOTS waits
+      // for ticket b, so its history + (XLG_SLOTS + 1) * max n1 samples are never overwritten while still needed
+      if (ring_ensure(h.b2.ring, next_pow2(history_reach(h.b2.geo.T2, h.b2.geo.L2) +
+                                           (size_t)(XLG_SLOTS + 1) * (size_t)h.out_cap)))
+        return -EIO;
       g->n_casc++;
-      if (h.L2 == 1) g->n_casc_int++;
+      if (h.b2.geo.L2 == 1) g->n_casc_int++;
     }
     if (dev_assign(&g->d_taps2, &g->cap_taps2, taps2.data(), taps2.size() * sizeof(float))) return -EIO;
     for (float2 *p : g->dead_rings) cudaFree(p);
     g->dead_rings.clear();
-    for (Slot &s : g->slots) {
-      if (s.cblk_cap >= (size_t)g->n_casc) continue;
-      if (s.d_cblk) cudaFree(s.d_cblk);
-      if (s.h_cblk) cudaFreeHost(s.h_cblk);
-      s.d_cblk = s.h_cblk = nullptr;
-      s.cblk_cap = std::max<size_t>((size_t)g->n_casc * 2, 16);
-      CU_OK(cudaMalloc(&s.d_cblk, s.cblk_cap * sizeof(CascBlk)));
-      CU_OK(cudaHostAlloc(&s.h_cblk, s.cblk_cap * sizeof(CascBlk), cudaHostAllocDefault));
-    }
-    const int n_rat = g->n_casc - g->n_casc_int;
-    for (Slot &s : g->slots) {
-      if (s.pblk_cap >= (size_t)n_rat) continue;
-      if (s.d_pblk) cudaFree(s.d_pblk);
-      if (s.h_pblk) cudaFreeHost(s.h_pblk);
-      s.d_pblk = s.h_pblk = nullptr;
-      s.pblk_cap = std::max<size_t>((size_t)n_rat * 2, 16);
-      CU_OK(cudaMalloc(&s.d_pblk, s.pblk_cap * sizeof(CascPolyBlk)));
-      CU_OK(cudaHostAlloc(&s.h_pblk, s.pblk_cap * sizeof(CascPolyBlk), cudaHostAllocDefault));
-    }
+    for (Slot &s : g->slots)
+      if (s.cblk.reserve((size_t)g->n_casc) || s.pblk.reserve((size_t)(g->n_casc - g->n_casc_int))) return -EIO;
   }
   if (rebuild_subbands(g, out_total)) return -EIO;
   if (ensure_ring(g, max_hist, g->qring != nullptr)) return -EIO;
@@ -1690,8 +1657,7 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
     }
   if (cudaFuncSetAttribute(fir_long2_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W2_SMEM) != cudaSuccess ||
       cudaFuncSetAttribute(fir_long4_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W4_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(cascade_fir_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem) != cudaSuccess ||
-      cudaFuncSetAttribute(cascade_fir_poly_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem) != cudaSuccess) {
+      cascade_stage_b_init() != cudaSuccess) {
     XL_LOG("cannot raise dynamic shared memory to %d bytes", kTileMaxSmem);
     return fail(-EIO);
   }
@@ -1815,7 +1781,7 @@ extern "C" void xlg_destroy(xlg_group *g) {
   if (g->d_sbmem) cudaFree(g->d_sbmem);
   if (g->d_sbtaps) cudaFree(g->d_sbtaps);
   for (HostClient &h : g->clients)
-    if (h.d_cring) cudaFree(h.d_cring);
+    if (h.b2.ring.p) cudaFree(h.b2.ring.p);
   for (float2 *p : g->dead_rings) cudaFree(p);
   if (g->ev_user) cudaEventDestroy(g->ev_user);
   if (g->s_in) cudaStreamDestroy(g->s_in);
@@ -1912,16 +1878,9 @@ extern "C" int xlg_add_client_rational_ex(xlg_group *g, uint32_t interp, uint32_
                                           size_t taps_len, int32_t center_freq, const xlg_client_state *state,
                                           int *client_id) {
   if (g == nullptr || client_id == nullptr) return -EINVAL;
-  if (interp == 0 || decim == 0) {
-    XL_LOG("rational client: interpolation %u and decimation %u must both be at least 1", interp, decim);
-    return -EINVAL;
-  }
-  if ((uint64_t)interp * g->fs > UINT32_MAX) {
-    XL_LOG("rational client: %u x %u Hz upsampled rate exceeds UINT32_MAX", interp, g->fs);
-    return -EINVAL;
-  }
-  if ((uint64_t)interp * (g->max_input_len / 2) >= (1ull << 31)) {
-    XL_LOG("rational client: %u x %u samples per block upsampled exceed 2^31", interp, g->max_input_len / 2);
+  const char *why = rational_refusal(g->fs, g->max_input_len, interp, decim);
+  if (why != nullptr) {
+    XL_LOG("rational client %u/%u at %u Hz, blocks of %u: %s", interp, decim, g->fs, g->max_input_len, why);
     return -EINVAL;
   }
   if (interp == 1) return xlg_add_client_ex(g, decim, taps, taps_len, center_freq, state, client_id);
@@ -1943,64 +1902,29 @@ extern "C" int xlg_add_client_cascade_rational(xlg_group *g, uint32_t decim1, co
                                                int32_t center_freq, uint32_t interp2, uint32_t decim2,
                                                const float *taps2, size_t taps2_len, int *client_id) {
   if (g == nullptr || client_id == nullptr) return -EINVAL;
-  if (decim1 == 0 || decim2 == 0 || taps1_len == 0 || taps2_len == 0 || taps1 == nullptr || taps2 == nullptr) {
-    XL_LOG("cascade client: decimations (%u, %u) and tap counts (%zu, %zu) must all be at least 1", decim1, decim2,
-           taps1_len, taps2_len);
+  if (taps1_len == 0 || taps2_len == 0 || taps1 == nullptr || taps2 == nullptr) {
+    XL_LOG("cascade client: tap counts (%zu, %zu) must both be at least 1", taps1_len, taps2_len);
     return -EINVAL;
   }
-  if (interp2 == 0) {
-    XL_LOG("cascade client: stage-B interpolation must be at least 1");
-    return -EINVAL;
-  }
-  if (interp2 > 1 && (uint64_t)interp2 * ((uint64_t)g->max_input_len / 2 / decim1 + 2) >= (1ull << 31)) {
-    XL_LOG("cascade client: %u x %u stage-A samples per block upsampled exceed 2^31", interp2,
-           g->max_input_len / 2 / decim1 + 2);
+  const char *why = cascade_refusal(g->max_input_len, decim1, interp2, decim2, taps2_len);
+  if (why != nullptr) {
+    XL_LOG("cascade client %u x %u/%u with %zu + %zu taps, blocks of %u: %s", decim1, interp2, decim2, taps1_len,
+           taps2_len, g->max_input_len, why);
     return -EINVAL;
   }
   if (g->flags & XLG_TRACK_STATE) {
     XL_LOG("cascade client: an XLG_TRACK_STATE group cannot carry the state of two stages");
     return -ENOTSUP;
   }
-  const size_t Tb2 = (taps2_len + interp2 - 1) / interp2;
-  if (taps2_len > (size_t)INT32_MAX ||
-      (interp2 == 1 ? cascade_smem(1, (int)decim2, (int)taps2_len)
-                    : cascade_poly_smem(1, (int)interp2, (int)decim2, (int)Tb2)) > (size_t)kTileMaxSmem) {
-    XL_LOG("cascade client: %zu stage-B taps (interpolation %u) exceed the stage-B kernel's shared memory", taps2_len,
-           interp2);
-    return -EINVAL;
-  }
-  // stage B: the reference filter at interp2 * fs / D1 with centre 0 -- its rotated taps are (h, +-0), so the
-  // real parts of the reversed taps (the even-length quirk included) are all it needs; at centre 0 the rate
-  // only enters the rotation, so clamping it changes nothing
-  const uint64_t rate2 = (uint64_t)interp2 * std::max<uint32_t>(g->fs / decim1, 1);
-  xl_client_consts k2;
-  int rc = xl_client_consts_build(taps2, taps2_len, decim2, 0, (uint32_t)std::min<uint64_t>(rate2, UINT32_MAX), &k2);
+  StageB b2;
+  int rc = stage_b_init(&b2, taps2, taps2_len, interp2, decim2, g->fs / decim1);
   if (rc) return rc;
-  std::vector<float> rev2(taps2_len);
-  if (interp2 == 1) {
-    for (size_t j = 0; j < taps2_len; j++) rev2[j] = k2.rev_cf32[2 * j];
-  } else {
-    // branch-major P[r][t] = rev2[r + t * L2], zero-padded to Tb2 taps per branch
-    std::vector<float> packed(2 * (size_t)interp2 * Tb2);
-    xl_poly_pack(k2.rev_cf32, taps2_len, interp2, packed.data());
-    rev2.resize((size_t)interp2 * Tb2);
-    for (size_t j = 0; j < rev2.size(); j++) rev2[j] = packed[2 * j];
-  }
-  xl_client_consts_free(&k2);
   int id = -1;
   rc = attach_client(g, 1, decim1, g->fs, taps1, taps1_len, center_freq, nullptr, &id);
   if (rc) return rc;
   HostClient &h = g->clients[id];
   h.casc = true;
-  h.L2 = interp2;
-  h.D2 = decim2;
-  h.T2 = taps2_len;
-  h.rev2.swap(rev2);
-  h.hist2 = (long long)taps2_len - 1;  // src/xlating.c:552 (upsampled samples when L2 > 1)
-  if (interp2 > 1) {
-    h.Tb2 = (int)Tb2;
-    h.ko2 = cascade_poly_ko((int)interp2, (int)decim2, h.Tb2);
-  }
+  h.b2 = std::move(b2);
   *client_id = id;
   return 0;
 }
@@ -2019,9 +1943,9 @@ extern "C" int xlg_remove_client(xlg_group *g, int client_id) {
       g->clients[client_id].sb)
     return -EINVAL;
   g->clients[client_id].active = false;
-  if (g->clients[client_id].d_cring) g->dead_rings.push_back(g->clients[client_id].d_cring);  // in-flight tickets read it
-  g->clients[client_id].d_cring = nullptr;
-  g->clients[client_id].rev2.clear();
+  if (g->clients[client_id].b2.ring.p) g->dead_rings.push_back(g->clients[client_id].b2.ring.p);  // in-flight tickets read it
+  g->clients[client_id].b2 = StageB();
+  g->clients[client_id].mtaps.clear();
   g->clients[client_id].rev.clear();
   g->clients[client_id].rev_q15.clear();
   g->dirty = true;
@@ -2039,7 +1963,7 @@ extern "C" int xlg_client_info(const xlg_group *g, int client_id, size_t *histor
   if (g == nullptr || client_id < 0 || client_id >= (int)g->clients.size() || !g->clients[client_id].active ||
       g->clients[client_id].sb)
     return -EINVAL;
-  if (history) *history = (size_t)(g->clients[client_id].mem ? g->clients[client_id].hist2 : g->clients[client_id].hist);
+  if (history) *history = (size_t)(g->clients[client_id].mem ? g->clients[client_id].b2.geo.hist2 : g->clients[client_id].hist);
   if (kernel_kind) *kernel_kind = g->clients[client_id].casc ? 5 : g->clients[client_id].kind;
   return 0;
 }
@@ -2052,7 +1976,7 @@ extern "C" int xlg_cascade_info(const xlg_group *g, int client_id, int *stage_a_
   const HostClient &h = g->clients[client_id];
   if (stage_a_kind) *stage_a_kind = h.kind;
   if (stage_a_history) *stage_a_history = (size_t)h.hist;
-  if (stage_b_history) *stage_b_history = (size_t)h.hist2;
+  if (stage_b_history) *stage_b_history = (size_t)h.b2.geo.hist2;
   return 0;
 }
 
@@ -2169,20 +2093,16 @@ extern "C" int xlg_add_client_subband_rational(xlg_group *g, int subband_id, uin
   h.mem = true;
   h.sb_cid = sb;
   h.D = 0;
-  h.L2 = interp2;
-  h.D2 = decim2;
-  h.T2 = taps2_len;
-  h.Tb2 = (int)Tb2;
+  h.b2.geo = stage_b_geom(interp2, decim2, taps2_len);
   if (interp2 == 1) {
-    h.rev2.assign(k.rev_cf32, k.rev_cf32 + 2 * taps2_len);
+    h.mtaps.assign(k.rev_cf32, k.rev_cf32 + 2 * taps2_len);
   } else {
-    h.rev2.resize(2 * (size_t)interp2 * Tb2);  // branch-major P[r][t] = rev[r + t * L2], zero-padded
-    xl_poly_pack(k.rev_cf32, taps2_len, interp2, h.rev2.data());
+    h.mtaps.resize(2 * (size_t)interp2 * Tb2);  // branch-major P[r][t] = rev[r + t * L2], zero-padded
+    xl_poly_pack(k.rev_cf32, taps2_len, interp2, h.mtaps.data());
   }
   h.incr_re = k.incr_re;
   h.incr_im = k.incr_im;
-  h.hist2 = (long long)taps2_len - 1;  // src/xlating.c:552 (upsampled samples when L2 > 1)
-  h.zb2 = g->clients[sb].a_pos;
+  h.zb2 = g->clients[sb].b2.ring.pos;
   h.is_new = true;
   xl_client_consts_free(&k);
   g->dirty = true;
@@ -2198,7 +2118,7 @@ extern "C" int xlg_subband_info(const xlg_group *g, int client_id, int *subband_
   const HostClient &h = g->clients[client_id];
   if (subband_id) *subband_id = g->clients[h.sb_cid].sb_id;
   if (stage_a_kind) *stage_a_kind = g->clients[h.sb_cid].kind;
-  if (member_history) *member_history = (size_t)h.hist2;
+  if (member_history) *member_history = (size_t)h.b2.geo.hist2;
   return 0;
 }
 
@@ -2304,7 +2224,8 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
   s.in_samples = (uint64_t)n;
   int max_generic_out = 0, poly_warps = 0, max_poly4_out = 0, n_casc = 0, max_n1 = 0, max_n2 = 0;
   int n_cint = 0, n_crat = 0, max_rat_ctas = 0;  // integer / rational stage B; CTAs per rational client
-  size_t casc_smem = 0, casc_poly_smem = 0;
+  int casc_ko = C_KO;                             // integer stage B: the smallest ko of its clients
+  size_t casc_poly_smem = 0;
   for (size_t i = 0; i < g->clients.size(); i++) {
     HostClient &h = g->clients[i];
     if (!h.active || h.mem) continue;
@@ -2331,53 +2252,30 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     }
     if (q15 || h.kind == 0) max_generic_out = std::max(max_generic_out, n_out);
     if (h.casc) {
-      // stage B: the reference's walk over this block's n_out stage-A samples, upsampled by L2 (the
-      // zero-stuffed stream u[L2 * n] = y[n]; the same integers for L2 = 1)
-      const long long first2 = (long long)h.L2 * h.a_pos - h.hist2;
-      const int n2 = xl_walk(&h.hist2, (long long)h.L2 * n_out, h.T2, h.D2, h.fin_cap);
-      CascBlk &cb = s.h_cblk[h.L2 == 1 ? n_cint++ : g->n_casc_int + n_crat];
-      cb.ring = h.d_cring;
-      cb.a_pos = h.a_pos;
-      cb.first = first2;
-      cb.mask = (unsigned)(h.cring_cap - 1);
-      cb.a_off = h.out_off;
-      cb.n1 = n_out;
-      cb.n2 = n2;
-      cb.D2 = (int)h.D2;
-      cb.T2 = (int)h.T2;
-      cb.taps_off = h.taps2_off;
-      cb.out_off = h.fin_off;
-      if (h.L2 == 1) {
-        max_n2 = std::max(max_n2, n2);
-        casc_smem = std::max(casc_smem, cascade_smem(C_KO, cb.D2, cb.T2));
-        s.casc_macs += (uint64_t)n2 * h.T2;
+      const StageBGeom &b = h.b2.geo;
+      const StageBStep w = stage_b_walk(h.b2.geo, h.b2.ring.pos, n_out, h.b2.fin_cap);
+      if (b.L2 == 1) {
+        stage_b_fill(h.b2, w, n_out, h.out_off, &s.cblk.h[n_cint++], nullptr);
+        max_n2 = std::max(max_n2, w.n2);
+        casc_ko = std::min(casc_ko, h.b2.ko);
+        s.casc_macs += (uint64_t)w.n2 * b.T2;
       } else {
         // only the appends read this client's CascBlk; cascade_fir_poly_cf32_kernel reads its CascPolyBlk
-        CascPolyBlk &pb = s.h_pblk[n_crat++];
-        pb.ring = h.d_cring;
-        pb.first = first2;
-        pb.mask = cb.mask;
-        pb.n2 = n2;
-        pb.L2 = (int)h.L2;
-        pb.M2 = (int)h.D2;
-        pb.Tb2 = h.Tb2;
-        pb.ko = h.ko2;
-        pb.taps_off = h.taps2_off;
-        pb.out_off = h.fin_off;
-        max_rat_ctas = std::max(max_rat_ctas, (n2 + h.ko2 - 1) / h.ko2);
-        casc_poly_smem = std::max(casc_poly_smem, cascade_poly_smem(h.ko2, pb.L2, pb.M2, pb.Tb2));
-        s.casc_macs += (uint64_t)n2 * (uint64_t)h.Tb2;
+        stage_b_fill(h.b2, w, n_out, h.out_off, &s.cblk.h[g->n_casc_int + n_crat], &s.pblk.h[n_crat]);
+        n_crat++;
+        max_rat_ctas = std::max(max_rat_ctas, (w.n2 + h.b2.ko - 1) / h.b2.ko);
+        casc_poly_smem = std::max(casc_poly_smem, cascade_poly_smem(h.b2.ko, (int)b.L2, (int)b.D2, b.Tb2));
+        s.casc_macs += (uint64_t)w.n2 * (uint64_t)b.Tb2;
       }
       n_casc++;
-      h.a_pos += n_out;
-      h.last_n2 = n2;
+      h.b2.ring.pos += n_out;
+      h.last_n2 = w.n2;
       max_n1 = std::max(max_n1, n_out);
     }
   }
 
-  // sub-band members: each class walks its sub-band's n1 new samples with the reference's count formula, in
-  // sub-band coordinates (the sub-band's a_pos before this block's samples), upsampled by L2 for a rational
-  // class
+  // sub-band members: each class walks its sub-band's n1 new samples from the sub-band ring's position before
+  // them
   const int n_sb = (int)g->sb_list.size();
   int max_sb_n1 = 0, max_sb_n2 = 0;
   int max_sbr_ctas = 0, max_sbr_l2 = 0;  // rational classes: output tiles of the longest residue, largest L2
@@ -2388,19 +2286,19 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       const SbClassHost &ch = g->sb_classes[c];
       const HostClient &a = g->clients[ch.sb_cid];
       const HostClient &m0 = g->clients[ch.members[0]];
-      long long hist2 = m0.hist2;
-      const long long first2 = (long long)ch.L2 * a.a_pos - hist2;
-      const int n2 = xl_walk(&hist2, (long long)ch.L2 * ho.n_out[ch.sb_cid], m0.T2, m0.D2, m0.out_cap);
-      SbBlk &b = s.h_sbblk[c];
-      b.ring = a.d_cring;
-      b.first = first2;
+      StageBGeom geo = m0.b2.geo;
+      const StageBStep w = stage_b_walk(geo, a.b2.ring.pos, ho.n_out[ch.sb_cid], m0.out_cap);
+      const int n2 = w.n2;
+      SbBlk &b = s.sbblk.h[c];
+      b.ring = a.b2.ring.p;
+      b.first = w.first;
       b.zb = ch.zb;
-      b.mask = (unsigned)(a.cring_cap - 1);
+      b.mask = (unsigned)(a.b2.ring.cap - 1);
       b.n2 = n2;
-      b.D2 = (int)m0.D2;
+      b.D2 = (int)geo.D2;
       b.T2 = ch.Tb;
       for (int id : ch.members) {
-        g->clients[id].hist2 = hist2;
+        g->clients[id].b2.geo.hist2 = geo.hist2;
         ho.n_out[id] = n2;
         ho.out_off[id] = g->clients[id].out_off;
       }
@@ -2418,14 +2316,14 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       const int i = g->sb_list[k];
       HostClient &a = g->clients[i];
       const int n1 = ho.n_out[i];
-      CascBlk &cb = s.h_sbcb[k];
+      CascBlk &cb = s.sbcb.h[k];
       memset(&cb, 0, sizeof(cb));
-      cb.ring = a.d_cring;
-      cb.a_pos = a.a_pos;
-      cb.mask = (unsigned)(a.cring_cap - 1);
+      cb.ring = a.b2.ring.p;
+      cb.a_pos = a.b2.ring.pos;
+      cb.mask = (unsigned)(a.b2.ring.cap - 1);
       cb.a_off = a.out_off;
       cb.n1 = n1;
-      a.a_pos += n1;
+      a.b2.ring.pos += n1;
       s.sb_rows += (uint64_t)n1;
       max_sb_n1 = std::max(max_sb_n1, n1);
     }
@@ -2800,26 +2698,18 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       CU_OK(cudaEventRecord(s.pf_casc[0], cs));
       s.pf_cb = true;
     }
-    CU_OK(cudaMemcpyAsync(s.d_cblk, s.h_cblk, (size_t)n_casc * sizeof(CascBlk), cudaMemcpyHostToDevice, cs));
-    if (n_crat > 0)
-      CU_OK(cudaMemcpyAsync(s.d_pblk, s.h_pblk, (size_t)n_crat * sizeof(CascPolyBlk), cudaMemcpyHostToDevice, cs));
-    if (max_n1 > 0) cascade_append_kernel<<<dim3((max_n1 + 255) / 256, n_casc), 256, 0, cs>>>(s.d_cblk, s.d_out);
+    CU_OK(s.cblk.upload((size_t)n_casc, cs));
+    if (n_crat > 0) CU_OK(s.pblk.upload((size_t)n_crat, cs));
+    if (max_n1 > 0) cascade_launch_append(s.cblk.d, n_casc, max_n1, s.d_out, cs);
     if (max_n2 > 0) {
-      // fewer outputs per CTA where a long stage-B window would not fit (attach checked that one output fits)
-      int ko = C_KO;
-      while (ko > 1 && casc_smem > (size_t)kTileMaxSmem) {
-        ko /= 2;
-        casc_smem = 0;
-        for (int c = 0; c < n_cint; c++)
-          casc_smem = std::max(casc_smem, cascade_smem(ko, s.h_cblk[c].D2, s.h_cblk[c].T2));
-      }
-      cascade_fir_cf32_kernel<<<dim3((max_n2 + ko - 1) / ko, n_cint), C_THREADS, casc_smem, cs>>>(s.d_cblk, g->d_taps2,
-                                                                                                s.d_out, ko);
+      // one launch at the largest ko that fits every client: each client's ko (cascade_ko) is C_KO halved until
+      // its window fits and cascade_smem grows with ko, so that is the smallest client's ko
+      size_t smem = 0;
+      for (int c = 0; c < n_cint; c++) smem = std::max(smem, cascade_smem(casc_ko, s.cblk.h[c].D2, s.cblk.h[c].T2));
+      cascade_launch_fir(s.cblk.d, n_cint, max_n2, casc_ko, smem, g->d_taps2, s.d_out, cs);
     }
     // rational stage B: each client's CTA size was fixed at attach to fit the shared memory
-    if (max_rat_ctas > 0)
-      cascade_fir_poly_cf32_kernel<<<dim3(max_rat_ctas, n_crat), C_THREADS, casc_poly_smem, cs>>>(s.d_pblk, g->d_taps2,
-                                                                                                s.d_out);
+    if (max_rat_ctas > 0) cascade_launch_fir_poly(s.pblk.d, n_crat, max_rat_ctas, casc_poly_smem, g->d_taps2, s.d_out, cs);
     if (g->profiling) CU_OK(cudaEventRecord(s.pf_casc[1], cs));
     CU_OK(cudaEventRecord(s.ev_casc, cs));
     g->ev_last_casc = s.ev_casc;
@@ -2828,7 +2718,7 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     for (size_t i = 0; i < g->clients.size(); i++)
       if (g->clients[i].active && g->clients[i].casc) {
         ho.n_out[i] = g->clients[i].last_n2;
-        ho.out_off[i] = g->clients[i].fin_off;
+        ho.out_off[i] = g->clients[i].b2.fin_off;
       }
   }
   // ---- sub-bands: append their outputs to their rings, then the members' oscillators and FIR ----
@@ -2840,18 +2730,18 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       CU_OK(cudaEventRecord(s.pf_sb[0], cs));
       s.pf_sbk = true;
     }
-    CU_OK(cudaMemcpyAsync(s.d_sbcb, s.h_sbcb, (size_t)n_sb * sizeof(CascBlk), cudaMemcpyHostToDevice, cs));
-    if (max_sb_n1 > 0) cascade_append_kernel<<<dim3((max_sb_n1 + 255) / 256, n_sb), 256, 0, cs>>>(s.d_sbcb, s.d_out);
+    CU_OK(s.sbcb.upload((size_t)n_sb, cs));
+    if (max_sb_n1 > 0) cascade_launch_append(s.sbcb.d, n_sb, max_sb_n1, s.d_out, cs);
     if (max_sb_n2 > 0 || max_sbr_ctas > 0) {
-      CU_OK(cudaMemcpyAsync(s.d_sbblk, s.h_sbblk, g->sb_classes.size() * sizeof(SbBlk), cudaMemcpyHostToDevice, cs));
-      subband_phase_kernel<<<(g->n_sb_mem + 31) / 32, 32, 0, cs>>>(g->d_clients, g->d_sbmem, s.d_sbblk, s.d_sbph);
+      CU_OK(s.sbblk.upload(g->sb_classes.size(), cs));
+      subband_phase_kernel<<<(g->n_sb_mem + 31) / 32, 32, 0, cs>>>(g->d_clients, g->d_sbmem, s.sbblk.d, s.d_sbph);
       if (max_sb_n2 > 0)
         subband_fir_cf32_kernel<<<dim3((max_sb_n2 + SB_KO - 1) / SB_KO, g->n_sb_groups_int), SB_THREADS, sb_smem,
-                                  cs>>>(s.d_sbblk, g->d_sbgrp, g->d_sbtaps, s.d_sbph, s.d_out);
+                                  cs>>>(s.sbblk.d, g->d_sbgrp, g->d_sbtaps, s.d_sbph, s.d_out);
       // rational classes: their groups follow the integer ones, one CTA layer per residue
       if (max_sbr_ctas > 0)
         subband_fir_poly_cf32_kernel<<<dim3(max_sbr_ctas, g->n_sb_groups - g->n_sb_groups_int, max_sbr_l2), SB_THREADS,
-                                       sbr_smem, cs>>>(s.d_sbblk, g->d_sbgrp + g->n_sb_groups_int, g->d_sbtaps,
+                                       sbr_smem, cs>>>(s.sbblk.d, g->d_sbgrp + g->n_sb_groups_int, g->d_sbtaps,
                                                        s.d_sbph, s.d_out);
     }
     if (g->profiling) CU_OK(cudaEventRecord(s.pf_sb[1], cs));
@@ -3133,7 +3023,7 @@ extern "C" int xlg_profile_read(xlg_group *g, xlg_profile *p, int reset) {
   return 0;
 }
 
-// ---- stage-B launchers for the per-filter engine (cascade_stage_b.cuh) ----
+// ---- stage-B launchers of both engines (cascade_stage_b.cuh) ----
 namespace xl {
 
 cudaError_t cascade_stage_b_init() {
