@@ -120,6 +120,7 @@ struct HostClient {
   bool casc = false;
   StageB b2;                     // (its fin_off / fin_cap: the final row of the slot's output arena)
   int last_n2 = 0;               // stage-B outputs of the block being submitted
+  int cblk = 0;                  // integer stage B: its entry in the per-slot CascBlk table
   // sub-band (xlg_add_subband): an integer client, not visible to the caller, whose row lies after every
   // host-visible row; b2.ring is its history ring
   bool sb = false;
@@ -396,6 +397,10 @@ struct xlg_group {
   size_t cap_taps2 = 0;
   int n_casc = 0;                           // active cascade clients
   int n_casc_int = 0;                       // of which integer stage B (their CascBlk entries come first)
+  struct CascRun {
+    int ko, c0, c1;                         // the integer CascBlk entries [c0, c1) have outputs per CTA ko
+  };
+  std::vector<CascRun> casc_runs;           // integer stage B by ko, largest first: one launch each
   std::vector<float2 *> dead_rings;         // rings of removed cascade clients, freed once the pipeline is drained
   cudaEvent_t ev_last_casc = nullptr;       // ev_casc of the last block with cascade clients or sub-bands
   bool have_last_casc = false;
@@ -910,6 +915,20 @@ static int rebuild_layout(xlg_group *g) {
         return -EIO;
       g->n_casc++;
       if (h.b2.geo.L2 == 1) g->n_casc_int++;
+    }
+    // integer entries ordered by ko, one stage-B launch per distinct ko: a client's lanes walk its taps as they
+    // would in a group of its own, whatever ko its neighbours have
+    std::vector<int> ints;
+    for (int i = 0; i < nc; i++)
+      if (g->clients[i].active && g->clients[i].casc && g->clients[i].b2.geo.L2 == 1) ints.push_back(i);
+    std::stable_sort(ints.begin(), ints.end(),
+                     [g](int a, int b) { return g->clients[a].b2.ko > g->clients[b].b2.ko; });
+    g->casc_runs.clear();
+    for (int e = 0; e < (int)ints.size(); e++) {
+      HostClient &h = g->clients[ints[e]];
+      h.cblk = e;
+      if (g->casc_runs.empty() || g->casc_runs.back().ko != h.b2.ko) g->casc_runs.push_back({h.b2.ko, e, e});
+      g->casc_runs.back().c1 = e + 1;
     }
     if (dev_assign(&g->d_taps2, &g->cap_taps2, taps2.data(), taps2.size() * sizeof(float))) return -EIO;
     for (float2 *p : g->dead_rings) cudaFree(p);
@@ -2222,9 +2241,8 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
   s.q15 = q15;
   s.tile_macs = s.algo_macs = s.out_samples = s.poly_macs = s.casc_macs = s.d2h_bytes = 0;
   s.in_samples = (uint64_t)n;
-  int max_generic_out = 0, poly_warps = 0, max_poly4_out = 0, n_casc = 0, max_n1 = 0, max_n2 = 0;
-  int n_cint = 0, n_crat = 0, max_rat_ctas = 0;  // integer / rational stage B; CTAs per rational client
-  int casc_ko = C_KO;                             // integer stage B: the smallest ko of its clients
+  int max_generic_out = 0, poly_warps = 0, max_poly4_out = 0, n_casc = 0, max_n1 = 0;
+  int n_crat = 0, max_rat_ctas = 0;  // rational stage B; CTAs per rational client
   size_t casc_poly_smem = 0;
   for (size_t i = 0; i < g->clients.size(); i++) {
     HostClient &h = g->clients[i];
@@ -2255,9 +2273,7 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       const StageBGeom &b = h.b2.geo;
       const StageBStep w = stage_b_walk(h.b2.geo, h.b2.ring.pos, n_out, h.b2.fin_cap);
       if (b.L2 == 1) {
-        stage_b_fill(h.b2, w, n_out, h.out_off, &s.cblk.h[n_cint++], nullptr);
-        max_n2 = std::max(max_n2, w.n2);
-        casc_ko = std::min(casc_ko, h.b2.ko);
+        stage_b_fill(h.b2, w, n_out, h.out_off, &s.cblk.h[h.cblk], nullptr);
         s.casc_macs += (uint64_t)w.n2 * b.T2;
       } else {
         // only the appends read this client's CascBlk; cascade_fir_poly_cf32_kernel reads its CascPolyBlk
@@ -2701,12 +2717,16 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     CU_OK(s.cblk.upload((size_t)n_casc, cs));
     if (n_crat > 0) CU_OK(s.pblk.upload((size_t)n_crat, cs));
     if (max_n1 > 0) cascade_launch_append(s.cblk.d, n_casc, max_n1, s.d_out, cs);
-    if (max_n2 > 0) {
-      // one launch at the largest ko that fits every client: each client's ko (cascade_ko) is C_KO halved until
-      // its window fits and cascade_smem grows with ko, so that is the smallest client's ko
+    // integer stage B: one launch per ko, as the drop-in engine launches it (the kernel's summation order
+    // depends on ko: with even D2 output k is summed by lane (k mod ko) mod 32)
+    for (const xlg_group::CascRun &r : g->casc_runs) {
+      int run_n2 = 0;
       size_t smem = 0;
-      for (int c = 0; c < n_cint; c++) smem = std::max(smem, cascade_smem(casc_ko, s.cblk.h[c].D2, s.cblk.h[c].T2));
-      cascade_launch_fir(s.cblk.d, n_cint, max_n2, casc_ko, smem, g->d_taps2, s.d_out, cs);
+      for (int c = r.c0; c < r.c1; c++) {
+        run_n2 = std::max(run_n2, s.cblk.h[c].n2);
+        smem = std::max(smem, cascade_smem(r.ko, s.cblk.h[c].D2, s.cblk.h[c].T2));
+      }
+      if (run_n2 > 0) cascade_launch_fir(s.cblk.d + r.c0, r.c1 - r.c0, run_n2, r.ko, smem, g->d_taps2, s.d_out, cs);
     }
     // rational stage B: each client's CTA size was fixed at attach to fit the shared memory
     if (max_rat_ctas > 0) cascade_launch_fir_poly(s.pblk.d, n_crat, max_rat_ctas, casc_poly_smem, g->d_taps2, s.d_out, cs);

@@ -16,6 +16,13 @@ usage: _dropin_cascade_worker.py <scenario> [arg]   -> one JSON line, exit code 
   neighbours              overlay on: integer and rational filters of one band on exact stimuli give the same
                           bits with and without cascade filters alive, and still join their band's group
   q15refuse               two refused Q15 calls leave a cascade filter's cf32 stream untouched
+  mixedko                 61.44 Msps plan filters (even D2, 256 outputs per stage-B CTA) next to filters with 16
+                          and 4 in the same batches: each filter gives the bits of the same client in a group of
+                          them all (skipped under XLATING_B200_DROPIN=group)
+  fullring                stage-A rings exactly full (T2 - 1 + one call's stage-A outputs = 8192: D1 = 6,
+                          T2 = 2730) and one sample past it (T2 = 2731), odd and even D2, over full calls that wrap
+                          them: exact taps against the float64 composition, random taps against the kernel model
+                          of an integer filter's rows
   pool <dir> [fresh]      cascade, rational and integer filters created and destroyed interleaved (the cascade
                           arena grows and is reused, filter memory comes from the pool): every cascade filter's
                           calls saved to <dir>; fresh: one filter in a fresh process
@@ -33,6 +40,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from oracle import pyoracle as po  # noqa: E402  (checker)
 from cascade import CascadeOracle, f64_filter, small_taps  # noqa: E402
+from cascade_exact import f64_stage_b, stage_b_ko, stage_b_model  # noqa: E402
 from cascade_rational import RationalCascadeOracle, f64_composition  # noqa: E402
 from exact import exact_input, to_complex  # noqa: E402
 from rational import oracle_filter, stuff  # noqa: E402
@@ -282,6 +290,68 @@ def scenario_q15refuse(out):
     out["refused"] = refused
 
 
+# ---- stage-B CTA sizes ----
+def scenario_mixedko(out):
+    rng = np.random.default_rng(37)
+    fs, fmt = 61440000, "cs16"
+    plan = pkg.cascade_plan(fs, [48000] * 3)
+    d1, t1n = plan[0]["d1"], plan[0]["taps1"][1:-1].copy()
+    specs = [(p["d1"], p["taps1"], p["center"], p["d2"], p["taps2"]) for p in plan]
+    specs += [(d1, t1n, -17, D2, (rng.standard_normal(64) / 8).astype(np.float32)) for D2 in (1024, 5000)]
+    blocks = [rand_block(rng, fmt, MAX_IN) for _ in range(24)]
+    filters = [pkg.XlatingFilter.cascade(*s, fs, MAX_IN) for s in specs]
+    outs = [[] for _ in specs]
+    run_threads([lambda b, i=i: outs[i].append(filters[i].process_cf32(fmt, blocks[b].copy()))
+                 for i in range(len(specs))], len(blocks))
+    for f in filters:
+        f.close()
+    if not GROUP_MODEL:
+        g = pkg.Group(fs, MAX_IN, flags=pkg.XLG_FORCE_GENERIC)
+        cids = [g.add_client_cascade(*s) for s in specs]
+        got = [[] for _ in specs]
+        for x in blocks:
+            t = g.submit(fmt, x)
+            g.wait(t)
+            for i, c in enumerate(cids):
+                got[i].append(np.array(g.output(t, c), copy=True))
+        g.close()
+        for i in range(len(specs)):
+            same_bits(outs[i], got[i], f"cascade {i} (D2 {specs[i][3]}) against the group")
+        out["batches"], out["calls"], out["shared"] = pkg.dropin_stats()
+    out["ko"] = [stage_b_ko(1, s[3], len(s[4])) for s in specs]
+    out["outputs"] = [sum(y.size for y in o) for o in outs]
+
+
+def scenario_fullring(out):
+    rng = np.random.default_rng(43)
+    fs, fmt, d1 = 2016000, "cs16", 6
+    blocks = [exact_input(rng, fmt, MAX_IN) for _ in range(8)]
+    t1 = small_taps(rng, 3, 1)
+    twin = pkg.XlatingFilter(d1, t1, 0, fs, MAX_IN)
+    rows = [twin.process_cf32(fmt, x) for x in blocks]
+    twin.close()
+    ref_a = f64_filter(t1, d1, 0, fs, [to_complex(fmt, x) for x in blocks])
+    assert all(np.array_equal(y, r.astype(np.complex64)) for y, r in zip(rows, ref_a))
+    checked = []
+    for T2 in (2730, 2731):
+        for D2 in (4, 5):
+            t2e = small_taps(rng, T2, 1)
+            t2r = (rng.standard_normal(T2) / np.sqrt(T2)).astype(np.float32)
+            for t2, exact in ((t2e, True), (t2r, False)):
+                f = pkg.XlatingFilter.cascade(d1, t1, 0, D2, t2, fs, MAX_IN)
+                got = [f.process_cf32(fmt, x) for x in blocks]
+                f.close()
+                if exact:
+                    want = [r.astype(np.complex64) for r in f64_stage_b(rows, 0, 1, D2, t2)]
+                else:
+                    want = stage_b_model(rows, 0, 1, D2, t2, fs // d1, stage_b_ko(1, D2, T2))
+                for b, (y, r) in enumerate(zip(got, want)):
+                    assert y.shape == r.shape and np.array_equal(y, r), (T2, D2, exact, b)
+                checked.append(sum(y.size for y in got))
+    out["checked"] = checked
+    out["stage_a"] = sum(y.size for y in rows)
+
+
 # ---- pool and arena reuse ----
 def scenario_pool(out, dump, fresh=False):
     rng = np.random.default_rng(31)
@@ -351,6 +421,10 @@ def main():
             scenario_neighbours(out)
         elif sc == "q15refuse":
             scenario_q15refuse(out)
+        elif sc == "mixedko":
+            scenario_mixedko(out)
+        elif sc == "fullring":
+            scenario_fullring(out)
         elif sc == "pool":
             scenario_pool(out, args[0], fresh=len(args) > 1 and args[1] == "fresh")
         else:

@@ -107,6 +107,21 @@ def test_refused_q15_call_consumes_nothing():
     assert line["stderr"].count("<3>") == 1
 
 
+def test_mixed_cta_sizes_give_the_group_bits():
+    """Filters launched at 256, 16 and 4 stage-B outputs per CTA in shared batches give the bits of the same
+    clients in one group: each keeps the CTA size it has alone, in both engines."""
+    line = run("mixedko")
+    assert line["ko"] == [256, 256, 256, 16, 4] and min(line["outputs"]) > 0
+    assert line["shared"] > 0
+
+
+def test_stage_a_ring_exactly_full():
+    """A private stage-A ring of exactly T2 - 1 + one call's outputs (8192) and one of 16384 at T2 + 1, wrapped
+    by full calls: bit for bit against the float64 composition and the kernel model."""
+    line = run("fullring", env=PRIVATE)
+    assert len(line["checked"]) == 8 and min(line["checked"]) > 1000 and line["stage_a"] > 2 * 8192
+
+
 def test_pool_reuse_starts_from_zero_history(tmp_path):
     """Cascade, rational and integer filters created and destroyed interleaved, the cascade arena growing under
     filters that have run: every cascade filter's calls equal those of one filter in a fresh process."""
