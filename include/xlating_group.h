@@ -192,12 +192,34 @@ int xlg_add_client_subband_rational(xlg_group *g, int subband_id, uint32_t inter
  * member's history_offset in sub-band samples (upsampled samples for a rational member).  -EINVAL for any
  * client that is not a member. */
 int xlg_subband_info(const xlg_group *g, int client_id, int *subband_id, int *stage_a_kind, size_t *member_history);
+/* Extension: bank sub-bands (DESIGN.md section 5, "Bank sub-bands").  A BANK cuts every sub-band fs / (2 * decim1)
+ * apart out of the band with one polyphase filter bank, instead of each sub-band running its own first stage.
+ *   A bank of decimation D1 and real taps h (taps1, T1 = taps1_len, copied) attached before the next submitted
+ *   block, at stream position P, has K = 2 * D1 channels.  Channel k in [-D1, D1) is centred at k * fs / K and
+ *   its output m is
+ *     y_k[m] = sum_{j < T1} x[s_m + j] * h[T1-1-j] * e^{-2 pi i k (s_m + j - P) / K},
+ *   x read as zero before P, s_m and the outputs per block those of an integer client (D1, T1) attached at P
+ *   (xlg_add_client's walk).  For odd T1 this is, in exact arithmetic, xlg_add_subband(g, D1, h, T1,
+ *   k * fs / K) attached at P.  Bank ids come from a small-integer space of their own.  -EINVAL (logged) for
+ *   decim1 or taps1_len of 0, fs % (2 * decim1) != 0, or taps too long for the bank kernel's shared memory
+ *   (about 16000 taps, less at large decim1); -ENOTSUP (logged) on an XLG_TRACK_STATE group.  A group with a
+ *   bank refuses XLG_PATH_Q15 submits (-ENOTSUP, logged, nothing enqueued). */
+int xlg_add_bank(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, int *bank_id);
+/* Materialise channel `channel` of a bank: an ordinary sub-band id.  xlg_add_client_subband[_rational] and
+ * xlg_remove_subband work on it unchanged (-EBUSY while it has members); xlg_subband_info reports
+ * stage_a_kind 7 for its members.  Its rows are the bank's from P, whenever it is materialised; its members
+ * get zero history at their own attach point.  -EINVAL (logged) for an unknown bank or a channel outside
+ * [-D1, D1), -EEXIST (logged) for a channel already materialised. */
+int xlg_add_bank_subband(xlg_group *g, int bank_id, int32_t channel, int *subband_id);
+/* -EBUSY (logged) while the bank still has channels; -EINVAL for an unknown id. */
+int xlg_remove_bank(xlg_group *g, int bank_id);
 /* Size the per-ticket result arenas (device and pinned host) for `output_samples_per_block` complex output
  * samples per block summed over all clients (a client at decimation D produces about max_input_len/2/D + 2).
  * A cascade client counts two rows, each rounded up to a multiple of 4 samples: its stage-A row of
  * n1 = max_input_len/2/decim1 + 2 samples, which stays on the device, and its final row of
  * floor(n1 * interp2 / decim2) + 2 (interp2 = 1 for xlg_add_client_cascade).  A sub-band counts one row of
- * n1 = max_input_len/2/decim1 + 2 samples, rounded up to 4, which stays on the device; a member counts its
+ * n1 = max_input_len/2/decim1 + 2 samples, rounded up to 4, which stays on the device (a bank's channel counts
+ * one row like a sub-band); a member counts its
  * final row of floor(n1 * interp2 / decim2) + 2, rounded up to 4 (interp2 = 1 for xlg_add_client_subband).
  * Optional: the arenas grow on demand when clients are added, but a growth re-allocates every ring entry and
  * the results still waiting in the ring are lost (-ESTALE for consumers that had not read them yet, like a
@@ -308,11 +330,22 @@ typedef struct {
 } xlg_subband_profile;
 int xlg_subband_profile_read(xlg_group *g, xlg_subband_profile *p, int reset);
 
+/* Banks (xlg_add_bank), counted like xlg_profile's while profiling is enabled.  xlg_profile does not count
+ * banks; their channels' ring appends and members are xlg_subband_profile's. */
+typedef struct {
+  double bank_ms;            /* the bank kernel */
+  uint64_t bank_launches;
+  uint64_t poly_macs;        /* real-by-complex MACs of the polyphase sums: sum n1 * T1 */
+  uint64_t dft_macs;         /* complex MACs of the channel sums: sum n1 * C * K, C materialised channels */
+} xlg_bank_profile;
+int xlg_bank_profile_read(xlg_group *g, xlg_bank_profile *p, int reset);
+
 /* Introspection for tests: history length (src/xlating.c:29 history_offset; upsampled samples for a
  * rational client, stage A's for a cascade client) and which kernel currently serves the client
  * (0 = generic, 1 = tiled, 2 = long-filter split-K, 3 = rational, polyphase generic, 4 = rational, tiled: at
  * least 8 clients with identical (interp, decim, taps_len, window alignment), gcd(interp, decim) = 1, whose
- * branches fit the tiled kernel's shared memory, 5 = cascade, 6 = sub-band member). */
+ * branches fit the tiled kernel's shared memory, 5 = cascade, 6 = sub-band member; 7, as a sub-band's kind in
+ * xlg_subband_info only, = a bank's channel). */
 int xlg_client_info(const xlg_group *g, int client_id, size_t *history, int *kernel_kind);
 /* A cascade client's stages: the kind (0, 1 or 2, as xlg_client_info) of the kernel serving stage A, and the
  * history_offset of each stage (stage B's in stage-A samples, upsampled by interp2 for a rational cascade

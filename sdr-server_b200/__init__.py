@@ -55,7 +55,7 @@ DROPIN_EXTENSION_SYMBOLS = ["create_rational_frequency_xlating_filter", "create_
 GROUP_SYMBOLS = [
     "xlg_create", "xlg_create_ex", "xlg_destroy", "xlg_add_client", "xlg_add_client_ex", "xlg_add_client_rational_ex", "xlg_remove_client", "xlg_reserve", "xlg_client_count", "xlg_submit",
     "xlg_wait", "xlg_input_consumed", "xlg_output", "xlg_read_output", "xlg_copy_output", "xlg_alloc_pinned", "xlg_free_pinned", "xlg_wait_stream", "xlg_partition_active", "xlg_timer_start",
-    "xlg_timer_stop", "xlg_profile_enable", "xlg_profile_read", "xlg_client_info", "xlg_add_client_rational", "xlg_poly_profile_read", "xlg_add_client_cascade", "xlg_add_client_cascade_rational", "xlg_cascade_info", "xlg_cascade_profile_read", "xlg_add_subband", "xlg_remove_subband", "xlg_add_client_subband", "xlg_add_client_subband_rational", "xlg_subband_info", "xlg_subband_profile_read", "xlg_dropin_stats", "xlg_dropin_stream_stats", "xlg_dropin_stream_times",
+    "xlg_timer_stop", "xlg_profile_enable", "xlg_profile_read", "xlg_client_info", "xlg_add_client_rational", "xlg_poly_profile_read", "xlg_add_client_cascade", "xlg_add_client_cascade_rational", "xlg_cascade_info", "xlg_cascade_profile_read", "xlg_add_subband", "xlg_remove_subband", "xlg_add_client_subband", "xlg_add_client_subband_rational", "xlg_subband_info", "xlg_subband_profile_read", "xlg_add_bank", "xlg_add_bank_subband", "xlg_remove_bank", "xlg_bank_profile_read", "xlg_dropin_stats", "xlg_dropin_stream_stats", "xlg_dropin_stream_times",
 ]
 
 
@@ -88,6 +88,11 @@ class XlgCascadeProfile(C.Structure):
 class XlgSubbandProfile(C.Structure):
     _fields_ = [("member_ms", C.c_double), ("member_launches", C.c_uint64), ("member_macs", C.c_uint64),
                 ("row_samples", C.c_uint64)]
+
+
+class XlgBankProfile(C.Structure):
+    _fields_ = [("bank_ms", C.c_double), ("bank_launches", C.c_uint64), ("poly_macs", C.c_uint64),
+                ("dft_macs", C.c_uint64)]
 
 
 def build(verbose: bool = False) -> None:
@@ -164,6 +169,14 @@ def lib() -> C.CDLL:
     L.xlg_subband_info.restype = C.c_int
     L.xlg_subband_profile_read.argtypes = [vp, C.POINTER(XlgSubbandProfile), C.c_int]
     L.xlg_subband_profile_read.restype = C.c_int
+    L.xlg_add_bank.argtypes = [vp, u32, fp, sz, C.POINTER(C.c_int)]
+    L.xlg_add_bank.restype = C.c_int
+    L.xlg_add_bank_subband.argtypes = [vp, C.c_int, i32, C.POINTER(C.c_int)]
+    L.xlg_add_bank_subband.restype = C.c_int
+    L.xlg_remove_bank.argtypes = [vp, C.c_int]
+    L.xlg_remove_bank.restype = C.c_int
+    L.xlg_bank_profile_read.argtypes = [vp, C.POINTER(XlgBankProfile), C.c_int]
+    L.xlg_bank_profile_read.restype = C.c_int
     L.xl_poly_pack.argtypes = [C.POINTER(C.c_float), sz, u32, C.POINTER(C.c_float)]
     L.xl_poly_pack.restype = None
     L.xlg_reserve.argtypes = [vp, sz]
@@ -450,6 +463,30 @@ class Group:
             raise ValueError(code)
         return sid.value, kind.value, h.value
 
+    def add_bank(self, decim1: int, taps1) -> int:
+        """A channel bank (include/xlating_group.h, xlg_add_bank): K = 2 * decim1 channels k * fs / K apart,
+        each the sub-band (decim1, taps1) centred there, from one polyphase pass.  Returns a bank id."""
+        t1 = np.ascontiguousarray(taps1, dtype=np.float32)
+        bid = C.c_int(-1)
+        code = self._L.xlg_add_bank(self._h, decim1, t1.ctypes.data_as(C.POINTER(C.c_float)), len(t1), C.byref(bid))
+        if code != 0:
+            raise ValueError(code)
+        return bid.value
+
+    def add_bank_subband(self, bid: int, channel: int) -> int:
+        """Channel `channel` in [-decim1, decim1) of bank `bid` (xlg_add_bank_subband): an ordinary sub-band id,
+        centred at channel * fs / (2 * decim1), that takes members through add_client_subband."""
+        sid = C.c_int(-1)
+        code = self._L.xlg_add_bank_subband(self._h, bid, channel, C.byref(sid))
+        if code != 0:
+            raise ValueError(code)
+        return sid.value
+
+    def remove_bank(self, bid: int) -> None:
+        code = self._L.xlg_remove_bank(self._h, bid)
+        if code != 0:
+            raise ValueError(code)
+
     def remove_client(self, cid: int) -> None:
         code = self._L.xlg_remove_client(self._h, cid)
         if code != 0:
@@ -584,6 +621,11 @@ class Group:
         p = XlgSubbandProfile()
         self._L.xlg_subband_profile_read(self._h, C.byref(p), 1 if reset else 0)
         return {k: getattr(p, k) for k, _ in XlgSubbandProfile._fields_}
+
+    def bank_profile_read(self, reset: bool = True) -> dict:
+        p = XlgBankProfile()
+        self._L.xlg_bank_profile_read(self._h, C.byref(p), 1 if reset else 0)
+        return {k: getattr(p, k) for k, _ in XlgBankProfile._fields_}
 
     def close(self):
         if self._h:
@@ -736,7 +778,16 @@ def subband_member_fits(interp2: int, decim2: int, t2: int) -> bool:
             <= 200 * 1024)
 
 
-def subband_plan(fs: int, clients):
+def bank_fits(d1: int, t1: int) -> bool:
+    """Whether the bank kernel's shared memory holds a bank (xlg_add_bank refuses the others): the taps padded
+    to a multiple of K = 2 * d1 and of 4, the window of 32 frames, K twiddles and 32 rows of K + 1 polyphase
+    sums, bank_smem in csrc/xlating_kernels.cuh against the 200 KiB the kernel is given."""
+    K = 2 * d1
+    tpad = ((-(-t1 // K) * K) + 3) & ~3
+    return 16 + 4 * tpad + 8 * ((31 * d1 + t1 + 2) & ~1) + 8 * K + 8 * 32 * (K + 1) <= 200 * 1024
+
+
+def subband_plan(fs: int, clients, bank: bool = False):
     """Sub-band clients for `clients`, a list of (center, rate).  For every D1 >= 2 that divides fs with
     fs1 = fs / D1 even, fs1 > 2 * max rate and every rate dividing fs1: sub-band centres fs1 / 2 apart from
     the lowest client centre up across the occupied span, each client assigned to the nearest one (so its
@@ -749,7 +800,14 @@ def subband_plan(fs: int, clients):
     interp2 = 1 where the rate divides fs1) with taps create_low_pass_filter(interp2, interp2 * fs1, rate / 2,
     rate / 5), and a D1 with a member the kernel would refuse (subband_member_fits) is skipped.  Returns
     {"d1", "taps1", "e", "subbands": [{"center"}], "members": [{"subband", "center", "rate", "interp2", "d2",
-    "offset", "taps2"}] in the order of `clients`, "fmas"}."""
+    "offset", "taps2"}] in the order of `clients`, "fmas"}.
+
+    bank=True plans the sub-bands as channels of one bank (Group.add_bank, add_bank_subband): each client is
+    assigned to the nearest centre j * fs1 / 2 of the bank's grid (|offset| <= fs1 / 4 still), every sub-band
+    entry also carries its "channel" k in [-D1, D1) (j wrapped: the channel at +fs / 2 is the one at -fs / 2,
+    and a member's offset stays relative to its own grid point), a D1 whose bank the kernel would refuse (bank_fits) is skipped, and the first stage costs
+    2 * T1 / D1 + 8 * C FMAs per input sample (one polyphase pass, C channel sums of K complex MACs per frame)
+    instead of 4 * T1 / D1 per sub-band."""
     centers = [int(c) for c, _ in clients]
     rates = [int(r) for _, r in clients]
     rmax = max(rates)
@@ -770,23 +828,36 @@ def subband_plan(fs: int, clients):
             if rational and not all(subband_member_fits(L2, M2, t.size) for L2, M2, t in shapes.values()):
                 continue
             half = fs1 // 2
-            n_cent = (hi - lo + half - 1) // half + 1
-            assign = [min(range(n_cent), key=lambda k: abs(c - (lo + k * half))) for c in centers]
-            used = sorted(set(assign))
             e = fs1 // 4 + rmax // 2
             t1 = create_low_pass_filter(1.0, fs, fs1 // 2, fs1 - 2 * e)
-            cost = subband_fmas(fs, d1, t1.size, len(used), [(r, shapes[r][2].size, shapes[r][0]) for r in rates])
+            if bank:
+                if not bank_fits(d1, t1.size):
+                    continue
+                base = 0  # the grid j * half, j = round(c / half), and j's channel
+                grid = [(2 * c + half) // (2 * half) for c in centers]
+                assign = [(j + d1) % (2 * d1) - d1 for j in grid]
+                used = sorted(set(assign))
+                cost = 2.0 * t1.size / d1 + 8.0 * len(used) + subband_fmas(
+                    fs, d1, t1.size, 0, [(r, shapes[r][2].size, shapes[r][0]) for r in rates])
+            else:
+                base = lo
+                grid = None
+                n_cent = (hi - lo + half - 1) // half + 1
+                assign = [min(range(n_cent), key=lambda k: abs(c - (lo + k * half))) for c in centers]
+                used = sorted(set(assign))
+                cost = subband_fmas(fs, d1, t1.size, len(used), [(r, shapes[r][2].size, shapes[r][0]) for r in rates])
             if best is None or cost < best[0]:
-                best = (cost, d1, fs1, half, e, t1, shapes, used, assign)
+                best = (cost, d1, fs1, half, e, t1, shapes, used, assign, base, grid)
         if best is not None:
             break
     if best is None:
         raise ValueError(f"{fs} has no divisor D1 >= 2 whose sub-band rate serves the rates {sorted(set(rates))}")
-    cost, d1, fs1, half, e, t1, shapes, used, assign = best
+    cost, d1, fs1, half, e, t1, shapes, used, assign, base, grid = best
     index = {k: i for i, k in enumerate(used)}
-    subbands = [{"center": lo + k * half} for k in used]
+    subbands = [{"center": base + k * half, "channel": k} if bank else {"center": base + k * half} for k in used]
     members = [{"subband": index[k], "center": c, "rate": r, "interp2": shapes[r][0], "d2": shapes[r][1],
-                "offset": c - (lo + k * half), "taps2": shapes[r][2]} for c, r, k in zip(centers, rates, assign)]
+                "offset": c - (base + (grid[i] if bank else k) * half), "taps2": shapes[r][2]}
+               for i, (c, r, k) in enumerate(zip(centers, rates, assign))]
     return {"d1": d1, "fs1": fs1, "taps1": t1, "e": e, "subbands": subbands, "members": members, "fmas": cost}
 
 

@@ -133,6 +133,24 @@ struct HostClient {
   int sb_cid = -1;               // its sub-band's client index
   long long zb2 = 0;             // sub-band position of its attach point: earlier samples read as zero
   int ph_row = 0;                // its rows of the slot's member oscillator table
+  // bank channel (xlg_add_bank_subband): a sub-band (sb) whose row bank_cf32_kernel writes; D and T are its
+  // bank's, and it is not an integer client (inactive ClientDev, no oscillator, no tap row)
+  int bank = -1;                 // its bank's id
+  int chan = 0;                  // its channel k in [-D1, D1)
+};
+
+// a channel bank (xlg_add_bank): reversed padded taps, twiddles, and the walk of an integer client (D1, T1)
+// attached at P
+struct BankHost {
+  bool active = false;
+  uint32_t D1 = 0;
+  size_t T1 = 0;
+  int K = 0, tpad = 0;
+  std::vector<float> taps;   // h[T1-1-j] at j, zero to tpad
+  std::vector<float2> tw;    // e^{-2 pi i j / K}
+  long long P = 0, hist = 0;
+  std::vector<int> cids;     // its materialised channels' client indices (the layout's)
+  int taps_off = 0, tw_off = 0, ch_off = 0;
 };
 
 // members of one sub-band that read the same windows: equal (L2, D2, T2, hist2) and, until their windows have
@@ -202,6 +220,10 @@ struct Slot {
   cudaEvent_t pf_sb[2] = {nullptr, nullptr};
   bool pf_sbk = false;
   uint64_t sb_macs = 0, sb_rows = 0;
+  BlkTable<BankBlk> bkblk;       // banks with channels: this block's windows, counts and channel tables
+  cudaEvent_t pf_bk[2] = {nullptr, nullptr};
+  bool pf_bkk = false;
+  uint64_t bk_poly = 0, bk_dft = 0;
   std::atomic<int64_t> ticket{-1};
   bool q15 = false;
   bool harvested = true;
@@ -414,6 +436,13 @@ struct xlg_group {
   float2 *d_sbtaps = nullptr;
   size_t cap_sbgrp = 0, cap_sbmem = 0, cap_sbtaps = 0, sbph_cap = 0;
   xlg_subband_profile sb_prof;
+  std::vector<BankHost> banks;              // bank id -> bank (inactive = free)
+  std::vector<int> bank_live;               // banks with channels, in BankBlk order
+  float *d_bktaps = nullptr;
+  float2 *d_bktw = nullptr;
+  int2 *d_bkch = nullptr;
+  size_t cap_bktaps = 0, cap_bktw = 0, cap_bkch = 0;
+  xlg_bank_profile bank_prof;
   int n_generic = 0;
   int max_client = 0;     // highest active id + 1
   bool dirty = true;
@@ -475,6 +504,7 @@ static void slot_free(Slot &s) {
   s.pblk.release();
   s.sbcb.release();
   s.sbblk.release();
+  s.bkblk.release();
   if (s.d_sbph) cudaFree(s.d_sbph);
   s.d_sbph = nullptr;
   s.d_pscratch = nullptr;
@@ -558,6 +588,12 @@ static void harvest_locked(xlg_group *g, Slot &s) {
   }
   g->sb_prof.member_macs += s.sb_macs;
   g->sb_prof.row_samples += s.sb_rows;
+  if (s.pf_bkk && cudaEventElapsedTime(&ms, s.pf_bk[0], s.pf_bk[1]) == cudaSuccess) {
+    g->bank_prof.bank_ms += ms;
+    g->bank_prof.bank_launches++;
+  }
+  g->bank_prof.poly_macs += s.bk_poly;
+  g->bank_prof.dft_macs += s.bk_dft;
   g->prof.blocks++;
   g->prof.out_samples += s.out_samples;
   g->prof.in_samples += s.in_samples;
@@ -841,6 +877,42 @@ static int rebuild_subbands(xlg_group *g, size_t &out_total) {
   return 0;
 }
 
+// Banks (the pipeline is drained, the channels' rows are placed): one arena each for the taps, the twiddles and
+// the channel tables of the banks that have channels, and the per-slot tables.
+static int rebuild_banks(xlg_group *g) {
+  g->bank_live.clear();
+  std::vector<float> taps;
+  std::vector<float2> tw;
+  std::vector<int2> chans;
+  for (int b = 0; b < (int)g->banks.size(); b++) {
+    BankHost &k = g->banks[b];
+    k.cids.clear();
+    if (!k.active) continue;
+    for (int i = 0; i < (int)g->clients.size(); i++)
+      if (g->clients[i].active && g->clients[i].bank == b) k.cids.push_back(i);
+    if (k.cids.empty()) continue;
+    k.ch_off = (int)chans.size();
+    for (int i : k.cids) chans.push_back(make_int2((g->clients[i].chan + k.K) % k.K, g->clients[i].out_off));
+    k.taps_off = (int)taps.size();
+    taps.insert(taps.end(), k.taps.begin(), k.taps.end());
+    k.tw_off = (int)tw.size();
+    tw.insert(tw.end(), k.tw.begin(), k.tw.end());
+    g->bank_live.push_back(b);
+  }
+  if (g->bank_live.empty()) return 0;
+  CU_OK(cudaFuncSetAttribute(bank_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem));
+  if (dev_assign(&g->d_bktaps, &g->cap_bktaps, taps.data(), taps.size() * sizeof(float)) ||
+      dev_assign(&g->d_bktw, &g->cap_bktw, tw.data(), tw.size() * sizeof(float2)) ||
+      dev_assign(&g->d_bkch, &g->cap_bkch, chans.data(), chans.size() * sizeof(int2)))
+    return -EIO;
+  for (Slot &s : g->slots) {
+    if (s.pf_bk[0] == nullptr)
+      for (cudaEvent_t &ev : s.pf_bk) CU_OK(cudaEventCreate(&ev));
+    if (s.bkblk.reserve(g->bank_live.size())) return -EIO;
+  }
+  return 0;
+}
+
 static int rebuild_layout(xlg_group *g) {
   // XLATING_B200_REBUILD_TIMING=1: where a re-layout spends its time (logged per call)
   static const bool timing = getenv("XLATING_B200_REBUILD_TIMING") != nullptr;
@@ -895,6 +967,8 @@ static int rebuild_layout(xlg_group *g) {
     taps_total += h.rev.size() / 2;
     max_hist = std::max(max_hist, history_reach(h.T, h.L));
   }
+  for (const BankHost &k : g->banks)  // a bank walks (and its channels read history) without channels too
+    if (k.active) max_hist = std::max(max_hist, k.T1 - 1);
   // cascade clients: stage-A rows after every host-visible row (the D2H copy ends before them), stage-B taps,
   // and a zeroed history ring for each new client (its positions before the attach read as zero)
   {
@@ -937,6 +1011,7 @@ static int rebuild_layout(xlg_group *g) {
       if (s.cblk.reserve((size_t)g->n_casc) || s.pblk.reserve((size_t)(g->n_casc - g->n_casc_int))) return -EIO;
   }
   if (rebuild_subbands(g, out_total)) return -EIO;
+  if (rebuild_banks(g)) return -EIO;
   if (ensure_ring(g, max_hist, g->qring != nullptr)) return -EIO;
   if (ensure_arenas(g, out_total, g->q_alloc)) return -EIO;
 
@@ -946,7 +1021,7 @@ static int rebuild_layout(xlg_group *g) {
   qtaps.resize(std::max<size_t>(taps_total, 1));
   for (int i = 0; i < nc; i++) {
     const HostClient &h = g->clients[i];
-    if (!h.active) continue;
+    if (!h.active || h.bank >= 0) continue;  // (a bank channel has no taps of its own)
     memcpy(&taps[h.taps_off], h.rev.data(), h.rev.size() * sizeof(float));  // both interleaved (re, im)
     memcpy(&qtaps[h.taps_off], h.rev_q15.data(), h.rev_q15.size() * sizeof(int16_t));
   }
@@ -1000,6 +1075,10 @@ static int rebuild_layout(xlg_group *g) {
     if (!h.active) continue;
     if (h.mem) {
       h.kind = 6;  // served by subband_fir_cf32_kernel (subband_fir_poly_cf32_kernel when L2 > 1)
+      continue;
+    }
+    if (h.bank >= 0) {
+      h.kind = 7;  // a bank channel: bank_cf32_kernel writes its row
       continue;
     }
     h.kind = h.L > 1 ? 3 : 0;
@@ -1268,7 +1347,8 @@ static int rebuild_layout(xlg_group *g) {
     }
     std::vector<int> loose;
     for (int i = 0; i < nc; i++)
-      if (g->clients[i].active && !g->clients[i].mem && (g->clients[i].kind == 0 || g->clients[i].kind >= 3))
+      if (g->clients[i].active && !g->clients[i].mem && g->clients[i].bank < 0 &&
+          (g->clients[i].kind == 0 || g->clients[i].kind >= 3))
         loose.push_back(i);
     for (size_t base = 0; base < loose.size(); base += 32) {
       int cap = 0;
@@ -1367,7 +1447,7 @@ static int rebuild_layout(xlg_group *g) {
     d.qtaps_off = h.taps_off;
     d.out_off = h.out_off;
     d.out_cap = h.out_cap;
-    d.active = h.mem ? 0 : 1;  // a member's entry only carries its oscillator (subband_phase_kernel)
+    d.active = h.mem || h.bank >= 0 ? 0 : 1;  // a member's entry only carries its oscillator (subband_phase_kernel)
     d.kind = h.kind;
     d.renorm = (g->flags & XLG_NO_RENORM) ? 0 : 1;
     d.ph_off = h.ph_off;
@@ -1454,7 +1534,7 @@ static void choose_partition(xlg_group *g) {
     const double n = (double)(g->max_input_len / 2);
     double steps = 0, fma = 0;
     for (const HostClient &h : g->clients) {
-      if (!h.active || h.mem) continue;
+      if (!h.active || h.mem || h.bank >= 0) continue;  // (no oscillator chain, no FIR of their own)
       const double n_out = n * h.L / (double)h.D;
       steps = std::max(steps, n_out);
       fma += 4.0 * n_out * (double)((h.T + h.L - 1) / h.L);
@@ -1585,6 +1665,7 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
   memset(&g->poly_prof, 0, sizeof(g->poly_prof));
   memset(&g->casc_prof, 0, sizeof(g->casc_prof));
   memset(&g->sb_prof, 0, sizeof(g->sb_prof));
+  memset(&g->bank_prof, 0, sizeof(g->bank_prof));
   g->device = device;
   g->fs = sampling_freq;
   g->max_input_len = max_input_len;
@@ -1767,6 +1848,8 @@ extern "C" void xlg_destroy(xlg_group *g) {
     if (s.ev_casc) cudaEventDestroy(s.ev_casc);
     for (cudaEvent_t ev : s.pf_sb)
       if (ev) cudaEventDestroy(ev);
+    for (cudaEvent_t ev : s.pf_bk)
+      if (ev) cudaEventDestroy(ev);
   }
   for (HostOut &h : g->ring_out) {
     if (h.h_out) cudaFreeHost(h.h_out);
@@ -1799,6 +1882,9 @@ extern "C" void xlg_destroy(xlg_group *g) {
   if (g->d_sbgrp) cudaFree(g->d_sbgrp);
   if (g->d_sbmem) cudaFree(g->d_sbmem);
   if (g->d_sbtaps) cudaFree(g->d_sbtaps);
+  if (g->d_bktaps) cudaFree(g->d_bktaps);
+  if (g->d_bktw) cudaFree(g->d_bktw);
+  if (g->d_bkch) cudaFree(g->d_bkch);
   for (HostClient &h : g->clients)
     if (h.b2.ring.p) cudaFree(h.b2.ring.p);
   for (float2 *p : g->dead_rings) cudaFree(p);
@@ -2141,6 +2227,131 @@ extern "C" int xlg_subband_info(const xlg_group *g, int client_id, int *subband_
   return 0;
 }
 
+extern "C" int xlg_add_bank(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, int *bank_id) {
+  if (g == nullptr || bank_id == nullptr) return -EINVAL;
+  if (decim1 == 0 || taps1_len == 0 || taps1 == nullptr) {
+    XL_LOG("bank: decimation %u and tap count %zu must both be at least 1", decim1, taps1_len);
+    return -EINVAL;
+  }
+  if (decim1 > (uint32_t)(INT32_MAX / 2) || g->fs % (2 * decim1) != 0) {
+    XL_LOG("bank: 2 x decimation %u does not divide the band rate %u (channel centres are in Hz at fs / %u)", decim1,
+           g->fs, 2 * decim1);
+    return -EINVAL;
+  }
+  if (taps1_len > (size_t)INT32_MAX / 8 || bank_smem((int)decim1, (int)taps1_len) > (size_t)kTileMaxSmem) {
+    XL_LOG("bank: %zu taps at decimation %u exceed the bank kernel's shared memory", taps1_len, decim1);
+    return -EINVAL;
+  }
+  if (g->flags & XLG_TRACK_STATE) {
+    XL_LOG("bank: an XLG_TRACK_STATE group cannot carry the state of two stages");
+    return -ENOTSUP;
+  }
+  BankHost k;
+  k.active = true;
+  k.D1 = decim1;
+  k.T1 = taps1_len;
+  k.K = 2 * (int)decim1;
+  k.tpad = bank_tpad(k.K, (int)taps1_len);
+  k.taps.assign((size_t)k.tpad, 0.f);
+  for (size_t j = 0; j < taps1_len; j++) k.taps[j] = taps1[taps1_len - 1 - j];
+  k.tw.resize((size_t)k.K);
+  // e^{-2 pi i j / K} = (-i)^q e^{-i t}, 4j = qK + rem, t = 2 pi rem / 4K in [0, pi/2): quarter turns are exact
+  // (W = 1, -i, -1, i where 4j % K == 0)
+  for (int j = 0; j < k.K; j++) {
+    const int q = 4 * j / k.K, rem = 4 * j - q * k.K;
+    const double t = 2.0 * 3.14159265358979323846 * (double)rem / (4.0 * (double)k.K);
+    const float c = (float)cos(t), sn = (float)sin(t);
+    k.tw[j] = q == 0 ? make_float2(c, -sn) : q == 1 ? make_float2(-sn, -c) : q == 2 ? make_float2(-c, sn) : make_float2(sn, c);
+  }
+  k.P = g->S;
+  k.hist = (long long)taps1_len - 1;  // a fresh filter's history: T1 - 1 samples, zero before P
+  int id = 0;
+  while (id < (int)g->banks.size() && g->banks[id].active) id++;
+  if (id == (int)g->banks.size()) g->banks.emplace_back();
+  g->banks[id] = std::move(k);
+  g->dirty = true;  // the input ring's history bound
+  *bank_id = id;
+  return 0;
+}
+
+static BankHost *bank_of(xlg_group *g, int bank_id) {
+  if (bank_id < 0 || bank_id >= (int)g->banks.size() || !g->banks[bank_id].active) return nullptr;
+  return &g->banks[bank_id];
+}
+
+extern "C" int xlg_remove_bank(xlg_group *g, int bank_id) {
+  if (g == nullptr) return -EINVAL;
+  BankHost *k = bank_of(g, bank_id);
+  if (k == nullptr) {
+    XL_LOG("bank %d does not exist", bank_id);
+    return -EINVAL;
+  }
+  int chans = 0;
+  for (const HostClient &h : g->clients) chans += h.active && h.bank == bank_id ? 1 : 0;
+  if (chans > 0) {
+    XL_LOG("bank %d still has %d channels; remove them first", bank_id, chans);
+    return -EBUSY;
+  }
+  *k = BankHost();
+  g->dirty = true;
+  return 0;
+}
+
+extern "C" int xlg_add_bank_subband(xlg_group *g, int bank_id, int32_t channel, int *subband_id) {
+  if (g == nullptr || subband_id == nullptr) return -EINVAL;
+  const BankHost *k = bank_of(g, bank_id);
+  if (k == nullptr) {
+    XL_LOG("bank channel: bank %d does not exist", bank_id);
+    return -EINVAL;
+  }
+  if (channel < -(int32_t)k->D1 || channel >= (int32_t)k->D1) {
+    XL_LOG("bank channel: channel %d is outside [-%u, %u)", channel, k->D1, k->D1);
+    return -EINVAL;
+  }
+  for (const HostClient &h : g->clients)
+    if (h.active && h.bank == bank_id && h.chan == channel) {
+      XL_LOG("bank channel: channel %d of bank %d already exists (sub-band %d)", channel, bank_id, h.sb_id);
+      return -EEXIST;
+    }
+  int cid = -1;
+  for (size_t i = 0; i < g->clients.size(); i++)
+    if (!g->clients[i].active) {
+      cid = (int)i;
+      break;
+    }
+  if (cid < 0) {
+    g->clients.emplace_back();
+    cid = (int)g->clients.size() - 1;
+  }
+  HostClient &h = g->clients[cid];
+  h = HostClient();
+  h.active = true;
+  h.D = k->D1;
+  h.T = k->T1;
+  h.hist = k->hist;
+  h.zero_before = k->P;
+  h.is_new = true;
+  h.bank = bank_id;
+  h.chan = channel;
+  int id = 0;
+  while (id < (int)g->subbands.size() && g->subbands[id] >= 0) id++;
+  if (id == (int)g->subbands.size()) g->subbands.push_back(-1);
+  g->subbands[id] = cid;
+  h.sb = true;
+  h.sb_id = id;
+  g->dirty = true;
+  *subband_id = id;
+  return 0;
+}
+
+extern "C" int xlg_bank_profile_read(xlg_group *g, xlg_bank_profile *p, int reset) {
+  if (g == nullptr || p == nullptr) return -EINVAL;
+  std::lock_guard<std::mutex> lk(g->mu);
+  *p = g->bank_prof;
+  if (reset) memset(&g->bank_prof, 0, sizeof(g->bank_prof));
+  return 0;
+}
+
 template <int FMT>
 static void launch_convert(bool q15, const void *raw, xlg_group *g, long long S, int n, cudaStream_t st) {
   const int threads = 256, blocks = (n + threads - 1) / threads;
@@ -2164,6 +2375,12 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     return -EINVAL;
   }
   const bool q15 = (flags & XLG_PATH_Q15) != 0;
+  if (q15)
+    for (const BankHost &k : g->banks)
+      if (k.active) {
+        XL_LOG("the Q15 path does not serve banks; submit without XLG_PATH_Q15");
+        return -ENOTSUP;
+      }
   if (q15)
     for (const HostClient &h : g->clients)
       if (h.active && (h.L > 1 || h.casc)) {
@@ -2246,7 +2463,7 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
   size_t casc_poly_smem = 0;
   for (size_t i = 0; i < g->clients.size(); i++) {
     HostClient &h = g->clients[i];
-    if (!h.active || h.mem) continue;
+    if (!h.active || h.mem || h.bank >= 0) continue;
     // upsampled coordinates (the same integers for L = 1)
     const long long Su = S * h.L, Eu = (S + n) * h.L;
     const long long first = Su - h.hist;
@@ -2288,6 +2505,43 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
       h.last_n2 = w.n2;
       max_n1 = std::max(max_n1, n_out);
     }
+  }
+
+  // banks: each walks the block as an integer client (D1, T1) attached at P; its channels are sub-bands of n1
+  // samples
+  int n_bk = 0, max_bk_n1 = 0, max_bk_cg = 0;
+  size_t bk_smem = 0;
+  s.bk_poly = s.bk_dft = 0;
+  for (int b = 0; b < (int)g->banks.size(); b++) {
+    BankHost &k = g->banks[b];
+    if (!k.active) continue;
+    const long long first = S - k.hist;
+    const int n1 = xl_walk(&k.hist, n, k.T1, k.D1, (int)((uint64_t)g->max_input_len / 2 / k.D1 + 2));
+    for (int i : k.cids) {
+      g->clients[i].hist = k.hist;
+      ho.n_out[i] = n1;
+      ho.out_off[i] = g->clients[i].out_off;
+    }
+    if (k.cids.empty()) continue;
+    BankBlk &e = s.bkblk.h[n_bk++];
+    e.taps = g->d_bktaps + k.taps_off;
+    e.tw = g->d_bktw + k.tw_off;
+    e.chans = g->d_bkch + k.ch_off;
+    e.first = first;
+    e.zb = k.P;
+    e.mask = mask;
+    e.n1 = n1;
+    e.D1 = (int)k.D1;
+    e.T1 = (int)k.T1;
+    e.K = k.K;
+    e.tpad = k.tpad;
+    e.n_ch = (int)k.cids.size();
+    e.r0 = (int)(((first - k.P) % k.K + k.K) % k.K);
+    max_bk_n1 = std::max(max_bk_n1, n1);
+    max_bk_cg = std::max(max_bk_cg, (e.n_ch + BK_CG - 1) / BK_CG);
+    bk_smem = std::max(bk_smem, bank_smem((int)k.D1, (int)k.T1));
+    s.bk_poly += (uint64_t)n1 * k.T1;
+    s.bk_dft += (uint64_t)n1 * k.cids.size() * (uint64_t)k.K;
   }
 
   // sub-band members: each class walks its sub-band's n1 new samples from the sub-band ring's position before
@@ -2414,8 +2668,21 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     g->have_last_conv = true;
   }
 
-  // ---- oscillator pre-pass (own stream: chains only on the previous pre-pass) ----
-  if (nc > 0) {
+  // ---- banks: after the conversions the FIR kernels wait for, not after the pre-pass (they have no oscillator) ----
+  s.pf_bkk = false;
+  if (n_bk > 0 && max_bk_n1 > 0) {
+    if (g->profiling) {
+      CU_OK(cudaEventRecord(s.pf_bk[0], cs));
+      s.pf_bkk = true;
+    }
+    CU_OK(s.bkblk.upload((size_t)n_bk, cs));
+    bank_cf32_kernel<<<dim3((max_bk_n1 + BK_F - 1) / BK_F, n_bk, max_bk_cg), BK_THREADS, bk_smem, cs>>>(
+        s.bkblk.d, g->ring, s.d_out);
+    if (g->profiling) CU_OK(cudaEventRecord(s.pf_bk[1], cs));
+  }
+
+  // ---- oscillator pre-pass (own stream: chains only on the previous pre-pass; none without a client to walk) ----
+  if (nc > 0 && (q15 || g->n_order > 0)) {
     const bool tl_phase = g->timeline && !(g->spec_valid && !q15);  // a pre-pass that ran ahead was stamped then
     if (g->profiling) CU_OK(cudaEventRecord(s.pf[2], g->s_ph));
     if (tl_phase) CU_OK(cudaEventRecord(s.tl_ph[(ticket / XLG_SLOTS) & 1][0], g->s_ph));

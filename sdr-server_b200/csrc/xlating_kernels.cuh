@@ -1556,4 +1556,121 @@ subband_fir_poly_cf32_kernel(const SbBlk *__restrict__ blk, const SbGroup *__res
   }
 }
 
+// ---------------------------------------------------------------------------
+// bank sub-bands (xlg_add_bank, xlg_add_bank_subband).  A bank of decimation D1 and real taps h (T1) is a
+// 2x-oversampled polyphase filter bank of K = 2 * D1 channels: channel k in [-D1, D1), centred at k * fs / K,
+// writes the row
+//     y_k[m] = sum_{j < T1} x[s_m + j] * h[T1-1-j] * e^{-2 pi i k (s_m + j - P) / K}
+// (P the bank's attach point, x zero before it, s_m the window starts of an integer client (D1, T1) attached
+// at P).  With r_m = (s_m - P) mod K and p = j mod K the rotation only depends on p + r_m, so
+//     v[m][p] = sum_q x[s_m + p + qK] * h[T1-1-p-qK]                          (phase 1, real taps)
+//     y_k[m]  = sum_{p < min(K, T1)} v[m][p] * W[(k (p + r_m)) mod K],   W[j] = e^{-2 pi i j / K}   (phase 2)
+// Order (the test model copies it): phase 1 is two fmaf chains (re, im) over q ascending from 0; phase 2 is
+// the 4-fmaf complex chain of the member kernels over p ascending from 0.  Both start from +0.
+// ---------------------------------------------------------------------------
+constexpr int BK_THREADS = 256;
+constexpr int BK_F = 32;   // frames per CTA
+constexpr int BK_CG = 32;  // channels per CTA (wide banks spread their channel sums over more CTAs)
+
+struct BankBlk {        // one bank, this block
+  const float *taps;    // h reversed (h[T1-1-j] at j), zero-padded to bank_tpad
+  const float2 *tw;     // W[j], j < K (built in double on the host by quarter turns, rounded once)
+  const int2 *chans;    // per materialised channel: (k mod K, its row in the slot's arena)
+  long long first;      // stream position of frame 0's window
+  long long zb;         // the bank's attach point P: earlier samples read as zero
+  unsigned mask;        // input ring capacity - 1
+  int n1, D1, T1, K, tpad, n_ch;
+  int r0;               // (first - P) mod K
+};
+
+// taps padded to a multiple of K and to whole float4s (one bulk copy)
+__host__ __device__ constexpr int bank_tpad(int K, int T1) { return ((T1 + K - 1) / K * K + 3) & ~3; }
+// shared memory of a CTA: mbarrier, the taps, the window of BK_F frames (+1 for an odd start, even), the
+// twiddles and the polyphase sums (rows of K + 1: an odd stride in float2)
+__host__ __device__ constexpr size_t bank_smem(int D1, int T1) {
+  return 16 + (size_t)bank_tpad(2 * D1, T1) * 4 + (((size_t)(BK_F - 1) * D1 + T1 + 2) & ~(size_t)1) * 8 +
+         (size_t)2 * D1 * 8 + (size_t)BK_F * (2 * D1 + 1) * 8;
+}
+
+// CTA (x, b, z) computes frames [x*BK_F, x*BK_F + BK_F) of the materialised channels [z*BK_CG, z*BK_CG + BK_CG)
+// of bank b.  One TMA bulk copy stages the taps, one or two (the ring wraps) the window; an odd window start
+// is fetched from one sample earlier.  Phase 1 gives thread e the sum (frame e / KP, phase e % KP); phase 2
+// gives it channel e / BK_F at frame e % BK_F, so a warp stores 32 consecutive samples of one row.
+__global__ void __launch_bounds__(BK_THREADS)
+bank_cf32_kernel(const BankBlk *__restrict__ blk, const float2 *__restrict__ ring, float2 *__restrict__ out) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  uint64_t *bar = reinterpret_cast<uint64_t *>(smem);
+  const BankBlk b = blk[blockIdx.y];
+  const int f0 = blockIdx.x * BK_F, c0 = blockIdx.z * BK_CG;
+  if (f0 >= b.n1 || c0 >= b.n_ch) return;
+  const int nch = min(BK_CG, b.n_ch - c0);
+  const int D1 = b.D1, T1 = b.T1, K = b.K;
+  const int nf = min(BK_F, b.n1 - f0);
+  float *ts = reinterpret_cast<float *>(smem + 16);
+  float2 *xs = reinterpret_cast<float2 *>(ts + b.tpad);
+  const long long w0 = b.first + (long long)f0 * D1;
+  const unsigned idx = (unsigned)((unsigned long long)w0) & b.mask;
+  const unsigned shift = idx & 1u;
+  const unsigned need = ((unsigned)((nf - 1) * D1 + T1) + shift + 1u) & ~1u;
+  float2 *tw = xs + need;
+  float2 *v = tw + K;
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    mbar_init(bar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  __syncthreads();
+  if (tid == 0) {
+    const unsigned tbytes = (unsigned)b.tpad * 4u;
+    const unsigned p1 = min(need, b.mask + 1u - (idx - shift));
+    mbar_expect_tx(bar, tbytes + need * 8u);
+    tma_bulk_g2s(ts, b.taps, tbytes, bar);
+    tma_bulk_g2s(xs, ring + (idx - shift), p1 * 8u, bar);
+    if (p1 < need) tma_bulk_g2s(xs + p1, ring, (need - p1) * 8u, bar);
+  }
+  for (int i = tid; i < K; i += BK_THREADS) tw[i] = b.tw[i];
+  mbar_wait(bar, 0);
+  const long long base = w0 - (long long)shift;
+  if (b.zb > base)  // windows that reach back before the attach point read zeros there
+    for (unsigned i = tid; i < need; i += BK_THREADS)
+      if (base + (long long)i < b.zb) xs[i] = make_float2(0.f, 0.f);
+  __syncthreads();
+  const int KP = min(K, T1), rs = K + 1;
+  for (int e = tid; e < nf * KP; e += BK_THREADS) {
+    const int f = e / KP, p = e - f * KP;
+    const float2 *x = xs + shift + f * D1 + p;
+    const float *h = ts + p;
+    float2 acc = make_float2(0.f, 0.f);
+    for (int j = 0; j < T1 - p; j += K) {
+      const float2 xv = x[j];
+      const float hv = h[j];
+      acc.x = fmaf(xv.x, hv, acc.x);
+      acc.y = fmaf(xv.y, hv, acc.y);
+    }
+    v[f * rs + p] = acc;
+  }
+  __syncthreads();
+  for (int e = tid; e < nch * BK_F; e += BK_THREADS) {
+    const int c = e / BK_F, f = e - c * BK_F;
+    if (f >= nf) continue;
+    const int2 ch = b.chans[c0 + c];
+    const int kk = ch.x;
+    const int r = (int)(((long long)b.r0 + (long long)(f0 + f) * D1) % K);
+    int t = (int)(((long long)kk * r) % K);
+    const float2 *vf = v + f * rs;
+    float2 acc = make_float2(0.f, 0.f);
+    for (int p = 0; p < KP; p++) {
+      const float2 a = vf[p], w = tw[t];
+      acc.x = fmaf(a.x, w.x, acc.x);
+      acc.x = fmaf(-a.y, w.y, acc.x);
+      acc.y = fmaf(a.x, w.y, acc.y);
+      acc.y = fmaf(a.y, w.x, acc.y);
+      t += kk;
+      if (t >= K) t -= K;
+    }
+    out[ch.y + f0 + f] = acc;
+  }
+}
+
 }  // namespace xl

@@ -1,7 +1,8 @@
-"""Throughput of sub-band clients (xlg_add_subband + xlg_add_client_subband) against single-stage and
-per-client cascade clients of the same centres and rates.
+"""Throughput of sub-band clients (xlg_add_subband + xlg_add_client_subband) and of bank sub-bands
+(xlg_add_bank + xlg_add_bank_subband) against single-stage and per-client cascade clients of the same centres
+and rates.
 
-    python tools/subband_bench.py [--blocks K] [--warmup W] [--rounds R] [--only NAME]
+    python tools/subband_bench.py [--blocks K] [--warmup W] [--rounds R] [--only NAME] [--plans P,...]
 
 Workloads (centres drawn uniformly across the band from a fixed seed):
   61M_1024   1024 clients at 48 kHz on a 61.44 Msps cs16 stream
@@ -12,14 +13,16 @@ Workloads (centres drawn uniformly across the band from a fixed seed):
   20M_256    256 clients at 48 kHz on a 20 Msps cs8 stream (HackRF)
 Plans, alternated within every round: "single" (one client each: client_plan's taps as an integer client, or
 rational_plan's as a rational client where the rate does not divide fs), "cascade" (cascade_plan) and
-"subband" (subband_plan; at the last three rates its members resample by a rational L2 / M2).
+"subband" (subband_plan; at the last three rates its members resample by a rational L2 / M2) and "bank"
+(subband_plan(bank=True): the same kind of members on the channels of one bank).
 
 Per workload and plan (one JSON line each): input MS/s and step time over K pipelined blocks (CUDA events,
 xlg_timer_*), algorithmic real FMAs per input sample from the shapes, and from a profiled run of its own (one
 compute stream, CUDA events around each launch) the time per block of the oscillator pre-pass, the integer
 FIR kernels, the cascades' stage B and the sub-band members' work (ring appends, member oscillators and
-member kernel).  Every run checks its last timed block of sampled clients against the tests' oracles (1e-5
-norm-wise).  Blocks are 262144 bytes, as in bench.py.  The card's name and power limit are printed first,
+member kernel) and the bank kernel.  Every run checks its last timed block of sampled clients against the tests' oracles (1e-5
+norm-wise; a bank's members against the float64 bank rows fed to the reference's float path, since the bank
+has no float oscillator to share with an oracle).  Blocks are 262144 bytes, as in bench.py.  The card's name and power limit are printed first,
 read in the same call.  Nothing is written to the tree.
 """
 import argparse
@@ -45,7 +48,7 @@ WORKLOADS = {  # fs, format, clients, rates
     "10M_256": (10000000, "cs16", 256, (48000,)),
     "20M_256": (20000000, "cs8", 256, (48000,)),
 }
-PLANS = ("single", "cascade", "subband")
+PLANS = ("single", "cascade", "subband", "bank")
 SAMPLED = 3
 
 
@@ -64,6 +67,7 @@ def build(name, plan, profile):
     from cascade_rational import RationalCascadeOracle
     from oracle import pyoracle as po
     from rational import oracle_filter, stuff
+    from bank_exact import BankMemberOracle
     from subband_rational import RationalSubbandOracle
     fs, fmt, n, _ = WORKLOADS[name]
     clients = workload_clients(name)
@@ -98,13 +102,22 @@ def build(name, plan, profile):
                  if p["interp2"] > 1 else cascade_oracle(p["d1"], p["taps1"], c, p["d2"], p["taps2"], fs, BLOCK))
             oracles.append((ids[k], lambda x, o=o: o.process_cf32(fmt, x)))
     else:
-        p = pkg.subband_plan(fs, clients)
-        sids = [g.add_subband(p["d1"], p["taps1"], sb["center"]) for sb in p["subbands"]]
+        p = pkg.subband_plan(fs, clients, bank=plan == "bank")
+        if plan == "bank":
+            bid = g.add_bank(p["d1"], p["taps1"])
+            sids = [g.add_bank_subband(bid, sb["channel"]) for sb in p["subbands"]]
+        else:
+            sids = [g.add_subband(p["d1"], p["taps1"], sb["center"]) for sb in p["subbands"]]
         ids = [g.add_client_subband(sids[m["subband"]], m["d2"], m["taps2"], m["offset"], m["interp2"])
                for m in p["members"]]
         fmas = p["fmas"]
         for k in picks:
             m = p["members"][k]
+            if plan == "bank":
+                o = BankMemberOracle(p["d1"], p["taps1"], p["subbands"][m["subband"]]["channel"], m["d2"], m["taps2"],
+                                     m["offset"], m["interp2"], fs)
+                oracles.append((ids[k], lambda x, o=o: o.process_cf32(fmt, x)))
+                continue
             o = RationalSubbandOracle(p["d1"], p["taps1"], p["subbands"][m["subband"]]["center"], fs, BLOCK)
             o.add_member(0, m["d2"], m["taps2"], m["offset"], m["interp2"])
             oracles.append((ids[k], lambda x, o=o: o.process_cf32(fmt, x)[0]))
@@ -145,17 +158,18 @@ def run(name, plan, blocks, warmup):
     g, ids, _, _ = build(name, plan, True)
     for i in range(warmup):
         g.wait(g.submit(fmt, data[i % 4]))
-    for read in (g.profile_read, g.cascade_profile_read, g.subband_profile_read):
+    for read in (g.profile_read, g.cascade_profile_read, g.subband_profile_read, g.bank_profile_read):
         read(reset=True)
     for i in range(blocks):
         g.wait(g.submit(fmt, data[i % 4]))
-    prof, cp, sp = g.profile_read(), g.cascade_profile_read(), g.subband_profile_read()
+    prof, cp, sp, bp = g.profile_read(), g.cascade_profile_read(), g.subband_profile_read(), g.bank_profile_read()
     g.close()
     per = max(prof["blocks"], 1)
     res["phase_ms_per_block"] = prof["phase_ms"] / per
     res["fir_ms_per_block"] = (prof["fir_tile_ms"] + prof["fir_generic_ms"] + prof["fir_long_ms"]) / per
     res["stage_b_ms_per_block"] = cp["stage_b_ms"] / per
     res["member_ms_per_block"] = sp["member_ms"] / per
+    res["bank_ms_per_block"] = bp["bank_ms"] / per
     return res
 
 
@@ -165,6 +179,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--only", default=None, help="one workload")
+    ap.add_argument("--plans", default=",".join(PLANS), help="plans to alternate, comma-separated")
     args = ap.parse_args()
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
                           capture_output=True, text=True).stdout.strip().splitlines()[0]
@@ -172,7 +187,7 @@ def main():
     names = [args.only] if args.only else list(WORKLOADS)
     for r in range(args.rounds):
         for name in names:
-            for plan in PLANS:
+            for plan in args.plans.split(","):
                 res = run(name, plan, args.blocks, args.warmup)
                 res["round"] = r
                 print(json.dumps(res), flush=True)
