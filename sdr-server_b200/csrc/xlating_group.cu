@@ -188,6 +188,10 @@ struct BlkTable {
   }
 };
 
+// Timed spans of a block: each has a begin and an end event per slot.  Profiling records every span; the
+// timeline (XLATING_B200_TIMELINE) records the convert and tile spans too.
+enum Span { SP_CONV, SP_PHASE, SP_TILE, SP_GEN, SP_LONG, SP_POLY_GEN, SP_POLY_TILE, SP_STAGE_B, SP_SB, SP_BANK, SP_N };
+
 struct Slot {
   void *d_raw = nullptr, *h_raw = nullptr;
   float2 *d_out = nullptr;
@@ -199,11 +203,9 @@ struct Slot {
   float2 *d_endph = nullptr;  // XLG_TRACK_STATE: every client's oscillator after this block (same capacity as d_blk)
   size_t blk_cap = 0;
   cudaEvent_t ev_h2d = nullptr, ev_conv = nullptr, ev_phase = nullptr, ev_fir = nullptr, ev_done = nullptr;
-  cudaEvent_t pf[10] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  cudaEvent_t pf[SP_N][2] = {};  // begin / end of each span
+  bool pf_on[SP_N] = {};         // the span ran in this block (its events are recorded, or, for the pre-pass, stamped)
   cudaEvent_t tl_ph[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // timeline: pre-pass stamps, by occupancy parity (it runs a block ahead)
-  bool pf_conv = false, pf_phase = false, pf_tile = false, pf_gen = false, pf_long = false;
-  cudaEvent_t pf_poly[4] = {nullptr, nullptr, nullptr, nullptr};  // around the polyphase generic / tiled kernels
-  bool pf_pg = false, pf_pt = false;
   float2 *d_pscratch = nullptr;  // kind 4: unrotated outputs per branch (ClientDev::poly_off)
   BlkInfo *d_vblk = nullptr, *h_vblk = nullptr;  // kind 4: per branch class, this block's window start and count
   uint64_t poly_macs = 0;
@@ -211,18 +213,12 @@ struct Slot {
                                  // (integer stage B first, then the rational ones)
   BlkTable<CascPolyBlk> pblk;    // rational cascade clients: this block's stage B
   cudaEvent_t ev_casc = nullptr;                 // stage B of this block done (its rings' appends are ordered on it)
-  cudaEvent_t pf_casc[2] = {nullptr, nullptr};
-  bool pf_cb = false;
   uint64_t casc_macs = 0, d2h_bytes = 0;
   BlkTable<CascBlk> sbcb;        // sub-bands: this block's ring appends
   BlkTable<SbBlk> sbblk;         // member classes: this block's windows and counts
   float2 *d_sbph = nullptr;                      // member oscillator table (HostClient::ph_row)
-  cudaEvent_t pf_sb[2] = {nullptr, nullptr};
-  bool pf_sbk = false;
   uint64_t sb_macs = 0, sb_rows = 0;
   BlkTable<BankBlk> bkblk;       // banks with channels: this block's windows, counts and channel tables
-  cudaEvent_t pf_bk[2] = {nullptr, nullptr};
-  bool pf_bkk = false;
   uint64_t bk_poly = 0, bk_dft = 0;
   std::atomic<int64_t> ticket{-1};
   bool q15 = false;
@@ -330,6 +326,27 @@ struct TileClassHost {
   long long minv = 0;        // decimation^-1 mod interp
 };
 
+// A tiled launch at KT outputs per CTA being assembled: its classes, CTAs and shared memory
+struct TileBatch {
+  TileLaunch P;
+  int KT, ctas = 0;
+  size_t smem = 0;
+  explicit TileBatch(int kt) : KT(kt) { memset(&P, 0, sizeof(P)); }
+  // n_out outputs of class ch, output 0 reading the window at first; returns the MACs its CTAs issue
+  uint64_t add(const TileClassHost &ch, long long first, int n_out) {
+    TileClass k = ch.k;
+    k.first = first;
+    k.n_out = n_out;
+    k.tiles = (n_out + KT - 1) / KT;
+    k.xs_len = (KT - 1) * k.Dp + k.L + (ch.merged ? k.D : 0);
+    k.cta_begin = ctas;
+    ctas += k.tiles * k.n_groups;
+    smem = std::max(smem, (size_t)T_SMEM_FIXED + ((size_t)k.xs_len + 10) * sizeof(float2));
+    P.cls[P.n_classes++] = k;
+    return (uint64_t)k.tiles * KT * (uint64_t)k.L * (uint64_t)ch.members.size();
+  }
+};
+
 }  // namespace
 
 struct xlg_group {
@@ -400,6 +417,7 @@ struct xlg_group {
   int *d_member_cid = nullptr;      // client id per member slot (-1 = padding)
   float2 *d_member_incr = nullptr;  // oscillator step per member slot (same indexing as d_members)
   int *d_order = nullptr;   // clients in oscillator-table order, 32 per group, -1 = padding
+  size_t cap_order = 0;
   int n_order = 0;
   size_t phase_cap = 0;     // float2 per slot oscillator table
   size_t arena_cap = 0;   // complex samples per slot arena
@@ -487,6 +505,55 @@ static size_t next_pow2(size_t v) {
 
 static int elem_bytes(int fmt) { return fmt == XLG_FMT_CS16 ? 2 : 1; }
 
+// (re)fill a device array; the allocation is reused while it is large enough (a re-layout per attach must not
+// pay a cudaFree + cudaMalloc -- each an implicit device synchronisation -- for every table)
+template <typename T>
+static int dev_assign(T **dptr, size_t *cap_bytes, const void *src, size_t bytes) {
+  if (bytes == 0) return 0;
+  if (*dptr == nullptr || *cap_bytes < bytes) {
+    if (*dptr) cudaFree(*dptr);
+    *dptr = nullptr;
+    const size_t want = bytes + bytes / 4 + 4096;
+    CU_OK(cudaMalloc(dptr, want));
+    *cap_bytes = want;
+  }
+  CU_OK(cudaMemcpy(*dptr, src, bytes, cudaMemcpyHostToDevice));
+  return 0;
+}
+
+// replace a device buffer whose contents need not survive by an uninitialised one of `bytes` (its caller has
+// decided that it grows)
+template <typename T>
+static int dev_grow(T **dptr, size_t bytes) {
+  if (*dptr) cudaFree(*dptr);
+  *dptr = nullptr;
+  CU_OK(cudaMalloc(dptr, bytes));
+  return 0;
+}
+
+// Move a power-of-two ring of cap samples into a new one of ncap (the pipeline is drained): the `keep` samples
+// before stream position pos stay at their positions mod ncap, all others read zero.  A ring that does not exist
+// yet (*ring == nullptr) becomes a zeroed one.
+template <typename T>
+static int ring_rehome(T **ring, size_t cap, size_t ncap, long long pos, size_t keep) {
+  T *fresh = nullptr;
+  CU_OK(cudaMalloc(&fresh, ncap * sizeof(T)));
+  if (*ring == nullptr) {
+    CU_OK(cudaMemset(fresh, 0, ncap * sizeof(T)));
+  } else {
+    std::vector<T> old(cap), h(ncap, T{});
+    CU_OK(cudaMemcpy(old.data(), *ring, cap * sizeof(T), cudaMemcpyDeviceToHost));
+    for (size_t k = 1; k <= keep; k++) {
+      const unsigned long long ab = (unsigned long long)(pos - (long long)k);
+      h[ab & (ncap - 1)] = old[ab & (cap - 1)];
+    }
+    CU_OK(cudaMemcpy(fresh, h.data(), ncap * sizeof(T), cudaMemcpyHostToDevice));
+    cudaFree(*ring);
+  }
+  *ring = fresh;
+  return 0;
+}
+
 static void slot_free(Slot &s) {
   if (s.d_raw) cudaFree(s.d_raw);
   if (s.h_raw) cudaFreeHost(s.h_raw);
@@ -531,67 +598,62 @@ static int drain(xlg_group *g) {
   return 0;
 }
 
+// a span's events are recorded while profiling, the convert and tile spans also for the timeline
+static bool span_timed(const xlg_group *g, Span sp) {
+  return g->profiling || (g->timeline && (sp == SP_CONV || sp == SP_TILE));
+}
+
+static int span_begin(xlg_group *g, Slot &s, Span sp, cudaStream_t st) {
+  if (!span_timed(g, sp)) return 0;
+  CU_OK(cudaEventRecord(s.pf[sp][0], st));
+  s.pf_on[sp] = true;
+  return 0;
+}
+
+static int span_end(xlg_group *g, Slot &s, Span sp, cudaStream_t st) {
+  if (span_timed(g, sp)) CU_OK(cudaEventRecord(s.pf[sp][1], st));
+  return 0;
+}
+
 static void harvest_locked(xlg_group *g, Slot &s) {
   if (s.harvested) return;
   s.harvested = true;
-  if (g->timeline && g->base_recorded && s.pf_conv && s.pf_phase && s.pf_tile) {
+  if (g->timeline && g->base_recorded && s.pf_on[SP_CONV] && s.pf_on[SP_PHASE] && s.pf_on[SP_TILE]) {
+    const int par = (int)((s.ticket.load() / XLG_SLOTS) & 1);
+    const cudaEvent_t e[6] = {s.pf[SP_CONV][0], s.pf[SP_CONV][1], s.tl_ph[par][0], s.tl_ph[par][1], s.pf[SP_TILE][0],
+                              s.pf[SP_TILE][1]};
     std::array<float, 7> r;
     r[0] = (float)s.ticket.load();
-    const int par = (int)((s.ticket.load() / XLG_SLOTS) & 1);
-    for (int i = 0; i < 6; i++) {
-      cudaEvent_t e = (i == 2 || i == 3) ? s.tl_ph[par][i - 2] : s.pf[i];
-      if (cudaEventElapsedTime(&r[1 + i], g->ev_base, e) != cudaSuccess) r[1 + i] = -1.f;
-    }
+    for (int i = 0; i < 6; i++)
+      if (cudaEventElapsedTime(&r[1 + i], g->ev_base, e[i]) != cudaSuccess) r[1 + i] = -1.f;
     g->tl.push_back(r);
     cudaGetLastError();
   }
   if (!g->profiling) return;
-  float ms = 0;
-  if (s.pf_conv && cudaEventElapsedTime(&ms, s.pf[0], s.pf[1]) == cudaSuccess) {
-    g->prof.convert_ms += ms;
-    g->prof.convert_launches++;
-  }
-  if (s.pf_phase && cudaEventElapsedTime(&ms, s.pf[2], s.pf[3]) == cudaSuccess) {
-    g->prof.phase_ms += ms;
-    g->prof.phase_launches++;
-  }
-  if (s.pf_tile && cudaEventElapsedTime(&ms, s.pf[4], s.pf[5]) == cudaSuccess) {
-    g->prof.fir_tile_ms += ms;
-    g->prof.fir_tile_launches++;
-  }
-  if (s.pf_gen && cudaEventElapsedTime(&ms, s.pf[6], s.pf[7]) == cudaSuccess) {
-    g->prof.fir_generic_ms += ms;
-    g->prof.fir_generic_launches++;
-  }
-  if (s.pf_long && cudaEventElapsedTime(&ms, s.pf[8], s.pf[9]) == cudaSuccess) {
-    g->prof.fir_long_ms += ms;
-    g->prof.fir_long_launches++;
-  }
-  if (s.pf_pg && cudaEventElapsedTime(&ms, s.pf_poly[0], s.pf_poly[1]) == cudaSuccess) {
-    g->poly_prof.fir_poly_generic_ms += ms;
-    g->poly_prof.fir_poly_generic_launches++;
-  }
-  if (s.pf_pt && cudaEventElapsedTime(&ms, s.pf_poly[2], s.pf_poly[3]) == cudaSuccess) {
-    g->poly_prof.fir_poly_tile_ms += ms;
-    g->poly_prof.fir_poly_tile_launches++;
+  // where each span's time and launch count go, in Span order
+  const std::pair<double *, uint64_t *> sink[SP_N] = {
+      {&g->prof.convert_ms, &g->prof.convert_launches},
+      {&g->prof.phase_ms, &g->prof.phase_launches},
+      {&g->prof.fir_tile_ms, &g->prof.fir_tile_launches},
+      {&g->prof.fir_generic_ms, &g->prof.fir_generic_launches},
+      {&g->prof.fir_long_ms, &g->prof.fir_long_launches},
+      {&g->poly_prof.fir_poly_generic_ms, &g->poly_prof.fir_poly_generic_launches},
+      {&g->poly_prof.fir_poly_tile_ms, &g->poly_prof.fir_poly_tile_launches},
+      {&g->casc_prof.stage_b_ms, &g->casc_prof.stage_b_launches},
+      {&g->sb_prof.member_ms, &g->sb_prof.member_launches},
+      {&g->bank_prof.bank_ms, &g->bank_prof.bank_launches}};
+  for (int sp = 0; sp < SP_N; sp++) {
+    float ms = 0;
+    if (s.pf_on[sp] && cudaEventElapsedTime(&ms, s.pf[sp][0], s.pf[sp][1]) == cudaSuccess) {
+      *sink[sp].first += ms;
+      (*sink[sp].second)++;
+    }
   }
   g->poly_prof.poly_macs += s.poly_macs;
-  if (s.pf_cb && cudaEventElapsedTime(&ms, s.pf_casc[0], s.pf_casc[1]) == cudaSuccess) {
-    g->casc_prof.stage_b_ms += ms;
-    g->casc_prof.stage_b_launches++;
-  }
   g->casc_prof.stage_b_macs += s.casc_macs;
   g->casc_prof.d2h_bytes += s.d2h_bytes;
-  if (s.pf_sbk && cudaEventElapsedTime(&ms, s.pf_sb[0], s.pf_sb[1]) == cudaSuccess) {
-    g->sb_prof.member_ms += ms;
-    g->sb_prof.member_launches++;
-  }
   g->sb_prof.member_macs += s.sb_macs;
   g->sb_prof.row_samples += s.sb_rows;
-  if (s.pf_bkk && cudaEventElapsedTime(&ms, s.pf_bk[0], s.pf_bk[1]) == cudaSuccess) {
-    g->bank_prof.bank_ms += ms;
-    g->bank_prof.bank_launches++;
-  }
   g->bank_prof.poly_macs += s.bk_poly;
   g->bank_prof.dft_macs += s.bk_dft;
   g->prof.blocks++;
@@ -609,44 +671,14 @@ static int ensure_ring(xlg_group *g, size_t need_hist, bool need_q) {
   const size_t cap = next_pow2((XLG_SLOTS + 1) * max_n + hist_cap + 64);
   if (drain(g)) return -EIO;
   if (!g->ring || cap != g->ring_cap) {
-    float2 *nr = nullptr;
-    CU_OK(cudaMalloc(&nr, cap * sizeof(float2)));
-    CU_OK(cudaMemset(nr, 0, cap * sizeof(float2)));
-    if (g->ring) {
-      // keep the most recent samples at their new ring positions
-      const size_t keep = std::min<size_t>(g->ring_cap, (size_t)std::max<long long>(g->S, 0));
-      std::vector<float2> tmp(g->ring_cap);
-      CU_OK(cudaMemcpy(tmp.data(), g->ring, g->ring_cap * sizeof(float2), cudaMemcpyDeviceToHost));
-      std::vector<float2> fresh(cap, make_float2(0.f, 0.f));
-      for (size_t i = 1; i <= keep; i++) {
-        const unsigned long long ab = (unsigned long long)(g->S - (long long)i);
-        fresh[ab & (cap - 1)] = tmp[ab & (g->ring_cap - 1)];
-      }
-      CU_OK(cudaMemcpy(nr, fresh.data(), cap * sizeof(float2), cudaMemcpyHostToDevice));
-      cudaFree(g->ring);
-    }
-    g->ring = nr;
-    if (g->qring) {
-      short2 *nq = nullptr;
-      CU_OK(cudaMalloc(&nq, cap * sizeof(short2)));
-      const size_t keep = std::min<size_t>(g->ring_cap, (size_t)std::max<long long>(g->qS, 0));
-      std::vector<short2> tmp(g->ring_cap);
-      CU_OK(cudaMemcpy(tmp.data(), g->qring, g->ring_cap * sizeof(short2), cudaMemcpyDeviceToHost));
-      std::vector<short2> fresh(cap, make_short2(0, 0));
-      for (size_t i = 1; i <= keep; i++) {
-        const unsigned long long ab = (unsigned long long)(g->qS - (long long)i);
-        fresh[ab & (cap - 1)] = tmp[ab & (g->ring_cap - 1)];
-      }
-      CU_OK(cudaMemcpy(nq, fresh.data(), cap * sizeof(short2), cudaMemcpyHostToDevice));
-      cudaFree(g->qring);
-      g->qring = nq;
-    }
+    // keep the most recent samples at their new ring positions
+    auto keep = [g](long long pos) { return std::min<size_t>(g->ring_cap, (size_t)std::max<long long>(pos, 0)); };
+    if (ring_rehome(&g->ring, g->ring_cap, cap, g->S, keep(g->S)) ||
+        (g->qring && ring_rehome(&g->qring, g->ring_cap, cap, g->qS, keep(g->qS))))
+      return -EIO;
     g->ring_cap = cap;
   }
-  if (need_q && !g->qring) {
-    CU_OK(cudaMalloc(&g->qring, g->ring_cap * sizeof(short2)));
-    CU_OK(cudaMemset(g->qring, 0, g->ring_cap * sizeof(short2)));
-  }
+  if (need_q && !g->qring && ring_rehome(&g->qring, 0, g->ring_cap, 0, 0)) return -EIO;
   g->hist_cap = hist_cap;
   return 0;
 }
@@ -655,19 +687,10 @@ static int ensure_arenas(xlg_group *g, size_t need, bool need_q) {
   const bool dev_out = (g->flags & XLG_OUT_DEVICE) != 0;
   if (need > g->arena_cap) {
     const size_t cap = std::max<size_t>(need + need / 4, 1024);
-    for (Slot &s : g->slots) {
-      if (s.d_out) cudaFree(s.d_out);
-      s.d_out = nullptr;
-      CU_OK(cudaMalloc(&s.d_out, cap * sizeof(float2)));
-      if (g->q_alloc) {
-        if (s.d_qout) cudaFree(s.d_qout);
-        if (s.d_qphases) cudaFree(s.d_qphases);
-        s.d_qout = nullptr;
-        s.d_qphases = nullptr;
-        CU_OK(cudaMalloc(&s.d_qout, cap * sizeof(short2)));
-        CU_OK(cudaMalloc(&s.d_qphases, cap * sizeof(short2)));
-      }
-    }
+    for (Slot &s : g->slots)
+      if (dev_grow(&s.d_out, cap * sizeof(float2)) ||
+          (g->q_alloc && (dev_grow(&s.d_qout, cap * sizeof(short2)) || dev_grow(&s.d_qphases, cap * sizeof(short2)))))
+        return -EIO;
     for (HostOut &h : g->ring_out) {
       float2 *n_out = nullptr;
       short2 *n_qout = nullptr;
@@ -687,10 +710,10 @@ static int ensure_arenas(xlg_group *g, size_t need, bool need_q) {
     g->arena_cap = cap;
   }
   if (need_q && !g->q_alloc) {
-    for (Slot &s : g->slots) {
-      CU_OK(cudaMalloc(&s.d_qout, std::max<size_t>(g->arena_cap, 1) * sizeof(short2)));
-      CU_OK(cudaMalloc(&s.d_qphases, std::max<size_t>(g->arena_cap, 1) * sizeof(short2)));
-    }
+    for (Slot &s : g->slots)
+      if (dev_grow(&s.d_qout, std::max<size_t>(g->arena_cap, 1) * sizeof(short2)) ||
+          dev_grow(&s.d_qphases, std::max<size_t>(g->arena_cap, 1) * sizeof(short2)))
+        return -EIO;
     if (!dev_out)
       for (HostOut &h : g->ring_out)
         CU_OK(cudaHostAlloc(&h.h_qout, std::max<size_t>(g->arena_cap, 1) * sizeof(short2), cudaHostAllocDefault));
@@ -703,41 +726,12 @@ static int ensure_arenas(xlg_group *g, size_t need, bool need_q) {
 // arenas, kernel classes.  Dynamic per-client state (hist, phase) lives on the
 // device and is preserved.
 static void choose_partition(xlg_group *g);
-// (re)fill a device array; the allocation is reused while it is large enough (a re-layout per attach must not
-// pay a cudaFree + cudaMalloc -- each an implicit device synchronisation -- for every table)
-template <typename T>
-static int dev_assign(T **dptr, size_t *cap_bytes, const void *src, size_t bytes) {
-  if (bytes == 0) return 0;
-  if (*dptr == nullptr || *cap_bytes < bytes) {
-    if (*dptr) cudaFree(*dptr);
-    *dptr = nullptr;
-    const size_t want = bytes + bytes / 4 + 4096;
-    CU_OK(cudaMalloc(dptr, want));
-    *cap_bytes = want;
-  }
-  CU_OK(cudaMemcpy(*dptr, src, bytes, cudaMemcpyHostToDevice));
-  return 0;
-}
 // Give a cascade's or a sub-band's history ring room for cap samples (a power of two; the pipeline is drained):
 // a new ring is zero, which its positions before the attach read, and a grown one keeps its last samples at
 // their new places.
 static int ring_ensure(HistRing &r, size_t cap) {
   if (r.p != nullptr && cap <= r.cap) return 0;
-  float2 *ring = nullptr;
-  CU_OK(cudaMalloc(&ring, cap * sizeof(float2)));
-  if (r.p == nullptr) {
-    CU_OK(cudaMemset(ring, 0, cap * sizeof(float2)));
-  } else {
-    std::vector<float2> old(r.cap), fresh(cap, make_float2(0.f, 0.f));
-    CU_OK(cudaMemcpy(old.data(), r.p, r.cap * sizeof(float2), cudaMemcpyDeviceToHost));
-    for (size_t k = 1; k <= r.cap; k++) {
-      const unsigned long long p = (unsigned long long)(r.pos - (long long)k);
-      fresh[p & (cap - 1)] = old[p & (r.cap - 1)];
-    }
-    CU_OK(cudaMemcpy(ring, fresh.data(), cap * sizeof(float2), cudaMemcpyHostToDevice));
-    cudaFree(r.p);
-  }
-  r.p = ring;
+  if (ring_rehome(&r.p, r.cap, cap, r.pos, r.cap)) return -EIO;
   r.cap = cap;
   return 0;
 }
@@ -864,16 +858,10 @@ static int rebuild_subbands(xlg_group *g, size_t &out_total) {
   const size_t n_sb = g->sb_list.size(), n_cls = g->sb_classes.size();
   const bool grow_ph = rows > g->sbph_cap;
   if (grow_ph) g->sbph_cap = rows + rows / 4 + 1024;
-  for (Slot &s : g->slots) {
-    if (s.pf_sb[0] == nullptr)
-      for (cudaEvent_t &ev : s.pf_sb) CU_OK(cudaEventCreate(&ev));
-    if (s.sbcb.reserve(n_sb) || s.sbblk.reserve(n_cls)) return -EIO;
-    if ((grow_ph || s.d_sbph == nullptr) && g->sbph_cap > 0) {
-      if (s.d_sbph) cudaFree(s.d_sbph);
-      s.d_sbph = nullptr;
-      CU_OK(cudaMalloc(&s.d_sbph, g->sbph_cap * sizeof(float2)));
-    }
-  }
+  for (Slot &s : g->slots)
+    if (s.sbcb.reserve(n_sb) || s.sbblk.reserve(n_cls) ||
+        ((grow_ph || s.d_sbph == nullptr) && g->sbph_cap > 0 && dev_grow(&s.d_sbph, g->sbph_cap * sizeof(float2))))
+      return -EIO;
   return 0;
 }
 
@@ -905,12 +893,107 @@ static int rebuild_banks(xlg_group *g) {
       dev_assign(&g->d_bktw, &g->cap_bktw, tw.data(), tw.size() * sizeof(float2)) ||
       dev_assign(&g->d_bkch, &g->cap_bkch, chans.data(), chans.size() * sizeof(int2)))
     return -EIO;
-  for (Slot &s : g->slots) {
-    if (s.pf_bk[0] == nullptr)
-      for (cudaEvent_t &ev : s.pf_bk) CU_OK(cudaEventCreate(&ev));
+  for (Slot &s : g->slots)
     if (s.bkblk.reserve(g->bank_live.size())) return -EIO;
-  }
   return 0;
+}
+
+// Cascade clients (the pipeline is drained): stage-A rows after every host-visible row (the D2H copy ends before
+// them), stage-B taps, and a zeroed history ring for each new client (its positions before the attach read as
+// zero)
+static int rebuild_cascades(xlg_group *g, size_t &out_total) {
+  const int nc = (int)g->clients.size();
+  std::vector<float> taps2;
+  g->n_casc = g->n_casc_int = 0;
+  for (int i = 0; i < nc; i++) {
+    HostClient &h = g->clients[i];
+    if (!h.active || !h.casc) continue;
+    h.out_off = (int)out_total;
+    out_total += (size_t)h.out_cap;
+    out_total = (out_total + 3) & ~(size_t)3;
+    h.b2.taps_off = (int)taps2.size();
+    taps2.insert(taps2.end(), h.b2.taps.begin(), h.b2.taps.end());
+    // stage B of block b reads stage-A outputs of earlier blocks; the submit of block b + XLG_SLOTS waits
+    // for ticket b, so its history + (XLG_SLOTS + 1) * max n1 samples are never overwritten while still needed
+    if (ring_ensure(h.b2.ring, next_pow2(history_reach(h.b2.geo.T2, h.b2.geo.L2) +
+                                         (size_t)(XLG_SLOTS + 1) * (size_t)h.out_cap)))
+      return -EIO;
+    g->n_casc++;
+    if (h.b2.geo.L2 == 1) g->n_casc_int++;
+  }
+  // integer entries ordered by ko, one stage-B launch per distinct ko: a client's lanes walk its taps as they
+  // would in a group of its own, whatever ko its neighbours have
+  std::vector<int> ints;
+  for (int i = 0; i < nc; i++)
+    if (g->clients[i].active && g->clients[i].casc && g->clients[i].b2.geo.L2 == 1) ints.push_back(i);
+  std::stable_sort(ints.begin(), ints.end(),
+                   [g](int a, int b) { return g->clients[a].b2.ko > g->clients[b].b2.ko; });
+  g->casc_runs.clear();
+  for (int e = 0; e < (int)ints.size(); e++) {
+    HostClient &h = g->clients[ints[e]];
+    h.cblk = e;
+    if (g->casc_runs.empty() || g->casc_runs.back().ko != h.b2.ko) g->casc_runs.push_back({h.b2.ko, e, e});
+    g->casc_runs.back().c1 = e + 1;
+  }
+  if (dev_assign(&g->d_taps2, &g->cap_taps2, taps2.data(), taps2.size() * sizeof(float))) return -EIO;
+  for (float2 *p : g->dead_rings) cudaFree(p);
+  g->dead_rings.clear();
+  for (Slot &s : g->slots)
+    if (s.cblk.reserve((size_t)g->n_casc) || s.pblk.reserve((size_t)(g->n_casc - g->n_casc_int))) return -EIO;
+  return 0;
+}
+
+// How the tiled kernels read a class of (D, T): natural or skewed input layout at pitch Dp, L flat taps per slot,
+// and whether it is a split-K long-filter class and can be tiled at all
+struct TileMode {
+  bool natural, as_long, eligible;
+  int Dp, L;
+};
+
+// A tiled class over `slots` (T_CG per group, -1 = padding) of clients with T taps at decimation D: its kernel
+// entry (the caller adds what is particular to its family) and its taps, appended to tile_taps as
+// [group][flat tap f][T_CG slots] with tap j = q * D + r at f = q * Dp + r.  taps(id) is a member's T reversed
+// taps (re, im interleaved).
+template <typename Taps>
+static TileClassHost tile_class(const std::vector<int> &slots, const std::vector<int> &real, uint32_t D, size_t T,
+                                const TileMode &m, int members_off, std::vector<float2> &tile_taps, Taps taps) {
+  TileClassHost ch;
+  memset(&ch.k, 0, sizeof(ch.k));
+  ch.T = T;
+  ch.members = slots;
+  ch.real = real;
+  ch.k.D = (int)D;
+  ch.k.Dp = m.Dp;
+  ch.k.L = m.L;
+  ch.k.n_groups = (int)(slots.size() / T_CG);
+  ch.k.n_members = (int)real.size();
+  ch.k.natural = m.natural ? 1 : 0;
+  ch.k.members_off = members_off;
+  ch.k.taps_off = (long long)tile_taps.size();
+  const size_t base = tile_taps.size();
+  tile_taps.resize(base + slots.size() * (size_t)m.L, make_float2(0.f, 0.f));
+  // one 256-byte line (all 32 slots of a tap) at a time -- slot-major packing touched a new cache line for every
+  // tap of every client (1.5 ms per re-layout at 1000 clients)
+  for (size_t gi = 0; gi < slots.size() / T_CG; gi++) {
+    float2 *dst = tile_taps.data() + base + gi * (size_t)m.L * T_CG;
+    const float *src[T_CG];
+    for (int sl = 0; sl < T_CG; sl++) {
+      const int id = slots[gi * T_CG + sl];
+      src[sl] = id < 0 ? nullptr : taps(id);
+    }
+    size_t q = 0, r = 0;  // j = q * D + r
+    for (size_t j = 0; j < T; j++) {
+      const size_t f = q * m.Dp + r;
+      if (++r == D) {
+        r = 0;
+        q++;
+      }
+      float2 *row = dst + f * T_CG;
+      for (int sl = 0; sl < T_CG; sl++)
+        if (src[sl]) row[sl] = make_float2(src[sl][2 * j], src[sl][2 * j + 1]);
+    }
+  }
+  return ch;
 }
 
 static int rebuild_layout(xlg_group *g) {
@@ -969,47 +1052,7 @@ static int rebuild_layout(xlg_group *g) {
   }
   for (const BankHost &k : g->banks)  // a bank walks (and its channels read history) without channels too
     if (k.active) max_hist = std::max(max_hist, k.T1 - 1);
-  // cascade clients: stage-A rows after every host-visible row (the D2H copy ends before them), stage-B taps,
-  // and a zeroed history ring for each new client (its positions before the attach read as zero)
-  {
-    std::vector<float> taps2;
-    g->n_casc = g->n_casc_int = 0;
-    for (int i = 0; i < nc; i++) {
-      HostClient &h = g->clients[i];
-      if (!h.active || !h.casc) continue;
-      h.out_off = (int)out_total;
-      out_total += (size_t)h.out_cap;
-      out_total = (out_total + 3) & ~(size_t)3;
-      h.b2.taps_off = (int)taps2.size();
-      taps2.insert(taps2.end(), h.b2.taps.begin(), h.b2.taps.end());
-      // stage B of block b reads stage-A outputs of earlier blocks; the submit of block b + XLG_SLOTS waits
-      // for ticket b, so its history + (XLG_SLOTS + 1) * max n1 samples are never overwritten while still needed
-      if (ring_ensure(h.b2.ring, next_pow2(history_reach(h.b2.geo.T2, h.b2.geo.L2) +
-                                           (size_t)(XLG_SLOTS + 1) * (size_t)h.out_cap)))
-        return -EIO;
-      g->n_casc++;
-      if (h.b2.geo.L2 == 1) g->n_casc_int++;
-    }
-    // integer entries ordered by ko, one stage-B launch per distinct ko: a client's lanes walk its taps as they
-    // would in a group of its own, whatever ko its neighbours have
-    std::vector<int> ints;
-    for (int i = 0; i < nc; i++)
-      if (g->clients[i].active && g->clients[i].casc && g->clients[i].b2.geo.L2 == 1) ints.push_back(i);
-    std::stable_sort(ints.begin(), ints.end(),
-                     [g](int a, int b) { return g->clients[a].b2.ko > g->clients[b].b2.ko; });
-    g->casc_runs.clear();
-    for (int e = 0; e < (int)ints.size(); e++) {
-      HostClient &h = g->clients[ints[e]];
-      h.cblk = e;
-      if (g->casc_runs.empty() || g->casc_runs.back().ko != h.b2.ko) g->casc_runs.push_back({h.b2.ko, e, e});
-      g->casc_runs.back().c1 = e + 1;
-    }
-    if (dev_assign(&g->d_taps2, &g->cap_taps2, taps2.data(), taps2.size() * sizeof(float))) return -EIO;
-    for (float2 *p : g->dead_rings) cudaFree(p);
-    g->dead_rings.clear();
-    for (Slot &s : g->slots)
-      if (s.cblk.reserve((size_t)g->n_casc) || s.pblk.reserve((size_t)(g->n_casc - g->n_casc_int))) return -EIO;
-  }
+  if (rebuild_cascades(g, out_total)) return -EIO;
   if (rebuild_subbands(g, out_total)) return -EIO;
   if (rebuild_banks(g)) return -EIO;
   if (ensure_ring(g, max_hist, g->qring != nullptr)) return -EIO;
@@ -1044,12 +1087,8 @@ static int rebuild_layout(xlg_group *g) {
   // tile of RK = 4: decides eligibility (smaller shapes need less; RK = 5 is used only where its tile fits)
   const int KT = 64;
   const size_t smem_fixed = (size_t)T_SMEM_FIXED;
-  struct Mode {
-    bool natural, as_long, eligible;
-    int Dp, L;
-  };
   auto mode_of = [&](uint32_t D, size_t T) {
-    Mode m;
+    TileMode m;
     const unsigned g16 = (D % 16 == 0) ? 16u : (D % 8 == 0) ? 8u : (D % 4 == 0) ? 4u : (D % 2 == 0) ? 2u : 1u;
     m.natural = g16 <= 2 && !env_skewed;
     m.Dp = m.natural ? (int)D : (int)(D | 1u);
@@ -1088,7 +1127,7 @@ static int rebuild_layout(xlg_group *g) {
       // rational: a tiled class per (L, M, T, alignment) where every branch is an integer class the tiled
       // kernel takes (gcd(L, M) = 1: each block uses every branch, outputs L apart)
       const size_t Tb = (h.T + h.L - 1) / h.L;
-      const Mode m = mode_of(h.D, Tb);
+      const TileMode m = mode_of(h.D, Tb);
       if ((g->flags & XLG_FORCE_GENERIC) || !g->poly_tile || std::gcd(h.L, h.D) != 1 || !m.eligible || m.as_long)
         continue;
       if (!poly_settled(g, h)) {
@@ -1098,15 +1137,13 @@ static int rebuild_layout(xlg_group *g) {
       pbuckets[std::make_tuple(h.L, h.D, h.T, h.hist)].push_back(i);
       continue;
     }
-    const long long first = g->S - h.hist;
-    const bool settled = (h.zero_before == 0 && g->S < (long long)g->ring_cap / 2) || h.zero_before <= first;
     if (g->flags & XLG_FORCE_GENERIC) continue;
-    const Mode m = mode_of(h.D, h.T);
+    const TileMode m = mode_of(h.D, h.T);
     if (!m.eligible) {
       h.tile_ineligible = true;
       continue;
     }
-    if (!settled) {
+    if (!poly_settled(g, h)) {
       h.pending_settle = true;  // re-derive the layout once its window has passed
       continue;
     }
@@ -1122,7 +1159,7 @@ static int rebuild_layout(xlg_group *g) {
     const uint32_t D = std::get<0>(kv.first);
     const size_t T = std::get<1>(kv.first);
     const bool merged = std::get<2>(kv.first) < 0;
-    const Mode m = mode_of(D, T);
+    const TileMode m = mode_of(D, T);
     // subgroups of 8 slots with one window alignment each
     std::map<long long, std::vector<int>> by_align;
     for (int id : kv.second) by_align[merged ? (long long)(T - 1) - g->clients[id].hist : 0].push_back(id);
@@ -1147,23 +1184,7 @@ static int rebuild_layout(xlg_group *g) {
       continue;
     }
     while (slots.size() % T_CG != 0) slots.push_back(-1);
-    TileClassHost ch;
-    memset(&ch.k, 0, sizeof(ch.k));
-    ch.T = T;
-    ch.members = slots;
-    ch.real = real;
-    ch.merged = merged;
-    ch.k.D = (int)D;
-    ch.k.Dp = m.Dp;
-    ch.k.L = m.L;
-    ch.k.n_groups = (int)(slots.size() / T_CG);
-    ch.k.n_members = (int)real.size();
-    ch.k.natural = m.natural ? 1 : 0;
-    ch.k.nseg = m.as_long ? (ch.k.L + W_JS - 1) / W_JS : 0;
-    ch.k.members_off = (int)members.size();
-    ch.k.taps_off = (long long)tile_taps.size();
-    const size_t base = tile_taps.size();
-    tile_taps.resize(base + slots.size() * (size_t)m.L, make_float2(0.f, 0.f));
+    const int members_off = (int)members.size();
     for (size_t sl = 0; sl < slots.size(); sl++) {
       const int id = slots[sl];
       member_cid.push_back(id);
@@ -1177,27 +1198,10 @@ static int rebuild_layout(xlg_group *g) {
       member_incr.push_back(make_float2(h.incr_re, h.incr_im));
       h.kind = m.as_long ? 2 : 1;
     }
-    // taps into [group][flat tap f][32 slots]: one 256-byte line (all 32 slots of a tap) at a time -- slot-major
-    // packing touched a new cache line for every tap of every client (1.5 ms per re-layout at 1000 clients)
-    for (size_t gi = 0; gi < slots.size() / T_CG; gi++) {
-      float2 *dst = tile_taps.data() + base + gi * (size_t)m.L * T_CG;
-      const float *src[T_CG];
-      for (int sl = 0; sl < T_CG; sl++) {
-        const int id = slots[gi * T_CG + sl];
-        src[sl] = id < 0 ? nullptr : g->clients[id].rev.data();
-      }
-      size_t q = 0, r = 0;  // j = q * D + r
-      for (size_t j = 0; j < T; j++) {
-        const size_t f = q * m.Dp + r;
-        if (++r == D) {
-          r = 0;
-          q++;
-        }
-        float2 *row = dst + f * T_CG;
-        for (int sl = 0; sl < T_CG; sl++)
-          if (src[sl]) row[sl] = make_float2(src[sl][2 * j], src[sl][2 * j + 1]);
-      }
-    }
+    TileClassHost ch = tile_class(slots, real, D, T, m, members_off, tile_taps,
+                                  [g](int id) { return g->clients[id].rev.data(); });
+    ch.merged = merged;
+    ch.k.nseg = m.as_long ? (ch.k.L + W_JS - 1) / W_JS : 0;
     dest.push_back(ch);
   }
   // rational tiled classes: one tiled class per polyphase branch r, members in the same slots of every branch
@@ -1208,7 +1212,7 @@ static int rebuild_layout(xlg_group *g) {
     const size_t T = std::get<2>(kv.first), Tb = (T + L - 1) / L;
     std::vector<int> &real = kv.second;
     if ((int)real.size() < kTileMinClients || g->poly_classes.size() + L > (size_t)T_MAX_CLASSES) continue;
-    const Mode m = mode_of(M, Tb);
+    const TileMode m = mode_of(M, Tb);
     std::vector<int> slots(real);
     while (slots.size() % T_CG != 0) slots.push_back(-1);
     long long minv = 0;  // M^-1 mod L (extended Euclid)
@@ -1232,40 +1236,19 @@ static int rebuild_layout(xlg_group *g) {
       max_rowcap = std::max(max_rowcap, h.poly_rowcap);
     }
     for (uint32_t r = 0; r < L; r++) {
-      TileClassHost ch;
-      memset(&ch.k, 0, sizeof(ch.k));
-      ch.T = Tb;
-      ch.members = slots;
-      ch.real = real;
-      ch.branch = (int)r;
-      ch.interp = L;
-      ch.minv = minv;
-      ch.k.D = (int)M;
-      ch.k.Dp = m.Dp;
-      ch.k.L = m.L;
-      ch.k.n_groups = (int)(slots.size() / T_CG);
-      ch.k.n_members = (int)real.size();
-      ch.k.natural = m.natural ? 1 : 0;
-      ch.k.members_off = (int)members.size();
-      ch.k.taps_off = (long long)tile_taps.size();
+      const int members_off = (int)members.size();
       const int v = (int)g->poly_classes.size();  // the tiled kernel reads this class's BlkInfo at d_vblk[v]
       for (int id : slots) {
         member_cid.push_back(id < 0 ? -1 : v);
         members.push_back(id < 0 ? -1 : g->clients[id].poly_off + (int)r * g->clients[id].poly_rowcap);
         member_incr.push_back(make_float2(1.f, 0.f));
       }
-      const size_t base = tile_taps.size();
-      tile_taps.resize(base + slots.size() * (size_t)m.L, make_float2(0.f, 0.f));
-      for (size_t gi = 0; gi < slots.size() / T_CG; gi++) {
-        float2 *dst = tile_taps.data() + base + gi * (size_t)m.L * T_CG;
-        for (int sl = 0; sl < T_CG; sl++) {
-          const int id = slots[gi * T_CG + sl];
-          if (id < 0) continue;
-          const float *src = g->clients[id].rev.data() + 2 * (size_t)r * Tb;  // branch r (xl_poly_pack)
-          for (size_t t = 0; t < Tb; t++)
-            dst[((t / M) * m.Dp + t % M) * T_CG + sl] = make_float2(src[2 * t], src[2 * t + 1]);
-        }
-      }
+      // branch r of every member (xl_poly_pack)
+      TileClassHost ch = tile_class(slots, real, M, Tb, m, members_off, tile_taps,
+                                    [g, r, Tb](int id) { return g->clients[id].rev.data() + 2 * (size_t)r * Tb; });
+      ch.branch = (int)r;
+      ch.interp = L;
+      ch.minv = minv;
       g->poly_classes.push_back(ch);
     }
   }
@@ -1364,13 +1347,8 @@ static int rebuild_layout(xlg_group *g) {
       }
       table += (size_t)cap * 32;
     }
-    if (g->d_order) cudaFree(g->d_order);
-    g->d_order = nullptr;
     g->n_order = (int)order.size();
-    if (!order.empty()) {
-      CU_OK(cudaMalloc(&g->d_order, order.size() * sizeof(int)));
-      CU_OK(cudaMemcpy(g->d_order, order.data(), order.size() * sizeof(int), cudaMemcpyHostToDevice));
-    }
+    if (dev_assign(&g->d_order, &g->cap_order, order.data(), order.size() * sizeof(int))) return -EIO;
     {
       size_t part = 0;
       for (TileClassHost &ch : g->long_classes) {
@@ -1384,38 +1362,27 @@ static int rebuild_layout(xlg_group *g) {
       }
       if (part > g->partial_cap) {
         g->partial_cap = part;
-        for (Slot &sl : g->slots) {
-          if (sl.d_partial) cudaFree(sl.d_partial);
-          sl.d_partial = nullptr;
-          CU_OK(cudaMalloc(&sl.d_partial, g->partial_cap * sizeof(float2)));
-        }
+        for (Slot &sl : g->slots)
+          if (dev_grow(&sl.d_partial, g->partial_cap * sizeof(float2))) return -EIO;
       }
     }
     if (pscratch > g->pscratch_cap) {
       g->pscratch_cap = pscratch + pscratch / 4 + 1024;
-      for (Slot &sl : g->slots) {
-        if (sl.d_pscratch) cudaFree(sl.d_pscratch);
-        sl.d_pscratch = nullptr;
-        CU_OK(cudaMalloc(&sl.d_pscratch, g->pscratch_cap * sizeof(float2)));
-      }
+      for (Slot &sl : g->slots)
+        if (dev_grow(&sl.d_pscratch, g->pscratch_cap * sizeof(float2))) return -EIO;
     }
     // the tiled kernel reads the phase of output j at [32 * (j / 2) + client slot]: a table of ones that long
     const size_t ones = ((size_t)max_rowcap / 2 + 2) * 32;
     if (!g->poly_classes.empty() && ones > g->ones_cap) {
-      if (g->d_ones) cudaFree(g->d_ones);
-      g->d_ones = nullptr;
       g->ones_cap = ones;
       std::vector<float2> one(ones, make_float2(1.f, 0.f));
-      CU_OK(cudaMalloc(&g->d_ones, ones * sizeof(float2)));
+      if (dev_grow(&g->d_ones, ones * sizeof(float2))) return -EIO;
       CU_OK(cudaMemcpy(g->d_ones, one.data(), ones * sizeof(float2), cudaMemcpyHostToDevice));
     }
     if (table > g->phase_cap) {
       g->phase_cap = table + table / 4 + 1024;
-      for (Slot &sl : g->slots) {
-        if (sl.d_phases) cudaFree(sl.d_phases);
-        sl.d_phases = nullptr;
-        CU_OK(cudaMalloc(&sl.d_phases, g->phase_cap * sizeof(float2)));
-      }
+      for (Slot &sl : g->slots)
+        if (dev_grow(&sl.d_phases, g->phase_cap * sizeof(float2))) return -EIO;
     }
   }
 
@@ -1467,26 +1434,20 @@ static int rebuild_layout(xlg_group *g) {
       return -EIO;
   }
   if ((size_t)nc > g->d_clients_cap) {
-    if (g->d_clients) cudaFree(g->d_clients);
-    g->d_clients = nullptr;
     g->d_clients_cap = std::max<size_t>((size_t)nc * 2, 64);
-    CU_OK(cudaMalloc(&g->d_clients, g->d_clients_cap * sizeof(ClientDev)));
+    if (dev_grow(&g->d_clients, g->d_clients_cap * sizeof(ClientDev))) return -EIO;
     CU_OK(cudaMemset(g->d_clients, 0, g->d_clients_cap * sizeof(ClientDev)));
-    if (g->d_clients_backup) cudaFree(g->d_clients_backup);
-    g->d_clients_backup = nullptr;
-    CU_OK(cudaMalloc(&g->d_clients_backup, g->d_clients_cap * sizeof(SpecSave)));
+    if (dev_grow(&g->d_clients_backup, g->d_clients_cap * sizeof(SpecSave))) return -EIO;
   }
   if (nc > 0) CU_OK(cudaMemcpy(g->d_clients, tab.data(), (size_t)nc * sizeof(ClientDev), cudaMemcpyHostToDevice));
 
   for (Slot &s : g->slots) {
     if (s.blk_cap < (size_t)std::max(nc, 1)) {
-      if (s.d_blk) cudaFree(s.d_blk);
-      s.d_blk = nullptr;
       s.blk_cap = std::max<size_t>((size_t)nc * 2, 64);
-      CU_OK(cudaMalloc(&s.d_blk, s.blk_cap * sizeof(BlkInfo)));
-      if (s.d_endph) cudaFree(s.d_endph);
-      s.d_endph = nullptr;
-      if (g->flags & XLG_TRACK_STATE) CU_OK(cudaMalloc(&s.d_endph, s.blk_cap * sizeof(float2)));
+      // (d_endph exists in XLG_TRACK_STATE groups only)
+      if (dev_grow(&s.d_blk, s.blk_cap * sizeof(BlkInfo)) ||
+          ((g->flags & XLG_TRACK_STATE) && dev_grow(&s.d_endph, s.blk_cap * sizeof(float2))))
+        return -EIO;
     }
   }
   if (g->flags & XLG_TRACK_STATE) {
@@ -1717,12 +1678,9 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
     cudaEvent_t *evs[] = {&s.ev_h2d, &s.ev_conv, &s.ev_phase, &s.ev_fir, &s.ev_done};
     for (cudaEvent_t *ev : evs)
       if (cudaEventCreateWithFlags(ev, cudaEventDisableTiming) != cudaSuccess) return fail(-EIO);
-    for (int i = 0; i < 10; i++)
-      if (cudaEventCreate(&s.pf[i]) != cudaSuccess) return fail(-EIO);
-    for (cudaEvent_t &ev : s.pf_poly)
-      if (cudaEventCreate(&ev) != cudaSuccess) return fail(-EIO);
-    for (cudaEvent_t &ev : s.pf_casc)
-      if (cudaEventCreate(&ev) != cudaSuccess) return fail(-EIO);
+    for (auto &span : s.pf)
+      for (cudaEvent_t &ev : span)
+        if (cudaEventCreate(&ev) != cudaSuccess) return fail(-EIO);
     if (cudaEventCreateWithFlags(&s.ev_casc, cudaEventDisableTiming) != cudaSuccess) return fail(-EIO);
     if (cudaMalloc(&s.d_vblk, T_MAX_CLASSES * sizeof(BlkInfo)) != cudaSuccess ||
         cudaHostAlloc(&s.h_vblk, T_MAX_CLASSES * sizeof(BlkInfo), cudaHostAllocDefault) != cudaSuccess)
@@ -1839,17 +1797,10 @@ extern "C" void xlg_destroy(xlg_group *g) {
     cudaEvent_t evs[] = {s.ev_h2d, s.ev_conv, s.ev_phase, s.ev_fir, s.ev_done};
     for (cudaEvent_t ev : evs)
       if (ev) cudaEventDestroy(ev);
-    for (int i = 0; i < 10; i++)
-      if (s.pf[i]) cudaEventDestroy(s.pf[i]);
-    for (cudaEvent_t ev : s.pf_poly)
-      if (ev) cudaEventDestroy(ev);
-    for (cudaEvent_t ev : s.pf_casc)
-      if (ev) cudaEventDestroy(ev);
+    for (auto &span : s.pf)
+      for (cudaEvent_t ev : span)
+        if (ev) cudaEventDestroy(ev);
     if (s.ev_casc) cudaEventDestroy(s.ev_casc);
-    for (cudaEvent_t ev : s.pf_sb)
-      if (ev) cudaEventDestroy(ev);
-    for (cudaEvent_t ev : s.pf_bk)
-      if (ev) cudaEventDestroy(ev);
   }
   for (HostOut &h : g->ring_out) {
     if (h.h_out) cudaFreeHost(h.h_out);
@@ -2344,14 +2295,6 @@ extern "C" int xlg_add_bank_subband(xlg_group *g, int bank_id, int32_t channel, 
   return 0;
 }
 
-extern "C" int xlg_bank_profile_read(xlg_group *g, xlg_bank_profile *p, int reset) {
-  if (g == nullptr || p == nullptr) return -EINVAL;
-  std::lock_guard<std::mutex> lk(g->mu);
-  *p = g->bank_prof;
-  if (reset) memset(&g->bank_prof, 0, sizeof(g->bank_prof));
-  return 0;
-}
-
 template <int FMT>
 static void launch_convert(bool q15, const void *raw, xlg_group *g, long long S, int n, cudaStream_t st) {
   const int threads = 256, blocks = (n + threads - 1) / threads;
@@ -2365,6 +2308,623 @@ static void launch_convert(bool q15, const void *raw, xlg_group *g, long long S,
   } else {
     convert_cf32_kernel<FMT><<<blocks, threads, 0, st>>>(raw, g->ring, mask, S, n);
   }
+}
+
+// One block being submitted: where it goes, and what the walks over its clients, banks and sub-bands found (the
+// sizes of each kernel family's launch)
+struct Block {
+  xlg_group *g;
+  Slot &s;
+  HostOut &ho;
+  int64_t ticket;
+  long long S;  // stream position of its first sample, on its path
+  int n;        // complex samples (src/xlating.c:387)
+  bool q15;
+  unsigned mask;
+  int nc;       // client table entries the kernels walk
+  cudaStream_t cs = nullptr, cvs = nullptr;  // its compute stream, the stream of its raw -> ring conversion
+  // client walk
+  int max_generic_out = 0, poly_warps = 0, max_poly4_out = 0;
+  int n_casc = 0, max_n1 = 0;
+  int n_crat = 0, max_rat_ctas = 0;  // rational stage B; CTAs per rational client
+  size_t casc_poly_smem = 0;
+  // bank walk
+  int n_bk = 0, max_bk_n1 = 0, max_bk_cg = 0;
+  size_t bk_smem = 0;
+  // sub-band walk
+  int n_sb = 0, max_sb_n1 = 0, max_sb_n2 = 0;
+  int max_sbr_ctas = 0, max_sbr_l2 = 0;  // rational classes: output tiles of the longest residue, largest L2
+  size_t sb_smem = 0, sbr_smem = 0;
+};
+
+// Clients: each one's outputs in this block (the host mirror of the oscillator pre-pass kernel's integer formula),
+// its next window (h.hist) and, for a cascade, its stage-B walk
+static void walk_clients(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  HostOut &ho = b.ho;
+  for (size_t i = 0; i < g->clients.size(); i++) {
+    HostClient &h = g->clients[i];
+    if (!h.active || h.mem || h.bank >= 0) continue;
+    // upsampled coordinates (the same integers for L = 1)
+    const long long Su = b.S * h.L, Eu = (b.S + b.n) * h.L;
+    const long long first = Su - h.hist;
+    const long long last_ok = Eu - (long long)h.T;
+    int n_out = 0;
+    if (last_ok >= first) n_out = (int)((last_ok - first) / (long long)h.D) + 1;
+    if (n_out > h.out_cap) n_out = h.out_cap;
+    ho.n_out[i] = n_out;
+    ho.out_off[i] = h.out_off;
+    h.hist = Eu - (first + (long long)n_out * (long long)h.D);
+    if (g->flags & XLG_TRACK_STATE) ho.hist_after[i] = h.hist;
+    s.out_samples += (uint64_t)n_out;
+    const uint64_t macs = (uint64_t)n_out * ((h.T + h.L - 1) / h.L);
+    s.algo_macs += macs;
+    if (h.kind >= 3) s.poly_macs += macs;
+    if (h.kind == 4) b.max_poly4_out = std::max(b.max_poly4_out, n_out);
+    if (h.kind == 3) {
+      // warps of fir_poly_generic_cf32_kernel: min(L, n_out) residues x groups of G_OPW outputs
+      const int per = (int)((n_out + (long long)h.L - 1) / h.L);
+      b.poly_warps = std::max(b.poly_warps, (int)std::min<long long>(h.L, n_out) * ((per + G_OPW - 1) / G_OPW));
+    }
+    if (b.q15 || h.kind == 0) b.max_generic_out = std::max(b.max_generic_out, n_out);
+    if (h.casc) {
+      const StageBGeom &geo = h.b2.geo;
+      const StageBStep w = stage_b_walk(h.b2.geo, h.b2.ring.pos, n_out, h.b2.fin_cap);
+      if (geo.L2 == 1) {
+        stage_b_fill(h.b2, w, n_out, h.out_off, &s.cblk.h[h.cblk], nullptr);
+        s.casc_macs += (uint64_t)w.n2 * geo.T2;
+      } else {
+        // only the appends read this client's CascBlk; cascade_fir_poly_cf32_kernel reads its CascPolyBlk
+        stage_b_fill(h.b2, w, n_out, h.out_off, &s.cblk.h[g->n_casc_int + b.n_crat], &s.pblk.h[b.n_crat]);
+        b.n_crat++;
+        b.max_rat_ctas = std::max(b.max_rat_ctas, (w.n2 + h.b2.ko - 1) / h.b2.ko);
+        b.casc_poly_smem = std::max(b.casc_poly_smem, cascade_poly_smem(h.b2.ko, (int)geo.L2, (int)geo.D2, geo.Tb2));
+        s.casc_macs += (uint64_t)w.n2 * (uint64_t)geo.Tb2;
+      }
+      b.n_casc++;
+      h.b2.ring.pos += n_out;
+      h.last_n2 = w.n2;
+      b.max_n1 = std::max(b.max_n1, n_out);
+    }
+  }
+}
+
+// Banks: each walks the block as an integer client (D1, T1) attached at P; its channels are sub-bands of n1
+// samples
+static void walk_banks(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  s.bk_poly = s.bk_dft = 0;
+  for (int bi = 0; bi < (int)g->banks.size(); bi++) {
+    BankHost &k = g->banks[bi];
+    if (!k.active) continue;
+    const long long first = b.S - k.hist;
+    const int n1 = xl_walk(&k.hist, b.n, k.T1, k.D1, (int)((uint64_t)g->max_input_len / 2 / k.D1 + 2));
+    for (int i : k.cids) {
+      g->clients[i].hist = k.hist;
+      b.ho.n_out[i] = n1;
+      b.ho.out_off[i] = g->clients[i].out_off;
+    }
+    if (k.cids.empty()) continue;
+    BankBlk &e = s.bkblk.h[b.n_bk++];
+    e.taps = g->d_bktaps + k.taps_off;
+    e.tw = g->d_bktw + k.tw_off;
+    e.chans = g->d_bkch + k.ch_off;
+    e.first = first;
+    e.zb = k.P;
+    e.mask = b.mask;
+    e.n1 = n1;
+    e.D1 = (int)k.D1;
+    e.T1 = (int)k.T1;
+    e.K = k.K;
+    e.tpad = k.tpad;
+    e.n_ch = (int)k.cids.size();
+    e.r0 = (int)(((first - k.P) % k.K + k.K) % k.K);
+    b.max_bk_n1 = std::max(b.max_bk_n1, n1);
+    b.max_bk_cg = std::max(b.max_bk_cg, (e.n_ch + BK_CG - 1) / BK_CG);
+    b.bk_smem = std::max(b.bk_smem, bank_smem((int)k.D1, (int)k.T1));
+    s.bk_poly += (uint64_t)n1 * k.T1;
+    s.bk_dft += (uint64_t)n1 * k.cids.size() * (uint64_t)k.K;
+  }
+}
+
+// Sub-band members: each class walks its sub-band's n1 new samples (ho.n_out of the sub-band) from the sub-band
+// ring's position before them; then the sub-bands' appends
+static void walk_subbands(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  HostOut &ho = b.ho;
+  b.n_sb = (int)g->sb_list.size();
+  s.sb_macs = s.sb_rows = 0;
+  if (b.n_sb == 0) return;
+  for (size_t c = 0; c < g->sb_classes.size(); c++) {
+    const SbClassHost &ch = g->sb_classes[c];
+    const HostClient &a = g->clients[ch.sb_cid];
+    const HostClient &m0 = g->clients[ch.members[0]];
+    StageBGeom geo = m0.b2.geo;
+    const StageBStep w = stage_b_walk(geo, a.b2.ring.pos, ho.n_out[ch.sb_cid], m0.out_cap);
+    const int n2 = w.n2;
+    SbBlk &e = s.sbblk.h[c];
+    e.ring = a.b2.ring.p;
+    e.first = w.first;
+    e.zb = ch.zb;
+    e.mask = (unsigned)(a.b2.ring.cap - 1);
+    e.n2 = n2;
+    e.D2 = (int)geo.D2;
+    e.T2 = ch.Tb;
+    for (int id : ch.members) {
+      g->clients[id].b2.geo.hist2 = geo.hist2;
+      ho.n_out[id] = n2;
+      ho.out_off[id] = g->clients[id].out_off;
+    }
+    s.sb_macs += (uint64_t)n2 * ch.Tb * ch.members.size();
+    if (ch.L2 == 1) {
+      b.max_sb_n2 = std::max(b.max_sb_n2, n2);
+      b.sb_smem = std::max(b.sb_smem, subband_smem(e.D2, e.T2));
+    } else if (n2 > 0) {
+      b.max_sbr_ctas = std::max(b.max_sbr_ctas, ((n2 + ch.L2 - 1) / ch.L2 + SB_KO - 1) / SB_KO);
+      b.max_sbr_l2 = std::max(b.max_sbr_l2, ch.L2);
+      b.sbr_smem = std::max(b.sbr_smem, subband_smem(e.D2, e.T2));
+    }
+  }
+  for (int k = 0; k < b.n_sb; k++) {
+    const int i = g->sb_list[k];
+    HostClient &a = g->clients[i];
+    const int n1 = ho.n_out[i];
+    CascBlk &cb = s.sbcb.h[k];
+    memset(&cb, 0, sizeof(cb));
+    cb.ring = a.b2.ring.p;
+    cb.a_pos = a.b2.ring.pos;
+    cb.mask = (unsigned)(a.b2.ring.cap - 1);
+    cb.a_off = a.out_off;
+    cb.n1 = n1;
+    a.b2.ring.pos += n1;
+    s.sb_rows += (uint64_t)n1;
+    b.max_sb_n1 = std::max(b.max_sb_n1, n1);
+  }
+}
+
+// Input staging, then the conversion (its own stream: never behind the FIR CTAs of earlier blocks that still wait
+// for an SM), which the compute stream waits for
+static int stage_and_convert(Block &b, int fmt, const void *input, uint32_t flags) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  const int n = b.n;
+  const void *d_in = input;
+  if (!(flags & XLG_INPUT_DEVICE) && n > 0) {
+    const size_t bytes = (size_t)n * 2 * elem_bytes(fmt);
+    cudaPointerAttributes attr;
+    bool pinned = false;
+    if (cudaPointerGetAttributes(&attr, input) == cudaSuccess)
+      pinned = attr.type == cudaMemoryTypeHost;
+    else
+      cudaGetLastError();
+    const void *src = input;
+    if (!pinned) {
+      memcpy(s.h_raw, input, bytes);
+      src = s.h_raw;
+    }
+    CU_OK(cudaMemcpyAsync(s.d_raw, src, bytes, cudaMemcpyHostToDevice, g->s_in));
+    CU_OK(cudaEventRecord(s.ev_h2d, g->s_in));
+    CU_OK(cudaStreamWaitEvent(b.cvs, s.ev_h2d, 0));
+    // caller-owned pinned memory is read by the copy engine AFTER this call returns: unless
+    // the caller promised to leave it alone (XLG_INPUT_KEEP), wait for the copy (a 256 KiB
+    // block is ~10 us) so that the buffer may be reused at once, like a pageable one
+    if (pinned && !(flags & XLG_INPUT_KEEP)) CU_OK(cudaEventSynchronize(s.ev_h2d));
+    d_in = s.d_raw;
+  }
+
+  if (g->user_wait_pending) {
+    // (in-order streams: later submits' conversions queue behind this one's, so one wait is enough)
+    CU_OK(cudaStreamWaitEvent(b.cvs, g->ev_user, 0));
+    CU_OK(cudaStreamWaitEvent(g->s_in, g->ev_user, 0));
+    if (!g->conv_own_stream)
+      for (int i = 0; i < g->n_cs; i++) CU_OK(cudaStreamWaitEvent(g->s_cs[i], g->ev_user, 0));
+    g->user_wait_pending = false;
+  }
+  if (n > 0) {
+    if (g->timeline && !g->base_recorded) {
+      CU_OK(cudaEventRecord(g->ev_base, b.cvs));
+      g->base_recorded = true;
+    }
+    if (span_begin(g, s, SP_CONV, b.cvs)) return -EIO;
+    if (fmt == XLG_FMT_CU8)
+      launch_convert<0>(b.q15, d_in, g, b.S, n, b.cvs);
+    else if (fmt == XLG_FMT_CS8)
+      launch_convert<1>(b.q15, d_in, g, b.S, n, b.cvs);
+    else
+      launch_convert<2>(b.q15, d_in, g, b.S, n, b.cvs);
+    if (span_end(g, s, SP_CONV, b.cvs)) return -EIO;
+    CU_OK(cudaEventRecord(s.ev_conv, b.cvs));
+  }
+  // the FIR reads this block's samples and, as history, the previous blocks'
+  // (s_cv is in order: waiting for THIS block's conversion covers the earlier ones -- one driver call less)
+  if (g->have_last_conv && (b.cvs == b.cs || n == 0)) CU_OK(cudaStreamWaitEvent(b.cs, g->ev_last_conv_ref, 0));
+  if (n > 0) {
+    if (b.cvs != b.cs) CU_OK(cudaStreamWaitEvent(b.cs, s.ev_conv, 0));
+    g->ev_last_conv_ref = s.ev_conv;
+    g->have_last_conv = true;
+  }
+  return 0;
+}
+
+// Banks: after the conversions the FIR kernels wait for, not after the pre-pass (they have no oscillator)
+static int launch_banks(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  if (b.n_bk == 0 || b.max_bk_n1 <= 0) return 0;
+  if (span_begin(g, s, SP_BANK, b.cs)) return -EIO;
+  CU_OK(s.bkblk.upload((size_t)b.n_bk, b.cs));
+  bank_cf32_kernel<<<dim3((b.max_bk_n1 + BK_F - 1) / BK_F, b.n_bk, b.max_bk_cg), BK_THREADS, b.bk_smem, b.cs>>>(
+      s.bkblk.d, g->ring, s.d_out);
+  return span_end(g, s, SP_BANK, b.cs);
+}
+
+// Oscillator pre-pass (own stream: chains only on the previous pre-pass; none without a client to walk), and the
+// next block's, speculatively
+static int launch_prepass(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  const bool q15 = b.q15;
+  const int64_t ticket = b.ticket;
+  const long long S = b.S;
+  const int n = b.n, nc = b.nc;
+  if (nc <= 0 || !(q15 || g->n_order > 0)) return 0;
+  const bool tl_phase = g->timeline && !(g->spec_valid && !q15);  // a pre-pass that ran ahead was stamped then
+  if (span_begin(g, s, SP_PHASE, g->s_ph)) return -EIO;
+  if (tl_phase) CU_OK(cudaEventRecord(s.tl_ph[(ticket / XLG_SLOTS) & 1][0], g->s_ph));
+  if (g->timeline) s.pf_on[SP_PHASE] = true;  // (harvest_locked writes the block's timeline row by it)
+  bool ran_ahead = false;
+  if (q15) {
+    phase_q15_kernel<<<(nc + P_QTHREADS - 1) / P_QTHREADS, P_QTHREADS, 0, g->s_ph>>>(g->d_clients, nc, s.d_blk,
+                                                                                    s.d_qphases, S, n);
+  } else if (g->spec_valid) {
+    // guessed right (checked on entry): this block's pre-pass was launched with the previous
+    // block and s.ev_phase was recorded then
+    ran_ahead = true;
+    g->spec_valid = false;
+    g->spec_hits++;
+  } else {
+    phase_cf32_kernel<<<g->n_order / 32, P_THREADS, 0, g->s_ph>>>(g->d_clients, g->d_order, s.d_blk, s.d_phases,
+                                                                 s.d_endph, nullptr, S, n);
+  }
+  if (span_end(g, s, SP_PHASE, g->s_ph)) return -EIO;
+  if (tl_phase) CU_OK(cudaEventRecord(s.tl_ph[(ticket / XLG_SLOTS) & 1][1], g->s_ph));
+  if (!ran_ahead) CU_OK(cudaEventRecord(s.ev_phase, g->s_ph));
+  CU_OK(cudaStreamWaitEvent(b.cs, s.ev_phase, 0));
+  // ... and the NEXT block's pre-pass, assuming it is as long as this one
+  if (!q15 && g->speculate && !g->profiling && n > 0 && g->n_order > 0 && g->d_clients_backup != nullptr) {
+    Slot &ns = g->slots[(ticket + 1) % XLG_SLOTS];
+    if (ns.ticket.load() >= 0) CU_OK(cudaStreamWaitEvent(g->s_ph, ns.ev_done, 0));  // its tables are still in use
+    // (the kernel itself saves every client's state before it advances it: no copy on the critical path)
+    if (g->timeline) CU_OK(cudaEventRecord(ns.tl_ph[((ticket + 1) / XLG_SLOTS) & 1][0], g->s_ph));
+    phase_cf32_kernel<<<g->n_order / 32, P_THREADS, 0, g->s_ph>>>(g->d_clients, g->d_order, ns.d_blk, ns.d_phases,
+                                                                 ns.d_endph, g->d_clients_backup, S + n, n);
+    if (g->timeline) CU_OK(cudaEventRecord(ns.tl_ph[((ticket + 1) / XLG_SLOTS) & 1][1], g->s_ph));
+    CU_OK(cudaEventRecord(ns.ev_phase, g->s_ph));
+    g->spec_valid = true;
+    g->spec_S = S + n;
+    g->spec_n = n;
+    g->spec_ticket = ticket + 1;
+  }
+  return 0;
+}
+
+// Integer tiled classes.  Tile shape for this launch: the largest thread tile (best FMA : load ratio) that
+// still yields about two CTAs per SM; fewer clients / outputs -> smaller tiles.
+// (The natural input layout is 2-way bank conflicting for even D, which 16 output
+// lanes absorb and 32 would not, so the production shapes all have LO = 16.
+// Measured on cfg2: an isolated launch takes ~94 us with every shape -- finer tiles
+// balance better but pay more shared loads per FMA -- while in steady state, where
+// consecutive blocks overlap, RK = 4 is 25 % faster than RK = 1.)
+// The 128-output tile of 4 warps (two output sets) must fit 3 CTAs per SM, and it is taken only
+// when its waves are at least 70 % full: its CTAs are twice as long, so a thin last wave idles SMs
+// for longer (measured on H100: cfg2 at 0.80 and c1000 at 0.72 run faster with it, c512 at 0.54
+// ran 4 % slower).
+static int launch_tiled(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  HostOut &ho = b.ho;
+  if (b.q15 || g->classes.empty()) return 0;
+  // input tile + tap stages of a class at KT outputs per CTA (the merged layout reads D more samples)
+  auto tile_smem = [](const TileClassHost &ch, int KT) {
+    return (size_t)T_SMEM_FIXED + ((size_t)(KT - 1) * ch.k.Dp + ch.k.L + ch.k.D + 10) * sizeof(float2);
+  };
+  int si = kTileSmallest;
+  for (int i = 0; i <= kTileSmallest; i++) {
+    const TileShapeHost &sh = kTileShapes[i];
+    const int kt = sh.kt();
+    int ctas = 0;
+    bool fits = true;
+    for (TileClassHost &ch : g->classes) {
+      int n_out = 0;
+      for (int id : ch.real) n_out = std::max(n_out, ho.n_out[id]);
+      if (n_out > 0) ctas += ((n_out + kt - 1) / kt) * ch.k.n_groups;
+      if (sh.min_ctas > 0 && tile_smem(ch, kt) > (size_t)(kSmSmem / sh.min_ctas - 1024)) fits = false;
+    }
+    const int slots = sh.min_ctas * g->fir_sms;  // resident CTAs per wave
+    if (sh.min_ctas > 0 && ctas > 0 && 10 * ctas < 7 * ((ctas + slots - 1) / slots) * slots) fits = false;
+    if (fits && ctas >= 2 * g->fir_sms) {
+      si = i;
+      break;
+    }
+  }
+  if (g->tile_force > 0) {  // a shape of kTileShapes (checked in xlg_create_ex)
+    si = tile_shape_index(g->tile_force);
+    for (TileClassHost &ch : g->classes)  // an experiment must not overflow shared memory
+      if (tile_smem(ch, kTileShapes[si].kt()) > (size_t)kTileMaxSmem) si = kTileSmallest;
+  }
+  const TileShapeHost &shape = kTileShapes[si];
+  TileBatch t(shape.kt());
+  for (TileClassHost &ch : g->classes) {
+    int n_out = 0;
+    for (int id : ch.real) n_out = std::max(n_out, ho.n_out[id]);
+    if (n_out <= 0) continue;
+    // merged: the earliest possible window start of this block (history = T-1); every member's window starts
+    // delta in [0, D) samples later, read on the device from BlkInfo.  Otherwise identical alignment: recover
+    // this block's start from the walked hist
+    const HostClient &h0 = g->clients[ch.real[0]];
+    const long long first = ch.merged ? b.S - (long long)(ch.T - 1)
+                                      : (b.S + b.n) - h0.hist - (long long)ho.n_out[ch.real[0]] * (long long)h0.D;
+    s.tile_macs += t.add(ch, first, n_out);
+  }
+  if (t.ctas == 0) return 0;
+  if (span_begin(g, s, SP_TILE, b.cs)) return -EIO;
+  long long *trace_ptr = nullptr;
+  if (g->d_trace != nullptr && t.ctas <= T_TRACE_CTAS) {
+    const int tslot = (int)(g->trace_launches % T_TRACE_LAUNCHES);
+    trace_ptr = g->d_trace + (size_t)tslot * T_TRACE_REC * T_TRACE_CTAS;
+    g->trace_n[tslot] = t.ctas;
+    g->trace_launches++;
+    g->trace_ctas = t.ctas;
+  }
+  shape.kernel<<<t.ctas, shape.threads, t.smem, b.cs>>>(t.P, g->ring, b.mask, (const float2 *)g->d_tile_taps,
+                                                        g->d_members, g->d_member_cid, g->d_member_incr, s.d_blk,
+                                                        s.d_phases, s.d_out, trace_ptr);
+  return span_end(g, s, SP_TILE, b.cs);
+}
+
+// Long filters: split-K partial sums, then the ordered reduction
+static int launch_long(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  HostOut &ho = b.ho;
+  if (b.q15 || g->long_classes.empty()) return 0;
+  TileLaunch P;
+  memset(&P, 0, sizeof(P));
+  int ctas = 0, max_out = 0, max_groups = 0;
+  // fir_long4's TMA bulk copies need 16-byte aligned strips: with even D every strip has the parity of
+  // the window start, and an odd start is fetched from one sample earlier.  One odd-D class sends the
+  // whole launch to fir_long2, which falls back to 8-byte cp.async for unaligned strips.
+  bool pipelined = true;
+  for (TileClassHost &ch : g->long_classes)
+    if (ho.n_out[ch.real[0]] > 0 && (g->clients[ch.real[0]].D & 1) != 0) pipelined = false;
+  int n_live = 0;
+  for (TileClassHost &ch : g->long_classes) n_live += ho.n_out[ch.real[0]] > 0 ? 1 : 0;
+  for (TileClassHost &ch : g->long_classes) {
+    const HostClient &h0 = g->clients[ch.real[0]];
+    const int n_out = ho.n_out[ch.real[0]];
+    if (n_out <= 0) continue;
+    TileClass k = ch.k;
+    k.first = (b.S + b.n) - h0.hist - (long long)n_out * (long long)h0.D;
+    k.n_out = n_out;
+    k.tiles = (n_out + W2_KT - 1) / W2_KT;
+    k.cta_begin = ctas;
+    k.nslab = k.nseg;
+    k.ksplit = k.nseg;
+    k.seg_per = 1;
+    if (pipelined) {
+      // one resident CTA per SM: as many CTAs along the tap axis as fill one wave of this class's share
+      const int units = ((n_out + W4_KT - 1) / W4_KT) * ((k.n_groups + W4_GROUPS - 1) / W4_GROUPS);
+      k.tiles = (n_out + W4_KT - 1) / W4_KT;  // (kpad, a multiple of 56, covers 2 x 28 too)
+      const int share = std::max(1, g->fir_sms / std::max(n_live, 1));
+      const int want = std::max(1, share / std::max(1, units));
+      k.seg_per = (k.nseg + std::min(want, k.nseg) - 1) / std::min(want, k.nseg);
+      k.ksplit = (k.nseg + k.seg_per - 1) / k.seg_per;
+      k.nslab = k.ksplit;
+      ctas += k.ksplit * units;
+    } else {
+      ctas += k.nseg * k.tiles * k.n_groups;
+    }
+    max_out = std::max(max_out, n_out);
+    max_groups = std::max(max_groups, k.n_groups);
+    P.cls[P.n_classes++] = k;
+    s.tile_macs += (uint64_t)k.tiles * W2_KT * (uint64_t)k.L * (uint64_t)ch.members.size();
+  }
+  if (ctas == 0) return 0;
+  if (span_begin(g, s, SP_LONG, b.cs)) return -EIO;
+  if (pipelined) {
+    // the first class gets the tensor map for its strips (all long clients of a stream normally share one D);
+    // tmap_w = 0 (no map) sends every stage down the per-strip bulk copies
+    strip_map_update(g, P.cls[0].D);
+    P.cls[0].tmap_w = g->strip_w;
+    fir_long4_cf32_kernel<<<ctas, W4_THREADS, W4_SMEM, b.cs>>>(P, g->ring, b.mask, (const float2 *)g->d_tile_taps,
+                                                              s.d_partial, g->strip_map);
+  } else {
+    fir_long2_cf32_kernel<<<ctas, W2_THREADS, W2_SMEM, b.cs>>>(P, g->ring, b.mask, (const float2 *)g->d_tile_taps,
+                                                              s.d_partial);
+  }
+  dim3 rgrid((max_out + 7) / 8, max_groups, P.n_classes);
+  fir_long_reduce_kernel<<<rgrid, 256, 0, b.cs>>>(P, s.d_partial, g->d_members, g->d_member_incr, s.d_phases,
+                                                  s.d_out);
+  return span_end(g, s, SP_LONG, b.cs);
+}
+
+static int launch_generic(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  if (b.nc <= 0 || b.max_generic_out <= 0) return 0;
+  dim3 grid((b.max_generic_out + G_OPC - 1) / G_OPC, b.nc);
+  if (span_begin(g, s, SP_GEN, b.cs)) return -EIO;
+  if (b.q15)
+    fir_generic_q15_kernel<<<grid, G_THREADS, 0, b.cs>>>(g->d_clients, s.d_blk, g->qring, b.mask, g->d_qtaps,
+                                                         s.d_qphases, s.d_qout);
+  else
+    fir_generic_cf32_kernel<<<grid, G_THREADS, 0, b.cs>>>(g->d_clients, s.d_blk, g->ring, b.mask, g->d_taps,
+                                                          s.d_phases, s.d_out);
+  return span_end(g, s, SP_GEN, b.cs);
+}
+
+// Rational tiled classes: the tiled kernel over one class per polyphase branch, then the placement
+static int launch_poly_tiled(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  HostOut &ho = b.ho;
+  if (b.q15 || g->poly_classes.empty() || b.max_poly4_out <= 0) return 0;
+  // largest tile that still gives about two CTAs per SM, among the shapes that fit any CTA count per SM (every
+  // one fits: eligibility was checked at 64)
+  int si = kTileSmallest;
+  for (int i = 0; i <= kTileSmallest; i++) {
+    if (kTileShapes[i].min_ctas != 0) continue;
+    const int kt = kTileShapes[i].kt();
+    int ctas = 0;
+    for (const TileClassHost &ch : g->poly_classes)
+      ctas += ((ho.n_out[ch.real[0]] / (int)ch.interp + 1 + kt - 1) / kt) * ch.k.n_groups;
+    if (ctas >= 2 * g->fir_sms) {
+      si = i;
+      break;
+    }
+  }
+  const TileShapeHost &shape = kTileShapes[si];
+  TileBatch t(shape.kt());
+  for (size_t v = 0; v < g->poly_classes.size(); v++) {
+    const TileClassHost &ch = g->poly_classes[v];
+    const HostClient &h0 = g->clients[ch.real[0]];
+    const int n_out = ho.n_out[ch.real[0]];
+    const long long L = ch.interp, M = h0.D;
+    // this block's first upsampled window (hist was advanced by the walk); branch r serves k = rho + j*L
+    const long long first_u = (b.S + b.n) * L - h0.hist - (long long)n_out * M;
+    const long long a = (((-(first_u + ch.branch)) % L) + L) % L;
+    const long long rho = (a * ch.minv) % L;
+    const int nv = rho < n_out ? (int)((n_out - 1 - rho) / L) + 1 : 0;
+    s.h_vblk[v].first = (first_u + rho * M + ch.branch) / L;  // exact: the window start is -r mod L
+    s.h_vblk[v].n_out = nv;
+    s.h_vblk[v].pad_ = 0;
+    if (nv > 0) s.tile_macs += t.add(ch, s.h_vblk[v].first, nv);
+  }
+  if (t.ctas == 0) return 0;
+  if (span_begin(g, s, SP_POLY_TILE, b.cs)) return -EIO;
+  CU_OK(cudaMemcpyAsync(s.d_vblk, s.h_vblk, g->poly_classes.size() * sizeof(BlkInfo), cudaMemcpyHostToDevice, b.cs));
+  shape.kernel<<<t.ctas, shape.threads, t.smem, b.cs>>>(t.P, g->ring, b.mask, (const float2 *)g->d_tile_taps,
+                                                        g->d_members, g->d_member_cid, g->d_member_incr, s.d_vblk,
+                                                        g->d_ones, s.d_pscratch, nullptr);
+  dim3 pgrid((b.max_poly4_out + 255) / 256, g->n_poly4);
+  poly_tile_place_cf32_kernel<<<pgrid, 256, 0, b.cs>>>(g->d_clients, g->d_poly4, s.d_blk, s.d_pscratch, s.d_phases,
+                                                       s.d_out);
+  return span_end(g, s, SP_POLY_TILE, b.cs);
+}
+
+static int launch_poly_generic(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  if (b.q15 || g->n_poly3 <= 0 || b.poly_warps <= 0) return 0;
+  constexpr int warps_per_cta = G_THREADS / 32;
+  dim3 grid((b.poly_warps + warps_per_cta - 1) / warps_per_cta, g->n_poly3);
+  if (span_begin(g, s, SP_POLY_GEN, b.cs)) return -EIO;
+  fir_poly_generic_cf32_kernel<<<grid, G_THREADS, 0, b.cs>>>(g->d_clients, g->d_poly3, s.d_blk, g->ring, b.mask,
+                                                             g->d_taps, s.d_phases, s.d_out);
+  return span_end(g, s, SP_POLY_GEN, b.cs);
+}
+
+// Cascade clients: append the stage-A outputs to their rings, then stage B; from then on a client's results are
+// its final row
+static int launch_stage_b(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  const cudaStream_t cs = b.cs;
+  if (b.q15 || b.n_casc == 0) return 0;
+  // the rings are appended in block order: after the previous block's stage B, whichever stream ran it
+  if (g->have_last_casc) CU_OK(cudaStreamWaitEvent(cs, g->ev_last_casc, 0));
+  if (span_begin(g, s, SP_STAGE_B, cs)) return -EIO;
+  CU_OK(s.cblk.upload((size_t)b.n_casc, cs));
+  if (b.n_crat > 0) CU_OK(s.pblk.upload((size_t)b.n_crat, cs));
+  if (b.max_n1 > 0) cascade_launch_append(s.cblk.d, b.n_casc, b.max_n1, s.d_out, cs);
+  // integer stage B: one launch per ko, as the drop-in engine launches it (the kernel's summation order
+  // depends on ko: with even D2 output k is summed by lane (k mod ko) mod 32)
+  for (const xlg_group::CascRun &r : g->casc_runs) {
+    int run_n2 = 0;
+    size_t smem = 0;
+    for (int c = r.c0; c < r.c1; c++) {
+      run_n2 = std::max(run_n2, s.cblk.h[c].n2);
+      smem = std::max(smem, cascade_smem(r.ko, s.cblk.h[c].D2, s.cblk.h[c].T2));
+    }
+    if (run_n2 > 0) cascade_launch_fir(s.cblk.d + r.c0, r.c1 - r.c0, run_n2, r.ko, smem, g->d_taps2, s.d_out, cs);
+  }
+  // rational stage B: each client's CTA size was fixed at attach to fit the shared memory
+  if (b.max_rat_ctas > 0)
+    cascade_launch_fir_poly(s.pblk.d, b.n_crat, b.max_rat_ctas, b.casc_poly_smem, g->d_taps2, s.d_out, cs);
+  if (span_end(g, s, SP_STAGE_B, cs)) return -EIO;
+  CU_OK(cudaEventRecord(s.ev_casc, cs));
+  g->ev_last_casc = s.ev_casc;
+  g->have_last_casc = true;
+  for (size_t i = 0; i < g->clients.size(); i++)
+    if (g->clients[i].active && g->clients[i].casc) {
+      b.ho.n_out[i] = g->clients[i].last_n2;
+      b.ho.out_off[i] = g->clients[i].b2.fin_off;
+    }
+  return 0;
+}
+
+// Sub-bands: append their outputs to their rings, then the members' oscillators and FIR
+static int launch_members(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  const cudaStream_t cs = b.cs;
+  if (b.n_sb == 0) return 0;
+  // the rings are appended in block order (the cascades' event orders both)
+  if (g->have_last_casc) CU_OK(cudaStreamWaitEvent(cs, g->ev_last_casc, 0));
+  if (span_begin(g, s, SP_SB, cs)) return -EIO;
+  CU_OK(s.sbcb.upload((size_t)b.n_sb, cs));
+  if (b.max_sb_n1 > 0) cascade_launch_append(s.sbcb.d, b.n_sb, b.max_sb_n1, s.d_out, cs);
+  if (b.max_sb_n2 > 0 || b.max_sbr_ctas > 0) {
+    CU_OK(s.sbblk.upload(g->sb_classes.size(), cs));
+    subband_phase_kernel<<<(g->n_sb_mem + 31) / 32, 32, 0, cs>>>(g->d_clients, g->d_sbmem, s.sbblk.d, s.d_sbph);
+    if (b.max_sb_n2 > 0)
+      subband_fir_cf32_kernel<<<dim3((b.max_sb_n2 + SB_KO - 1) / SB_KO, g->n_sb_groups_int), SB_THREADS, b.sb_smem,
+                                cs>>>(s.sbblk.d, g->d_sbgrp, g->d_sbtaps, s.d_sbph, s.d_out);
+    // rational classes: their groups follow the integer ones, one CTA layer per residue
+    if (b.max_sbr_ctas > 0)
+      subband_fir_poly_cf32_kernel<<<dim3(b.max_sbr_ctas, g->n_sb_groups - g->n_sb_groups_int, b.max_sbr_l2),
+                                     SB_THREADS, b.sbr_smem, cs>>>(s.sbblk.d, g->d_sbgrp + g->n_sb_groups_int,
+                                                                   g->d_sbtaps, s.d_sbph, s.d_out);
+  }
+  if (span_end(g, s, SP_SB, cs)) return -EIO;
+  CU_OK(cudaEventRecord(s.ev_casc, cs));
+  g->ev_last_casc = s.ev_casc;
+  g->have_last_casc = true;
+  // a sub-band is not a client: nothing to read, and the D2H copy ends before its row
+  for (int i : g->sb_list) {
+    b.ho.n_out[i] = 0;
+    b.ho.out_off[i] = 0;
+  }
+  return 0;
+}
+
+// Results back to the host (the final rows), or, for XLG_OUT_DEVICE groups, done = FIR done
+static int copy_back(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  HostOut &ho = b.ho;
+  if ((g->flags & XLG_OUT_DEVICE) || g->arena_cap == 0 || b.nc <= 0) {
+    CU_OK(cudaEventRecord(s.ev_done, b.cs));  // results stay on the device: no hop through s_out
+    return 0;
+  }
+  size_t used = 0;
+  for (size_t i = 0; i < g->clients.size(); i++)
+    if (g->clients[i].active) used = std::max(used, (size_t)ho.out_off[i] + (size_t)ho.n_out[i]);
+  CU_OK(cudaStreamWaitEvent(g->s_out, s.ev_fir, 0));
+  if (used > 0) {
+    if (b.q15)
+      CU_OK(cudaMemcpyAsync(ho.h_qout, s.d_qout, used * sizeof(short2), cudaMemcpyDeviceToHost, g->s_out));
+    else
+      CU_OK(cudaMemcpyAsync(ho.h_out, s.d_out, used * sizeof(float2), cudaMemcpyDeviceToHost, g->s_out));
+    s.d2h_bytes = used * (b.q15 ? sizeof(short2) : sizeof(float2));
+  }
+  if ((g->flags & XLG_TRACK_STATE) && !b.q15 && s.d_endph != nullptr && ho.h_endph != nullptr)
+    CU_OK(cudaMemcpyAsync(ho.h_endph, s.d_endph, (size_t)b.nc * sizeof(float2), cudaMemcpyDeviceToHost, g->s_out));
+  CU_OK(cudaEventRecord(s.ev_done, g->s_out));
+  return 0;
 }
 
 extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t input_len, uint32_t flags) {
@@ -2391,8 +2951,6 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
         return -ENOTSUP;
       }
   CU_OK(cudaSetDevice(g->device));
-  const bool dev_in = (flags & XLG_INPUT_DEVICE) != 0;
-  const bool dev_out = (g->flags & XLG_OUT_DEVICE) != 0;
 
   // clients whose zero-history window has passed may move to a tiled / long class
   if (!g->dirty && !q15) {
@@ -2438,13 +2996,7 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     std::lock_guard<std::mutex> lk(g->mu);
     harvest_locked(g, s);
   }
-  const int n = (int)(input_len / 2);  // complex samples (src/xlating.c:387)
-  const long long S = q15 ? g->qS : g->S;
-  const int nc = g->max_client;
-  const unsigned mask = (unsigned)(g->ring_cap - 1);
-
-  // host mirror of the per-client output counts (same integer formula as the
-  // oscillator pre-pass kernel)
+  Block b{g, s, ho, ticket, q15 ? g->qS : g->S, (int)(input_len / 2), q15, (unsigned)(g->ring_cap - 1), g->max_client};
   {
     // consumers read this entry's metadata under the same mutex (xlg_output) / spinlock (xlg_copy_output)
     std::lock_guard<std::mutex> lk(g->mu);
@@ -2457,618 +3009,35 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
   }
   s.q15 = q15;
   s.tile_macs = s.algo_macs = s.out_samples = s.poly_macs = s.casc_macs = s.d2h_bytes = 0;
-  s.in_samples = (uint64_t)n;
-  int max_generic_out = 0, poly_warps = 0, max_poly4_out = 0, n_casc = 0, max_n1 = 0;
-  int n_crat = 0, max_rat_ctas = 0;  // rational stage B; CTAs per rational client
-  size_t casc_poly_smem = 0;
-  for (size_t i = 0; i < g->clients.size(); i++) {
-    HostClient &h = g->clients[i];
-    if (!h.active || h.mem || h.bank >= 0) continue;
-    // upsampled coordinates (the same integers for L = 1)
-    const long long Su = S * h.L, Eu = (S + n) * h.L;
-    const long long first = Su - h.hist;
-    const long long last_ok = Eu - (long long)h.T;
-    int n_out = 0;
-    if (last_ok >= first) n_out = (int)((last_ok - first) / (long long)h.D) + 1;
-    if (n_out > h.out_cap) n_out = h.out_cap;
-    ho.n_out[i] = n_out;
-    ho.out_off[i] = h.out_off;
-    h.hist = Eu - (first + (long long)n_out * (long long)h.D);
-    if (g->flags & XLG_TRACK_STATE) ho.hist_after[i] = h.hist;
-    s.out_samples += (uint64_t)n_out;
-    const uint64_t macs = (uint64_t)n_out * ((h.T + h.L - 1) / h.L);
-    s.algo_macs += macs;
-    if (h.kind >= 3) s.poly_macs += macs;
-    if (h.kind == 4) max_poly4_out = std::max(max_poly4_out, n_out);
-    if (h.kind == 3) {
-      // warps of fir_poly_generic_cf32_kernel: min(L, n_out) residues x groups of G_OPW outputs
-      const int per = (int)((n_out + (long long)h.L - 1) / h.L);
-      poly_warps = std::max(poly_warps, (int)std::min<long long>(h.L, n_out) * ((per + G_OPW - 1) / G_OPW));
-    }
-    if (q15 || h.kind == 0) max_generic_out = std::max(max_generic_out, n_out);
-    if (h.casc) {
-      const StageBGeom &b = h.b2.geo;
-      const StageBStep w = stage_b_walk(h.b2.geo, h.b2.ring.pos, n_out, h.b2.fin_cap);
-      if (b.L2 == 1) {
-        stage_b_fill(h.b2, w, n_out, h.out_off, &s.cblk.h[h.cblk], nullptr);
-        s.casc_macs += (uint64_t)w.n2 * b.T2;
-      } else {
-        // only the appends read this client's CascBlk; cascade_fir_poly_cf32_kernel reads its CascPolyBlk
-        stage_b_fill(h.b2, w, n_out, h.out_off, &s.cblk.h[g->n_casc_int + n_crat], &s.pblk.h[n_crat]);
-        n_crat++;
-        max_rat_ctas = std::max(max_rat_ctas, (w.n2 + h.b2.ko - 1) / h.b2.ko);
-        casc_poly_smem = std::max(casc_poly_smem, cascade_poly_smem(h.b2.ko, (int)b.L2, (int)b.D2, b.Tb2));
-        s.casc_macs += (uint64_t)w.n2 * (uint64_t)b.Tb2;
-      }
-      n_casc++;
-      h.b2.ring.pos += n_out;
-      h.last_n2 = w.n2;
-      max_n1 = std::max(max_n1, n_out);
-    }
-  }
-
-  // banks: each walks the block as an integer client (D1, T1) attached at P; its channels are sub-bands of n1
-  // samples
-  int n_bk = 0, max_bk_n1 = 0, max_bk_cg = 0;
-  size_t bk_smem = 0;
-  s.bk_poly = s.bk_dft = 0;
-  for (int b = 0; b < (int)g->banks.size(); b++) {
-    BankHost &k = g->banks[b];
-    if (!k.active) continue;
-    const long long first = S - k.hist;
-    const int n1 = xl_walk(&k.hist, n, k.T1, k.D1, (int)((uint64_t)g->max_input_len / 2 / k.D1 + 2));
-    for (int i : k.cids) {
-      g->clients[i].hist = k.hist;
-      ho.n_out[i] = n1;
-      ho.out_off[i] = g->clients[i].out_off;
-    }
-    if (k.cids.empty()) continue;
-    BankBlk &e = s.bkblk.h[n_bk++];
-    e.taps = g->d_bktaps + k.taps_off;
-    e.tw = g->d_bktw + k.tw_off;
-    e.chans = g->d_bkch + k.ch_off;
-    e.first = first;
-    e.zb = k.P;
-    e.mask = mask;
-    e.n1 = n1;
-    e.D1 = (int)k.D1;
-    e.T1 = (int)k.T1;
-    e.K = k.K;
-    e.tpad = k.tpad;
-    e.n_ch = (int)k.cids.size();
-    e.r0 = (int)(((first - k.P) % k.K + k.K) % k.K);
-    max_bk_n1 = std::max(max_bk_n1, n1);
-    max_bk_cg = std::max(max_bk_cg, (e.n_ch + BK_CG - 1) / BK_CG);
-    bk_smem = std::max(bk_smem, bank_smem((int)k.D1, (int)k.T1));
-    s.bk_poly += (uint64_t)n1 * k.T1;
-    s.bk_dft += (uint64_t)n1 * k.cids.size() * (uint64_t)k.K;
-  }
-
-  // sub-band members: each class walks its sub-band's n1 new samples from the sub-band ring's position before
-  // them
-  const int n_sb = (int)g->sb_list.size();
-  int max_sb_n1 = 0, max_sb_n2 = 0;
-  int max_sbr_ctas = 0, max_sbr_l2 = 0;  // rational classes: output tiles of the longest residue, largest L2
-  size_t sb_smem = 0, sbr_smem = 0;
-  s.sb_macs = s.sb_rows = 0;
-  if (n_sb > 0) {
-    for (size_t c = 0; c < g->sb_classes.size(); c++) {
-      const SbClassHost &ch = g->sb_classes[c];
-      const HostClient &a = g->clients[ch.sb_cid];
-      const HostClient &m0 = g->clients[ch.members[0]];
-      StageBGeom geo = m0.b2.geo;
-      const StageBStep w = stage_b_walk(geo, a.b2.ring.pos, ho.n_out[ch.sb_cid], m0.out_cap);
-      const int n2 = w.n2;
-      SbBlk &b = s.sbblk.h[c];
-      b.ring = a.b2.ring.p;
-      b.first = w.first;
-      b.zb = ch.zb;
-      b.mask = (unsigned)(a.b2.ring.cap - 1);
-      b.n2 = n2;
-      b.D2 = (int)geo.D2;
-      b.T2 = ch.Tb;
-      for (int id : ch.members) {
-        g->clients[id].b2.geo.hist2 = geo.hist2;
-        ho.n_out[id] = n2;
-        ho.out_off[id] = g->clients[id].out_off;
-      }
-      s.sb_macs += (uint64_t)n2 * ch.Tb * ch.members.size();
-      if (ch.L2 == 1) {
-        max_sb_n2 = std::max(max_sb_n2, n2);
-        sb_smem = std::max(sb_smem, subband_smem(b.D2, b.T2));
-      } else if (n2 > 0) {
-        max_sbr_ctas = std::max(max_sbr_ctas, ((n2 + ch.L2 - 1) / ch.L2 + SB_KO - 1) / SB_KO);
-        max_sbr_l2 = std::max(max_sbr_l2, ch.L2);
-        sbr_smem = std::max(sbr_smem, subband_smem(b.D2, b.T2));
-      }
-    }
-    for (int k = 0; k < n_sb; k++) {
-      const int i = g->sb_list[k];
-      HostClient &a = g->clients[i];
-      const int n1 = ho.n_out[i];
-      CascBlk &cb = s.sbcb.h[k];
-      memset(&cb, 0, sizeof(cb));
-      cb.ring = a.b2.ring.p;
-      cb.a_pos = a.b2.ring.pos;
-      cb.mask = (unsigned)(a.b2.ring.cap - 1);
-      cb.a_off = a.out_off;
-      cb.n1 = n1;
-      a.b2.ring.pos += n1;
-      s.sb_rows += (uint64_t)n1;
-      max_sb_n1 = std::max(max_sb_n1, n1);
-    }
-  }
+  s.in_samples = (uint64_t)b.n;
+  std::fill(std::begin(s.pf_on), std::end(s.pf_on), false);
+  // The walks, in this order: the client walk advances every client's hist, from which the tiled and long launches
+  // recover each class's window start; the bank walk counts its channels' outputs, which the sub-band walk reads.
+  walk_clients(b);
+  walk_banks(b);
+  walk_subbands(b);
 
   // consecutive blocks alternate between two compute streams so that the tail of
   // one block's FIR overlaps the head of the next (each block's launch alone
   // cannot fill 132 SMs evenly); per-kernel profiling keeps a single stream so
   // that event-timed durations are not inflated by the overlap
-  cudaStream_t cs = g->profiling ? g->s_cs[0] : g->s_cs[ticket % g->n_cs];
-  cudaStream_t cvs = g->conv_own_stream ? g->s_cv : cs;  // stream of the raw -> ring conversion
-
-  // ---- input staging ----
-  const void *d_in = input;
-  if (!dev_in && n > 0) {
-    const size_t bytes = (size_t)n * 2 * elem_bytes(fmt);
-    cudaPointerAttributes attr;
-    bool pinned = false;
-    if (cudaPointerGetAttributes(&attr, input) == cudaSuccess)
-      pinned = attr.type == cudaMemoryTypeHost;
-    else
-      cudaGetLastError();
-    const void *src = input;
-    if (!pinned) {
-      memcpy(s.h_raw, input, bytes);
-      src = s.h_raw;
-    }
-    CU_OK(cudaMemcpyAsync(s.d_raw, src, bytes, cudaMemcpyHostToDevice, g->s_in));
-    CU_OK(cudaEventRecord(s.ev_h2d, g->s_in));
-    CU_OK(cudaStreamWaitEvent(cvs, s.ev_h2d, 0));
-    // caller-owned pinned memory is read by the copy engine AFTER this call returns: unless
-    // the caller promised to leave it alone (XLG_INPUT_KEEP), wait for the copy (a 256 KiB
-    // block is ~10 us) so that the buffer may be reused at once, like a pageable one
-    if (pinned && !(flags & XLG_INPUT_KEEP)) CU_OK(cudaEventSynchronize(s.ev_h2d));
-    d_in = s.d_raw;
-  }
-
-  if (g->user_wait_pending) {
-    // (in-order streams: later submits' conversions queue behind this one's, so one wait is enough)
-    CU_OK(cudaStreamWaitEvent(cvs, g->ev_user, 0));
-    CU_OK(cudaStreamWaitEvent(g->s_in, g->ev_user, 0));
-    if (!g->conv_own_stream)
-      for (int i = 0; i < g->n_cs; i++) CU_OK(cudaStreamWaitEvent(g->s_cs[i], g->ev_user, 0));
-    g->user_wait_pending = false;
-  }
-  // ---- convert (its own stream: never behind the FIR CTAs of earlier blocks that still wait for an SM) ----
-  s.pf_conv = s.pf_phase = s.pf_tile = s.pf_gen = false;
-  if (n > 0) {
-    if (g->timeline && !g->base_recorded) {
-      CU_OK(cudaEventRecord(g->ev_base, cvs));
-      g->base_recorded = true;
-    }
-    if (g->profiling || g->timeline) {
-      CU_OK(cudaEventRecord(s.pf[0], cvs));
-      s.pf_conv = true;
-    }
-    if (fmt == XLG_FMT_CU8)
-      launch_convert<0>(q15, d_in, g, S, n, cvs);
-    else if (fmt == XLG_FMT_CS8)
-      launch_convert<1>(q15, d_in, g, S, n, cvs);
-    else
-      launch_convert<2>(q15, d_in, g, S, n, cvs);
-    if (g->profiling || g->timeline) CU_OK(cudaEventRecord(s.pf[1], cvs));
-    CU_OK(cudaEventRecord(s.ev_conv, cvs));
-  }
-  // the FIR reads this block's samples and, as history, the previous blocks'
-  // (s_cv is in order: waiting for THIS block's conversion covers the earlier ones -- one driver call less)
-  if (g->have_last_conv && (cvs == cs || n == 0)) CU_OK(cudaStreamWaitEvent(cs, g->ev_last_conv_ref, 0));
-  if (n > 0) {
-    if (cvs != cs) CU_OK(cudaStreamWaitEvent(cs, s.ev_conv, 0));
-    g->ev_last_conv_ref = s.ev_conv;
-    g->have_last_conv = true;
-  }
-
-  // ---- banks: after the conversions the FIR kernels wait for, not after the pre-pass (they have no oscillator) ----
-  s.pf_bkk = false;
-  if (n_bk > 0 && max_bk_n1 > 0) {
-    if (g->profiling) {
-      CU_OK(cudaEventRecord(s.pf_bk[0], cs));
-      s.pf_bkk = true;
-    }
-    CU_OK(s.bkblk.upload((size_t)n_bk, cs));
-    bank_cf32_kernel<<<dim3((max_bk_n1 + BK_F - 1) / BK_F, n_bk, max_bk_cg), BK_THREADS, bk_smem, cs>>>(
-        s.bkblk.d, g->ring, s.d_out);
-    if (g->profiling) CU_OK(cudaEventRecord(s.pf_bk[1], cs));
-  }
-
-  // ---- oscillator pre-pass (own stream: chains only on the previous pre-pass; none without a client to walk) ----
-  if (nc > 0 && (q15 || g->n_order > 0)) {
-    const bool tl_phase = g->timeline && !(g->spec_valid && !q15);  // a pre-pass that ran ahead was stamped then
-    if (g->profiling) CU_OK(cudaEventRecord(s.pf[2], g->s_ph));
-    if (tl_phase) CU_OK(cudaEventRecord(s.tl_ph[(ticket / XLG_SLOTS) & 1][0], g->s_ph));
-    if (g->profiling || g->timeline) s.pf_phase = true;
-    bool ran_ahead = false;
-    if (q15) {
-      phase_q15_kernel<<<(nc + P_QTHREADS - 1) / P_QTHREADS, P_QTHREADS, 0, g->s_ph>>>(g->d_clients, nc, s.d_blk,
-                                                                                      s.d_qphases, S, n);
-    } else if (g->spec_valid) {
-      // guessed right (checked on entry): this block's pre-pass was launched with the previous
-      // block and s.ev_phase was recorded then
-      ran_ahead = true;
-      g->spec_valid = false;
-      g->spec_hits++;
-    } else {
-      phase_cf32_kernel<<<g->n_order / 32, P_THREADS, 0, g->s_ph>>>(g->d_clients, g->d_order, s.d_blk, s.d_phases,
-                                                                   s.d_endph, nullptr, S, n);
-    }
-    if (g->profiling) CU_OK(cudaEventRecord(s.pf[3], g->s_ph));
-    if (tl_phase) CU_OK(cudaEventRecord(s.tl_ph[(ticket / XLG_SLOTS) & 1][1], g->s_ph));
-    if (!ran_ahead) CU_OK(cudaEventRecord(s.ev_phase, g->s_ph));
-    CU_OK(cudaStreamWaitEvent(cs, s.ev_phase, 0));
-    // ... and the NEXT block's pre-pass, assuming it is as long as this one
-    if (!q15 && g->speculate && !g->profiling && n > 0 && g->n_order > 0 && g->d_clients_backup != nullptr) {
-      Slot &ns = g->slots[(ticket + 1) % XLG_SLOTS];
-      if (ns.ticket.load() >= 0) CU_OK(cudaStreamWaitEvent(g->s_ph, ns.ev_done, 0));  // its tables are still in use
-      // (the kernel itself saves every client's state before it advances it: no copy on the critical path)
-      if (g->timeline) CU_OK(cudaEventRecord(ns.tl_ph[((ticket + 1) / XLG_SLOTS) & 1][0], g->s_ph));
-      phase_cf32_kernel<<<g->n_order / 32, P_THREADS, 0, g->s_ph>>>(g->d_clients, g->d_order, ns.d_blk, ns.d_phases,
-                                                                   ns.d_endph, g->d_clients_backup, S + n, n);
-      if (g->timeline) CU_OK(cudaEventRecord(ns.tl_ph[((ticket + 1) / XLG_SLOTS) & 1][1], g->s_ph));
-      CU_OK(cudaEventRecord(ns.ev_phase, g->s_ph));
-      g->spec_valid = true;
-      g->spec_S = S + n;
-      g->spec_n = n;
-      g->spec_ticket = ticket + 1;
-    }
-  }
-
-  // ---- FIR ----
-  if (!q15 && !g->classes.empty()) {
-    // Tile shape for this launch: the largest thread tile (best FMA : load ratio) that
-    // still yields about two CTAs per SM; fewer clients / outputs -> smaller tiles.
-    // (The natural input layout is 2-way bank conflicting for even D, which 16 output
-    // lanes absorb and 32 would not, so the production shapes all have LO = 16.
-    // Measured on cfg2: an isolated launch takes ~94 us with every shape -- finer tiles
-    // balance better but pay more shared loads per FMA -- while in steady state, where
-    // consecutive blocks overlap, RK = 4 is 25 % faster than RK = 1.)
-    // The 128-output tile of 4 warps (two output sets) must fit 3 CTAs per SM, and it is taken only
-    // when its waves are at least 70 % full: its CTAs are twice as long, so a thin last wave idles SMs
-    // for longer (measured on H100: cfg2 at 0.80 and c1000 at 0.72 run faster with it, c512 at 0.54
-    // ran 4 % slower).
-    // input tile + tap stages of a class at KT outputs per CTA (the merged layout reads D more samples)
-    auto tile_smem = [](const TileClassHost &ch, int KT) {
-      return (size_t)T_SMEM_FIXED + ((size_t)(KT - 1) * ch.k.Dp + ch.k.L + ch.k.D + 10) * sizeof(float2);
-    };
-    int si = kTileSmallest;
-    for (int i = 0; i <= kTileSmallest; i++) {
-      const TileShapeHost &sh = kTileShapes[i];
-      const int kt = sh.kt();
-      int ctas = 0;
-      bool fits = true;
-      for (TileClassHost &ch : g->classes) {
-        int n_out = 0;
-        for (int id : ch.real) n_out = std::max(n_out, ho.n_out[id]);
-        if (n_out > 0) ctas += ((n_out + kt - 1) / kt) * ch.k.n_groups;
-        if (sh.min_ctas > 0 && tile_smem(ch, kt) > (size_t)(kSmSmem / sh.min_ctas - 1024)) fits = false;
-      }
-      const int slots = sh.min_ctas * g->fir_sms;  // resident CTAs per wave
-      if (sh.min_ctas > 0 && ctas > 0 && 10 * ctas < 7 * ((ctas + slots - 1) / slots) * slots) fits = false;
-      if (fits && ctas >= 2 * g->fir_sms) {
-        si = i;
-        break;
-      }
-    }
-    if (g->tile_force > 0) {  // a shape of kTileShapes (checked in xlg_create_ex)
-      si = tile_shape_index(g->tile_force);
-      for (TileClassHost &ch : g->classes)  // an experiment must not overflow shared memory
-        if (tile_smem(ch, kTileShapes[si].kt()) > (size_t)kTileMaxSmem) si = kTileSmallest;
-    }
-    const TileShapeHost &shape = kTileShapes[si];
-    const int KT = shape.kt();
-    TileLaunch P;
-    memset(&P, 0, sizeof(P));
-    int ctas = 0;
-    size_t smem = 0;
-    for (TileClassHost &ch : g->classes) {
-      int n_out = 0;
-      for (int id : ch.real) n_out = std::max(n_out, ho.n_out[id]);
-      if (n_out <= 0) continue;
-      TileClass k = ch.k;
-      if (ch.merged) {
-        // earliest possible window start of this block (history = T-1); every member's
-        // window starts delta in [0, D) samples later, read on the device from BlkInfo
-        k.first = S - (long long)(ch.T - 1);
-      } else {
-        // identical alignment: hist was already advanced above; recover this block's start
-        const HostClient &h0 = g->clients[ch.real[0]];
-        k.first = (S + n) - h0.hist - (long long)ho.n_out[ch.real[0]] * (long long)h0.D;
-      }
-      k.n_out = n_out;
-      k.tiles = (n_out + KT - 1) / KT;
-      k.xs_len = (KT - 1) * k.Dp + k.L + (ch.merged ? k.D : 0);
-      k.cta_begin = ctas;
-      ctas += k.tiles * k.n_groups;
-      smem = std::max(smem, (size_t)T_SMEM_FIXED + ((size_t)k.xs_len + 10) * sizeof(float2));
-      P.cls[P.n_classes++] = k;
-      s.tile_macs += (uint64_t)k.tiles * KT * (uint64_t)k.L * (uint64_t)ch.members.size();
-    }
-    if (ctas > 0) {
-      if (g->profiling || g->timeline) {
-        CU_OK(cudaEventRecord(s.pf[4], cs));
-        s.pf_tile = true;
-      }
-      const float2 *tt = (const float2 *)g->d_tile_taps;
-      long long *trace_ptr = nullptr;
-      if (g->d_trace != nullptr && ctas <= T_TRACE_CTAS) {
-        const int tslot = (int)(g->trace_launches % T_TRACE_LAUNCHES);
-        trace_ptr = g->d_trace + (size_t)tslot * T_TRACE_REC * T_TRACE_CTAS;
-        g->trace_n[tslot] = ctas;
-        g->trace_launches++;
-        g->trace_ctas = ctas;
-      }
-      shape.kernel<<<ctas, shape.threads, smem, cs>>>(P, g->ring, mask, tt, g->d_members, g->d_member_cid,
-                                                      g->d_member_incr, s.d_blk, s.d_phases, s.d_out, trace_ptr);
-      if (g->profiling || g->timeline) CU_OK(cudaEventRecord(s.pf[5], cs));
-    }
-  }
-  // ---- long filters: split-K partial sums, then the ordered reduction ----
-  s.pf_long = false;
-  if (!q15 && !g->long_classes.empty()) {
-    TileLaunch P;
-    memset(&P, 0, sizeof(P));
-    int ctas = 0, max_out = 0, max_groups = 0;
-    // fir_long4's TMA bulk copies need 16-byte aligned strips: with even D every strip has the parity of
-    // the window start, and an odd start is fetched from one sample earlier.  One odd-D class sends the
-    // whole launch to fir_long2, which falls back to 8-byte cp.async for unaligned strips.
-    bool pipelined = true;
-    for (TileClassHost &ch : g->long_classes)
-      if (ho.n_out[ch.real[0]] > 0 && (g->clients[ch.real[0]].D & 1) != 0) pipelined = false;
-    int n_live = 0;
-    for (TileClassHost &ch : g->long_classes) n_live += ho.n_out[ch.real[0]] > 0 ? 1 : 0;
-    for (TileClassHost &ch : g->long_classes) {
-      const HostClient &h0 = g->clients[ch.real[0]];
-      const int n_out = ho.n_out[ch.real[0]];
-      if (n_out <= 0) continue;
-      TileClass k = ch.k;
-      k.first = (S + n) - h0.hist - (long long)n_out * (long long)h0.D;
-      k.n_out = n_out;
-      k.tiles = (n_out + W2_KT - 1) / W2_KT;
-      k.cta_begin = ctas;
-      k.nslab = k.nseg;
-      k.ksplit = k.nseg;
-      k.seg_per = 1;
-      if (pipelined) {
-        // one resident CTA per SM: as many CTAs along the tap axis as fill one wave of this class's share
-        const int units = ((n_out + W4_KT - 1) / W4_KT) * ((k.n_groups + W4_GROUPS - 1) / W4_GROUPS);
-        k.tiles = (n_out + W4_KT - 1) / W4_KT;  // (kpad, a multiple of 56, covers 2 x 28 too)
-        const int share = std::max(1, g->fir_sms / std::max(n_live, 1));
-        const int want = std::max(1, share / std::max(1, units));
-        k.seg_per = (k.nseg + std::min(want, k.nseg) - 1) / std::min(want, k.nseg);
-        k.ksplit = (k.nseg + k.seg_per - 1) / k.seg_per;
-        k.nslab = k.ksplit;
-        ctas += k.ksplit * units;
-      } else {
-        ctas += k.nseg * k.tiles * k.n_groups;
-      }
-      max_out = std::max(max_out, n_out);
-      max_groups = std::max(max_groups, k.n_groups);
-      P.cls[P.n_classes++] = k;
-      s.tile_macs += (uint64_t)k.tiles * W2_KT * (uint64_t)k.L * (uint64_t)ch.members.size();
-    }
-    if (ctas > 0) {
-      if (g->profiling) {
-        CU_OK(cudaEventRecord(s.pf[8], cs));
-        s.pf_long = true;
-      }
-      if (pipelined) {
-        // the first class gets the tensor map for its strips (all long clients of a stream normally share one D);
-        // tmap_w = 0 (no map) sends every stage down the per-strip bulk copies
-        strip_map_update(g, P.cls[0].D);
-        P.cls[0].tmap_w = g->strip_w;
-        fir_long4_cf32_kernel<<<ctas, W4_THREADS, W4_SMEM, cs>>>(P, g->ring, mask, (const float2 *)g->d_tile_taps,
-                                                                s.d_partial, g->strip_map);
-      } else {
-        fir_long2_cf32_kernel<<<ctas, W2_THREADS, W2_SMEM, cs>>>(P, g->ring, mask, (const float2 *)g->d_tile_taps,
-                                                                s.d_partial);
-      }
-      dim3 rgrid((max_out + 7) / 8, max_groups, P.n_classes);
-      fir_long_reduce_kernel<<<rgrid, 256, 0, cs>>>(P, s.d_partial, g->d_members, g->d_member_incr, s.d_phases,
-                                                    s.d_out);
-      if (g->profiling) CU_OK(cudaEventRecord(s.pf[9], cs));
-    }
-  }
-  if (nc > 0 && max_generic_out > 0) {
-    dim3 grid((max_generic_out + G_OPC - 1) / G_OPC, nc);
-    if (g->profiling) {
-      CU_OK(cudaEventRecord(s.pf[6], cs));
-      s.pf_gen = true;
-    }
-    if (q15)
-      fir_generic_q15_kernel<<<grid, G_THREADS, 0, cs>>>(g->d_clients, s.d_blk, g->qring, mask, g->d_qtaps,
-                                                             s.d_qphases, s.d_qout);
-    else
-      fir_generic_cf32_kernel<<<grid, G_THREADS, 0, cs>>>(g->d_clients, s.d_blk, g->ring, mask, g->d_taps,
-                                                              s.d_phases, s.d_out);
-    if (g->profiling) CU_OK(cudaEventRecord(s.pf[7], cs));
-  }
-  // ---- rational tiled classes: the tiled kernel over one class per polyphase branch, then the placement ----
-  s.pf_pt = false;
-  if (!q15 && !g->poly_classes.empty() && max_poly4_out > 0) {
-    TileLaunch P;
-    memset(&P, 0, sizeof(P));
-    // largest tile that still gives about two CTAs per SM (every shape fits: eligibility was checked at 64)
-    static const int kPolyShapes[][2] = {{16, 4}, {16, 2}, {16, 1}};
-    int lo = 16, rk = 1;
-    for (const auto &sh : kPolyShapes) {
-      int ctas = 0;
-      for (const TileClassHost &ch : g->poly_classes)
-        ctas += ((ho.n_out[ch.real[0]] / (int)ch.interp + 1 + sh[0] * sh[1] - 1) / (sh[0] * sh[1])) * ch.k.n_groups;
-      if (ctas >= 2 * g->fir_sms) {
-        lo = sh[0];
-        rk = sh[1];
-        break;
-      }
-    }
-    const int KT = lo * rk;
-    int ctas = 0;
-    size_t smem = 0;
-    for (size_t v = 0; v < g->poly_classes.size(); v++) {
-      const TileClassHost &ch = g->poly_classes[v];
-      const HostClient &h0 = g->clients[ch.real[0]];
-      const int n_out = ho.n_out[ch.real[0]];
-      const long long L = ch.interp, M = h0.D;
-      // this block's first upsampled window (hist was advanced above); branch r serves k = rho + j*L
-      const long long first_u = (S + n) * L - h0.hist - (long long)n_out * M;
-      const long long a = (((-(first_u + ch.branch)) % L) + L) % L;
-      const long long rho = (a * ch.minv) % L;
-      const int nv = rho < n_out ? (int)((n_out - 1 - rho) / L) + 1 : 0;
-      s.h_vblk[v].first = (first_u + rho * M + ch.branch) / L;  // exact: the window start is -r mod L
-      s.h_vblk[v].n_out = nv;
-      s.h_vblk[v].pad_ = 0;
-      if (nv <= 0) continue;
-      TileClass k = ch.k;
-      k.first = s.h_vblk[v].first;
-      k.n_out = nv;
-      k.tiles = (nv + KT - 1) / KT;
-      k.xs_len = (KT - 1) * k.Dp + k.L;
-      k.cta_begin = ctas;
-      ctas += k.tiles * k.n_groups;
-      smem = std::max(smem, (size_t)T_SMEM_FIXED + ((size_t)k.xs_len + 10) * sizeof(float2));
-      P.cls[P.n_classes++] = k;
-      s.tile_macs += (uint64_t)k.tiles * KT * (uint64_t)k.L * (uint64_t)ch.members.size();
-    }
-    if (ctas > 0) {
-      if (g->profiling) {
-        CU_OK(cudaEventRecord(s.pf_poly[2], cs));
-        s.pf_pt = true;
-      }
-      CU_OK(cudaMemcpyAsync(s.d_vblk, s.h_vblk, g->poly_classes.size() * sizeof(BlkInfo), cudaMemcpyHostToDevice, cs));
-      const float2 *tt = (const float2 *)g->d_tile_taps;
-#define XL_LAUNCH_PTILE(RK_)                                                                                     \
-  fir_tile_cf32_kernel<16, RK_, 1><<<ctas, TileShape<16, RK_, 1>::kThreads, smem, cs>>>(                          \
-      P, g->ring, mask, tt, g->d_members, g->d_member_cid, g->d_member_incr, s.d_vblk, g->d_ones, s.d_pscratch, nullptr)
-      if (rk == 4)
-        XL_LAUNCH_PTILE(4);
-      else if (rk == 2)
-        XL_LAUNCH_PTILE(2);
-      else
-        XL_LAUNCH_PTILE(1);
-#undef XL_LAUNCH_PTILE
-      dim3 pgrid((max_poly4_out + 255) / 256, g->n_poly4);
-      poly_tile_place_cf32_kernel<<<pgrid, 256, 0, cs>>>(g->d_clients, g->d_poly4, s.d_blk, s.d_pscratch, s.d_phases,
-                                                         s.d_out);
-      if (g->profiling) CU_OK(cudaEventRecord(s.pf_poly[3], cs));
-    }
-  }
-  s.pf_pg = false;
-  if (!q15 && g->n_poly3 > 0 && poly_warps > 0) {
-    constexpr int warps_per_cta = G_THREADS / 32;
-    dim3 grid((poly_warps + warps_per_cta - 1) / warps_per_cta, g->n_poly3);
-    if (g->profiling) {
-      CU_OK(cudaEventRecord(s.pf_poly[0], cs));
-      s.pf_pg = true;
-    }
-    fir_poly_generic_cf32_kernel<<<grid, G_THREADS, 0, cs>>>(g->d_clients, g->d_poly3, s.d_blk, g->ring, mask, g->d_taps,
-                                                             s.d_phases, s.d_out);
-    if (g->profiling) CU_OK(cudaEventRecord(s.pf_poly[1], cs));
-  }
-  // ---- cascade clients: append the stage-A outputs to their rings, then stage B ----
-  s.pf_cb = false;
-  if (!q15 && n_casc > 0) {
-    // the rings are appended in block order: after the previous block's stage B, whichever stream ran it
-    if (g->have_last_casc) CU_OK(cudaStreamWaitEvent(cs, g->ev_last_casc, 0));
-    if (g->profiling) {
-      CU_OK(cudaEventRecord(s.pf_casc[0], cs));
-      s.pf_cb = true;
-    }
-    CU_OK(s.cblk.upload((size_t)n_casc, cs));
-    if (n_crat > 0) CU_OK(s.pblk.upload((size_t)n_crat, cs));
-    if (max_n1 > 0) cascade_launch_append(s.cblk.d, n_casc, max_n1, s.d_out, cs);
-    // integer stage B: one launch per ko, as the drop-in engine launches it (the kernel's summation order
-    // depends on ko: with even D2 output k is summed by lane (k mod ko) mod 32)
-    for (const xlg_group::CascRun &r : g->casc_runs) {
-      int run_n2 = 0;
-      size_t smem = 0;
-      for (int c = r.c0; c < r.c1; c++) {
-        run_n2 = std::max(run_n2, s.cblk.h[c].n2);
-        smem = std::max(smem, cascade_smem(r.ko, s.cblk.h[c].D2, s.cblk.h[c].T2));
-      }
-      if (run_n2 > 0) cascade_launch_fir(s.cblk.d + r.c0, r.c1 - r.c0, run_n2, r.ko, smem, g->d_taps2, s.d_out, cs);
-    }
-    // rational stage B: each client's CTA size was fixed at attach to fit the shared memory
-    if (max_rat_ctas > 0) cascade_launch_fir_poly(s.pblk.d, n_crat, max_rat_ctas, casc_poly_smem, g->d_taps2, s.d_out, cs);
-    if (g->profiling) CU_OK(cudaEventRecord(s.pf_casc[1], cs));
-    CU_OK(cudaEventRecord(s.ev_casc, cs));
-    g->ev_last_casc = s.ev_casc;
-    g->have_last_casc = true;
-    // from here on the client's results are its final row
-    for (size_t i = 0; i < g->clients.size(); i++)
-      if (g->clients[i].active && g->clients[i].casc) {
-        ho.n_out[i] = g->clients[i].last_n2;
-        ho.out_off[i] = g->clients[i].b2.fin_off;
-      }
-  }
-  // ---- sub-bands: append their outputs to their rings, then the members' oscillators and FIR ----
-  s.pf_sbk = false;
-  if (n_sb > 0) {
-    // the rings are appended in block order (the cascades' event orders both)
-    if (g->have_last_casc) CU_OK(cudaStreamWaitEvent(cs, g->ev_last_casc, 0));
-    if (g->profiling) {
-      CU_OK(cudaEventRecord(s.pf_sb[0], cs));
-      s.pf_sbk = true;
-    }
-    CU_OK(s.sbcb.upload((size_t)n_sb, cs));
-    if (max_sb_n1 > 0) cascade_launch_append(s.sbcb.d, n_sb, max_sb_n1, s.d_out, cs);
-    if (max_sb_n2 > 0 || max_sbr_ctas > 0) {
-      CU_OK(s.sbblk.upload(g->sb_classes.size(), cs));
-      subband_phase_kernel<<<(g->n_sb_mem + 31) / 32, 32, 0, cs>>>(g->d_clients, g->d_sbmem, s.sbblk.d, s.d_sbph);
-      if (max_sb_n2 > 0)
-        subband_fir_cf32_kernel<<<dim3((max_sb_n2 + SB_KO - 1) / SB_KO, g->n_sb_groups_int), SB_THREADS, sb_smem,
-                                  cs>>>(s.sbblk.d, g->d_sbgrp, g->d_sbtaps, s.d_sbph, s.d_out);
-      // rational classes: their groups follow the integer ones, one CTA layer per residue
-      if (max_sbr_ctas > 0)
-        subband_fir_poly_cf32_kernel<<<dim3(max_sbr_ctas, g->n_sb_groups - g->n_sb_groups_int, max_sbr_l2), SB_THREADS,
-                                       sbr_smem, cs>>>(s.sbblk.d, g->d_sbgrp + g->n_sb_groups_int, g->d_sbtaps,
-                                                       s.d_sbph, s.d_out);
-    }
-    if (g->profiling) CU_OK(cudaEventRecord(s.pf_sb[1], cs));
-    CU_OK(cudaEventRecord(s.ev_casc, cs));
-    g->ev_last_casc = s.ev_casc;
-    g->have_last_casc = true;
-    // (the FIR launches above sized themselves by these counts) a sub-band is not a client: nothing to
-    // read, and the D2H copy ends before its row
-    for (int i : g->sb_list) {
-      ho.n_out[i] = 0;
-      ho.out_off[i] = 0;
-    }
-  }
+  b.cs = g->profiling ? g->s_cs[0] : g->s_cs[ticket % g->n_cs];
+  b.cvs = g->conv_own_stream ? g->s_cv : b.cs;
+  // The launches, in stream order.  Each sizes itself by the walks' counts in ho: stage B switches the cascades'
+  // counts to their final rows, and the member launch zeroes the sub-bands', only after their own launches.  Both
+  // append to their rings in block order, chained on ev_last_casc.
+  if (stage_and_convert(b, fmt, input, flags) || launch_banks(b) || launch_prepass(b) || launch_tiled(b) ||
+      launch_long(b) || launch_generic(b) || launch_poly_tiled(b) || launch_poly_generic(b) || launch_stage_b(b) ||
+      launch_members(b))
+    return -EIO;
   CU_OK(cudaGetLastError());
-  CU_OK(cudaEventRecord(s.ev_fir, cs));
-
-  // ---- results back to the host ----
-  if (!dev_out && g->arena_cap > 0 && nc > 0) {
-    size_t used = 0;
-    for (size_t i = 0; i < g->clients.size(); i++)
-      if (g->clients[i].active) used = std::max(used, (size_t)ho.out_off[i] + (size_t)ho.n_out[i]);  // final rows
-    CU_OK(cudaStreamWaitEvent(g->s_out, s.ev_fir, 0));
-    if (used > 0) {
-      if (q15)
-        CU_OK(cudaMemcpyAsync(ho.h_qout, s.d_qout, used * sizeof(short2), cudaMemcpyDeviceToHost, g->s_out));
-      else
-        CU_OK(cudaMemcpyAsync(ho.h_out, s.d_out, used * sizeof(float2), cudaMemcpyDeviceToHost, g->s_out));
-      s.d2h_bytes = used * (q15 ? sizeof(short2) : sizeof(float2));
-    }
-    if ((g->flags & XLG_TRACK_STATE) && !q15 && s.d_endph != nullptr && ho.h_endph != nullptr)
-      CU_OK(cudaMemcpyAsync(ho.h_endph, s.d_endph, (size_t)nc * sizeof(float2), cudaMemcpyDeviceToHost, g->s_out));
-    CU_OK(cudaEventRecord(s.ev_done, g->s_out));
-  } else {
-    CU_OK(cudaEventRecord(s.ev_done, cs));  // results stay on the device: done = FIR done, no hop through s_out
-  }
+  CU_OK(cudaEventRecord(s.ev_fir, b.cs));
+  if (copy_back(b)) return -EIO;
 
   if (q15)
-    g->qS += n;
+    g->qS += b.n;
   else
-    g->S += n;
+    g->S += b.n;
   s.ticket.store(ticket);
   ho.ticket.store(ticket);
   s.harvested = false;
@@ -3271,28 +3240,30 @@ extern "C" int xlg_profile_enable(xlg_group *g, int on) {
   return 0;
 }
 
-extern "C" int xlg_poly_profile_read(xlg_group *g, xlg_poly_profile *p, int reset) {
+// one kernel family's counters (the profile structs after xlg_profile)
+template <typename P>
+static int family_profile_read(xlg_group *g, P xlg_group::*prof, P *p, int reset) {
   if (g == nullptr || p == nullptr) return -EINVAL;
   std::lock_guard<std::mutex> lk(g->mu);
-  *p = g->poly_prof;
-  if (reset) memset(&g->poly_prof, 0, sizeof(g->poly_prof));
+  *p = g->*prof;
+  if (reset) memset(&(g->*prof), 0, sizeof(P));
   return 0;
+}
+
+extern "C" int xlg_poly_profile_read(xlg_group *g, xlg_poly_profile *p, int reset) {
+  return family_profile_read(g, &xlg_group::poly_prof, p, reset);
 }
 
 extern "C" int xlg_cascade_profile_read(xlg_group *g, xlg_cascade_profile *p, int reset) {
-  if (g == nullptr || p == nullptr) return -EINVAL;
-  std::lock_guard<std::mutex> lk(g->mu);
-  *p = g->casc_prof;
-  if (reset) memset(&g->casc_prof, 0, sizeof(g->casc_prof));
-  return 0;
+  return family_profile_read(g, &xlg_group::casc_prof, p, reset);
 }
 
 extern "C" int xlg_subband_profile_read(xlg_group *g, xlg_subband_profile *p, int reset) {
-  if (g == nullptr || p == nullptr) return -EINVAL;
-  std::lock_guard<std::mutex> lk(g->mu);
-  *p = g->sb_prof;
-  if (reset) memset(&g->sb_prof, 0, sizeof(g->sb_prof));
-  return 0;
+  return family_profile_read(g, &xlg_group::sb_prof, p, reset);
+}
+
+extern "C" int xlg_bank_profile_read(xlg_group *g, xlg_bank_profile *p, int reset) {
+  return family_profile_read(g, &xlg_group::bank_prof, p, reset);
 }
 
 extern "C" int xlg_profile_read(xlg_group *g, xlg_profile *p, int reset) {
