@@ -7,6 +7,10 @@
 * bank_model: what bank_cf32_kernel computes, in its fmaf order (DESIGN.md section 5, "Bank sub-bands"), with
   a `mutation` argument that models a plausible kernel bug (MUTATIONS).
 * twiddles: the library's table W[j] = e^{-2 pi i j / K}, built by quarter turns in double and rounded once.
+* bank_member_model: bank_model's rows of a channel fed to subband_exact.member_model, bit for bit what a
+  member of a bank channel computes on any taps and input.
+* ring_cap, bank_ctas: the group's input ring capacity and, per block and bank CTA, its window, parity, wrap
+  split and zeroing before P (the edges the GPU tests assert they reached).
 """
 import math
 
@@ -16,6 +20,9 @@ from subband_exact import fmaf
 
 F = np.float32
 MUTATIONS = ("twiddle_plus_1", "r0_negated", "zero_point_minus_1", "taps_not_reversed")
+XLG_SLOTS = 4  # tickets in flight (include/xlating_group.h)
+BK_F = 32      # frames per bank CTA (xlating_kernels.cuh)
+BK_CG = 32     # channels per bank CTA
 
 
 def bank_tpad(K, T1):
@@ -85,7 +92,8 @@ def bank_model(taps, D1, channels, x, P, sizes, mutation=None):
 
     Frame m (window s_m, r_m = (s_m - P) mod K): phase 1 sums v[p] = fmaf chains (re, im) over q ascending of
     x[s_m + p + qK] * hr[p + qK], hr[j] = h[T1-1-j], for p < min(K, T1); phase 2 sums y_k = the 4-fmaf complex
-    chain over p ascending of v[p] * W[(k mod K) * (p + r_m) mod K].  Both start from +0.
+    chain over p ascending of v[p] * W[(k mod K) * (p + r_m) mod K].  Both start from +0.  Each step of a
+    chain is one fmaf over every (frame, p) or (channel, frame) at once, so wide banks stay affordable.
 
     mutation (MUTATIONS): twiddle_plus_1 reads W one index further; r0_negated takes r_m = (P - s_m) mod K;
     zero_point_minus_1 reads the sample just before P; taps_not_reversed multiplies x[s_m + j] by h[j]."""
@@ -104,33 +112,89 @@ def bank_model(taps, D1, channels, x, P, sizes, mutation=None):
     vre = np.zeros((total, KP), F)
     vim = np.zeros((total, KP), F)
     xr, xi = X.real.astype(F), X.imag.astype(F)
-    for p in range(KP):
-        are = np.zeros(total, F)
-        aim = np.zeros(total, F)
-        for j in range(p, T1, K):
-            are = fmaf(xr[:, j], hr[j], are)
-            aim = fmaf(xi[:, j], hr[j], aim)
-        vre[:, p], vim[:, p] = are, aim
+    for q in range(-(-T1 // K)):  # tap p + qK of every phase p that has one
+        j = q * K + np.arange(min(KP, T1 - q * K))
+        p = j - q * K
+        vre[:, p] = fmaf(xr[:, j], hr[j], vre[:, p])
+        vim[:, p] = fmaf(xi[:, j], hr[j], vim[:, p])
     W = twiddles(K)
     wre, wim = W.real.astype(F), W.imag.astype(F)
     r = (s - P) % K if mutation != "r0_negated" else (P - s) % K
+    chans = list(channels)
+    kk = np.array([k % K for k in chans], np.int64)[:, None]
+    are = np.zeros((len(chans), total), F)
+    aim = np.zeros((len(chans), total), F)
+    for p in range(KP):
+        t = (kk * (p + r)[None, :]) % K
+        if mutation == "twiddle_plus_1":
+            t = (t + 1) % K
+        a, b, c, d = vre[None, :, p], vim[None, :, p], wre[t], wim[t]
+        are = fmaf(a, c, are)
+        are = fmaf(-b, d, are)
+        aim = fmaf(a, d, aim)
+        aim = fmaf(b, c, aim)
     out = {}
-    for k in channels:
-        kk = k % K
-        are = np.zeros(total, F)
-        aim = np.zeros(total, F)
-        for p in range(KP):
-            t = (kk * (p + r)) % K
-            if mutation == "twiddle_plus_1":
-                t = (t + 1) % K
-            a, b, c, d = vre[:, p], vim[:, p], wre[t], wim[t]
-            are = fmaf(a, c, are)
-            are = fmaf(-b, d, are)
-            aim = fmaf(a, d, aim)
-            aim = fmaf(b, c, aim)
+    for i, k in enumerate(chans):
         y = np.empty(total, np.complex64)
-        y.real, y.imag = are, aim
+        y.real, y.imag = are[i], aim[i]
         out[k] = np.split(y, np.cumsum(counts)[:-1])
+    return out
+
+
+def bank_member_model(taps1, D1, k, x, P, sizes, members, fs, mat=0, attach=0, renorm=True, mutation=None):
+    """Members of channel k of a bank, as the bank kernel and the member kernels compute them: bank_model's
+    rows of the channel fed to member_model.
+
+    The bank (taps1, D1) is attached at stream position P of x; sizes are its blocks from P on.  The channel
+    was materialised before block `mat` of them (its ring reads zero before that block) and the members
+    (l2, d2, taps2, offset) before block `attach` of the channel's blocks.  Members of one shape form one class,
+    in the given order.  Returns per member one complex64 array per block from the attach on.
+
+    mutation: an entry of MUTATIONS (the bank) or of subband_exact.MUTATIONS (the members)."""
+    from subband_exact import MUTATIONS as SB_MUTATIONS, member_consts, member_model
+    assert mutation is None or mutation in MUTATIONS or mutation in SB_MUTATIONS, mutation
+    rows = bank_model(taps1, D1, [k], x, P, sizes, mutation=mutation if mutation in MUTATIONS else None)[k][mat:]
+    classes = {}
+    for i, (l2, d2, taps2, offset) in enumerate(members):
+        classes.setdefault((l2, d2, len(taps2)), []).append(i)
+    outs = [None] * len(members)
+    for (l2, d2, _), idx in classes.items():
+        consts = [member_consts(np.asarray(members[i][2], F), d2, members[i][3], l2, fs // D1) for i in idx]
+        got = member_model(rows, attach, l2, d2, [c[0] for c in consts], [c[1] for c in consts], renorm=renorm,
+                           mutation=mutation if mutation in SB_MUTATIONS else None)
+        for i, y in zip(idx, got):
+            outs[i] = y
+    return outs
+
+
+def next_pow2(n):
+    return 1 << max(0, int(n - 1).bit_length())
+
+
+def ring_cap(max_in, hist):
+    """The group's input ring capacity (ensure_ring): XLG_SLOTS + 1 blocks of max_in / 2 samples, the largest
+    history the group has needed (at least 4096) and 64 samples of slack, to a power of two."""
+    return next_pow2((XLG_SLOTS + 1) * (max_in // 2) + max(hist, 4096) + 64)
+
+
+def bank_ctas(sizes, T1, D1, P, cap):
+    """Per block of a bank attached at stream position P (sizes: its blocks from P on) and per CTA x of its
+    frames (BK_F each), what walk_banks and the kernel prologue compute: (w0, shift, need, split, pre_p) --
+    the window start, its parity in the ring, the samples staged, whether the staging is two bulk copies
+    (the window straddles the ring's wrap) and whether the CTA zeroes samples before P."""
+    counts, firsts = bank_walk(sizes, T1, D1)
+    out = []
+    for n1, first in zip(counts, firsts):
+        ctas = []
+        for f0 in range(0, n1, BK_F):
+            nf = min(BK_F, n1 - f0)
+            w0 = P + first + f0 * D1
+            idx = w0 & (cap - 1)
+            shift = idx & 1
+            need = ((nf - 1) * D1 + T1 + shift + 1) & ~1
+            p1 = min(need, cap - (idx - shift))
+            ctas.append((w0, shift, need, p1 < need, w0 - shift < P))
+        out.append(ctas)
     return out
 
 

@@ -5,6 +5,10 @@
 * the kernel model equals the float64 definition bit for bit on exact stimuli (dyadic taps, grid input,
   channels whose twiddles are +-1 or +-i), and is within float32 accuracy of it at any channel;
 * mutations of the model each fail the exact harness;
+* bank_member_model (the bank model's rows fed to the member model) equals the float64 composition on exact
+  stimuli, stays within float32 accuracy of the streaming oracle on random data, and every mutation of either
+  stage changes its output;
+* ring_cap and bank_ctas follow the walk;
 * subband_plan(bank=True) puts every sub-band on the bank's grid with offsets within fs1 / 4 and counts the
   first stage as one polyphase pass and C channel sums; the default plan is the one of the sub-band workloads.
 """
@@ -14,9 +18,13 @@ import sys
 import numpy as np
 import pytest
 
-from bank_exact import MUTATIONS, bank_model, bank_walk, f64_bank, twiddles
+import subband_exact
+from bank_exact import (MUTATIONS, BankMemberOracle, bank_ctas, bank_member_model, bank_model, bank_walk, f64_bank,
+                        ring_cap, twiddles)
 from cascade import f64_filter, filter_constants
 from exact import dyadic_taps, exact_input, to_complex
+from subband_exact import f64_member
+from subband_rig import dyadic_member
 from oracle import pyoracle as po
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools"))
@@ -198,3 +206,94 @@ def test_streaming_member_oracle_follows_the_definition():
             got = o.process_cf32("cu8", r)
             assert np.array_equal(got, w.astype(np.complex64)) or np.max(np.abs(got - w)) <= 1e-6 * max(
                 np.max(np.abs(w)), 1.0)
+
+
+# ---------------------------------------------------------------------------
+# the chain: bank rows into the member kernels
+# ---------------------------------------------------------------------------
+CHAIN_INT = [(1, 1), (3, 9), (4, 8), (5, 23), (2, 31)]  # (D2, T2)
+CHAIN_RAT = [(2, 5, 33), (3, 7, 40), (12, 5, 60)]       # (L2, M2, T2)
+
+
+@pytest.mark.parametrize("D1,T1,fmt", [(2, 9, "cu8"), (4, 31, "cs8"), (10, 61, "cs16"), (32, 70, "cs8")])
+def test_chain_is_exact_on_exact_stimuli(D1, T1, fmt):
+    """Dyadic bank taps, quarter-turn channels, dyadic full-length members at offset 0 within exact_bound:
+    the chain equals f64_bank's rows fed to f64_member, with the bank attached after block 0, the channel
+    materialised a block later and members attached at the channel's first block and two blocks on."""
+    rng = np.random.default_rng(D1 * 13 + T1)
+    fs = 2 * D1 * 96000
+    taps1 = dyadic_taps(rng, T1, fmt)
+    _, x = stream(rng, fmt, SIZES)
+    P, sizes = SIZES[0], SIZES[1:]
+    for k in exact_channels(D1):
+        for attach in (0, 2):
+            members = [(1, d2, dyadic_member(rng, taps1, T2, fmt), 0) for d2, T2 in CHAIN_INT]
+            members += [(l2, m2, dyadic_member(rng, taps1, T2, fmt), 0) for l2, m2, T2 in CHAIN_RAT]
+            got = bank_member_model(taps1, D1, k, x.astype(np.complex64), P, sizes, members, fs, mat=1,
+                                    attach=attach)
+            rows = f64_bank(taps1, D1, [k], x, P, sizes)[k][1:]
+            for (l2, d2, taps2, _), y in zip(members, got):
+                want = f64_member(rows[attach:], l2, d2, taps2, fs // D1)
+                assert len(y) == len(want)
+                for a, w in zip(y, want):
+                    assert np.array_equal(a, w), (fmt, k, l2, d2, taps2.size, attach)
+
+
+@pytest.mark.parametrize("D1,T1,fmt", [(3, 13, "cu8"), (7, 101, "cs8"), (20, 45, "cs16")])
+def test_chain_is_within_float32_of_the_oracle(D1, T1, fmt):
+    """Random taps and input, members at offsets 0, +-fs1/4 and arbitrary: within 1e-5 norm-wise of
+    BankMemberOracle (the float64 rows fed to the reference's float path)."""
+    rng = np.random.default_rng(T1 + 3)
+    fs = 2 * D1 * 48000
+    fs1 = fs // D1
+    taps1 = (rng.standard_normal(T1) / np.sqrt(T1)).astype(np.float32)
+    raw, x = stream(rng, fmt, SIZES)
+    offsets = [0, fs1 // 4, -fs1 // 4, int(rng.integers(-fs1 // 2, fs1 // 2))]
+    shapes = [(1, d2, T2) for d2, T2 in CHAIN_INT] + list(CHAIN_RAT)
+    for k in (-D1, 0, D1 - 1, 1):
+        members = [(l2, d2, (rng.standard_normal(T2) / np.sqrt(T2)).astype(np.float32), offsets[i % 4])
+                   for i, (l2, d2, T2) in enumerate(shapes)]
+        got = bank_member_model(taps1, D1, k, x.astype(np.complex64), 0, SIZES, members, fs)
+        for (l2, d2, taps2, off), y in zip(members, got):
+            o = BankMemberOracle(D1, taps1, k, d2, taps2, off, l2, fs)
+            want = [o.process_cf32(fmt, r) for r in raw]
+            a, b = np.concatenate(y), np.concatenate(want)
+            assert a.shape == b.shape
+            assert np.max(np.abs(a - b)) <= 1e-5 * np.max(np.abs(b)), (k, l2, d2, off)
+
+
+@pytest.mark.parametrize("mutation", MUTATIONS + subband_exact.MUTATIONS)
+def test_every_mutation_changes_the_chain(mutation):
+    """Random data: the bank attached at an odd P, the channel materialised with it, a class of 33 integer
+    members (odd Tb: tap rows of sb_tpad, not Tb, apart; one phase row past 32) at distinct offsets and a
+    rational class of L2 = 3, attached with the channel or (the member mutations) after its rows began."""
+    rng = np.random.default_rng(8)
+    D1, T1, fs = 5, 37, 960000
+    fs1 = fs // D1
+    taps1 = rng.standard_normal(T1).astype(np.float32)
+    _, x = stream(rng, "cs16", SIZES)
+    x = x.astype(np.complex64)
+    members = [(1, 4, rng.standard_normal(23).astype(np.float32), int(rng.integers(-fs1 // 2, fs1 // 2)))
+               for _ in range(33)]
+    members += [(3, 7, rng.standard_normal(40).astype(np.float32), 1000 * i) for i in range(3)]
+    P, sizes = sum(SIZES[:3]), SIZES[3:]
+    args = (taps1, D1, 3, x, P, sizes, members, fs)
+    attach = 0 if mutation in MUTATIONS else 3  # (the bank's: rows whose windows reach back before P)
+    base = bank_member_model(*args, attach=attach)
+    got = bank_member_model(*args, attach=attach, mutation=mutation)
+    assert any(not np.array_equal(a, b) for ya, yb in zip(base, got) for a, b in zip(ya, yb)), mutation
+
+
+def test_ring_cap_and_bank_ctas_follow_the_walk():
+    assert ring_cap(8192, 0) == 32768 and ring_cap(8192, 12300) == 65536 and ring_cap(65536, 4096) == 262144
+    sizes, T1, D1, P, cap = [1000, 37, 0, 2001], 300, 7, 5, 64
+    counts, firsts = bank_walk(sizes, T1, D1)
+    ctas = bank_ctas(sizes, T1, D1, P, cap)
+    assert [len(c) for c in ctas] == [-(-n // 32) for n in counts]
+    for n1, first, cs in zip(counts, firsts, ctas):
+        for x, (w0, shift, need, split, pre) in enumerate(cs):
+            nf = min(32, n1 - 32 * x)
+            assert w0 == P + first + 32 * x * D1 and shift == w0 % 2 and need % 2 == 0
+            assert need >= (nf - 1) * D1 + T1 + shift and split == ((w0 - shift) % cap + need > cap)
+            assert pre == (w0 - shift < P)
+    assert ctas[0][1][4] and not ctas[3][0][4]  # T1 > 32 D1: CTA 1 of the first block reads before P
