@@ -52,7 +52,11 @@ enum { XLG_FMT_CU8 = 0, XLG_FMT_CS8 = 1, XLG_FMT_CS16 = 2 };
                                   with the ticket's results: xlg_copy_output(..., state_after).  Used by the
                                   per-filter drop-in engine, which moves filters in and out of a group. */
 /* xlg_submit flags */
-#define XLG_INPUT_DEVICE 0x100u /* `input` is a device pointer on the group's GPU (already staged) */
+#define XLG_INPUT_DEVICE 0x100u /* `input` is a device pointer on the group's GPU (already staged), aligned to one
+                                   complex sample: 2 bytes for cu8 and cs8, 4 for cs16.  A misaligned one is
+                                   refused (-EINVAL, logged) before anything is enqueued; no ticket is taken.
+                                   The block may be overwritten once xlg_input_consumed(ticket) (or xlg_wait)
+                                   returns. */
 #define XLG_PATH_Q15 0x200u     /* Q15 integer path (src/xlating.c:92-140) instead of cf32 */
 #define XLG_INPUT_KEEP 0x400u   /* `input` is page-locked host memory that the caller leaves untouched until
                                    xlg_input_consumed(ticket) (or xlg_wait) returns: xlg_submit then returns
@@ -232,7 +236,10 @@ int xlg_client_count(const xlg_group *g);
  * XLG_SLOTS tickets are already in flight and the oldest has not completed. */
 int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t input_len, uint32_t flags);
 
-/* Block until the H2D copy of ticket's input block has completed (XLG_INPUT_KEEP submits). */
+/* Block until the group has read ticket's input block: its H2D copy for a host block (what XLG_INPUT_KEEP submits
+ * wait for), its conversion for an XLG_INPUT_DEVICE block (which may then be reused, also by work on another
+ * stream).  Returns at once for a block of no complex sample, and for a ticket whose slot a later ticket already
+ * uses (its input was read long ago).  -EINVAL for a ticket not yet submitted. */
 int xlg_input_consumed(xlg_group *g, int64_t ticket);
 
 /* Block until ticket's outputs are complete (in pinned host memory, or in HBM
@@ -263,7 +270,10 @@ void *xlg_alloc_pinned(size_t bytes);
 void xlg_free_pinned(void *p);
 
 /* Make the group's work wait for everything already enqueued on an external
- * CUDA stream (e.g. the torch/NCCL stream that produced a device input). */
+ * CUDA stream (e.g. the torch/NCCL stream that produced a device input).  Every
+ * call made since the last xlg_submit is honoured by the next one, so a block
+ * produced on several streams takes one call per stream.  Nothing is enqueued
+ * on the caller's stream. */
 int xlg_wait_stream(xlg_group *g, void *cuda_stream);
 
 /* SMs currently reserved for the oscillator pre-pass (0 = no partition active).  With XLG_SM_PARTITION the group

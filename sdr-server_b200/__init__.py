@@ -521,10 +521,18 @@ class Group:
         return t
 
     def submit_ptr(self, fmt_code: int, ptr: int, n: int, flags: int = 0) -> int:
+        """Submit n raw elements at address ptr: page-locked host memory (a PinnedBuffer's ptr, or a pinned torch
+        tensor's data_ptr(), plus any byte offset) or, with XLG_INPUT_DEVICE, device memory."""
         t = self._L.xlg_submit(self._h, fmt_code, ptr, n, flags)
         if t < 0:
             raise RuntimeError(f"xlg_submit -> {t}")
         return t
+
+    def input_consumed(self, ticket: int) -> None:
+        """xlg_input_consumed: returns once the group has read the ticket's input block."""
+        code = self._L.xlg_input_consumed(self._h, ticket)
+        if code != 0:
+            raise RuntimeError(f"xlg_input_consumed -> {code}")
 
     def wait(self, ticket: int) -> None:
         code = self._L.xlg_wait(self._h, ticket)

@@ -203,6 +203,7 @@ struct Slot {
   float2 *d_endph = nullptr;  // XLG_TRACK_STATE: every client's oscillator after this block (same capacity as d_blk)
   size_t blk_cap = 0;
   cudaEvent_t ev_h2d = nullptr, ev_conv = nullptr, ev_phase = nullptr, ev_fir = nullptr, ev_done = nullptr;
+  cudaEvent_t ev_input = nullptr;  // the last reader of this ticket's input: ev_h2d, ev_conv, or none for n = 0
   cudaEvent_t pf[SP_N][2] = {};  // begin / end of each span
   bool pf_on[SP_N] = {};         // the span ran in this block (its events are recorded, or, for the pre-pass, stamped)
   cudaEvent_t tl_ph[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // timeline: pre-pass stamps, by occupancy parity (it runs a block ahead)
@@ -357,8 +358,10 @@ struct xlg_group {
   cudaStream_t s_in = nullptr, s_ph = nullptr, s_out = nullptr;
   // raw -> ring conversion: its own stream, in the oscillator partition (or at high priority without one), so
   // that block b+1's conversion never queues behind the CTAs of block b's FIR that are still waiting for an SM
-  cudaEvent_t ev_user = nullptr;  // xlg_wait_stream: recorded on the caller's stream, waited for by the next submit's first reader
-  bool user_wait_pending = false;
+  // xlg_wait_stream: one event per call since the last submit, each recorded on the caller's stream and waited for
+  // by the next submit's first reader; the pool is reused, n_user_waits of it are pending
+  std::vector<cudaEvent_t> ev_user;
+  size_t n_user_waits = 0;
   cudaStream_t s_cv = nullptr;
   bool conv_own_stream = true;  // XLATING_B200_CONV_STREAM=0: convert on the block's compute stream (the old order)
   static constexpr int kMaxCs = 4;
@@ -1839,7 +1842,7 @@ extern "C" void xlg_destroy(xlg_group *g) {
   for (HostClient &h : g->clients)
     if (h.b2.ring.p) cudaFree(h.b2.ring.p);
   for (float2 *p : g->dead_rings) cudaFree(p);
-  if (g->ev_user) cudaEventDestroy(g->ev_user);
+  for (cudaEvent_t e : g->ev_user) cudaEventDestroy(e);
   if (g->s_in) cudaStreamDestroy(g->s_in);
   for (const xlg_group::StreamSet *ss : {&g->set_part, &g->set_plain}) {
     if (ss->ph) cudaStreamDestroy(ss->ph);
@@ -2515,14 +2518,17 @@ static int stage_and_convert(Block &b, int fmt, const void *input, uint32_t flag
     d_in = s.d_raw;
   }
 
-  if (g->user_wait_pending) {
-    // (in-order streams: later submits' conversions queue behind this one's, so one wait is enough)
-    CU_OK(cudaStreamWaitEvent(b.cvs, g->ev_user, 0));
-    CU_OK(cudaStreamWaitEvent(g->s_in, g->ev_user, 0));
+  // (in-order streams: later submits' conversions queue behind this one's, so one wait per event is enough)
+  for (size_t i = 0; i < g->n_user_waits; i++) {
+    const cudaEvent_t e = g->ev_user[i];
+    CU_OK(cudaStreamWaitEvent(b.cvs, e, 0));
+    CU_OK(cudaStreamWaitEvent(g->s_in, e, 0));
     if (!g->conv_own_stream)
-      for (int i = 0; i < g->n_cs; i++) CU_OK(cudaStreamWaitEvent(g->s_cs[i], g->ev_user, 0));
-    g->user_wait_pending = false;
+      for (int c = 0; c < g->n_cs; c++) CU_OK(cudaStreamWaitEvent(g->s_cs[c], e, 0));
   }
+  g->n_user_waits = 0;
+  // what xlg_input_consumed waits for: the copy out of a host block, the conversion that reads a device block
+  s.ev_input = n == 0 ? nullptr : (flags & XLG_INPUT_DEVICE) ? s.ev_conv : s.ev_h2d;
   if (n > 0) {
     if (g->timeline && !g->base_recorded) {
       CU_OK(cudaEventRecord(g->ev_base, b.cvs));
@@ -2934,6 +2940,13 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     XL_LOG("block of %zu elements exceeds max_input_len %u", input_len, g->max_input_len);
     return -EINVAL;
   }
+  // the conversion kernels load one complex sample at a time (uchar2 / char2 / short2); host inputs are staged
+  // into an aligned buffer, device inputs are read where they are
+  const size_t sample_bytes = 2 * elem_bytes(fmt);
+  if ((flags & XLG_INPUT_DEVICE) && input_len > 0 && (uintptr_t)input % sample_bytes != 0) {
+    XL_LOG("device input %p is not aligned to one complex sample (%zu bytes)", input, sample_bytes);
+    return -EINVAL;
+  }
   const bool q15 = (flags & XLG_PATH_Q15) != 0;
   if (q15)
     for (const BankHost &k : g->banks)
@@ -3159,9 +3172,10 @@ extern "C" int xlg_copy_output(xlg_group *g, int64_t ticket, int client_id, void
 extern "C" int xlg_input_consumed(xlg_group *g, int64_t ticket) {
   if (g == nullptr || ticket < 0 || ticket >= g->next_ticket.load()) return -EINVAL;
   Slot &s = g->slots[ticket % XLG_SLOTS];
-  if (s.ticket.load() != ticket) return 0;  // the slot serves a later ticket: this one's copy finished long ago
+  if (s.ticket.load() != ticket) return 0;  // the slot serves a later ticket: this one's input was read long ago
+  if (s.ev_input == nullptr) return 0;      // an empty block reads nothing
   cudaSetDevice(g->device);
-  CU_OK(cudaEventSynchronize(s.ev_h2d));
+  CU_OK(cudaEventSynchronize(s.ev_input));
   return 0;
 }
 
@@ -3182,12 +3196,17 @@ extern "C" int xlg_wait_stream(xlg_group *g, void *cuda_stream) {
   if (g == nullptr) return -EINVAL;
   cudaSetDevice(g->device);
   // Only the first reader of a device-resident input has to wait: the conversion (and the H2D stream, for
-  // symmetry with host inputs).  The event is recorded now and attached to the consuming stream by the next
+  // symmetry with host inputs).  An event is recorded now and attached to the consuming stream by the next
   // xlg_submit -- which knows the stream (a re-layout in between may switch stream sets) -- so a call costs one
-  // record here and one wait there instead of a wait on every stream of the group.
-  if (g->ev_user == nullptr) CU_OK(cudaEventCreateWithFlags(&g->ev_user, cudaEventDisableTiming));
-  CU_OK(cudaEventRecord(g->ev_user, (cudaStream_t)cuda_stream));
-  g->user_wait_pending = true;
+  // record here and one wait there instead of a wait on every stream of the group.  Every call since the last
+  // submit keeps its own event: a block may be produced on several streams.
+  if (g->n_user_waits == g->ev_user.size()) {
+    cudaEvent_t e = nullptr;
+    CU_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    g->ev_user.push_back(e);
+  }
+  CU_OK(cudaEventRecord(g->ev_user[g->n_user_waits], (cudaStream_t)cuda_stream));
+  g->n_user_waits++;
   return 0;
 }
 
