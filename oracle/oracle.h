@@ -59,6 +59,9 @@ size_t orc_xlating_process_q15(orc_xlating *f, int fmt, const void *input,
 size_t orc_xlating_history(const orc_xlating *f);
 void orc_xlating_phase(const orc_xlating *f, float *re, float *im);
 size_t orc_xlating_taps(const orc_xlating *f, const float **rev_taps_interleaved);
+/* the Q15 path's constants: reversed taps (interleaved re,im) and the oscillator step */
+size_t orc_xlating_q15_consts(const orc_xlating *f, const int16_t **rev_q15_interleaved, int16_t *qinc_re,
+                              int16_t *qinc_im);
 
 /* State hand-over, for the model check of the drop-in engine's stream overlay
  * (tests/stream_overlay_shim.cpp): the cf32 history the next call will prepend

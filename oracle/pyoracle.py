@@ -70,6 +70,9 @@ def orc() -> C.CDLL:
         lib.orc_xlating_phase.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float)]
         lib.orc_xlating_taps.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_float))]
         lib.orc_xlating_taps.restype = C.c_size_t
+        lib.orc_xlating_q15_consts.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_int16)), C.POINTER(C.c_int16),
+                                               C.POINTER(C.c_int16)]
+        lib.orc_xlating_q15_consts.restype = C.c_size_t
         lib.orc_xlating_set_state.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.c_size_t, C.c_float, C.c_float]
         lib.orc_xlating_set_state.restype = C.c_int
         _orc = lib
@@ -144,6 +147,14 @@ class OracleFilter:
         p = C.POINTER(C.c_float)()
         n = self._lib.orc_xlating_taps(self._h, C.byref(p))
         return np.ctypeslib.as_array(p, shape=(2 * n,)).copy().view(np.complex64)
+
+    @property
+    def q15_consts(self):
+        """((T, 2) int16 reversed Q15 taps, (qinc_re, qinc_im))."""
+        p = C.POINTER(C.c_int16)()
+        qr, qi = C.c_int16(), C.c_int16()
+        n = self._lib.orc_xlating_q15_consts(self._h, C.byref(p), C.byref(qr), C.byref(qi))
+        return np.ctypeslib.as_array(p, shape=(2 * n,)).copy().reshape(n, 2), (qr.value, qi.value)
 
     def close(self):
         if self._h:

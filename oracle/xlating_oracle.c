@@ -208,8 +208,12 @@ size_t orc_xlating_process_q15(orc_xlating *f, int fmt, const void *input,
       for (size_t j = 0; j < T; j++) { /* :108-116 */
         const int32_t xr = x[2 * j], xi = x[2 * j + 1];
         const int32_t tr = f->rev_q15[2 * j], ti = f->rev_q15[2 * j + 1];
-        acc_re += xr * tr - xi * ti;
-        acc_im += xr * ti + xi * tr;
+        /* each pair is summed in 32 bits before it meets the int64 accumulator.  The imaginary pair is
+         * 2^31 for x = tap = (-32768, -32768), which the reference's int arithmetic wraps to -2^31: wrap
+         * it here with unsigned arithmetic (defined) and gcc's modular conversion back to int32_t.  Each
+         * product fits in int32_t. */
+        acc_re += (int32_t)((uint32_t)(xr * tr) - (uint32_t)(xi * ti));
+        acc_im += (int32_t)((uint32_t)(xr * ti) + (uint32_t)(xi * tr));
       }
       const int16_t ar = sat16((int32_t)(acc_re >> 15)); /* :118-119 */
       const int16_t ai = sat16((int32_t)(acc_im >> 15));
@@ -230,6 +234,13 @@ size_t orc_xlating_process_q15(orc_xlating *f, int fmt, const void *input,
 }
 
 size_t orc_xlating_history(const orc_xlating *f) { return f->hist; }
+
+size_t orc_xlating_q15_consts(const orc_xlating *f, const int16_t **rev, int16_t *qinc_re, int16_t *qinc_im) {
+  *rev = f->rev_q15;
+  *qinc_re = f->qinc_re;
+  *qinc_im = f->qinc_im;
+  return f->ntaps;
+}
 
 void orc_xlating_phase(const orc_xlating *f, float *re, float *im) {
   *re = f->ph_re;

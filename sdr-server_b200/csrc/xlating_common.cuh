@@ -197,8 +197,11 @@ __device__ __forceinline__ float2 fir_warp_cf32(const float2 *__restrict__ ring,
 
 // Q15 integer path (src/xlating.c:92-140): int16 x int16 products accumulated in
 // int64 -- integer addition is associative, so the lane-split + shuffle reduction
-// is bit-exact against the reference's sequential loop.  Returns the filter output
-// already scaled and saturated (:118-119).
+// is bit-exact against the reference's sequential loop.  Each product pair is
+// summed in 32 bits first, as the reference's int arithmetic does (:114-115): the
+// imaginary pair of x = tap = (-32768, -32768) is 2^31 and wraps to -2^31 there, so
+// it wraps here too (unsigned add, then back to int), before it is widened.
+// Returns the filter output already scaled and saturated (:118-119).
 __device__ __forceinline__ short2 fir_warp_q15(const short2 *__restrict__ ring, unsigned mask, long long zb,
                                                const short2 *__restrict__ tp, int T, int D, long long w0,
                                                int lane) {
@@ -213,8 +216,10 @@ __device__ __forceinline__ short2 fir_warp_q15(const short2 *__restrict__ ring, 
       const long long ab = w0 + (long long)i * D + j;
       short2 x = ring[(unsigned)((unsigned long long)ab) & mask];  // unconditional: any masked index is in the ring
       if (ab < zb) x = make_short2(0, 0);
-      are[i] += (long long)((int)x.x * (int)t.x) - (long long)((int)x.y * (int)t.y);  // :114
-      aim[i] += (long long)((int)x.x * (int)t.y) + (long long)((int)x.y * (int)t.x);  // :115
+      const int pre = (int)((unsigned)((int)x.x * (int)t.x) - (unsigned)((int)x.y * (int)t.y));  // :114
+      const int pim = (int)((unsigned)((int)x.x * (int)t.y) + (unsigned)((int)x.y * (int)t.x));  // :115
+      are[i] += (long long)pre;
+      aim[i] += (long long)pim;
     }
   }
 #pragma unroll
