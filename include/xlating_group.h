@@ -217,6 +217,19 @@ int xlg_add_bank(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1
 int xlg_add_bank_subband(xlg_group *g, int bank_id, int32_t channel, int *subband_id);
 /* -EBUSY (logged) while the bank still has channels; -EINVAL for an unknown id. */
 int xlg_remove_bank(xlg_group *g, int bank_id);
+/* Extension: FFT bank sub-bands (DESIGN.md section 5, "FFT banks").  A bank whose channels are defined exactly as
+ * xlg_add_bank's (the same P, s_m, zero history and output counts) and whose channel stage is a K-point FFT of
+ * each frame's polyphase sums instead of a direct sum per channel: O(K log K) per frame, whatever the number of
+ * channels, which makes wide banks affordable.  Only the rounding differs from xlg_add_bank.  Its id comes from
+ * the same space as xlg_add_bank's; xlg_add_bank_subband, xlg_remove_bank, xlg_add_client_subband[_rational]
+ * and xlg_remove_subband work on it unchanged, xlg_subband_info reports stage_a_kind 8 for its members and
+ * xlg_reserve counts its channels as a bank's.  -EINVAL (logged) for decim1 or taps1_len of 0, K = 2 * decim1
+ * not a power of two or above 4096, fs % K != 0, or more than max(16 * K, 16384) taps; -ENOTSUP (logged) on an
+ * XLG_TRACK_STATE group.  A group with one refuses XLG_PATH_Q15 submits, as for every bank. */
+int xlg_add_bank_fft(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, int *bank_id);
+/* Real FP32 instructions of the butterflies of one K-point FFT bank frame (K a power of two): 28 per radix-4
+ * butterfly (16 adds and 3 complex products of 4), 4 per radix-2 butterfly.  The planner costs FFT banks by it. */
+uint64_t xlg_bank_fft_flops(uint32_t K);
 /* Size the per-ticket result arenas (device and pinned host) for `output_samples_per_block` complex output
  * samples per block summed over all clients (a client at decimation D produces about max_input_len/2/D + 2).
  * A cascade client counts two rows, each rounded up to a multiple of 4 samples: its stage-A row of
@@ -350,12 +363,22 @@ typedef struct {
 } xlg_bank_profile;
 int xlg_bank_profile_read(xlg_group *g, xlg_bank_profile *p, int reset);
 
+/* FFT banks (xlg_add_bank_fft), counted like xlg_profile's while profiling is enabled.  xlg_bank_profile counts
+ * direct banks only. */
+typedef struct {
+  double fft_ms;             /* the FFT bank kernel */
+  uint64_t fft_launches;
+  uint64_t poly_macs;        /* real-by-complex MACs of the polyphase sums: sum n1 * T1 */
+  uint64_t butterfly_flops;  /* real FP32 instructions of the butterflies: sum n1 * xlg_bank_fft_flops(K) */
+} xlg_bank_fft_profile;
+int xlg_bank_fft_profile_read(xlg_group *g, xlg_bank_fft_profile *p, int reset);
+
 /* Introspection for tests: history length (src/xlating.c:29 history_offset; upsampled samples for a
  * rational client, stage A's for a cascade client) and which kernel currently serves the client
  * (0 = generic, 1 = tiled, 2 = long-filter split-K, 3 = rational, polyphase generic, 4 = rational, tiled: at
  * least 8 clients with identical (interp, decim, taps_len, window alignment), gcd(interp, decim) = 1, whose
  * branches fit the tiled kernel's shared memory, 5 = cascade, 6 = sub-band member; 7, as a sub-band's kind in
- * xlg_subband_info only, = a bank's channel). */
+ * xlg_subband_info only, = a bank's channel, 8 likewise = an FFT bank's channel). */
 int xlg_client_info(const xlg_group *g, int client_id, size_t *history, int *kernel_kind);
 /* A cascade client's stages: the kind (0, 1 or 2, as xlg_client_info) of the kernel serving stage A, and the
  * history_offset of each stage (stage B's in stage-A samples, upsampled by interp2 for a rational cascade

@@ -95,6 +95,11 @@ class XlgBankProfile(C.Structure):
                 ("dft_macs", C.c_uint64)]
 
 
+class XlgBankFftProfile(C.Structure):
+    _fields_ = [("fft_ms", C.c_double), ("fft_launches", C.c_uint64), ("poly_macs", C.c_uint64),
+                ("butterfly_flops", C.c_uint64)]
+
+
 def build(verbose: bool = False) -> None:
     """Compile lib/libxlating_b200.so for sm_90a (nvcc cross-compiles without a GPU)."""
     subprocess.run(["make", "-C", HERE, "all"], check=True,
@@ -177,6 +182,12 @@ def lib() -> C.CDLL:
     L.xlg_remove_bank.restype = C.c_int
     L.xlg_bank_profile_read.argtypes = [vp, C.POINTER(XlgBankProfile), C.c_int]
     L.xlg_bank_profile_read.restype = C.c_int
+    L.xlg_add_bank_fft.argtypes = [vp, u32, fp, sz, C.POINTER(C.c_int)]
+    L.xlg_add_bank_fft.restype = C.c_int
+    L.xlg_bank_fft_profile_read.argtypes = [vp, C.POINTER(XlgBankFftProfile), C.c_int]
+    L.xlg_bank_fft_profile_read.restype = C.c_int
+    L.xlg_bank_fft_flops.argtypes = [u32]
+    L.xlg_bank_fft_flops.restype = C.c_uint64
     L.xl_poly_pack.argtypes = [C.POINTER(C.c_float), sz, u32, C.POINTER(C.c_float)]
     L.xl_poly_pack.restype = None
     L.xlg_reserve.argtypes = [vp, sz]
@@ -473,6 +484,18 @@ class Group:
             raise ValueError(code)
         return bid.value
 
+    def add_bank_fft(self, decim1: int, taps1) -> int:
+        """An FFT bank (xlg_add_bank_fft): add_bank's channels, cut by a K-point FFT per frame instead of a direct
+        sum per channel (K = 2 * decim1 a power of two up to 4096; bank_fft_fits bounds taps1).  Returns a bank
+        id from add_bank's id space."""
+        t1 = np.ascontiguousarray(taps1, dtype=np.float32)
+        bid = C.c_int(-1)
+        code = self._L.xlg_add_bank_fft(self._h, decim1, t1.ctypes.data_as(C.POINTER(C.c_float)), len(t1),
+                                        C.byref(bid))
+        if code != 0:
+            raise ValueError(code)
+        return bid.value
+
     def add_bank_subband(self, bid: int, channel: int) -> int:
         """Channel `channel` in [-decim1, decim1) of bank `bid` (xlg_add_bank_subband): an ordinary sub-band id,
         centred at channel * fs / (2 * decim1), that takes members through add_client_subband."""
@@ -635,6 +658,11 @@ class Group:
         self._L.xlg_bank_profile_read(self._h, C.byref(p), 1 if reset else 0)
         return {k: getattr(p, k) for k, _ in XlgBankProfile._fields_}
 
+    def bank_fft_profile_read(self, reset: bool = True) -> dict:
+        p = XlgBankFftProfile()
+        self._L.xlg_bank_fft_profile_read(self._h, C.byref(p), 1 if reset else 0)
+        return {k: getattr(p, k) for k, _ in XlgBankFftProfile._fields_}
+
     def close(self):
         if self._h:
             self._L.xlg_destroy(self._h)
@@ -795,7 +823,19 @@ def bank_fits(d1: int, t1: int) -> bool:
     return 16 + 4 * tpad + 8 * ((31 * d1 + t1 + 2) & ~1) + 8 * K + 8 * 32 * (K + 1) <= 200 * 1024
 
 
-def subband_plan(fs: int, clients, bank: bool = False):
+def bank_fft_fits(d1: int, t1: int) -> bool:
+    """Whether the FFT bank kernel takes a bank (xlg_add_bank_fft refuses the others): K = 2 * d1 a power of two
+    up to 4096 and at most max(16 * K, 16384) taps, bank_fft_max_taps in csrc/xlating_kernels.cuh."""
+    K = 2 * d1
+    return d1 >= 1 and K & (K - 1) == 0 and K <= 4096 and 1 <= t1 <= max(16 * K, 16384)
+
+
+def bank_fft_flops(K: int) -> int:
+    """Real FP32 instructions of the butterflies of one K-point FFT bank frame (xlg_bank_fft_flops)."""
+    return int(lib().xlg_bank_fft_flops(K))
+
+
+def subband_plan(fs: int, clients, bank: bool = False, fft: bool = False):
     """Sub-band clients for `clients`, a list of (center, rate).  For every D1 >= 2 that divides fs with
     fs1 = fs / D1 even, fs1 > 2 * max rate and every rate dividing fs1: sub-band centres fs1 / 2 apart from
     the lowest client centre up across the occupied span, each client assigned to the nearest one (so its
@@ -815,7 +855,13 @@ def subband_plan(fs: int, clients, bank: bool = False):
     entry also carries its "channel" k in [-D1, D1) (j wrapped: the channel at +fs / 2 is the one at -fs / 2,
     and a member's offset stays relative to its own grid point), a D1 whose bank the kernel would refuse (bank_fits) is skipped, and the first stage costs
     2 * T1 / D1 + 8 * C FMAs per input sample (one polyphase pass, C channel sums of K complex MACs per frame)
-    instead of 4 * T1 / D1 per sub-band."""
+    instead of 4 * T1 / D1 per sub-band.
+
+    fft=True (with bank=True) also considers FFT banks (Group.add_bank_fft) where bank_fft_fits: their channel
+    stage costs bank_fft_flops(K) / D1 per input sample instead of 8 * C.  At each D1 the cheaper kernel is
+    taken (the direct one on a tie), and the plan carries "kernel": "direct" or "fft"."""
+    if fft and not bank:
+        raise ValueError("fft=True plans banks: it needs bank=True")
     centers = [int(c) for c, _ in clients]
     rates = [int(r) for _, r in clients]
     rmax = max(rates)
@@ -838,14 +884,19 @@ def subband_plan(fs: int, clients, bank: bool = False):
             half = fs1 // 2
             e = fs1 // 4 + rmax // 2
             t1 = create_low_pass_filter(1.0, fs, fs1 // 2, fs1 - 2 * e)
+            kernel = None
             if bank:
-                if not bank_fits(d1, t1.size):
-                    continue
                 base = 0  # the grid j * half, j = round(c / half), and j's channel
                 grid = [(2 * c + half) // (2 * half) for c in centers]
                 assign = [(j + d1) % (2 * d1) - d1 for j in grid]
                 used = sorted(set(assign))
-                cost = 2.0 * t1.size / d1 + 8.0 * len(used) + subband_fmas(
+                stages = [(8.0 * len(used), "direct")] if bank_fits(d1, t1.size) else []
+                if fft and bank_fft_fits(d1, t1.size):
+                    stages.append((bank_fft_flops(2 * d1) / d1, "fft"))
+                if not stages:
+                    continue
+                stage, kernel = min(stages, key=lambda c: c[0])  # (a tie keeps the direct bank)
+                cost = 2.0 * t1.size / d1 + stage + subband_fmas(
                     fs, d1, t1.size, 0, [(r, shapes[r][2].size, shapes[r][0]) for r in rates])
             else:
                 base = lo
@@ -855,18 +906,21 @@ def subband_plan(fs: int, clients, bank: bool = False):
                 used = sorted(set(assign))
                 cost = subband_fmas(fs, d1, t1.size, len(used), [(r, shapes[r][2].size, shapes[r][0]) for r in rates])
             if best is None or cost < best[0]:
-                best = (cost, d1, fs1, half, e, t1, shapes, used, assign, base, grid)
+                best = (cost, d1, fs1, half, e, t1, shapes, used, assign, base, grid, kernel)
         if best is not None:
             break
     if best is None:
         raise ValueError(f"{fs} has no divisor D1 >= 2 whose sub-band rate serves the rates {sorted(set(rates))}")
-    cost, d1, fs1, half, e, t1, shapes, used, assign, base, grid = best
+    cost, d1, fs1, half, e, t1, shapes, used, assign, base, grid, kernel = best
     index = {k: i for i, k in enumerate(used)}
     subbands = [{"center": base + k * half, "channel": k} if bank else {"center": base + k * half} for k in used]
     members = [{"subband": index[k], "center": c, "rate": r, "interp2": shapes[r][0], "d2": shapes[r][1],
                 "offset": c - (base + (grid[i] if bank else k) * half), "taps2": shapes[r][2]}
                for i, (c, r, k) in enumerate(zip(centers, rates, assign))]
-    return {"d1": d1, "fs1": fs1, "taps1": t1, "e": e, "subbands": subbands, "members": members, "fmas": cost}
+    plan = {"d1": d1, "fs1": fs1, "taps1": t1, "e": e, "subbands": subbands, "members": members, "fmas": cost}
+    if fft:
+        plan["kernel"] = kernel
+    return plan
 
 
 # ---------------------------------------------------------------------------

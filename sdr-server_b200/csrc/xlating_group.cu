@@ -133,16 +133,17 @@ struct HostClient {
   int sb_cid = -1;               // its sub-band's client index
   long long zb2 = 0;             // sub-band position of its attach point: earlier samples read as zero
   int ph_row = 0;                // its rows of the slot's member oscillator table
-  // bank channel (xlg_add_bank_subband): a sub-band (sb) whose row bank_cf32_kernel writes; D and T are its
+  // bank channel (xlg_add_bank_subband): a sub-band (sb) whose row its bank's kernel writes; D and T are its
   // bank's, and it is not an integer client (inactive ClientDev, no oscillator, no tap row)
   int bank = -1;                 // its bank's id
   int chan = 0;                  // its channel k in [-D1, D1)
 };
 
-// a channel bank (xlg_add_bank): reversed padded taps, twiddles, and the walk of an integer client (D1, T1)
-// attached at P
+// a channel bank (xlg_add_bank, xlg_add_bank_fft): reversed padded taps, twiddles, and the walk of an integer
+// client (D1, T1) attached at P
 struct BankHost {
   bool active = false;
+  bool fft = false;          // its channel stage: bank_fft_cf32_kernel instead of bank_cf32_kernel
   uint32_t D1 = 0;
   size_t T1 = 0;
   int K = 0, tpad = 0;
@@ -190,7 +191,9 @@ struct BlkTable {
 
 // Timed spans of a block: each has a begin and an end event per slot.  Profiling records every span; the
 // timeline (XLATING_B200_TIMELINE) records the convert and tile spans too.
-enum Span { SP_CONV, SP_PHASE, SP_TILE, SP_GEN, SP_LONG, SP_POLY_GEN, SP_POLY_TILE, SP_STAGE_B, SP_SB, SP_BANK, SP_N };
+enum Span {
+  SP_CONV, SP_PHASE, SP_TILE, SP_GEN, SP_LONG, SP_POLY_GEN, SP_POLY_TILE, SP_STAGE_B, SP_SB, SP_BANK, SP_BANK_FFT, SP_N
+};
 
 struct Slot {
   void *d_raw = nullptr, *h_raw = nullptr;
@@ -221,6 +224,8 @@ struct Slot {
   uint64_t sb_macs = 0, sb_rows = 0;
   BlkTable<BankBlk> bkblk;       // banks with channels: this block's windows, counts and channel tables
   uint64_t bk_poly = 0, bk_dft = 0;
+  BlkTable<BankBlk> bfblk;       // the same for the FFT banks
+  uint64_t bf_poly = 0, bf_flops = 0;
   std::atomic<int64_t> ticket{-1};
   bool q15 = false;
   bool harvested = true;
@@ -464,6 +469,7 @@ struct xlg_group {
   int2 *d_bkch = nullptr;
   size_t cap_bktaps = 0, cap_bktw = 0, cap_bkch = 0;
   xlg_bank_profile bank_prof;
+  xlg_bank_fft_profile bank_fft_prof;
   int n_generic = 0;
   int max_client = 0;     // highest active id + 1
   bool dirty = true;
@@ -575,6 +581,7 @@ static void slot_free(Slot &s) {
   s.sbcb.release();
   s.sbblk.release();
   s.bkblk.release();
+  s.bfblk.release();
   if (s.d_sbph) cudaFree(s.d_sbph);
   s.d_sbph = nullptr;
   s.d_pscratch = nullptr;
@@ -644,7 +651,8 @@ static void harvest_locked(xlg_group *g, Slot &s) {
       {&g->poly_prof.fir_poly_tile_ms, &g->poly_prof.fir_poly_tile_launches},
       {&g->casc_prof.stage_b_ms, &g->casc_prof.stage_b_launches},
       {&g->sb_prof.member_ms, &g->sb_prof.member_launches},
-      {&g->bank_prof.bank_ms, &g->bank_prof.bank_launches}};
+      {&g->bank_prof.bank_ms, &g->bank_prof.bank_launches},
+      {&g->bank_fft_prof.fft_ms, &g->bank_fft_prof.fft_launches}};
   for (int sp = 0; sp < SP_N; sp++) {
     float ms = 0;
     if (s.pf_on[sp] && cudaEventElapsedTime(&ms, s.pf[sp][0], s.pf[sp][1]) == cudaSuccess) {
@@ -659,6 +667,8 @@ static void harvest_locked(xlg_group *g, Slot &s) {
   g->sb_prof.row_samples += s.sb_rows;
   g->bank_prof.poly_macs += s.bk_poly;
   g->bank_prof.dft_macs += s.bk_dft;
+  g->bank_fft_prof.poly_macs += s.bf_poly;
+  g->bank_fft_prof.butterfly_flops += s.bf_flops;
   g->prof.blocks++;
   g->prof.out_samples += s.out_samples;
   g->prof.in_samples += s.in_samples;
@@ -868,10 +878,21 @@ static int rebuild_subbands(xlg_group *g, size_t &out_total) {
   return 0;
 }
 
+// Where channel k of an FFT bank lies in its transformed row (bank_fft_cf32_kernel): the digit reversal of
+// k mod K, one base-4 digit per radix-4 stage (the first stage's digit is the most significant), then the radix-2
+// stage's bit
+static int bank_fft_pos(int k, int K) {
+  int pos = 0, L = K;
+  k = (k % K + K) % K;
+  for (; L >= 4; L >>= 2, k >>= 2) pos += (k & 3) * (L >> 2);
+  return L == 2 ? pos + (k & 1) : pos;
+}
+
 // Banks (the pipeline is drained, the channels' rows are placed): one arena each for the taps, the twiddles and
 // the channel tables of the banks that have channels, and the per-slot tables.
 static int rebuild_banks(xlg_group *g) {
   g->bank_live.clear();
+  size_t n_fft = 0;
   std::vector<float> taps;
   std::vector<float2> tw;
   std::vector<int2> chans;
@@ -883,7 +904,11 @@ static int rebuild_banks(xlg_group *g) {
       if (g->clients[i].active && g->clients[i].bank == b) k.cids.push_back(i);
     if (k.cids.empty()) continue;
     k.ch_off = (int)chans.size();
-    for (int i : k.cids) chans.push_back(make_int2((g->clients[i].chan + k.K) % k.K, g->clients[i].out_off));
+    for (int i : k.cids) {
+      const int c = g->clients[i].chan;
+      chans.push_back(make_int2(k.fft ? bank_fft_pos(c, k.K) : (c + k.K) % k.K, g->clients[i].out_off));
+    }
+    n_fft += k.fft ? 1 : 0;
     k.taps_off = (int)taps.size();
     taps.insert(taps.end(), k.taps.begin(), k.taps.end());
     k.tw_off = (int)tw.size();
@@ -897,7 +922,7 @@ static int rebuild_banks(xlg_group *g) {
       dev_assign(&g->d_bkch, &g->cap_bkch, chans.data(), chans.size() * sizeof(int2)))
     return -EIO;
   for (Slot &s : g->slots)
-    if (s.bkblk.reserve(g->bank_live.size())) return -EIO;
+    if (s.bkblk.reserve(g->bank_live.size() - n_fft) || s.bfblk.reserve(n_fft)) return -EIO;
   return 0;
 }
 
@@ -1120,7 +1145,7 @@ static int rebuild_layout(xlg_group *g) {
       continue;
     }
     if (h.bank >= 0) {
-      h.kind = 7;  // a bank channel: bank_cf32_kernel writes its row
+      h.kind = g->banks[h.bank].fft ? 8 : 7;  // a bank channel: bank_cf32_kernel (8: bank_fft_cf32_kernel) writes it
       continue;
     }
     h.kind = h.L > 1 ? 3 : 0;
@@ -1630,6 +1655,7 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
   memset(&g->casc_prof, 0, sizeof(g->casc_prof));
   memset(&g->sb_prof, 0, sizeof(g->sb_prof));
   memset(&g->bank_prof, 0, sizeof(g->bank_prof));
+  memset(&g->bank_fft_prof, 0, sizeof(g->bank_fft_prof));
   g->device = device;
   g->fs = sampling_freq;
   g->max_input_len = max_input_len;
@@ -2181,27 +2207,41 @@ extern "C" int xlg_subband_info(const xlg_group *g, int client_id, int *subband_
   return 0;
 }
 
-extern "C" int xlg_add_bank(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, int *bank_id) {
+// A bank (fft: its channel stage is bank_fft_cf32_kernel's) after the checks of its kernel
+static int add_bank(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, bool fft, int *bank_id) {
+  const char *what = fft ? "FFT bank" : "bank";
   if (g == nullptr || bank_id == nullptr) return -EINVAL;
   if (decim1 == 0 || taps1_len == 0 || taps1 == nullptr) {
-    XL_LOG("bank: decimation %u and tap count %zu must both be at least 1", decim1, taps1_len);
+    XL_LOG("%s: decimation %u and tap count %zu must both be at least 1", what, decim1, taps1_len);
     return -EINVAL;
   }
   if (decim1 > (uint32_t)(INT32_MAX / 2) || g->fs % (2 * decim1) != 0) {
-    XL_LOG("bank: 2 x decimation %u does not divide the band rate %u (channel centres are in Hz at fs / %u)", decim1,
-           g->fs, 2 * decim1);
+    XL_LOG("%s: 2 x decimation %u does not divide the band rate %u (channel centres are in Hz at fs / %u)", what,
+           decim1, g->fs, 2 * decim1);
     return -EINVAL;
   }
-  if (taps1_len > (size_t)INT32_MAX / 8 || bank_smem((int)decim1, (int)taps1_len) > (size_t)kTileMaxSmem) {
+  if (fft) {
+    const uint32_t K = 2 * decim1;
+    if ((K & (K - 1)) != 0 || K > 4096) {
+      XL_LOG("FFT bank: K = 2 x decimation %u = %u is not a power of two up to 4096", decim1, K);
+      return -EINVAL;
+    }
+    if (taps1_len > (size_t)bank_fft_max_taps((int)K)) {
+      XL_LOG("FFT bank: %zu taps at decimation %u exceed the kernel's bound of %lld", taps1_len, decim1,
+             bank_fft_max_taps((int)K));
+      return -EINVAL;
+    }
+  } else if (taps1_len > (size_t)INT32_MAX / 8 || bank_smem((int)decim1, (int)taps1_len) > (size_t)kTileMaxSmem) {
     XL_LOG("bank: %zu taps at decimation %u exceed the bank kernel's shared memory", taps1_len, decim1);
     return -EINVAL;
   }
   if (g->flags & XLG_TRACK_STATE) {
-    XL_LOG("bank: an XLG_TRACK_STATE group cannot carry the state of two stages");
+    XL_LOG("%s: an XLG_TRACK_STATE group cannot carry the state of two stages", what);
     return -ENOTSUP;
   }
   BankHost k;
   k.active = true;
+  k.fft = fft;
   k.D1 = decim1;
   k.T1 = taps1_len;
   k.K = 2 * (int)decim1;
@@ -2226,6 +2266,20 @@ extern "C" int xlg_add_bank(xlg_group *g, uint32_t decim1, const float *taps1, s
   g->dirty = true;  // the input ring's history bound
   *bank_id = id;
   return 0;
+}
+
+extern "C" int xlg_add_bank(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, int *bank_id) {
+  return add_bank(g, decim1, taps1, taps1_len, false, bank_id);
+}
+
+extern "C" int xlg_add_bank_fft(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, int *bank_id) {
+  return add_bank(g, decim1, taps1, taps1_len, true, bank_id);
+}
+
+extern "C" uint64_t xlg_bank_fft_flops(uint32_t K) {
+  uint64_t n = 0, L = K;
+  for (; L >= 4; L >>= 2) n += (uint64_t)K / 4 * 28;  // radix 4: 16 adds, 3 products of 4 instructions
+  return L == 2 ? n + (uint64_t)K / 2 * 4 : n;        // radix 2: 4 adds
 }
 
 static BankHost *bank_of(xlg_group *g, int bank_id) {
@@ -2334,6 +2388,8 @@ struct Block {
   // bank walk
   int n_bk = 0, max_bk_n1 = 0, max_bk_cg = 0;
   size_t bk_smem = 0;
+  int n_bf = 0, max_bf_ctas = 0;  // FFT banks
+  size_t bf_smem = 0;
   // sub-band walk
   int n_sb = 0, max_sb_n1 = 0, max_sb_n2 = 0;
   int max_sbr_ctas = 0, max_sbr_l2 = 0;  // rational classes: output tiles of the longest residue, largest L2
@@ -2399,6 +2455,7 @@ static void walk_banks(Block &b) {
   xlg_group *g = b.g;
   Slot &s = b.s;
   s.bk_poly = s.bk_dft = 0;
+  s.bf_poly = s.bf_flops = 0;
   for (int bi = 0; bi < (int)g->banks.size(); bi++) {
     BankHost &k = g->banks[bi];
     if (!k.active) continue;
@@ -2410,7 +2467,7 @@ static void walk_banks(Block &b) {
       b.ho.out_off[i] = g->clients[i].out_off;
     }
     if (k.cids.empty()) continue;
-    BankBlk &e = s.bkblk.h[b.n_bk++];
+    BankBlk &e = k.fft ? s.bfblk.h[b.n_bf++] : s.bkblk.h[b.n_bk++];
     e.taps = g->d_bktaps + k.taps_off;
     e.tw = g->d_bktw + k.tw_off;
     e.chans = g->d_bkch + k.ch_off;
@@ -2424,6 +2481,13 @@ static void walk_banks(Block &b) {
     e.tpad = k.tpad;
     e.n_ch = (int)k.cids.size();
     e.r0 = (int)(((first - k.P) % k.K + k.K) % k.K);
+    if (k.fft) {
+      b.max_bf_ctas = std::max(b.max_bf_ctas, (n1 + bank_fft_frames(k.K) - 1) / bank_fft_frames(k.K));
+      b.bf_smem = std::max(b.bf_smem, bank_fft_smem(k.K));
+      s.bf_poly += (uint64_t)n1 * k.T1;
+      s.bf_flops += (uint64_t)n1 * xlg_bank_fft_flops((uint32_t)k.K);
+      continue;
+    }
     b.max_bk_n1 = std::max(b.max_bk_n1, n1);
     b.max_bk_cg = std::max(b.max_bk_cg, (e.n_ch + BK_CG - 1) / BK_CG);
     b.bk_smem = std::max(b.bk_smem, bank_smem((int)k.D1, (int)k.T1));
@@ -2555,16 +2619,23 @@ static int stage_and_convert(Block &b, int fmt, const void *input, uint32_t flag
   return 0;
 }
 
-// Banks: after the conversions the FIR kernels wait for, not after the pre-pass (they have no oscillator)
+// Banks: after the conversions the FIR kernels wait for, not after the pre-pass (they have no oscillator); the
+// direct banks, then the FFT banks
 static int launch_banks(Block &b) {
   xlg_group *g = b.g;
   Slot &s = b.s;
-  if (b.n_bk == 0 || b.max_bk_n1 <= 0) return 0;
-  if (span_begin(g, s, SP_BANK, b.cs)) return -EIO;
-  CU_OK(s.bkblk.upload((size_t)b.n_bk, b.cs));
-  bank_cf32_kernel<<<dim3((b.max_bk_n1 + BK_F - 1) / BK_F, b.n_bk, b.max_bk_cg), BK_THREADS, b.bk_smem, b.cs>>>(
-      s.bkblk.d, g->ring, s.d_out);
-  return span_end(g, s, SP_BANK, b.cs);
+  if (b.n_bk > 0 && b.max_bk_n1 > 0) {
+    if (span_begin(g, s, SP_BANK, b.cs)) return -EIO;
+    CU_OK(s.bkblk.upload((size_t)b.n_bk, b.cs));
+    bank_cf32_kernel<<<dim3((b.max_bk_n1 + BK_F - 1) / BK_F, b.n_bk, b.max_bk_cg), BK_THREADS, b.bk_smem, b.cs>>>(
+        s.bkblk.d, g->ring, s.d_out);
+    if (span_end(g, s, SP_BANK, b.cs)) return -EIO;
+  }
+  if (b.n_bf == 0 || b.max_bf_ctas <= 0) return 0;
+  if (span_begin(g, s, SP_BANK_FFT, b.cs)) return -EIO;
+  CU_OK(s.bfblk.upload((size_t)b.n_bf, b.cs));
+  bank_fft_cf32_kernel<<<dim3(b.max_bf_ctas, b.n_bf), BF_THREADS, b.bf_smem, b.cs>>>(s.bfblk.d, g->ring, s.d_out);
+  return span_end(g, s, SP_BANK_FFT, b.cs);
 }
 
 // Oscillator pre-pass (own stream: chains only on the previous pre-pass; none without a client to walk), and the
@@ -3283,6 +3354,10 @@ extern "C" int xlg_subband_profile_read(xlg_group *g, xlg_subband_profile *p, in
 
 extern "C" int xlg_bank_profile_read(xlg_group *g, xlg_bank_profile *p, int reset) {
   return family_profile_read(g, &xlg_group::bank_prof, p, reset);
+}
+
+extern "C" int xlg_bank_fft_profile_read(xlg_group *g, xlg_bank_fft_profile *p, int reset) {
+  return family_profile_read(g, &xlg_group::bank_fft_prof, p, reset);
 }
 
 extern "C" int xlg_profile_read(xlg_group *g, xlg_profile *p, int reset) {

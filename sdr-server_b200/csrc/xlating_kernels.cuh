@@ -1673,4 +1673,93 @@ bank_cf32_kernel(const BankBlk *__restrict__ blk, const float2 *__restrict__ rin
   }
 }
 
+// ---------------------------------------------------------------------------
+// FFT bank sub-bands (xlg_add_bank_fft).  The channels are the bank's above; only the channel stage differs: a
+// K-point FFT, K = 2 * D1 a power of two up to 4096.  Phase 1's sums v[m][p] (p < min(K, T1), the direct bank's
+// two fmaf chains over q ascending from +0; zero for T1 <= p < K) are placed at u[(p + r_m) mod K], an exact
+// permutation, so that
+//     y_k[m] = sum_{p < K} u[p] * W[(k p) mod K]
+// which a decimation-in-frequency FFT computes in place: radix-4 stages at lengths L = K, K/4, ... while L >= 4,
+// then one radix-2 stage at L = 2 when log2 K is odd.  The radix-4 butterfly at length L, for every block of L
+// and j < L/4, reads a_q = u[b + j + q L/4] and writes (component-wise float adds, in this order)
+//     t0 = a0 + a2, t1 = a0 - a2, t2 = a1 + a3, t3 = a1 - a3
+//     y0 = t0 + t2, y1 = (t1.x + t3.y, t1.y - t3.x), y2 = t0 - t2, y3 = (t1.x - t3.y, t1.y + t3.x)
+//     u[b + j + q L/4] = y0 for q = 0, y_q * W[q j K / L] for q = 1, 2, 3
+// the radix-2 butterfly (a0, a1) -> (a0 + a1, a0 - a1), and every product y * w is
+//     (fmaf(-y.y, w.y, y.x * w.x), fmaf(y.y, w.x, y.x * w.y))     (rounded products, no contraction)
+// W is the direct bank's table read at stride K / L, so the quarter turns stay exact.  Channel k then lies at
+// the digit reversal of k mod K (bank_fft_pos in xlating_group.cu), which the channel table carries.
+// ---------------------------------------------------------------------------
+constexpr int BF_THREADS = 256;
+constexpr int BF_N = 2048;  // sums per CTA: BF_N / K frames, one frame at K = 4096
+__host__ __device__ constexpr int bank_fft_frames(int K) { return K >= BF_N ? 1 : BF_N / K; }
+__host__ __device__ constexpr size_t bank_fft_smem(int K) { return (size_t)bank_fft_frames(K) * K * 8; }
+// taps: a phase's chain is at most max(16, 16384 / K) terms long
+__host__ __device__ constexpr long long bank_fft_max_taps(int K) { return 16LL * K > 16384 ? 16LL * K : 16384; }
+
+__device__ __forceinline__ float2 cmul_tw(float2 y, float2 w) {
+  return make_float2(fmaf(-y.y, w.y, __fmul_rn(y.x, w.x)), fmaf(y.y, w.x, __fmul_rn(y.x, w.y)));
+}
+
+// CTA (x, b) computes frames [x F, x F + F) of bank b, F = bank_fft_frames(K): the rotated sums of each frame in
+// a row of K in shared memory (taps and window read through the L1: T1 is too long to stage), the FFT of every
+// row, then the materialised channels' samples, a channel's frames consecutively.  chans[c].x is the channel's
+// position in the transformed row.
+__global__ void __launch_bounds__(BF_THREADS)
+bank_fft_cf32_kernel(const BankBlk *__restrict__ blk, const float2 *__restrict__ ring, float2 *__restrict__ out) {
+  extern __shared__ __align__(16) float2 u[];
+  const BankBlk b = blk[blockIdx.y];
+  const int K = b.K, F = bank_fft_frames(K);
+  const int f0 = blockIdx.x * F;
+  if (f0 >= b.n1) return;
+  const int nf = min(F, b.n1 - f0), T1 = b.T1, tid = threadIdx.x;
+  const int lk = 31 - __clz(K);
+  for (int e = tid; e < nf * K; e += BF_THREADS) {
+    const int f = e >> lk, p = e & (K - 1);
+    const long long w = b.first + (long long)(f0 + f) * b.D1;
+    float2 acc = make_float2(0.f, 0.f);
+    for (int j = p; j < T1; j += K) {
+      const long long pos = w + j;
+      const float2 xv = pos < b.zb ? make_float2(0.f, 0.f) : ring[(unsigned)((unsigned long long)pos) & b.mask];
+      const float hv = __ldg(b.taps + j);
+      acc.x = fmaf(xv.x, hv, acc.x);
+      acc.y = fmaf(xv.y, hv, acc.y);
+    }
+    const int r = (int)(((long long)b.r0 + (long long)(f0 + f) * b.D1) & (K - 1));
+    u[(f << lk) + ((p + r) & (K - 1))] = acc;
+  }
+  __syncthreads();
+  int L = K;
+  for (; L >= 4; L >>= 2) {
+    const int q4 = L >> 2, s = K / L;
+    for (int e = tid; e < nf * (K >> 2); e += BF_THREADS) {
+      const int f = e >> (lk - 2), i = e & ((K >> 2) - 1), j = i & (q4 - 1);
+      float2 *x = u + (f << lk) + 4 * (i - j) + j;
+      const float2 a0 = x[0], a1 = x[q4], a2 = x[2 * q4], a3 = x[3 * q4];
+      const float2 t0 = make_float2(a0.x + a2.x, a0.y + a2.y), t1 = make_float2(a0.x - a2.x, a0.y - a2.y);
+      const float2 t2 = make_float2(a1.x + a3.x, a1.y + a3.y), t3 = make_float2(a1.x - a3.x, a1.y - a3.y);
+      x[0] = make_float2(t0.x + t2.x, t0.y + t2.y);
+      x[q4] = cmul_tw(make_float2(t1.x + t3.y, t1.y - t3.x), __ldg(b.tw + j * s));
+      x[2 * q4] = cmul_tw(make_float2(t0.x - t2.x, t0.y - t2.y), __ldg(b.tw + 2 * j * s));
+      x[3 * q4] = cmul_tw(make_float2(t1.x - t3.y, t1.y + t3.x), __ldg(b.tw + 3 * j * s));
+    }
+    __syncthreads();
+  }
+  if (L == 2) {
+    for (int e = tid; e < nf * (K >> 1); e += BF_THREADS) {
+      float2 *x = u + 2 * e;
+      const float2 a0 = x[0], a1 = x[1];
+      x[0] = make_float2(a0.x + a1.x, a0.y + a1.y);
+      x[1] = make_float2(a0.x - a1.x, a0.y - a1.y);
+    }
+    __syncthreads();
+  }
+  for (int e = tid; e < b.n_ch * F; e += BF_THREADS) {
+    const int c = e / F, f = e - c * F;
+    if (f >= nf) continue;
+    const int2 ch = b.chans[c];
+    out[ch.y + f0 + f] = u[(f << lk) + ch.x];
+  }
+}
+
 }  // namespace xl

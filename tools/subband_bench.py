@@ -2,7 +2,7 @@
 (xlg_add_bank + xlg_add_bank_subband) against single-stage and per-client cascade clients of the same centres
 and rates.
 
-    python tools/subband_bench.py [--blocks K] [--warmup W] [--rounds R] [--only NAME] [--plans P,...]
+    python tools/subband_bench.py [--blocks K] [--warmup W] [--rounds R] [--only NAME,...] [--plans P,...]
 
 Workloads (centres drawn uniformly across the band from a fixed seed):
   61M_1024   1024 clients at 48 kHz on a 61.44 Msps cs16 stream
@@ -13,14 +13,15 @@ Workloads (centres drawn uniformly across the band from a fixed seed):
   20M_256    256 clients at 48 kHz on a 20 Msps cs8 stream (HackRF)
 Plans, alternated within every round: "single" (one client each: client_plan's taps as an integer client, or
 rational_plan's as a rational client where the rate does not divide fs), "cascade" (cascade_plan) and
-"subband" (subband_plan; at the last three rates its members resample by a rational L2 / M2) and "bank"
-(subband_plan(bank=True): the same kind of members on the channels of one bank).
+"subband" (subband_plan; at the last three rates its members resample by a rational L2 / M2), "bank"
+(subband_plan(bank=True): the same kind of members on the channels of one bank) and "bank_fft"
+(subband_plan(bank=True, fft=True): the same with a direct or an FFT bank, whichever the planner costs lower).
 
 Per workload and plan (one JSON line each): input MS/s and step time over K pipelined blocks (CUDA events,
 xlg_timer_*), algorithmic real FMAs per input sample from the shapes, and from a profiled run of its own (one
 compute stream, CUDA events around each launch) the time per block of the oscillator pre-pass, the integer
 FIR kernels, the cascades' stage B and the sub-band members' work (ring appends, member oscillators and
-member kernel) and the bank kernel.  Every run checks its last timed block of sampled clients against the tests' oracles (1e-5
+member kernel), the bank kernel and the FFT bank kernel.  Every run checks its last timed block of sampled clients against the tests' oracles (1e-5
 norm-wise; a bank's members against the float64 bank rows fed to the reference's float path, since the bank
 has no float oscillator to share with an oracle).  Blocks are 262144 bytes, as in bench.py.  The card's name and power limit are printed first,
 read in the same call.  Nothing is written to the tree.
@@ -48,7 +49,7 @@ WORKLOADS = {  # fs, format, clients, rates
     "10M_256": (10000000, "cs16", 256, (48000,)),
     "20M_256": (20000000, "cs8", 256, (48000,)),
 }
-PLANS = ("single", "cascade", "subband", "bank")
+PLANS = ("single", "cascade", "subband", "bank", "bank_fft")
 SAMPLED = 3
 
 
@@ -74,6 +75,7 @@ def build(name, plan, profile):
     g = pkg.Group(fs, BLOCK)
     picks = [0, n // 2, n - 1]
     oracles = []
+    shape = {}
     if plan == "single" and any(fs % r for _, r in clients):
         rp = pkg.rational_plan(fs, [r for _, r in clients])
         ids = [g.add_client_rational(q["interp"], q["decim"], q["taps"], c) for q, (c, _) in zip(rp, clients)]
@@ -102,9 +104,13 @@ def build(name, plan, profile):
                  if p["interp2"] > 1 else cascade_oracle(p["d1"], p["taps1"], c, p["d2"], p["taps2"], fs, BLOCK))
             oracles.append((ids[k], lambda x, o=o: o.process_cf32(fmt, x)))
     else:
-        p = pkg.subband_plan(fs, clients, bank=plan == "bank")
-        if plan == "bank":
-            bid = g.add_bank(p["d1"], p["taps1"])
+        banked = plan in ("bank", "bank_fft")
+        p = (pkg.subband_plan(fs, clients, bank=True, fft=True) if plan == "bank_fft" else
+             pkg.subband_plan(fs, clients, bank=banked))
+        shape = {"d1": p["d1"], "subbands": len(p["subbands"]), "kernel": p.get("kernel")}
+        if banked:
+            add = g.add_bank_fft if p.get("kernel") == "fft" else g.add_bank
+            bid = add(p["d1"], p["taps1"])
             sids = [g.add_bank_subband(bid, sb["channel"]) for sb in p["subbands"]]
         else:
             sids = [g.add_subband(p["d1"], p["taps1"], sb["center"]) for sb in p["subbands"]]
@@ -113,7 +119,7 @@ def build(name, plan, profile):
         fmas = p["fmas"]
         for k in picks:
             m = p["members"][k]
-            if plan == "bank":
+            if banked:
                 o = BankMemberOracle(p["d1"], p["taps1"], p["subbands"][m["subband"]]["channel"], m["d2"], m["taps2"],
                                      m["offset"], m["interp2"], fs)
                 oracles.append((ids[k], lambda x, o=o: o.process_cf32(fmt, x)))
@@ -123,7 +129,7 @@ def build(name, plan, profile):
             oracles.append((ids[k], lambda x, o=o: o.process_cf32(fmt, x)[0]))
     if profile:
         g.profile_enable(True)
-    return g, ids, fmas, oracles
+    return g, ids, fmas, oracles, shape
 
 
 def run(name, plan, blocks, warmup):
@@ -132,9 +138,9 @@ def run(name, plan, blocks, warmup):
     dtype = pkg.NP_DTYPE[fmt]
     elems = BLOCK // np.dtype(dtype).itemsize
     data = [rng.integers(np.iinfo(dtype).min, np.iinfo(dtype).max, elems, dtype=dtype, endpoint=True) for _ in range(4)]
-    g, ids, fmas, oracles = build(name, plan, False)
+    g, ids, fmas, oracles, shape = build(name, plan, False)
     res = {"workload": name, "plan": plan, "fs": fs, "fmt": fmt, "clients": n, "blocks": blocks,
-           "fmas_per_input_sample": fmas}
+           "fmas_per_input_sample": fmas, **shape}
     for i in range(warmup):
         g.wait(g.submit(fmt, data[i % 4]))
     g.timer_start()
@@ -155,14 +161,16 @@ def run(name, plan, blocks, warmup):
     assert worst <= 1e-5, (name, plan, worst)
     res["checked_error"] = worst
     g.close()
-    g, ids, _, _ = build(name, plan, True)
+    g, ids, _, _, _ = build(name, plan, True)
     for i in range(warmup):
         g.wait(g.submit(fmt, data[i % 4]))
-    for read in (g.profile_read, g.cascade_profile_read, g.subband_profile_read, g.bank_profile_read):
+    for read in (g.profile_read, g.cascade_profile_read, g.subband_profile_read, g.bank_profile_read,
+                 g.bank_fft_profile_read):
         read(reset=True)
     for i in range(blocks):
         g.wait(g.submit(fmt, data[i % 4]))
     prof, cp, sp, bp = g.profile_read(), g.cascade_profile_read(), g.subband_profile_read(), g.bank_profile_read()
+    fp = g.bank_fft_profile_read()
     g.close()
     per = max(prof["blocks"], 1)
     res["phase_ms_per_block"] = prof["phase_ms"] / per
@@ -170,6 +178,7 @@ def run(name, plan, blocks, warmup):
     res["stage_b_ms_per_block"] = cp["stage_b_ms"] / per
     res["member_ms_per_block"] = sp["member_ms"] / per
     res["bank_ms_per_block"] = bp["bank_ms"] / per
+    res["fft_ms_per_block"] = fp["fft_ms"] / per
     return res
 
 
@@ -178,13 +187,13 @@ def main():
     ap.add_argument("--blocks", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=2)
-    ap.add_argument("--only", default=None, help="one workload")
+    ap.add_argument("--only", default=None, help="workloads, comma-separated")
     ap.add_argument("--plans", default=",".join(PLANS), help="plans to alternate, comma-separated")
     args = ap.parse_args()
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
                           capture_output=True, text=True).stdout.strip().splitlines()[0]
     print(json.dumps({"card": card}), flush=True)
-    names = [args.only] if args.only else list(WORKLOADS)
+    names = args.only.split(",") if args.only else list(WORKLOADS)
     for r in range(args.rounds):
         for name in names:
             for plan in args.plans.split(","):
