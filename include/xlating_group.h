@@ -64,6 +64,9 @@ enum { XLG_FMT_CU8 = 0, XLG_FMT_CS8 = 1, XLG_FMT_CS16 = 2 };
                                    be reused as soon as xlg_submit returns, exactly like a pageable one (which
                                    is staged through the group's own pinned buffer with a memcpy). */
 
+/* xlg_add_spectrum flags */
+#define XLG_SPECTRUM_POWER 0x1u /* rows of linear power v instead of the reference's 10 * log10f(v) dB */
+
 /* depth of the device pipeline (blocks in flight).  Outputs of ticket t stay valid
  * until ticket t + XLG_SLOTS (or t + host_ring, see xlg_create_ex) is submitted;
  * after that xlg_wait / xlg_output return -ESTALE. */
@@ -230,6 +233,40 @@ int xlg_add_bank_fft(xlg_group *g, uint32_t decim1, const float *taps1, size_t t
 /* Real FP32 instructions of the butterflies of one K-point FFT bank frame (K a power of two): 28 per radix-4
  * butterfly (16 adds and 3 complex products of 4), 4 per radix-2 butterfly.  The planner costs FFT banks by it. */
 uint64_t xlg_bank_fft_flops(uint32_t K);
+/* Extension: spectrum rows (DESIGN.md section 5, "Spectrum rows"): the reference spectrogram tool's rows
+ * (src/spectrogram/spectrogram.c) of the band, served beside the clients.
+ *   A spectrum of width W, frames_per_row F and skip_per_row S attached before the next submitted block, at
+ *   stream position P, has period R = F * W + S.  Row r covers the F frames x[P + r R + f W ... + W), f < F; no
+ *   frame reads before P.  For each frame, X = DFT_W(frame), c = X * (1/W) (1/W rounded to float once) and
+ *   p = c.re^2 + c.im^2 + 1e-20f; the row's value per bin is the max of p over its F frames.  The row is then
+ *   half swapped as spectrogram.c:156-163 does: for j < W/2 (rounded down) out[j] = v[W/2 + j] and
+ *   out[W/2 + j] = v[j]; for odd W out[W-1] = v[W-1] (not a true fftshift).  Each value is 10 * log10f(v), the
+ *   reference's dB row, or v itself with XLG_SPECTRUM_POWER.  The reference tool's rows are F = fs / W and
+ *   S = fs % W; its png_util_set_data turns a dB row into 8-bit grey with (int)(dB + 255) clamped to [0, 255].
+ *   A row is returned with the ticket whose block holds the row's last frame sample: a block completes zero,
+ *   one or many rows, and a row spans as many blocks as it needs.  Removing a spectrum drops its partial row.
+ *   W a power of two from 4 to 4096 runs an FFT per frame; any other W a direct DFT of W complex MACs per input
+ *   sample.  Spectrum ids come from a small-integer space of their own; xlg_client_count does not count them.
+ *   -EINVAL (logged) for W = 0 or above 4096, F = 0, R >= 2^31 or an unknown flag; -ENOTSUP (logged) on an
+ *   XLG_TRACK_STATE group.  A group with a spectrum refuses XLG_PATH_Q15 submits (-ENOTSUP, logged, nothing
+ *   enqueued).  Attaching or removing a spectrum changes no client's output. */
+int xlg_add_spectrum(xlg_group *g, uint32_t width, uint32_t frames_per_row, uint32_t skip_per_row, uint32_t flags,
+                     int *spectrum_id);
+/* Drops its partial row.  -EINVAL for an unknown id. */
+int xlg_remove_spectrum(xlg_group *g, int spectrum_id);
+/* The rows a spectrum completed in a ticket: *n_rows x W contiguous floats, in pinned host memory, or in HBM for
+ * XLG_OUT_DEVICE groups (valid as xlg_output's).  *n_rows is known when xlg_submit returns.  -EINVAL for a
+ * spectrum that was not attached when the ticket was submitted. */
+int xlg_spectrum_output(xlg_group *g, int64_t ticket, int spectrum_id, const float **rows, size_t *n_rows);
+/* The width W of a ticket's rows of a spectrum: the width the id had when the ticket was submitted (an id freed by
+ * xlg_remove_spectrum may come back with another width).  -EINVAL as xlg_spectrum_output. */
+int xlg_spectrum_width(xlg_group *g, int64_t ticket, int spectrum_id, uint32_t *width);
+/* Waits for the ticket and copies at most cap_rows of its rows (xlg_spectrum_width floats each) into dst;
+ * *n_rows = rows it has. */
+int xlg_read_spectrum(xlg_group *g, int64_t ticket, int spectrum_id, float *dst, size_t cap_rows, size_t *n_rows);
+/* The channel stage serving a spectrum (0 = direct DFT, 1 = FFT) and the rows completed by the blocks submitted
+ * so far. */
+int xlg_spectrum_info(const xlg_group *g, int spectrum_id, int *kernel, uint64_t *rows_done);
 /* Size the per-ticket result arenas (device and pinned host) for `output_samples_per_block` complex output
  * samples per block summed over all clients (a client at decimation D produces about max_input_len/2/D + 2).
  * A cascade client counts two rows, each rounded up to a multiple of 4 samples: its stage-A row of
@@ -238,6 +275,7 @@ uint64_t xlg_bank_fft_flops(uint32_t K);
  * n1 = max_input_len/2/decim1 + 2 samples, rounded up to 4, which stays on the device (a bank's channel counts
  * one row like a sub-band); a member counts its
  * final row of floor(n1 * interp2 / decim2) + 2, rounded up to 4 (interp2 = 1 for xlg_add_client_subband).
+ * A spectrum counts ceil((max_input_len/2/R + 1) * W / 2) samples, rounded up to 4: room for its rows of W floats.
  * Optional: the arenas grow on demand when clients are added, but a growth re-allocates every ring entry and
  * the results still waiting in the ring are lost (-ESTALE for consumers that had not read them yet, like a
  * block overwritten in the reference's queue).  A server that knows its client limit reserves once, up front. */
@@ -372,6 +410,16 @@ typedef struct {
   uint64_t butterfly_flops;  /* real FP32 instructions of the butterflies: sum n1 * xlg_bank_fft_flops(K) */
 } xlg_bank_fft_profile;
 int xlg_bank_fft_profile_read(xlg_group *g, xlg_bank_fft_profile *p, int reset);
+
+/* Spectra (xlg_add_spectrum), counted like xlg_profile's while profiling is enabled. */
+typedef struct {
+  double spectrum_ms;        /* the channel stages and the emit pass */
+  uint64_t spectrum_launches;
+  uint64_t frames;           /* W-point frames transformed */
+  uint64_t channel_flops;    /* FP32 instructions of the channel stages: per frame xlg_bank_fft_flops(W) + 6 W on
+                                the FFT path, 4 W^2 + 6 W on the direct path (an fmaf counts one) */
+} xlg_spectrum_profile;
+int xlg_spectrum_profile_read(xlg_group *g, xlg_spectrum_profile *p, int reset);
 
 /* Introspection for tests: history length (src/xlating.c:29 history_offset; upsampled samples for a
  * rational client, stage A's for a cascade client) and which kernel currently serves the client

@@ -43,6 +43,7 @@ XLG_TRACK_STATE = 0x20
 XLG_INPUT_DEVICE = 0x100
 XLG_PATH_Q15 = 0x200
 XLG_INPUT_KEEP = 0x400
+XLG_SPECTRUM_POWER = 0x1  # xlg_add_spectrum flag
 XLG_SLOTS = 4
 
 # every symbol the headers declare (checked by tests/test_abi.py)
@@ -98,6 +99,11 @@ class XlgBankProfile(C.Structure):
 class XlgBankFftProfile(C.Structure):
     _fields_ = [("fft_ms", C.c_double), ("fft_launches", C.c_uint64), ("poly_macs", C.c_uint64),
                 ("butterfly_flops", C.c_uint64)]
+
+
+class XlgSpectrumProfile(C.Structure):
+    _fields_ = [("spectrum_ms", C.c_double), ("spectrum_launches", C.c_uint64), ("frames", C.c_uint64),
+                ("channel_flops", C.c_uint64)]
 
 
 def build(verbose: bool = False) -> None:
@@ -188,6 +194,20 @@ def lib() -> C.CDLL:
     L.xlg_bank_fft_profile_read.restype = C.c_int
     L.xlg_bank_fft_flops.argtypes = [u32]
     L.xlg_bank_fft_flops.restype = C.c_uint64
+    L.xlg_add_spectrum.argtypes = [vp, u32, u32, u32, u32, C.POINTER(C.c_int)]
+    L.xlg_add_spectrum.restype = C.c_int
+    L.xlg_remove_spectrum.argtypes = [vp, C.c_int]
+    L.xlg_remove_spectrum.restype = C.c_int
+    L.xlg_spectrum_output.argtypes = [vp, C.c_int64, C.c_int, C.POINTER(C.POINTER(C.c_float)), C.POINTER(sz)]
+    L.xlg_spectrum_output.restype = C.c_int
+    L.xlg_spectrum_width.argtypes = [vp, C.c_int64, C.c_int, C.POINTER(C.c_uint32)]
+    L.xlg_spectrum_width.restype = C.c_int
+    L.xlg_read_spectrum.argtypes = [vp, C.c_int64, C.c_int, fp, sz, C.POINTER(sz)]
+    L.xlg_read_spectrum.restype = C.c_int
+    L.xlg_spectrum_info.argtypes = [vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint64)]
+    L.xlg_spectrum_info.restype = C.c_int
+    L.xlg_spectrum_profile_read.argtypes = [vp, C.POINTER(XlgSpectrumProfile), C.c_int]
+    L.xlg_spectrum_profile_read.restype = C.c_int
     L.xl_poly_pack.argtypes = [C.POINTER(C.c_float), sz, u32, C.POINTER(C.c_float)]
     L.xl_poly_pack.restype = None
     L.xlg_reserve.argtypes = [vp, sz]
@@ -510,6 +530,61 @@ class Group:
         if code != 0:
             raise ValueError(code)
 
+    def add_spectrum(self, width: int, frames_per_row: int, skip: int = 0, power: bool = False) -> int:
+        """A spectrum (xlg_add_spectrum) attached before the next submitted block: rows of the max-held power of
+        `frames_per_row` consecutive `width`-point DFT frames, `skip` samples skipped after each row, half swapped
+        as the reference's spectrogram; dB rows, or linear power with power=True.  spectrogram_params(fs, width)
+        gives the reference tool's frames_per_row and skip.  Returns a spectrum id."""
+        sid = C.c_int(-1)
+        code = self._L.xlg_add_spectrum(self._h, width, frames_per_row, skip, XLG_SPECTRUM_POWER if power else 0,
+                                        C.byref(sid))
+        if code != 0:
+            raise ValueError(code)
+        return sid.value
+
+    def remove_spectrum(self, sid: int) -> None:
+        code = self._L.xlg_remove_spectrum(self._h, sid)
+        if code != 0:
+            raise ValueError(code)
+
+    def spectrum_rows(self, ticket: int, sid: int) -> int:
+        """Rows spectrum `sid` completed in `ticket` (known when submit returns)."""
+        n = C.c_size_t(0)
+        code = self._L.xlg_spectrum_output(self._h, ticket, sid, None, C.byref(n))
+        if code != 0:
+            raise ValueError(code)
+        return n.value
+
+    def spectrum_width(self, ticket: int, sid: int) -> int:
+        """The width of the rows spectrum `sid` completed in `ticket`: the one the id had when the ticket was
+        submitted (xlg_spectrum_width)."""
+        w = C.c_uint32(0)
+        code = self._L.xlg_spectrum_width(self._h, ticket, sid, C.byref(w))
+        if code != 0:
+            raise ValueError(code)
+        return w.value
+
+    def read_spectrum(self, ticket: int, sid: int) -> np.ndarray:
+        """The rows spectrum `sid` completed in `ticket`, a (rows, width) float32 array of the width the ticket's
+        rows were made with (xlg_read_spectrum; waits for the ticket)."""
+        n = self.spectrum_rows(ticket, sid)
+        buf = np.zeros((n, self.spectrum_width(ticket, sid)), np.float32)
+        got = C.c_size_t(0)
+        code = self._L.xlg_read_spectrum(self._h, ticket, sid, buf.ctypes.data_as(C.POINTER(C.c_float)), n,
+                                         C.byref(got))
+        if code != 0:
+            raise ValueError(code)
+        assert got.value == n
+        return buf
+
+    def spectrum_info(self, sid: int):
+        """(kernel: 0 direct DFT, 1 FFT, rows completed by the blocks submitted so far)."""
+        kind, rows = C.c_int(-1), C.c_uint64(0)
+        code = self._L.xlg_spectrum_info(self._h, sid, C.byref(kind), C.byref(rows))
+        if code != 0:
+            raise ValueError(code)
+        return kind.value, rows.value
+
     def remove_client(self, cid: int) -> None:
         code = self._L.xlg_remove_client(self._h, cid)
         if code != 0:
@@ -662,6 +737,11 @@ class Group:
         p = XlgBankFftProfile()
         self._L.xlg_bank_fft_profile_read(self._h, C.byref(p), 1 if reset else 0)
         return {k: getattr(p, k) for k, _ in XlgBankFftProfile._fields_}
+
+    def spectrum_profile_read(self, reset: bool = True) -> dict:
+        p = XlgSpectrumProfile()
+        self._L.xlg_spectrum_profile_read(self._h, C.byref(p), 1 if reset else 0)
+        return {k: getattr(p, k) for k, _ in XlgSpectrumProfile._fields_}
 
     def close(self):
         if self._h:
@@ -833,6 +913,23 @@ def bank_fft_fits(d1: int, t1: int) -> bool:
 def bank_fft_flops(K: int) -> int:
     """Real FP32 instructions of the butterflies of one K-point FFT bank frame (xlg_bank_fft_flops)."""
     return int(lib().xlg_bank_fft_flops(K))
+
+
+def spectrogram_params(fs: int, width: int):
+    """(frames_per_row, skip) of the reference spectrogram tool at sampling rate fs and width W: one row per fs
+    samples, (fs // W, fs % W).  ValueError where the tool refuses: W or fs not positive, W > fs."""
+    if width <= 0 or fs <= 0:
+        raise ValueError(f"width {width} and sampling rate {fs} must be positive")
+    if width > fs:
+        raise ValueError(f"width {width} is too wide for sampling rate {fs}")
+    return fs // width, fs % width
+
+
+def spectrogram_pixels(rows) -> np.ndarray:
+    """8-bit grey pixels of dB rows, as the reference's png_util_set_data: (int)(dB + 255), truncated toward
+    zero, clamped to [0, 255]."""
+    v = np.asarray(rows, np.float32) + np.float32(255)
+    return np.clip(np.trunc(v), 0, 255).astype(np.uint8)
 
 
 def subband_plan(fs: int, clients, bank: bool = False, fft: bool = False):

@@ -154,6 +154,21 @@ struct BankHost {
   int taps_off = 0, tw_off = 0, ch_off = 0;
 };
 
+// a spectrum (xlg_add_spectrum): its device tables and hold rows, and its walk from P in 64-bit stream positions
+struct SpectrumHost {
+  bool active = false;
+  bool power = false;        // XLG_SPECTRUM_POWER
+  int W = 0, F = 0, S = 0, R = 0;
+  long long P = 0;
+  uint64_t rows_done = 0;    // rows completed by the blocks submitted so far
+  int fir = 0;               // frames of the current row completed so far
+  int rows_cap = 0, NR = 0;  // rows a block can complete; hold rows (rows_cap + 1: all that a block touches)
+  float2 *d_tw = nullptr;
+  int *d_map = nullptr;
+  unsigned *d_hold = nullptr;
+  int out_off = 0;           // its rows in the slot's arena, in complex samples
+};
+
 // members of one sub-band that read the same windows: equal (L2, D2, T2, hist2) and, until their windows have
 // passed it, the same attach point
 struct SbClassHost {
@@ -192,7 +207,8 @@ struct BlkTable {
 // Timed spans of a block: each has a begin and an end event per slot.  Profiling records every span; the
 // timeline (XLATING_B200_TIMELINE) records the convert and tile spans too.
 enum Span {
-  SP_CONV, SP_PHASE, SP_TILE, SP_GEN, SP_LONG, SP_POLY_GEN, SP_POLY_TILE, SP_STAGE_B, SP_SB, SP_BANK, SP_BANK_FFT, SP_N
+  SP_CONV, SP_PHASE, SP_TILE, SP_GEN, SP_LONG, SP_POLY_GEN, SP_POLY_TILE, SP_STAGE_B, SP_SB, SP_BANK, SP_BANK_FFT, SP_SPEC,
+  SP_N
 };
 
 struct Slot {
@@ -226,6 +242,9 @@ struct Slot {
   uint64_t bk_poly = 0, bk_dft = 0;
   BlkTable<BankBlk> bfblk;       // the same for the FFT banks
   uint64_t bf_poly = 0, bf_flops = 0;
+  BlkTable<SpecBlk> spblk;       // spectra with work in this block
+  uint64_t sp_frames = 0, sp_flops = 0;
+  cudaEvent_t ev_spec = nullptr;  // this block's spectra done (the hold rows are updated in block order on it)
   std::atomic<int64_t> ticket{-1};
   bool q15 = false;
   bool harvested = true;
@@ -317,6 +336,7 @@ struct HostOut {
   MetaArr<int> n_out;    // per client id
   MetaArr<int> out_off;  // per client id
   MetaArr<long long> hist_after;  // XLG_TRACK_STATE: per client id, history_offset after this ticket
+  MetaArr<int> sp_rows, sp_off, sp_w;  // per spectrum id: rows, their offset in floats, width (0: not attached)
   float2 *h_endph = nullptr;          // XLG_TRACK_STATE: pinned, oscillator after this ticket, per client id
   size_t endph_cap = 0;
 };
@@ -470,6 +490,11 @@ struct xlg_group {
   size_t cap_bktaps = 0, cap_bktw = 0, cap_bkch = 0;
   xlg_bank_profile bank_prof;
   xlg_bank_fft_profile bank_fft_prof;
+  std::vector<SpectrumHost> spectra;        // spectrum id -> spectrum (inactive = free)
+  std::vector<void *> dead_spec;            // tables and holds of removed spectra, freed once the pipeline is drained
+  cudaEvent_t ev_last_spec = nullptr;       // ev_spec of the last block with spectrum work
+  bool have_last_spec = false;
+  xlg_spectrum_profile spec_prof;
   int n_generic = 0;
   int max_client = 0;     // highest active id + 1
   bool dirty = true;
@@ -582,6 +607,7 @@ static void slot_free(Slot &s) {
   s.sbblk.release();
   s.bkblk.release();
   s.bfblk.release();
+  s.spblk.release();
   if (s.d_sbph) cudaFree(s.d_sbph);
   s.d_sbph = nullptr;
   s.d_pscratch = nullptr;
@@ -652,7 +678,8 @@ static void harvest_locked(xlg_group *g, Slot &s) {
       {&g->casc_prof.stage_b_ms, &g->casc_prof.stage_b_launches},
       {&g->sb_prof.member_ms, &g->sb_prof.member_launches},
       {&g->bank_prof.bank_ms, &g->bank_prof.bank_launches},
-      {&g->bank_fft_prof.fft_ms, &g->bank_fft_prof.fft_launches}};
+      {&g->bank_fft_prof.fft_ms, &g->bank_fft_prof.fft_launches},
+      {&g->spec_prof.spectrum_ms, &g->spec_prof.spectrum_launches}};
   for (int sp = 0; sp < SP_N; sp++) {
     float ms = 0;
     if (s.pf_on[sp] && cudaEventElapsedTime(&ms, s.pf[sp][0], s.pf[sp][1]) == cudaSuccess) {
@@ -669,6 +696,8 @@ static void harvest_locked(xlg_group *g, Slot &s) {
   g->bank_prof.dft_macs += s.bk_dft;
   g->bank_fft_prof.poly_macs += s.bf_poly;
   g->bank_fft_prof.butterfly_flops += s.bf_flops;
+  g->spec_prof.frames += s.sp_frames;
+  g->spec_prof.channel_flops += s.sp_flops;
   g->prof.blocks++;
   g->prof.out_samples += s.out_samples;
   g->prof.in_samples += s.in_samples;
@@ -926,6 +955,28 @@ static int rebuild_banks(xlg_group *g) {
   return 0;
 }
 
+// Spectra (the pipeline is drained): their rows after the clients' final rows, inside the D2H copy; a frame reads
+// at most W - 1 samples of earlier blocks
+static int rebuild_spectra(xlg_group *g, size_t &out_total, size_t &max_hist) {
+  for (void *p : g->dead_spec) cudaFree(p);
+  g->dead_spec.clear();
+  size_t n = 0;
+  for (SpectrumHost &p : g->spectra) {
+    if (!p.active) continue;
+    p.out_off = (int)out_total;
+    out_total += ((size_t)p.rows_cap * p.W + 1) / 2;
+    out_total = (out_total + 3) & ~(size_t)3;
+    max_hist = std::max(max_hist, (size_t)p.W - 1);
+    n++;
+  }
+  if (n == 0) return 0;
+  CU_OK(cudaFuncSetAttribute(spectrum_direct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             (int)spec_direct_smem(SPEC_MAX_W - 1)));
+  for (Slot &s : g->slots)
+    if (s.spblk.reserve(n)) return -EIO;
+  return 0;
+}
+
 // Cascade clients (the pipeline is drained): stage-A rows after every host-visible row (the D2H copy ends before
 // them), stage-B taps, and a zeroed history ring for each new client (its positions before the attach read as
 // zero)
@@ -1080,6 +1131,7 @@ static int rebuild_layout(xlg_group *g) {
   }
   for (const BankHost &k : g->banks)  // a bank walks (and its channels read history) without channels too
     if (k.active) max_hist = std::max(max_hist, k.T1 - 1);
+  if (rebuild_spectra(g, out_total, max_hist)) return -EIO;
   if (rebuild_cascades(g, out_total)) return -EIO;
   if (rebuild_subbands(g, out_total)) return -EIO;
   if (rebuild_banks(g)) return -EIO;
@@ -1656,6 +1708,7 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
   memset(&g->sb_prof, 0, sizeof(g->sb_prof));
   memset(&g->bank_prof, 0, sizeof(g->bank_prof));
   memset(&g->bank_fft_prof, 0, sizeof(g->bank_fft_prof));
+  memset(&g->spec_prof, 0, sizeof(g->spec_prof));
   g->device = device;
   g->fs = sampling_freq;
   g->max_input_len = max_input_len;
@@ -1665,6 +1718,7 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
     h.n_out.retired = &g->retired_meta_i;
     h.out_off.retired = &g->retired_meta_i;
     h.hist_after.retired = &g->retired_meta_ll;
+    h.sp_rows.retired = h.sp_off.retired = h.sp_w.retired = &g->retired_meta_i;
   }
   int rc = 0;
   auto fail = [&](int code) {
@@ -1711,6 +1765,7 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
       for (cudaEvent_t &ev : span)
         if (cudaEventCreate(&ev) != cudaSuccess) return fail(-EIO);
     if (cudaEventCreateWithFlags(&s.ev_casc, cudaEventDisableTiming) != cudaSuccess) return fail(-EIO);
+    if (cudaEventCreateWithFlags(&s.ev_spec, cudaEventDisableTiming) != cudaSuccess) return fail(-EIO);
     if (cudaMalloc(&s.d_vblk, T_MAX_CLASSES * sizeof(BlkInfo)) != cudaSuccess ||
         cudaHostAlloc(&s.h_vblk, T_MAX_CLASSES * sizeof(BlkInfo), cudaHostAllocDefault) != cudaSuccess)
       return fail(-ENOMEM);
@@ -1830,6 +1885,7 @@ extern "C" void xlg_destroy(xlg_group *g) {
       for (cudaEvent_t ev : span)
         if (ev) cudaEventDestroy(ev);
     if (s.ev_casc) cudaEventDestroy(s.ev_casc);
+    if (s.ev_spec) cudaEventDestroy(s.ev_spec);
   }
   for (HostOut &h : g->ring_out) {
     if (h.h_out) cudaFreeHost(h.h_out);
@@ -1838,6 +1894,9 @@ extern "C" void xlg_destroy(xlg_group *g) {
     h.n_out.release();
     h.out_off.release();
     h.hist_after.release();
+    h.sp_rows.release();
+    h.sp_off.release();
+    h.sp_w.release();
   }
   for (int *p : g->retired_meta_i) delete[] p;
   for (long long *p : g->retired_meta_ll) delete[] p;
@@ -1868,6 +1927,10 @@ extern "C" void xlg_destroy(xlg_group *g) {
   for (HostClient &h : g->clients)
     if (h.b2.ring.p) cudaFree(h.b2.ring.p);
   for (float2 *p : g->dead_rings) cudaFree(p);
+  for (const SpectrumHost &p : g->spectra)
+    for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold})
+      if (d) cudaFree(d);
+  for (void *p : g->dead_spec) cudaFree(p);
   for (cudaEvent_t e : g->ev_user) cudaEventDestroy(e);
   if (g->s_in) cudaStreamDestroy(g->s_in);
   for (const xlg_group::StreamSet *ss : {&g->set_part, &g->set_plain}) {
@@ -2207,6 +2270,19 @@ extern "C" int xlg_subband_info(const xlg_group *g, int client_id, int *subband_
   return 0;
 }
 
+// e^{-2 pi i j / K}, j < K, of the banks and spectra: (-i)^q e^{-i t}, 4j = qK + rem, t = 2 pi rem / 4K in
+// [0, pi/2), in double, rounded once: quarter turns are exact (W = 1, -i, -1, i where 4j % K == 0)
+static std::vector<float2> twiddle_table(int K) {
+  std::vector<float2> tw((size_t)K);
+  for (int j = 0; j < K; j++) {
+    const int q = (int)(4LL * j / K), rem = (int)(4LL * j - (long long)q * K);
+    const double t = 2.0 * 3.14159265358979323846 * (double)rem / (4.0 * (double)K);
+    const float c = (float)cos(t), sn = (float)sin(t);
+    tw[j] = q == 0 ? make_float2(c, -sn) : q == 1 ? make_float2(-sn, -c) : q == 2 ? make_float2(-c, sn) : make_float2(sn, c);
+  }
+  return tw;
+}
+
 // A bank (fft: its channel stage is bank_fft_cf32_kernel's) after the checks of its kernel
 static int add_bank(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, bool fft, int *bank_id) {
   const char *what = fft ? "FFT bank" : "bank";
@@ -2248,15 +2324,7 @@ static int add_bank(xlg_group *g, uint32_t decim1, const float *taps1, size_t ta
   k.tpad = bank_tpad(k.K, (int)taps1_len);
   k.taps.assign((size_t)k.tpad, 0.f);
   for (size_t j = 0; j < taps1_len; j++) k.taps[j] = taps1[taps1_len - 1 - j];
-  k.tw.resize((size_t)k.K);
-  // e^{-2 pi i j / K} = (-i)^q e^{-i t}, 4j = qK + rem, t = 2 pi rem / 4K in [0, pi/2): quarter turns are exact
-  // (W = 1, -i, -1, i where 4j % K == 0)
-  for (int j = 0; j < k.K; j++) {
-    const int q = 4 * j / k.K, rem = 4 * j - q * k.K;
-    const double t = 2.0 * 3.14159265358979323846 * (double)rem / (4.0 * (double)k.K);
-    const float c = (float)cos(t), sn = (float)sin(t);
-    k.tw[j] = q == 0 ? make_float2(c, -sn) : q == 1 ? make_float2(-sn, -c) : q == 2 ? make_float2(-c, sn) : make_float2(sn, c);
-  }
+  k.tw = twiddle_table(k.K);
   k.P = g->S;
   k.hist = (long long)taps1_len - 1;  // a fresh filter's history: T1 - 1 samples, zero before P
   int id = 0;
@@ -2352,6 +2420,95 @@ extern "C" int xlg_add_bank_subband(xlg_group *g, int bank_id, int32_t channel, 
   return 0;
 }
 
+extern "C" int xlg_add_spectrum(xlg_group *g, uint32_t width, uint32_t frames_per_row, uint32_t skip_per_row,
+                                uint32_t flags, int *spectrum_id) {
+  if (g == nullptr || spectrum_id == nullptr) return -EINVAL;
+  if (width == 0 || width > SPEC_MAX_W || frames_per_row == 0) {
+    XL_LOG("spectrum: width %u must be in [1, %d] and frames per row %u at least 1", width, SPEC_MAX_W, frames_per_row);
+    return -EINVAL;
+  }
+  const uint64_t R = (uint64_t)frames_per_row * width + skip_per_row;
+  if (R >= (1ull << 31)) {
+    XL_LOG("spectrum: a row period of %llu samples is not below 2^31", (unsigned long long)R);
+    return -EINVAL;
+  }
+  if (flags & ~XLG_SPECTRUM_POWER) {
+    XL_LOG("spectrum: unknown flags 0x%x", flags & ~XLG_SPECTRUM_POWER);
+    return -EINVAL;
+  }
+  if (g->flags & XLG_TRACK_STATE) {
+    XL_LOG("spectrum: an XLG_TRACK_STATE group does not serve spectra");
+    return -ENOTSUP;
+  }
+  CU_OK(cudaSetDevice(g->device));
+  SpectrumHost p;
+  p.active = true;
+  p.power = (flags & XLG_SPECTRUM_POWER) != 0;
+  p.W = (int)width;
+  p.F = (int)frames_per_row;
+  p.S = (int)skip_per_row;
+  p.R = (int)R;
+  p.P = g->S;
+  p.rows_cap = (int)((uint64_t)g->max_input_len / 2 / R + 1);
+  p.NR = p.rows_cap + 1;
+  const int W = p.W, half = W / 2;
+  std::vector<int> map((size_t)W);
+  for (int j = 0; j < W; j++) {
+    // spectrogram.c:156-163: the halves swapped, an odd width's last bin in place
+    const int bin = j < half ? half + j : j < 2 * half ? j - half : W - 1;
+    map[j] = spec_fft(W) ? bank_fft_pos(bin, W) : bin;
+  }
+  const std::vector<float2> tw = twiddle_table(W);
+  const size_t hold_bytes = (size_t)p.NR * W * sizeof(unsigned);
+  if (cudaMalloc(&p.d_tw, W * sizeof(float2)) != cudaSuccess || cudaMalloc(&p.d_map, W * sizeof(int)) != cudaSuccess ||
+      cudaMalloc(&p.d_hold, hold_bytes) != cudaSuccess) {
+    for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold})
+      if (d) cudaFree(d);
+    XL_LOG("spectrum: out of device memory");
+    return -ENOMEM;
+  }
+  CU_OK(cudaMemcpy(p.d_tw, tw.data(), W * sizeof(float2), cudaMemcpyHostToDevice));
+  CU_OK(cudaMemcpy(p.d_map, map.data(), W * sizeof(int), cudaMemcpyHostToDevice));
+  // (on a group stream, finished before the spectrum exists: the kernels' streams do not wait for the legacy one)
+  CU_OK(cudaMemsetAsync(p.d_hold, 0, hold_bytes, g->s_in));
+  CU_OK(cudaStreamSynchronize(g->s_in));
+  int id = 0;
+  while (id < (int)g->spectra.size() && g->spectra[id].active) id++;
+  if (id == (int)g->spectra.size()) g->spectra.emplace_back();
+  g->spectra[id] = p;
+  g->dirty = true;  // its rows in the arenas, the input ring's history bound
+  *spectrum_id = id;
+  return 0;
+}
+
+static SpectrumHost *spectrum_of(xlg_group *g, int id) {
+  if (id < 0 || id >= (int)g->spectra.size() || !g->spectra[id].active) return nullptr;
+  return &g->spectra[id];
+}
+
+extern "C" int xlg_remove_spectrum(xlg_group *g, int spectrum_id) {
+  if (g == nullptr) return -EINVAL;
+  SpectrumHost *p = spectrum_of(g, spectrum_id);
+  if (p == nullptr) {
+    XL_LOG("spectrum %d does not exist", spectrum_id);
+    return -EINVAL;
+  }
+  // in-flight tickets still read the tables and the hold: freed at the next re-layout, which drains
+  for (void *d : {(void *)p->d_tw, (void *)p->d_map, (void *)p->d_hold}) g->dead_spec.push_back(d);
+  *p = SpectrumHost();
+  g->dirty = true;
+  return 0;
+}
+
+extern "C" int xlg_spectrum_info(const xlg_group *g, int spectrum_id, int *kernel, uint64_t *rows_done) {
+  if (g == nullptr) return -EINVAL;
+  const SpectrumHost *p = spectrum_of(const_cast<xlg_group *>(g), spectrum_id);
+  if (p == nullptr) return -EINVAL;
+  if (kernel) *kernel = spec_fft(p->W) ? 1 : 0;
+  if (rows_done) *rows_done = p->rows_done;
+  return 0;
+}
+
 template <int FMT>
 static void launch_convert(bool q15, const void *raw, xlg_group *g, long long S, int n, cudaStream_t st) {
   const int threads = 256, blocks = (n + threads - 1) / threads;
@@ -2390,6 +2547,9 @@ struct Block {
   size_t bk_smem = 0;
   int n_bf = 0, max_bf_ctas = 0;  // FFT banks
   size_t bf_smem = 0;
+  // spectrum walk: entries, CTAs of the FFT and direct paths, row values to emit, the end of their rows in the arena
+  int n_spec = 0, max_spf_ctas = 0, max_spd_ctas = 0, max_spd_groups = 0, max_sp_values = 0;
+  size_t spf_smem = 0, spd_smem = 0, sp_used = 0;
   // sub-band walk
   int n_sb = 0, max_sb_n1 = 0, max_sb_n2 = 0;
   int max_sbr_ctas = 0, max_sbr_l2 = 0;  // rational classes: output tiles of the longest residue, largest L2
@@ -2493,6 +2653,60 @@ static void walk_banks(Block &b) {
     b.bk_smem = std::max(b.bk_smem, bank_smem((int)k.D1, (int)k.T1));
     s.bk_poly += (uint64_t)n1 * k.T1;
     s.bk_dft += (uint64_t)n1 * k.cids.size() * (uint64_t)k.K;
+  }
+}
+
+// Spectra: the frames this block completes (those whose last sample it holds) and the rows they complete, in
+// closed form from the frames completed since P
+static void walk_spectra(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  s.sp_frames = s.sp_flops = 0;
+  const long long E = b.S + b.n;
+  for (int id = 0; id < (int)g->spectra.size(); id++) {
+    SpectrumHost &p = g->spectra[id];
+    b.ho.sp_w[id] = p.active ? p.W : 0;
+    if (!p.active) continue;
+    const uint64_t d = (uint64_t)(E - p.P), F = (uint64_t)p.F;
+    const uint64_t total = d / (uint64_t)p.R * F + std::min<uint64_t>(F, d % (uint64_t)p.R / (uint64_t)p.W);
+    const int n_frames = (int)(total - (p.rows_done * F + (uint64_t)p.fir));
+    const int n_rows = (int)(total / F - p.rows_done);
+    b.ho.sp_rows[id] = n_rows;
+    b.ho.sp_off[id] = 2 * p.out_off;
+    if (n_frames > 0) {
+      SpecBlk &e = s.spblk.h[b.n_spec++];
+      e.tw = p.d_tw;
+      e.map = p.d_map;
+      e.hold = p.d_hold;
+      e.out = reinterpret_cast<float *>(s.d_out) + 2 * (size_t)p.out_off;
+      e.base = p.P + (long long)(p.rows_done * (uint64_t)p.R);
+      e.mask = b.mask;
+      e.W = p.W;
+      e.F = p.F;
+      e.R = p.R;
+      e.NR = p.NR;
+      e.f0 = (unsigned)p.fir;
+      e.n_frames = n_frames;
+      e.n_rows = n_rows;
+      e.slot0 = (int)(p.rows_done % (uint64_t)p.NR);
+      e.power = p.power ? 1 : 0;
+      e.inv_w = 1.0f / (float)p.W;
+      const uint64_t flops = spec_fft(p.W) ? xlg_bank_fft_flops((uint32_t)p.W) : 4ull * p.W * p.W;
+      s.sp_frames += (uint64_t)n_frames;
+      s.sp_flops += (uint64_t)n_frames * (flops + 6ull * p.W);
+      if (spec_fft(p.W)) {
+        b.max_spf_ctas = std::max(b.max_spf_ctas, (n_frames + bank_fft_frames(p.W) - 1) / bank_fft_frames(p.W));
+        b.spf_smem = std::max(b.spf_smem, bank_fft_smem(p.W));
+      } else {
+        b.max_spd_ctas = std::max(b.max_spd_ctas, (n_frames + spec_direct_frames(p.W) - 1) / spec_direct_frames(p.W));
+        b.max_spd_groups = std::max(b.max_spd_groups, spec_direct_groups(p.W));
+        b.spd_smem = std::max(b.spd_smem, spec_direct_smem(p.W));
+      }
+      b.max_sp_values = std::max(b.max_sp_values, n_rows * p.W);
+      b.sp_used = std::max(b.sp_used, (size_t)p.out_off + ((size_t)n_rows * p.W + 1) / 2);
+    }
+    p.rows_done = total / F;
+    p.fir = (int)(total % F);
   }
 }
 
@@ -2636,6 +2850,30 @@ static int launch_banks(Block &b) {
   CU_OK(s.bfblk.upload((size_t)b.n_bf, b.cs));
   bank_fft_cf32_kernel<<<dim3(b.max_bf_ctas, b.n_bf), BF_THREADS, b.bf_smem, b.cs>>>(s.bfblk.d, g->ring, s.d_out);
   return span_end(g, s, SP_BANK_FFT, b.cs);
+}
+
+// Spectra: after the clients' launches, so that no client kernel waits for them; each block's after the previous
+// one's, which emptied the hold rows it reuses
+static int launch_spectra(Block &b) {
+  xlg_group *g = b.g;
+  Slot &s = b.s;
+  if (b.n_spec == 0) return 0;
+  if (g->have_last_spec) CU_OK(cudaStreamWaitEvent(b.cs, g->ev_last_spec, 0));
+  if (span_begin(g, s, SP_SPEC, b.cs)) return -EIO;
+  CU_OK(s.spblk.upload((size_t)b.n_spec, b.cs));
+  if (b.max_spf_ctas > 0)
+    spectrum_fft_kernel<<<dim3(b.max_spf_ctas, b.n_spec), SPEC_THREADS, b.spf_smem, b.cs>>>(s.spblk.d, g->ring);
+  if (b.max_spd_ctas > 0)
+    spectrum_direct_kernel<<<dim3(b.max_spd_ctas, b.max_spd_groups, b.n_spec), SPEC_THREADS, b.spd_smem, b.cs>>>(
+        s.spblk.d, g->ring);
+  if (b.max_sp_values > 0)
+    spectrum_emit_kernel<<<dim3((b.max_sp_values + SPEC_THREADS - 1) / SPEC_THREADS, b.n_spec), SPEC_THREADS, 0,
+                           b.cs>>>(s.spblk.d);
+  if (span_end(g, s, SP_SPEC, b.cs)) return -EIO;
+  CU_OK(cudaEventRecord(s.ev_spec, b.cs));
+  g->ev_last_spec = s.ev_spec;
+  g->have_last_spec = true;
+  return 0;
 }
 
 // Oscillator pre-pass (own stream: chains only on the previous pre-pass; none without a client to walk), and the
@@ -2983,13 +3221,14 @@ static int copy_back(Block &b) {
   xlg_group *g = b.g;
   Slot &s = b.s;
   HostOut &ho = b.ho;
-  if ((g->flags & XLG_OUT_DEVICE) || g->arena_cap == 0 || b.nc <= 0) {
+  if ((g->flags & XLG_OUT_DEVICE) || g->arena_cap == 0 || (b.nc <= 0 && b.sp_used == 0)) {
     CU_OK(cudaEventRecord(s.ev_done, b.cs));  // results stay on the device: no hop through s_out
     return 0;
   }
   size_t used = 0;
   for (size_t i = 0; i < g->clients.size(); i++)
     if (g->clients[i].active) used = std::max(used, (size_t)ho.out_off[i] + (size_t)ho.n_out[i]);
+  used = std::max(used, b.sp_used);
   CU_OK(cudaStreamWaitEvent(g->s_out, s.ev_fir, 0));
   if (used > 0) {
     if (b.q15)
@@ -3019,6 +3258,12 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     return -EINVAL;
   }
   const bool q15 = (flags & XLG_PATH_Q15) != 0;
+  if (q15)
+    for (const SpectrumHost &p : g->spectra)
+      if (p.active) {
+        XL_LOG("the Q15 path does not serve spectra; submit without XLG_PATH_Q15");
+        return -ENOTSUP;
+      }
   if (q15)
     for (const BankHost &k : g->banks)
       if (k.active) {
@@ -3089,6 +3334,9 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
     ho.n_out.assign(g->clients.size(), 0);
     ho.out_off.assign(g->clients.size(), 0);
     if (g->flags & XLG_TRACK_STATE) ho.hist_after.assign(g->clients.size(), 0);
+    ho.sp_rows.assign(g->spectra.size(), 0);
+    ho.sp_off.assign(g->spectra.size(), 0);
+    ho.sp_w.assign(g->spectra.size(), 0);
     ho.q15 = q15;
   }
   s.q15 = q15;
@@ -3100,6 +3348,7 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
   walk_clients(b);
   walk_banks(b);
   walk_subbands(b);
+  walk_spectra(b);
 
   // consecutive blocks alternate between two compute streams so that the tail of
   // one block's FIR overlaps the head of the next (each block's launch alone
@@ -3112,7 +3361,7 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
   // append to their rings in block order, chained on ev_last_casc.
   if (stage_and_convert(b, fmt, input, flags) || launch_banks(b) || launch_prepass(b) || launch_tiled(b) ||
       launch_long(b) || launch_generic(b) || launch_poly_tiled(b) || launch_poly_generic(b) || launch_stage_b(b) ||
-      launch_members(b))
+      launch_members(b) || launch_spectra(b))
     return -EIO;
   CU_OK(cudaGetLastError());
   CU_OK(cudaEventRecord(s.ev_fir, b.cs));
@@ -3188,6 +3437,64 @@ extern "C" int xlg_read_output(xlg_group *g, int64_t ticket, int client_id, void
     memcpy(dst, src, bytes);
     // seqlock-style validation: xlg_submit marks the entry (ticket = -1) BEFORE it enqueues the
     // copy that overwrites it, so an unchanged ticket after our reads means they saw this ticket's data
+    std::atomic_thread_fence(std::memory_order_acquire);
+    if (ho.ticket.load() != ticket) return -ESTALE;
+  }
+  return 0;
+}
+
+// A ticket's rows of a spectrum: where they are, how many, and the width they were made with, read together under
+// the group's lock
+static int spectrum_rows(xlg_group *g, int64_t ticket, int spectrum_id, const float **rows, size_t *n_rows,
+                         uint32_t *width) {
+  if (g == nullptr || ticket < 0 || ticket >= g->next_ticket.load()) return -EINVAL;
+  HostOut &ho = g->ring_out[ticket % (int64_t)g->ring_out.size()];
+  std::lock_guard<std::mutex> lk(g->mu);
+  if (ho.ticket.load() != ticket) return -ESTALE;
+  if (spectrum_id < 0 || spectrum_id >= (int)ho.sp_w.size() || ho.sp_w[spectrum_id] == 0) return -EINVAL;
+  if (n_rows) *n_rows = (size_t)ho.sp_rows[spectrum_id];
+  if (width) *width = (uint32_t)ho.sp_w[spectrum_id];
+  if (rows) {
+    if (g->flags & XLG_OUT_DEVICE) {
+      Slot &s = g->slots[ticket % XLG_SLOTS];
+      if (s.ticket.load() != ticket) return -ESTALE;  // device arenas live XLG_SLOTS tickets
+      *rows = reinterpret_cast<const float *>(s.d_out) + ho.sp_off[spectrum_id];
+    } else {
+      *rows = reinterpret_cast<const float *>(ho.h_out) + ho.sp_off[spectrum_id];
+    }
+  }
+  return 0;
+}
+
+extern "C" int xlg_spectrum_output(xlg_group *g, int64_t ticket, int spectrum_id, const float **rows, size_t *n_rows) {
+  return spectrum_rows(g, ticket, spectrum_id, rows, n_rows, nullptr);
+}
+
+extern "C" int xlg_spectrum_width(xlg_group *g, int64_t ticket, int spectrum_id, uint32_t *width) {
+  if (width == nullptr) return -EINVAL;
+  return spectrum_rows(g, ticket, spectrum_id, nullptr, nullptr, width);
+}
+
+extern "C" int xlg_read_spectrum(xlg_group *g, int64_t ticket, int spectrum_id, float *dst, size_t cap_rows,
+                                 size_t *n_rows) {
+  if (g == nullptr || dst == nullptr) return -EINVAL;
+  int rc = xlg_wait(g, ticket);
+  if (rc != 0) return rc;
+  const float *src = nullptr;
+  size_t n = 0;
+  uint32_t W = 0;
+  rc = spectrum_rows(g, ticket, spectrum_id, &src, &n, &W);
+  if (rc != 0) return rc;
+  if (n_rows) *n_rows = n;
+  const size_t bytes = std::min(n, cap_rows) * W * sizeof(float);
+  if (bytes == 0) return 0;
+  if (g->flags & XLG_OUT_DEVICE) {
+    cudaSetDevice(g->device);
+    CU_OK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
+    if (g->slots[ticket % XLG_SLOTS].ticket.load() != ticket) return -ESTALE;
+  } else {
+    const HostOut &ho = g->ring_out[ticket % (int64_t)g->ring_out.size()];
+    memcpy(dst, src, bytes);
     std::atomic_thread_fence(std::memory_order_acquire);
     if (ho.ticket.load() != ticket) return -ESTALE;
   }
@@ -3358,6 +3665,10 @@ extern "C" int xlg_bank_profile_read(xlg_group *g, xlg_bank_profile *p, int rese
 
 extern "C" int xlg_bank_fft_profile_read(xlg_group *g, xlg_bank_fft_profile *p, int reset) {
   return family_profile_read(g, &xlg_group::bank_fft_prof, p, reset);
+}
+
+extern "C" int xlg_spectrum_profile_read(xlg_group *g, xlg_spectrum_profile *p, int reset) {
+  return family_profile_read(g, &xlg_group::spec_prof, p, reset);
 }
 
 extern "C" int xlg_profile_read(xlg_group *g, xlg_profile *p, int reset) {

@@ -1701,6 +1701,37 @@ __device__ __forceinline__ float2 cmul_tw(float2 y, float2 w) {
   return make_float2(fmaf(-y.y, w.y, __fmul_rn(y.x, w.x)), fmaf(y.y, w.x, __fmul_rn(y.x, w.y)));
 }
 
+// The in-place decimation-in-frequency FFT of nf rows of K (a power of two, lk = log2 K) in shared memory u, in
+// the order the header above states, tw[j] = e^{-2 pi i j / K}; every stage ends with a barrier
+template <int THREADS>
+__device__ __forceinline__ void fft_dif_rows(float2 *u, int nf, int K, int lk, const float2 *tw, int tid) {
+  int L = K;
+  for (; L >= 4; L >>= 2) {
+    const int q4 = L >> 2, s = K / L;
+    for (int e = tid; e < nf * (K >> 2); e += THREADS) {
+      const int f = e >> (lk - 2), i = e & ((K >> 2) - 1), j = i & (q4 - 1);
+      float2 *x = u + (f << lk) + 4 * (i - j) + j;
+      const float2 a0 = x[0], a1 = x[q4], a2 = x[2 * q4], a3 = x[3 * q4];
+      const float2 t0 = make_float2(a0.x + a2.x, a0.y + a2.y), t1 = make_float2(a0.x - a2.x, a0.y - a2.y);
+      const float2 t2 = make_float2(a1.x + a3.x, a1.y + a3.y), t3 = make_float2(a1.x - a3.x, a1.y - a3.y);
+      x[0] = make_float2(t0.x + t2.x, t0.y + t2.y);
+      x[q4] = cmul_tw(make_float2(t1.x + t3.y, t1.y - t3.x), __ldg(tw + j * s));
+      x[2 * q4] = cmul_tw(make_float2(t0.x - t2.x, t0.y - t2.y), __ldg(tw + 2 * j * s));
+      x[3 * q4] = cmul_tw(make_float2(t1.x - t3.y, t1.y + t3.x), __ldg(tw + 3 * j * s));
+    }
+    __syncthreads();
+  }
+  if (L == 2) {
+    for (int e = tid; e < nf * (K >> 1); e += THREADS) {
+      float2 *x = u + 2 * e;
+      const float2 a0 = x[0], a1 = x[1];
+      x[0] = make_float2(a0.x + a1.x, a0.y + a1.y);
+      x[1] = make_float2(a0.x - a1.x, a0.y - a1.y);
+    }
+    __syncthreads();
+  }
+}
+
 // CTA (x, b) computes frames [x F, x F + F) of bank b, F = bank_fft_frames(K): the rotated sums of each frame in
 // a row of K in shared memory (taps and window read through the L1: T1 is too long to stage), the FFT of every
 // row, then the materialised channels' samples, a channel's frames consecutively.  chans[c].x is the channel's
@@ -1729,37 +1760,173 @@ bank_fft_cf32_kernel(const BankBlk *__restrict__ blk, const float2 *__restrict__
     u[(f << lk) + ((p + r) & (K - 1))] = acc;
   }
   __syncthreads();
-  int L = K;
-  for (; L >= 4; L >>= 2) {
-    const int q4 = L >> 2, s = K / L;
-    for (int e = tid; e < nf * (K >> 2); e += BF_THREADS) {
-      const int f = e >> (lk - 2), i = e & ((K >> 2) - 1), j = i & (q4 - 1);
-      float2 *x = u + (f << lk) + 4 * (i - j) + j;
-      const float2 a0 = x[0], a1 = x[q4], a2 = x[2 * q4], a3 = x[3 * q4];
-      const float2 t0 = make_float2(a0.x + a2.x, a0.y + a2.y), t1 = make_float2(a0.x - a2.x, a0.y - a2.y);
-      const float2 t2 = make_float2(a1.x + a3.x, a1.y + a3.y), t3 = make_float2(a1.x - a3.x, a1.y - a3.y);
-      x[0] = make_float2(t0.x + t2.x, t0.y + t2.y);
-      x[q4] = cmul_tw(make_float2(t1.x + t3.y, t1.y - t3.x), __ldg(b.tw + j * s));
-      x[2 * q4] = cmul_tw(make_float2(t0.x - t2.x, t0.y - t2.y), __ldg(b.tw + 2 * j * s));
-      x[3 * q4] = cmul_tw(make_float2(t1.x - t3.y, t1.y + t3.x), __ldg(b.tw + 3 * j * s));
-    }
-    __syncthreads();
-  }
-  if (L == 2) {
-    for (int e = tid; e < nf * (K >> 1); e += BF_THREADS) {
-      float2 *x = u + 2 * e;
-      const float2 a0 = x[0], a1 = x[1];
-      x[0] = make_float2(a0.x + a1.x, a0.y + a1.y);
-      x[1] = make_float2(a0.x - a1.x, a0.y - a1.y);
-    }
-    __syncthreads();
-  }
+  fft_dif_rows<BF_THREADS>(u, nf, K, lk, b.tw, tid);
   for (int e = tid; e < b.n_ch * F; e += BF_THREADS) {
     const int c = e / F, f = e - c * F;
     if (f >= nf) continue;
     const int2 ch = b.chans[c];
     out[ch.y + f0 + f] = u[(f << lk) + ch.x];
   }
+}
+
+// ---------------------------------------------------------------------------
+// Spectrum rows (xlg_add_spectrum).  A spectrum of width W, F frames per row and S samples skipped per row,
+// attached at stream position P, has period R = F W + S; row r is the max-hold over the frames
+// x[P + r R + f W ... + W), f < F, of the power of each DFT bin (src/spectrogram/spectrogram.c).  Per frame and
+// bin, with X the frame's DFT and inv = 1/W rounded to float once, in this order (rounded operations, no
+// contraction):
+//     c = (X.x * inv, X.y * inv),   p = (c.x * c.x + c.y * c.y) + 1e-20f
+// X comes from one of two channel stages:
+//   FFT path (W a power of two, 4 <= W <= 4096): the frame in natural order through fft_dif_rows, the FFT bank's
+//     radix-4 (then radix-2) decimation in frequency with the twiddle table read at stride W / L; bin k then lies
+//     at position bank_fft_pos(k, W) of the row (digit reversal).  FP32 instructions per frame:
+//     xlg_bank_fft_flops(W) + 6 W.
+//   Direct path (every other W <= 4096): X_k = sum_{n < W} x[n] W_tab[(k n) mod W], two fmaf chains from +0 over
+//     n ascending, acc.x = fmaf(-x.y, w.y, fmaf(x.x, w.x, acc.x)), acc.y = fmaf(x.y, w.x, fmaf(x.x, w.y, acc.y)):
+//     W complex MACs per input sample, 4 W^2 + 6 W FP32 instructions per frame.
+// The table is the banks' e^{-2 pi i m / W}, built in double by quarter turns and rounded once.  Each p goes to
+// the spectrum's hold row of its frame's row by atomicMax on its bit pattern: p >= 1e-20 > 0, so integer order
+// is float order and the max does not depend on the order CTAs run in (0, the empty hold, is below every p).
+// The hold has NR rows used round-robin by row number (NR exceeds the rows a block touches); the emit pass reads
+// each row the block completed through the row map (out[j] = hold[map[j]]: the reference's half swap, then the
+// FFT path's digit reversal), writes v (XLG_SPECTRUM_POWER) or 10 * log10f(v), and zeroes what it read.
+// ---------------------------------------------------------------------------
+constexpr int SPEC_THREADS = 256;
+constexpr int SPEC_MAX_W = 4096;
+
+struct SpecBlk {          // one spectrum, this block
+  const float2 *tw;       // e^{-2 pi i m / W}, m < W
+  const int *map;         // output bin j reads hold position map[j]
+  unsigned *hold;         // NR rows of W: each row's running max (float bits), zero when empty
+  float *out;             // its rows in the slot's arena: n_rows x W
+  long long base;         // stream position of the first row this block touches: P + r R
+  unsigned mask;          // input ring capacity - 1
+  int W, F, R, NR;
+  unsigned f0;            // frames of that row done by earlier blocks
+  int n_frames;           // frames completed by this block
+  int n_rows;             // rows completed by this block (the first is row r)
+  int slot0;              // hold row of row r: r mod NR
+  int power;              // XLG_SPECTRUM_POWER: linear rows, else dB
+  float inv_w;
+};
+
+__host__ __device__ constexpr bool spec_fft(int W) { return W >= 4 && W <= SPEC_MAX_W && (W & (W - 1)) == 0; }
+// direct path: frames per CTA (W < SPEC_THREADS: one thread per (frame, bin)), CTAs per frame along y
+__host__ __device__ constexpr int spec_direct_frames(int W) { return W >= SPEC_THREADS ? 1 : SPEC_THREADS / W; }
+__host__ __device__ constexpr int spec_direct_groups(int W) { return (W + SPEC_THREADS - 1) / SPEC_THREADS; }
+__host__ __device__ constexpr size_t spec_direct_smem(int W) {
+  return ((size_t)spec_direct_frames(W) * W + W) * sizeof(float2);
+}
+
+// frame j of this block: its first sample's stream position and its hold row
+struct SpecFrame {
+  long long pos;
+  int hold_row;
+};
+__device__ __forceinline__ SpecFrame spec_frame(const SpecBlk &b, int j) {
+  const unsigned g = b.f0 + (unsigned)j, rr = g / (unsigned)b.F, ff = g - rr * (unsigned)b.F;
+  return {b.base + (long long)rr * b.R + (long long)ff * b.W, (int)(((unsigned)b.slot0 + rr) % (unsigned)b.NR)};
+}
+
+__device__ __forceinline__ unsigned spec_power(float2 X, float inv) {
+  const float cx = __fmul_rn(X.x, inv), cy = __fmul_rn(X.y, inv);
+  return __float_as_uint(__fadd_rn(__fadd_rn(__fmul_rn(cx, cx), __fmul_rn(cy, cy)), 1e-20f));
+}
+
+// CTA (x, s) transforms frames [x F, x F + F) of spectrum s, F = bank_fft_frames(W), one row of W each in shared
+// memory, and folds their powers into the hold (below W = 256 a CTA first takes the max over runs of its frames)
+__global__ void __launch_bounds__(SPEC_THREADS)
+spectrum_fft_kernel(const SpecBlk *__restrict__ blk, const float2 *__restrict__ ring) {
+  extern __shared__ __align__(16) float2 u[];
+  const SpecBlk b = blk[blockIdx.y];
+  if (!spec_fft(b.W)) return;
+  const int W = b.W, F = bank_fft_frames(W);
+  const int j0 = blockIdx.x * F;
+  if (j0 >= b.n_frames) return;
+  const int nf = min(F, b.n_frames - j0), tid = threadIdx.x, lw = 31 - __clz(W);
+  for (int e = tid; e < nf * W; e += SPEC_THREADS) {
+    const long long pos = spec_frame(b, j0 + (e >> lw)).pos + (e & (W - 1));
+    u[e] = ring[(unsigned)((unsigned long long)pos) & b.mask];
+  }
+  __syncthreads();
+  fft_dif_rows<SPEC_THREADS>(u, nf, W, lw, b.tw, tid);
+  if (W >= SPEC_THREADS) {  // at most 8 frames: one atomicMax per power
+    for (int e = tid; e < nf * W; e += SPEC_THREADS) {
+      const int h = spec_frame(b, j0 + (e >> lw)).hold_row;
+      atomicMax(b.hold + (size_t)h * W + (e & (W - 1)), spec_power(u[e], b.inv_w));
+    }
+    return;
+  }
+  // narrow rows, many frames: the powers' bits in place of the transformed rows, then a thread takes one position
+  // over a run of frames, keeps their max and issues one atomicMax per hold row the run meets (the max does not
+  // depend on the order)
+  unsigned *pw = reinterpret_cast<unsigned *>(u);
+  for (int e = tid; e < nf * W; e += SPEC_THREADS) pw[2 * e] = spec_power(u[e], b.inv_w);
+  __syncthreads();
+  // (W divides SPEC_THREADS: thread tid takes position tid mod W over run tid / W)
+  const int runs = SPEC_THREADS / W, per = (nf + runs - 1) / runs;
+  const int q = tid & (W - 1), f0 = (tid >> lw) * per, f1 = min(nf, f0 + per);
+  int h = -1;
+  unsigned m = 0u;
+  for (int f = f0; f < f1; f++) {
+    const int hf = spec_frame(b, j0 + f).hold_row;
+    if (hf != h) {
+      if (h >= 0) atomicMax(b.hold + (size_t)h * W + q, m);
+      h = hf;
+      m = 0u;
+    }
+    m = max(m, pw[2 * ((f << lw) + q)]);
+  }
+  if (h >= 0) atomicMax(b.hold + (size_t)h * W + q, m);
+}
+
+// CTA (x, y, s) computes bins [y 256, y 256 + 256) of frames [x Fd, x Fd + Fd) of spectrum s,
+// Fd = spec_direct_frames(W): the frames and the table in shared memory, one bin of one frame per thread
+__global__ void __launch_bounds__(SPEC_THREADS)
+spectrum_direct_kernel(const SpecBlk *__restrict__ blk, const float2 *__restrict__ ring) {
+  extern __shared__ __align__(16) float2 sm[];
+  const SpecBlk b = blk[blockIdx.z];
+  const int W = b.W;
+  if (spec_fft(W)) return;
+  const int Fd = spec_direct_frames(W), j0 = blockIdx.x * Fd, k0 = blockIdx.y * SPEC_THREADS;
+  if (j0 >= b.n_frames || k0 >= W) return;
+  const int nf = min(Fd, b.n_frames - j0), tid = threadIdx.x;
+  float2 *tw = sm, *xs = sm + W;
+  for (int i = tid; i < W; i += SPEC_THREADS) tw[i] = b.tw[i];
+  for (int e = tid; e < nf * W; e += SPEC_THREADS) {
+    const int f = e / W;
+    const long long pos = spec_frame(b, j0 + f).pos + (e - f * W);
+    xs[e] = ring[(unsigned)((unsigned long long)pos) & b.mask];
+  }
+  __syncthreads();
+  const int wb = min(W, SPEC_THREADS), f = tid / wb, k = k0 + tid - f * wb;
+  if (f >= nf || k >= W) return;
+  const float2 *x = xs + f * W;
+  float2 acc = make_float2(0.f, 0.f);
+  int t = 0;
+  for (int n = 0; n < W; n++) {
+    const float2 a = x[n], w = tw[t];
+    acc.x = fmaf(a.x, w.x, acc.x);
+    acc.x = fmaf(-a.y, w.y, acc.x);
+    acc.y = fmaf(a.x, w.y, acc.y);
+    acc.y = fmaf(a.y, w.x, acc.y);
+    t += k;
+    if (t >= W) t -= W;
+  }
+  atomicMax(b.hold + (size_t)spec_frame(b, j0 + f).hold_row * W + k, spec_power(acc, b.inv_w));
+}
+
+// CTA (x, s) writes values [x 256, x 256 + 256) of the n_rows x W values of the rows spectrum s completed in
+// this block, and empties what it read of the hold
+__global__ void __launch_bounds__(SPEC_THREADS) spectrum_emit_kernel(const SpecBlk *__restrict__ blk) {
+  const SpecBlk b = blk[blockIdx.y];
+  const int e = blockIdx.x * SPEC_THREADS + threadIdx.x;
+  if (e >= b.n_rows * b.W) return;
+  const int i = e / b.W, j = e - i * b.W;
+  unsigned *hold = b.hold + (size_t)((b.slot0 + i) % b.NR) * b.W + b.map[j];
+  const float v = __uint_as_float(*hold);
+  *hold = 0u;
+  b.out[e] = b.power ? v : __fmul_rn(10.f, log10f(v));
 }
 
 }  // namespace xl
