@@ -252,6 +252,20 @@ uint64_t xlg_bank_fft_flops(uint32_t K);
  *   enqueued).  Attaching or removing a spectrum changes no client's output. */
 int xlg_add_spectrum(xlg_group *g, uint32_t width, uint32_t frames_per_row, uint32_t skip_per_row, uint32_t flags,
                      int *spectrum_id);
+/* Spectrum rows of a source's output instead of the band: defined exactly as xlg_add_spectrum's, with x the
+ * source's cf32 output stream and P its output position when the next block is submitted (positions count from
+ * there, so a spectrum attached with its client, before the client's first block, covers the client's whole output:
+ * the reference tool's rows of the file sdr-server writes for it; spectrogram_params(client_rate, W) gives the tool's
+ * F and S).  A client's stream is what xlg_output returns for it, ticket after ticket (a cascade client's final
+ * row); a sub-band's or a bank channel's (a sub-band id) is its rows at fs / decim1.  The ids, rows, widths, info,
+ * profile and removal are xlg_add_spectrum's, and every refusal of xlg_add_spectrum applies; -EINVAL (logged) for
+ * an unknown client or sub-band id.  While a spectrum reads it, xlg_remove_client and xlg_remove_subband return
+ * -EBUSY (logged) for its source (and a bank with channels cannot be removed).  Attaching or removing one changes
+ * no client's output and no band spectrum's rows. */
+int xlg_add_client_spectrum(xlg_group *g, int client_id, uint32_t width, uint32_t frames_per_row,
+                            uint32_t skip_per_row, uint32_t flags, int *spectrum_id);
+int xlg_add_subband_spectrum(xlg_group *g, int subband_id, uint32_t width, uint32_t frames_per_row,
+                             uint32_t skip_per_row, uint32_t flags, int *spectrum_id);
 /* Drops its partial row.  -EINVAL for an unknown id. */
 int xlg_remove_spectrum(xlg_group *g, int spectrum_id);
 /* The rows a spectrum completed in a ticket: *n_rows x W contiguous floats, in pinned host memory, or in HBM for
@@ -276,6 +290,10 @@ int xlg_spectrum_info(const xlg_group *g, int spectrum_id, int *kernel, uint64_t
  * one row like a sub-band); a member counts its
  * final row of floor(n1 * interp2 / decim2) + 2, rounded up to 4 (interp2 = 1 for xlg_add_client_subband).
  * A spectrum counts ceil((max_input_len/2/R + 1) * W / 2) samples, rounded up to 4: room for its rows of W floats.
+ * A spectrum of a source (xlg_add_client_spectrum, xlg_add_subband_spectrum) counts the same with max_input_len/2
+ * replaced by its source's row capacity: out_cap = max_input_len/2 * L / D + 2 for a client, the final row's
+ * floor(out_cap * interp2 / decim2) + 2 for a cascade, n1 for a sub-band or bank channel, a member's final row for
+ * a sub-band member.
  * Optional: the arenas grow on demand when clients are added, but a growth re-allocates every ring entry and
  * the results still waiting in the ring are lost (-ESTALE for consumers that had not read them yet, like a
  * block overwritten in the reference's queue).  A server that knows its client limit reserves once, up front. */

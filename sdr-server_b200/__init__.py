@@ -196,6 +196,10 @@ def lib() -> C.CDLL:
     L.xlg_bank_fft_flops.restype = C.c_uint64
     L.xlg_add_spectrum.argtypes = [vp, u32, u32, u32, u32, C.POINTER(C.c_int)]
     L.xlg_add_spectrum.restype = C.c_int
+    L.xlg_add_client_spectrum.argtypes = [vp, C.c_int, u32, u32, u32, u32, C.POINTER(C.c_int)]
+    L.xlg_add_client_spectrum.restype = C.c_int
+    L.xlg_add_subband_spectrum.argtypes = [vp, C.c_int, u32, u32, u32, u32, C.POINTER(C.c_int)]
+    L.xlg_add_subband_spectrum.restype = C.c_int
     L.xlg_remove_spectrum.argtypes = [vp, C.c_int]
     L.xlg_remove_spectrum.restype = C.c_int
     L.xlg_spectrum_output.argtypes = [vp, C.c_int64, C.c_int, C.POINTER(C.POINTER(C.c_float)), C.POINTER(sz)]
@@ -538,6 +542,29 @@ class Group:
         sid = C.c_int(-1)
         code = self._L.xlg_add_spectrum(self._h, width, frames_per_row, skip, XLG_SPECTRUM_POWER if power else 0,
                                         C.byref(sid))
+        if code != 0:
+            raise ValueError(code)
+        return sid.value
+
+    def add_client_spectrum(self, cid: int, width: int, frames_per_row: int, skip: int = 0,
+                            power: bool = False) -> int:
+        """A spectrum of client `cid`'s output stream (xlg_add_client_spectrum): add_spectrum's rows of what
+        output() returns for it from the next submitted block on (a cascade client's final row).
+        spectrogram_params(client_rate, width) gives the reference tool's parameters for the client's file."""
+        sid = C.c_int(-1)
+        code = self._L.xlg_add_client_spectrum(self._h, cid, width, frames_per_row, skip,
+                                               XLG_SPECTRUM_POWER if power else 0, C.byref(sid))
+        if code != 0:
+            raise ValueError(code)
+        return sid.value
+
+    def add_subband_spectrum(self, sbid: int, width: int, frames_per_row: int, skip: int = 0,
+                             power: bool = False) -> int:
+        """A spectrum of sub-band (or bank channel) `sbid`'s rows at fs / decim1 (xlg_add_subband_spectrum),
+        from the next submitted block on: a zoomed waterfall of the sub-band."""
+        sid = C.c_int(-1)
+        code = self._L.xlg_add_subband_spectrum(self._h, sbid, width, frames_per_row, skip,
+                                                XLG_SPECTRUM_POWER if power else 0, C.byref(sid))
         if code != 0:
             raise ValueError(code)
         return sid.value

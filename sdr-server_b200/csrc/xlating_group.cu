@@ -154,12 +154,18 @@ struct BankHost {
   int taps_off = 0, tw_off = 0, ch_off = 0;
 };
 
-// a spectrum (xlg_add_spectrum): its device tables and hold rows, and its walk from P in 64-bit stream positions
+// a spectrum (xlg_add_spectrum, xlg_add_client_spectrum, xlg_add_subband_spectrum): its device tables and hold
+// rows, and its walk from P in 64-bit stream positions -- the band's, or its source's own, counted from the attach
 struct SpectrumHost {
   bool active = false;
   bool power = false;        // XLG_SPECTRUM_POWER
   int W = 0, F = 0, S = 0, R = 0;
   long long P = 0;
+  int src = -1;              // its source's client index (a client, a cascade's final row, a sub-band or bank
+                             // channel); -1: the band
+  long long pos = 0;         // source samples appended to d_ring so far (P = 0)
+  float2 *d_ring = nullptr;  // the source's samples at pos & ring_mask
+  unsigned ring_mask = 0;
   uint64_t rows_done = 0;    // rows completed by the blocks submitted so far
   int fir = 0;               // frames of the current row completed so far
   int rows_cap = 0, NR = 0;  // rows a block can complete; hold rows (rows_cap + 1: all that a block touches)
@@ -243,6 +249,8 @@ struct Slot {
   BlkTable<BankBlk> bfblk;       // the same for the FFT banks
   uint64_t bf_poly = 0, bf_flops = 0;
   BlkTable<SpecBlk> spblk;       // spectra with work in this block
+  BlkTable<const float2 *> spring;  // the ring each spblk entry reads
+  BlkTable<CascBlk> spcb;        // spectra of a source: this block's appends to their rings
   uint64_t sp_frames = 0, sp_flops = 0;
   cudaEvent_t ev_spec = nullptr;  // this block's spectra done (the hold rows are updated in block order on it)
   std::atomic<int64_t> ticket{-1};
@@ -608,6 +616,8 @@ static void slot_free(Slot &s) {
   s.bkblk.release();
   s.bfblk.release();
   s.spblk.release();
+  s.spcb.release();
+  s.spring.release();
   if (s.d_sbph) cudaFree(s.d_sbph);
   s.d_sbph = nullptr;
   s.d_pscratch = nullptr;
@@ -960,20 +970,23 @@ static int rebuild_banks(xlg_group *g) {
 static int rebuild_spectra(xlg_group *g, size_t &out_total, size_t &max_hist) {
   for (void *p : g->dead_spec) cudaFree(p);
   g->dead_spec.clear();
-  size_t n = 0;
+  size_t n = 0, n_src = 0;
   for (SpectrumHost &p : g->spectra) {
     if (!p.active) continue;
     p.out_off = (int)out_total;
     out_total += ((size_t)p.rows_cap * p.W + 1) / 2;
     out_total = (out_total + 3) & ~(size_t)3;
-    max_hist = std::max(max_hist, (size_t)p.W - 1);
+    if (p.src < 0)
+      max_hist = std::max(max_hist, (size_t)p.W - 1);
+    else
+      n_src++;  // (its frames read its own ring)
     n++;
   }
   if (n == 0) return 0;
   CU_OK(cudaFuncSetAttribute(spectrum_direct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              (int)spec_direct_smem(SPEC_MAX_W - 1)));
   for (Slot &s : g->slots)
-    if (s.spblk.reserve(n)) return -EIO;
+    if (s.spblk.reserve(n) || s.spring.reserve(n) || s.spcb.reserve(n_src)) return -EIO;
   return 0;
 }
 
@@ -1928,7 +1941,7 @@ extern "C" void xlg_destroy(xlg_group *g) {
     if (h.b2.ring.p) cudaFree(h.b2.ring.p);
   for (float2 *p : g->dead_rings) cudaFree(p);
   for (const SpectrumHost &p : g->spectra)
-    for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold})
+    for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold, (void *)p.d_ring})
       if (d) cudaFree(d);
   for (void *p : g->dead_spec) cudaFree(p);
   for (cudaEvent_t e : g->ev_user) cudaEventDestroy(e);
@@ -2086,10 +2099,22 @@ extern "C" int xlg_reserve(xlg_group *g, size_t output_samples_per_block) {
   return ensure_arenas(g, output_samples_per_block - output_samples_per_block / 5, g->q_alloc);
 }
 
+// the id of a spectrum whose source is client index cid, -1 if none reads it
+static int spectrum_reading(const xlg_group *g, int cid) {
+  for (int id = 0; id < (int)g->spectra.size(); id++)
+    if (g->spectra[id].active && g->spectra[id].src == cid) return id;
+  return -1;
+}
+
 extern "C" int xlg_remove_client(xlg_group *g, int client_id) {
   if (g == nullptr || client_id < 0 || client_id >= (int)g->clients.size() || !g->clients[client_id].active ||
       g->clients[client_id].sb)
     return -EINVAL;
+  if (spectrum_reading(g, client_id) >= 0) {
+    XL_LOG("client %d is the source of spectrum %d; remove the spectrum first", client_id,
+           spectrum_reading(g, client_id));
+    return -EBUSY;
+  }
   g->clients[client_id].active = false;
   if (g->clients[client_id].b2.ring.p) g->dead_rings.push_back(g->clients[client_id].b2.ring.p);  // in-flight tickets read it
   g->clients[client_id].b2 = StageB();
@@ -2173,6 +2198,10 @@ extern "C" int xlg_remove_subband(xlg_group *g, int subband_id) {
   for (const HostClient &h : g->clients) members += h.active && h.mem && h.sb_cid == cid ? 1 : 0;
   if (members > 0) {
     XL_LOG("sub-band %d still has %d members; remove them first", subband_id, members);
+    return -EBUSY;
+  }
+  if (spectrum_reading(g, cid) >= 0) {
+    XL_LOG("sub-band %d is the source of spectrum %d; remove the spectrum first", subband_id, spectrum_reading(g, cid));
     return -EBUSY;
   }
   g->clients[cid].sb = false;
@@ -2420,9 +2449,18 @@ extern "C" int xlg_add_bank_subband(xlg_group *g, int bank_id, int32_t channel, 
   return 0;
 }
 
-extern "C" int xlg_add_spectrum(xlg_group *g, uint32_t width, uint32_t frames_per_row, uint32_t skip_per_row,
-                                uint32_t flags, int *spectrum_id) {
-  if (g == nullptr || spectrum_id == nullptr) return -EINVAL;
+// Samples a block adds at most to the output stream of client index cid (the row capacity rebuild_layout gives
+// it): its row, a cascade's final row, a sub-band's or bank channel's n1
+static int source_cap(const xlg_group *g, const HostClient &h) {
+  const uint64_t half = (uint64_t)g->max_input_len / 2;
+  if (h.mem) return stage_b_rows(half / g->clients[h.sb_cid].D + 2, h.b2.geo.L2, h.b2.geo.D2);
+  const int cap = (int)(half * h.L / h.D + 2);
+  return h.casc ? stage_b_rows((uint64_t)cap, h.b2.geo.L2, h.b2.geo.D2) : cap;
+}
+
+// A spectrum of the band (src = -1) or of client index src's output stream, after the checks of its source
+static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_per_row, uint32_t skip_per_row,
+                        uint32_t flags, int *spectrum_id) {
   if (width == 0 || width > SPEC_MAX_W || frames_per_row == 0) {
     XL_LOG("spectrum: width %u must be in [1, %d] and frames per row %u at least 1", width, SPEC_MAX_W, frames_per_row);
     return -EINVAL;
@@ -2448,9 +2486,15 @@ extern "C" int xlg_add_spectrum(xlg_group *g, uint32_t width, uint32_t frames_pe
   p.F = (int)frames_per_row;
   p.S = (int)skip_per_row;
   p.R = (int)R;
-  p.P = g->S;
-  p.rows_cap = (int)((uint64_t)g->max_input_len / 2 / R + 1);
+  p.src = src;
+  // a source's positions count from here: P = 0 in its own stream
+  const uint64_t cap = src < 0 ? (uint64_t)g->max_input_len / 2 : (uint64_t)source_cap(g, g->clients[src]);
+  p.P = src < 0 ? g->S : 0;
+  p.rows_cap = (int)(cap / R + 1);
   p.NR = p.rows_cap + 1;
+  // a source's ring holds every sample of the frames a block completes: the block's own and W - 1 before them
+  const size_t ring_cap = src < 0 ? 0 : next_pow2((size_t)width - 1 + (size_t)cap);
+  p.ring_mask = (unsigned)(ring_cap - 1);
   const int W = p.W, half = W / 2;
   std::vector<int> map((size_t)W);
   for (int j = 0; j < W; j++) {
@@ -2461,8 +2505,9 @@ extern "C" int xlg_add_spectrum(xlg_group *g, uint32_t width, uint32_t frames_pe
   const std::vector<float2> tw = twiddle_table(W);
   const size_t hold_bytes = (size_t)p.NR * W * sizeof(unsigned);
   if (cudaMalloc(&p.d_tw, W * sizeof(float2)) != cudaSuccess || cudaMalloc(&p.d_map, W * sizeof(int)) != cudaSuccess ||
-      cudaMalloc(&p.d_hold, hold_bytes) != cudaSuccess) {
-    for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold})
+      cudaMalloc(&p.d_hold, hold_bytes) != cudaSuccess ||
+      (ring_cap > 0 && cudaMalloc(&p.d_ring, ring_cap * sizeof(float2)) != cudaSuccess)) {
+    for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold, (void *)p.d_ring})
       if (d) cudaFree(d);
     XL_LOG("spectrum: out of device memory");
     return -ENOMEM;
@@ -2481,6 +2526,34 @@ extern "C" int xlg_add_spectrum(xlg_group *g, uint32_t width, uint32_t frames_pe
   return 0;
 }
 
+extern "C" int xlg_add_spectrum(xlg_group *g, uint32_t width, uint32_t frames_per_row, uint32_t skip_per_row,
+                                uint32_t flags, int *spectrum_id) {
+  if (g == nullptr || spectrum_id == nullptr) return -EINVAL;
+  return add_spectrum(g, -1, width, frames_per_row, skip_per_row, flags, spectrum_id);
+}
+
+extern "C" int xlg_add_client_spectrum(xlg_group *g, int client_id, uint32_t width, uint32_t frames_per_row,
+                                       uint32_t skip_per_row, uint32_t flags, int *spectrum_id) {
+  if (g == nullptr || spectrum_id == nullptr) return -EINVAL;
+  if (client_id < 0 || client_id >= (int)g->clients.size() || !g->clients[client_id].active ||
+      g->clients[client_id].sb) {
+    XL_LOG("client spectrum: client %d does not exist", client_id);
+    return -EINVAL;
+  }
+  return add_spectrum(g, client_id, width, frames_per_row, skip_per_row, flags, spectrum_id);
+}
+
+extern "C" int xlg_add_subband_spectrum(xlg_group *g, int subband_id, uint32_t width, uint32_t frames_per_row,
+                                        uint32_t skip_per_row, uint32_t flags, int *spectrum_id) {
+  if (g == nullptr || spectrum_id == nullptr) return -EINVAL;
+  const int cid = subband_client(g, subband_id);
+  if (cid < 0) {
+    XL_LOG("sub-band spectrum: sub-band %d does not exist", subband_id);
+    return -EINVAL;
+  }
+  return add_spectrum(g, cid, width, frames_per_row, skip_per_row, flags, spectrum_id);
+}
+
 static SpectrumHost *spectrum_of(xlg_group *g, int id) {
   if (id < 0 || id >= (int)g->spectra.size() || !g->spectra[id].active) return nullptr;
   return &g->spectra[id];
@@ -2494,7 +2567,8 @@ extern "C" int xlg_remove_spectrum(xlg_group *g, int spectrum_id) {
     return -EINVAL;
   }
   // in-flight tickets still read the tables and the hold: freed at the next re-layout, which drains
-  for (void *d : {(void *)p->d_tw, (void *)p->d_map, (void *)p->d_hold}) g->dead_spec.push_back(d);
+  for (void *d : {(void *)p->d_tw, (void *)p->d_map, (void *)p->d_hold, (void *)p->d_ring})
+    if (d) g->dead_spec.push_back(d);
   *p = SpectrumHost();
   g->dirty = true;
   return 0;
@@ -2550,6 +2624,7 @@ struct Block {
   // spectrum walk: entries, CTAs of the FFT and direct paths, row values to emit, the end of their rows in the arena
   int n_spec = 0, max_spf_ctas = 0, max_spd_ctas = 0, max_spd_groups = 0, max_sp_values = 0;
   size_t spf_smem = 0, spd_smem = 0, sp_used = 0;
+  int n_spa = 0, max_spa_n = 0;  // appends to spectrum sources' rings, the longest
   // sub-band walk
   int n_sb = 0, max_sb_n1 = 0, max_sb_n2 = 0;
   int max_sbr_ctas = 0, max_sbr_l2 = 0;  // rational classes: output tiles of the longest residue, largest L2
@@ -2656,17 +2731,36 @@ static void walk_banks(Block &b) {
   }
 }
 
-// Spectra: the frames this block completes (those whose last sample it holds) and the rows they complete, in
-// closed form from the frames completed since P
+// Spectra: a source's new samples appended to the spectrum's ring, then the frames this block completes (those
+// whose last sample it holds) and the rows they complete, in closed form from the frames completed since P.  A
+// source's counts are read here, every block (a re-layout moves its row): a cascade's final row is h.last_n2 at
+// h.b2.fin_off (ho still holds stage A until launch_stage_b), and a sub-band's or bank channel's ho.n_out is
+// zeroed by launch_members after this walk.
 static void walk_spectra(Block &b) {
   xlg_group *g = b.g;
   Slot &s = b.s;
   s.sp_frames = s.sp_flops = 0;
-  const long long E = b.S + b.n;
   for (int id = 0; id < (int)g->spectra.size(); id++) {
     SpectrumHost &p = g->spectra[id];
     b.ho.sp_w[id] = p.active ? p.W : 0;
     if (!p.active) continue;
+    long long E = b.S + b.n;
+    if (p.src >= 0) {
+      const HostClient &h = g->clients[p.src];
+      const int n_src = h.casc ? h.last_n2 : b.ho.n_out[p.src];
+      if (n_src > 0) {
+        CascBlk &cb = s.spcb.h[b.n_spa++];
+        memset(&cb, 0, sizeof(cb));
+        cb.ring = p.d_ring;
+        cb.a_pos = p.pos;
+        cb.mask = p.ring_mask;
+        cb.a_off = h.casc ? h.b2.fin_off : h.out_off;
+        cb.n1 = n_src;
+        b.max_spa_n = std::max(b.max_spa_n, n_src);
+      }
+      p.pos += n_src;
+      E = p.pos;
+    }
     const uint64_t d = (uint64_t)(E - p.P), F = (uint64_t)p.F;
     const uint64_t total = d / (uint64_t)p.R * F + std::min<uint64_t>(F, d % (uint64_t)p.R / (uint64_t)p.W);
     const int n_frames = (int)(total - (p.rows_done * F + (uint64_t)p.fir));
@@ -2674,13 +2768,14 @@ static void walk_spectra(Block &b) {
     b.ho.sp_rows[id] = n_rows;
     b.ho.sp_off[id] = 2 * p.out_off;
     if (n_frames > 0) {
+      s.spring.h[b.n_spec] = p.src < 0 ? g->ring : p.d_ring;
       SpecBlk &e = s.spblk.h[b.n_spec++];
       e.tw = p.d_tw;
       e.map = p.d_map;
       e.hold = p.d_hold;
       e.out = reinterpret_cast<float *>(s.d_out) + 2 * (size_t)p.out_off;
       e.base = p.P + (long long)(p.rows_done * (uint64_t)p.R);
-      e.mask = b.mask;
+      e.mask = p.src < 0 ? b.mask : p.ring_mask;
       e.W = p.W;
       e.F = p.F;
       e.R = p.R;
@@ -2852,20 +2947,28 @@ static int launch_banks(Block &b) {
   return span_end(g, s, SP_BANK_FFT, b.cs);
 }
 
-// Spectra: after the clients' launches, so that no client kernel waits for them; each block's after the previous
-// one's, which emptied the hold rows it reuses
+// Spectra: after the clients' launches (every client, stage-B and member kernel is on b.cs before them), so that no
+// client kernel waits for them; each block's after the previous one's, which emptied the hold rows it reuses and
+// read the sources' rings it appends to.  One append launch for all sources, then the channel stages and the emit
 static int launch_spectra(Block &b) {
   xlg_group *g = b.g;
   Slot &s = b.s;
-  if (b.n_spec == 0) return 0;
+  if (b.n_spec == 0 && b.n_spa == 0) return 0;
   if (g->have_last_spec) CU_OK(cudaStreamWaitEvent(b.cs, g->ev_last_spec, 0));
   if (span_begin(g, s, SP_SPEC, b.cs)) return -EIO;
-  CU_OK(s.spblk.upload((size_t)b.n_spec, b.cs));
+  if (b.n_spa > 0) {
+    CU_OK(s.spcb.upload((size_t)b.n_spa, b.cs));
+    cascade_launch_append(s.spcb.d, b.n_spa, b.max_spa_n, s.d_out, b.cs);
+  }
+  if (b.n_spec > 0) {
+    CU_OK(s.spblk.upload((size_t)b.n_spec, b.cs));
+    CU_OK(s.spring.upload((size_t)b.n_spec, b.cs));
+  }
   if (b.max_spf_ctas > 0)
-    spectrum_fft_kernel<<<dim3(b.max_spf_ctas, b.n_spec), SPEC_THREADS, b.spf_smem, b.cs>>>(s.spblk.d, g->ring);
+    spectrum_fft_kernel<<<dim3(b.max_spf_ctas, b.n_spec), SPEC_THREADS, b.spf_smem, b.cs>>>(s.spblk.d, s.spring.d);
   if (b.max_spd_ctas > 0)
     spectrum_direct_kernel<<<dim3(b.max_spd_ctas, b.max_spd_groups, b.n_spec), SPEC_THREADS, b.spd_smem, b.cs>>>(
-        s.spblk.d, g->ring);
+        s.spblk.d, s.spring.d);
   if (b.max_sp_values > 0)
     spectrum_emit_kernel<<<dim3((b.max_sp_values + SPEC_THREADS - 1) / SPEC_THREADS, b.n_spec), SPEC_THREADS, 0,
                            b.cs>>>(s.spblk.d);

@@ -1770,8 +1770,10 @@ bank_fft_cf32_kernel(const BankBlk *__restrict__ blk, const float2 *__restrict__
 }
 
 // ---------------------------------------------------------------------------
-// Spectrum rows (xlg_add_spectrum).  A spectrum of width W, F frames per row and S samples skipped per row,
-// attached at stream position P, has period R = F W + S; row r is the max-hold over the frames
+// Spectrum rows (xlg_add_spectrum, and xlg_add_client_spectrum / xlg_add_subband_spectrum, whose stream x is a
+// source's output, appended by cascade_append_kernel to a ring of the spectrum's own and counted from its attach,
+// P = 0).  A spectrum of width W, F frames per row and S samples skipped per row, attached at stream position P,
+// has period R = F W + S; row r is the max-hold over the frames
 // x[P + r R + f W ... + W), f < F, of the power of each DFT bin (src/spectrogram/spectrogram.c).  Per frame and
 // bin, with X the frame's DFT and inv = 1/W rounded to float once, in this order (rounded operations, no
 // contraction):
@@ -1800,7 +1802,7 @@ struct SpecBlk {          // one spectrum, this block
   unsigned *hold;         // NR rows of W: each row's running max (float bits), zero when empty
   float *out;             // its rows in the slot's arena: n_rows x W
   long long base;         // stream position of the first row this block touches: P + r R
-  unsigned mask;          // input ring capacity - 1
+  unsigned mask;          // capacity - 1 of the ring it reads
   int W, F, R, NR;
   unsigned f0;            // frames of that row done by earlier blocks
   int n_frames;           // frames completed by this block
@@ -1809,6 +1811,8 @@ struct SpecBlk {          // one spectrum, this block
   int power;              // XLG_SPECTRUM_POWER: linear rows, else dB
   float inv_w;
 };
+// (the ring each entry reads comes in a table of its own, rings[s]: the group's input ring or the spectrum's source
+// ring, whose capacity - 1 is the entry's mask -- a pointer more in SpecBlk would change spectrum_emit_kernel too)
 
 __host__ __device__ constexpr bool spec_fft(int W) { return W >= 4 && W <= SPEC_MAX_W && (W & (W - 1)) == 0; }
 // direct path: frames per CTA (W < SPEC_THREADS: one thread per (frame, bin)), CTAs per frame along y
@@ -1836,9 +1840,10 @@ __device__ __forceinline__ unsigned spec_power(float2 X, float inv) {
 // CTA (x, s) transforms frames [x F, x F + F) of spectrum s, F = bank_fft_frames(W), one row of W each in shared
 // memory, and folds their powers into the hold (below W = 256 a CTA first takes the max over runs of its frames)
 __global__ void __launch_bounds__(SPEC_THREADS)
-spectrum_fft_kernel(const SpecBlk *__restrict__ blk, const float2 *__restrict__ ring) {
+spectrum_fft_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__restrict__ rings) {
   extern __shared__ __align__(16) float2 u[];
   const SpecBlk b = blk[blockIdx.y];
+  const float2 *__restrict__ ring = rings[blockIdx.y];
   if (!spec_fft(b.W)) return;
   const int W = b.W, F = bank_fft_frames(W);
   const int j0 = blockIdx.x * F;
@@ -1883,9 +1888,10 @@ spectrum_fft_kernel(const SpecBlk *__restrict__ blk, const float2 *__restrict__ 
 // CTA (x, y, s) computes bins [y 256, y 256 + 256) of frames [x Fd, x Fd + Fd) of spectrum s,
 // Fd = spec_direct_frames(W): the frames and the table in shared memory, one bin of one frame per thread
 __global__ void __launch_bounds__(SPEC_THREADS)
-spectrum_direct_kernel(const SpecBlk *__restrict__ blk, const float2 *__restrict__ ring) {
+spectrum_direct_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__restrict__ rings) {
   extern __shared__ __align__(16) float2 sm[];
   const SpecBlk b = blk[blockIdx.z];
+  const float2 *__restrict__ ring = rings[blockIdx.z];
   const int W = b.W;
   if (spec_fft(W)) return;
   const int Fd = spec_direct_frames(W), j0 = blockIdx.x * Fd, k0 = blockIdx.y * SPEC_THREADS;
