@@ -266,6 +266,36 @@ int xlg_add_client_spectrum(xlg_group *g, int client_id, uint32_t width, uint32_
                             uint32_t skip_per_row, uint32_t flags, int *spectrum_id);
 int xlg_add_subband_spectrum(xlg_group *g, int subband_id, uint32_t width, uint32_t frames_per_row,
                              uint32_t skip_per_row, uint32_t flags, int *spectrum_id);
+/* Windowed, overlapped and averaged spectra (Welch's method), of the band, a client or a sub-band (source, and
+ * source_id as for xlg_add_client_spectrum / xlg_add_subband_spectrum; ignored for the band).  The definition is
+ * xlg_add_spectrum's with three more parameters:
+ *   hop H >= 1 (0 means W): row period R = (F - 1) * H + W + S; row r covers the frames x[P + r R + f H ... + W),
+ *     f < F, so frames overlap by W - H samples when H < W.  With H = W this is xlg_add_spectrum's.
+ *   window w[0..W) (copied; NULL: none): each frame is z[n] = (x[n].re * w[n], x[n].im * w[n]), one rounded float
+ *     multiply each, before the DFT.  No window is bit for bit a window of ones.
+ *   reduce: XLG_SPECTRUM_MAX, the max of p over the row's frames as above, or XLG_SPECTRUM_MEAN: s = +0, then
+ *     s = s + p_f for f = 0 .. F - 1 in frame order (one rounded float add each), v = s / float(F) (float(F)
+ *     rounded to nearest, the division correctly rounded).
+ * p, the half swap, dB or linear power and the ticket a row comes with (the one whose block holds the row's last
+ * frame sample, P + r R + (F - 1) H + W - 1) are xlg_add_spectrum's.  With a window w W / sum(w), mean rows are
+ * scipy.signal.welch(x, window, nperseg=W, noverlap=W-H, detrend=False, return_onesided=False,
+ * scaling="spectrum") + 1e-20, up to float32 rounding and before the half swap.
+ * Ids, rows, widths, info, profile, removal and the sources' -EBUSY rules are xlg_add_spectrum's; xlg_reserve
+ * counts a spectrum's rows with this R.  A desc with H = W, no window and the max is served exactly as
+ * xlg_add_spectrum.  A mean spectrum keeps a frame buffer of ((cap - 1) / min(H, W + S) + 1) x W floats in HBM,
+ * cap being max_input_len/2 or the source's row capacity: the most frames a block completes.
+ * -EINVAL (logged, nothing changed) for every refusal of xlg_add_spectrum, a NULL desc, an unknown source, client
+ * or sub-band id, 8 H < W (more than 7/8 overlap), R >= 2^31, a window weight that is not finite or an unknown
+ * reduce; -ENOTSUP (logged) on an XLG_TRACK_STATE group. */
+enum { XLG_SPECTRUM_MAX = 0, XLG_SPECTRUM_MEAN = 1 };                        /* xlg_spectrum_desc.reduce */
+enum { XLG_SOURCE_BAND = 0, XLG_SOURCE_CLIENT = 1, XLG_SOURCE_SUBBAND = 2 }; /* xlg_add_spectrum_ex source */
+typedef struct {
+  uint32_t width, frames_per_row, skip_per_row, flags; /* as xlg_add_spectrum (flags: XLG_SPECTRUM_POWER) */
+  uint32_t hop;        /* samples from one frame's start to the next within a row; 0 means width */
+  uint32_t reduce;     /* XLG_SPECTRUM_MAX or XLG_SPECTRUM_MEAN */
+  const float *window; /* width weights, copied; NULL: none */
+} xlg_spectrum_desc;
+int xlg_add_spectrum_ex(xlg_group *g, int source, int source_id, const xlg_spectrum_desc *desc, int *spectrum_id);
 /* Drops its partial row.  -EINVAL for an unknown id. */
 int xlg_remove_spectrum(xlg_group *g, int spectrum_id);
 /* The rows a spectrum completed in a ticket: *n_rows x W contiguous floats, in pinned host memory, or in HBM for
@@ -431,11 +461,12 @@ int xlg_bank_fft_profile_read(xlg_group *g, xlg_bank_fft_profile *p, int reset);
 
 /* Spectra (xlg_add_spectrum), counted like xlg_profile's while profiling is enabled. */
 typedef struct {
-  double spectrum_ms;        /* the channel stages and the emit pass */
+  double spectrum_ms;        /* the channel stages, the mean's fold and the emit pass */
   uint64_t spectrum_launches;
-  uint64_t frames;           /* W-point frames transformed */
+  uint64_t frames;           /* W-point frames transformed (overlapped frames each count) */
   uint64_t channel_flops;    /* FP32 instructions of the channel stages: per frame xlg_bank_fft_flops(W) + 6 W on
-                                the FFT path, 4 W^2 + 6 W on the direct path (an fmaf counts one) */
+                                the FFT path, 4 W^2 + 6 W on the direct path (an fmaf counts one); 2 W more for a
+                                windowed spectrum's frame and W more for a mean spectrum's (the fold's adds) */
 } xlg_spectrum_profile;
 int xlg_spectrum_profile_read(xlg_group *g, xlg_spectrum_profile *p, int reset);
 

@@ -106,6 +106,12 @@ class XlgSpectrumProfile(C.Structure):
                 ("channel_flops", C.c_uint64)]
 
 
+class XlgSpectrumDesc(C.Structure):  # xlg_add_spectrum_ex
+    _fields_ = [("width", C.c_uint32), ("frames_per_row", C.c_uint32), ("skip_per_row", C.c_uint32),
+                ("flags", C.c_uint32), ("hop", C.c_uint32), ("reduce", C.c_uint32),
+                ("window", C.POINTER(C.c_float))]
+
+
 def build(verbose: bool = False) -> None:
     """Compile lib/libxlating_b200.so for sm_90a (nvcc cross-compiles without a GPU)."""
     subprocess.run(["make", "-C", HERE, "all"], check=True,
@@ -200,6 +206,8 @@ def lib() -> C.CDLL:
     L.xlg_add_client_spectrum.restype = C.c_int
     L.xlg_add_subband_spectrum.argtypes = [vp, C.c_int, u32, u32, u32, u32, C.POINTER(C.c_int)]
     L.xlg_add_subband_spectrum.restype = C.c_int
+    L.xlg_add_spectrum_ex.argtypes = [vp, C.c_int, C.c_int, C.POINTER(XlgSpectrumDesc), C.POINTER(C.c_int)]
+    L.xlg_add_spectrum_ex.restype = C.c_int
     L.xlg_remove_spectrum.argtypes = [vp, C.c_int]
     L.xlg_remove_spectrum.restype = C.c_int
     L.xlg_spectrum_output.argtypes = [vp, C.c_int64, C.c_int, C.POINTER(C.POINTER(C.c_float)), C.POINTER(sz)]
@@ -534,11 +542,33 @@ class Group:
         if code != 0:
             raise ValueError(code)
 
-    def add_spectrum(self, width: int, frames_per_row: int, skip: int = 0, power: bool = False) -> int:
+    def _add_spectrum_ex(self, source, source_id, width, frames_per_row, skip, power, hop, window, mean):
+        """xlg_add_spectrum_ex (hop None: width; window: `width` weights or None; mean: the mean of the row's
+        frames instead of their max)."""
+        w = None
+        if window is not None:
+            w = np.ascontiguousarray(window, np.float32)
+            if w.shape != (width,):
+                raise ValueError(f"window of shape {w.shape}, width {width}")
+        desc = XlgSpectrumDesc(width, frames_per_row, skip, XLG_SPECTRUM_POWER if power else 0,
+                               0 if hop is None else hop, 1 if mean else 0,
+                               None if w is None else w.ctypes.data_as(C.POINTER(C.c_float)))
+        sid = C.c_int(-1)
+        code = self._L.xlg_add_spectrum_ex(self._h, source, source_id, C.byref(desc), C.byref(sid))
+        if code != 0:
+            raise ValueError(code)
+        return sid.value
+
+    def add_spectrum(self, width: int, frames_per_row: int, skip: int = 0, power: bool = False,
+                     hop=None, window=None, mean: bool = False) -> int:
         """A spectrum (xlg_add_spectrum) attached before the next submitted block: rows of the max-held power of
         `frames_per_row` consecutive `width`-point DFT frames, `skip` samples skipped after each row, half swapped
         as the reference's spectrogram; dB rows, or linear power with power=True.  spectrogram_params(fs, width)
-        gives the reference tool's frames_per_row and skip.  Returns a spectrum id."""
+        gives the reference tool's frames_per_row and skip.  Returns a spectrum id.
+        With `hop` (samples between frame starts in a row), `window` (`width` float weights) or mean=True (the
+        mean of the frames' powers instead of their max) it is a Welch spectrum (xlg_add_spectrum_ex)."""
+        if hop is not None or window is not None or mean:
+            return self._add_spectrum_ex(0, 0, width, frames_per_row, skip, power, hop, window, mean)
         sid = C.c_int(-1)
         code = self._L.xlg_add_spectrum(self._h, width, frames_per_row, skip, XLG_SPECTRUM_POWER if power else 0,
                                         C.byref(sid))
@@ -547,10 +577,13 @@ class Group:
         return sid.value
 
     def add_client_spectrum(self, cid: int, width: int, frames_per_row: int, skip: int = 0,
-                            power: bool = False) -> int:
+                            power: bool = False, hop=None, window=None, mean: bool = False) -> int:
         """A spectrum of client `cid`'s output stream (xlg_add_client_spectrum): add_spectrum's rows of what
         output() returns for it from the next submitted block on (a cascade client's final row).
-        spectrogram_params(client_rate, width) gives the reference tool's parameters for the client's file."""
+        spectrogram_params(client_rate, width) gives the reference tool's parameters for the client's file.
+        hop, window and mean as for add_spectrum."""
+        if hop is not None or window is not None or mean:
+            return self._add_spectrum_ex(1, cid, width, frames_per_row, skip, power, hop, window, mean)
         sid = C.c_int(-1)
         code = self._L.xlg_add_client_spectrum(self._h, cid, width, frames_per_row, skip,
                                                XLG_SPECTRUM_POWER if power else 0, C.byref(sid))
@@ -559,9 +592,12 @@ class Group:
         return sid.value
 
     def add_subband_spectrum(self, sbid: int, width: int, frames_per_row: int, skip: int = 0,
-                             power: bool = False) -> int:
+                             power: bool = False, hop=None, window=None, mean: bool = False) -> int:
         """A spectrum of sub-band (or bank channel) `sbid`'s rows at fs / decim1 (xlg_add_subband_spectrum),
-        from the next submitted block on: a zoomed waterfall of the sub-band."""
+        from the next submitted block on: a zoomed waterfall of the sub-band.  hop, window and mean as for
+        add_spectrum."""
+        if hop is not None or window is not None or mean:
+            return self._add_spectrum_ex(2, sbid, width, frames_per_row, skip, power, hop, window, mean)
         sid = C.c_int(-1)
         code = self._L.xlg_add_subband_spectrum(self._h, sbid, width, frames_per_row, skip,
                                                 XLG_SPECTRUM_POWER if power else 0, C.byref(sid))

@@ -40,6 +40,7 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <cmath>
 #include <map>
 #include <mutex>
 #include <numeric>
@@ -173,6 +174,12 @@ struct SpectrumHost {
   int *d_map = nullptr;
   unsigned *d_hold = nullptr;
   int out_off = 0;           // its rows in the slot's arena, in complex samples
+  // xlg_add_spectrum_ex: served by the extended kernels when it has a hop other than W, a window or the mean
+  bool ext = false, mean = false;
+  int H = 0;                 // hop (W for today's spectra)
+  float *d_win = nullptr;    // W weights, or none
+  float *d_fbuf = nullptr;   // mean: fb_frames rows of W, the powers of the frames a block completes
+  int fb_frames = 0;
 };
 
 // members of one sub-band that read the same windows: equal (L2, D2, T2, hist2) and, until their windows have
@@ -250,6 +257,7 @@ struct Slot {
   uint64_t bf_poly = 0, bf_flops = 0;
   BlkTable<SpecBlk> spblk;       // spectra with work in this block
   BlkTable<const float2 *> spring;  // the ring each spblk entry reads
+  BlkTable<SpecExt> spext;       // the extended entries' hop, window and frame buffer (the tail of spblk)
   BlkTable<CascBlk> spcb;        // spectra of a source: this block's appends to their rings
   uint64_t sp_frames = 0, sp_flops = 0;
   cudaEvent_t ev_spec = nullptr;  // this block's spectra done (the hold rows are updated in block order on it)
@@ -618,6 +626,7 @@ static void slot_free(Slot &s) {
   s.spblk.release();
   s.spcb.release();
   s.spring.release();
+  s.spext.release();
   if (s.d_sbph) cudaFree(s.d_sbph);
   s.d_sbph = nullptr;
   s.d_pscratch = nullptr;
@@ -970,9 +979,10 @@ static int rebuild_banks(xlg_group *g) {
 static int rebuild_spectra(xlg_group *g, size_t &out_total, size_t &max_hist) {
   for (void *p : g->dead_spec) cudaFree(p);
   g->dead_spec.clear();
-  size_t n = 0, n_src = 0;
+  size_t n = 0, n_src = 0, n_ext = 0;
   for (SpectrumHost &p : g->spectra) {
     if (!p.active) continue;
+    n_ext += p.ext ? 1 : 0;
     p.out_off = (int)out_total;
     out_total += ((size_t)p.rows_cap * p.W + 1) / 2;
     out_total = (out_total + 3) & ~(size_t)3;
@@ -985,8 +995,10 @@ static int rebuild_spectra(xlg_group *g, size_t &out_total, size_t &max_hist) {
   if (n == 0) return 0;
   CU_OK(cudaFuncSetAttribute(spectrum_direct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              (int)spec_direct_smem(SPEC_MAX_W - 1)));
+  CU_OK(cudaFuncSetAttribute(spectrum_direct_ext_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             (int)spec_direct_smem(SPEC_MAX_W - 1)));
   for (Slot &s : g->slots)
-    if (s.spblk.reserve(n) || s.spring.reserve(n) || s.spcb.reserve(n_src)) return -EIO;
+    if (s.spblk.reserve(n) || s.spring.reserve(n) || s.spcb.reserve(n_src) || s.spext.reserve(n_ext)) return -EIO;
   return 0;
 }
 
@@ -1941,7 +1953,8 @@ extern "C" void xlg_destroy(xlg_group *g) {
     if (h.b2.ring.p) cudaFree(h.b2.ring.p);
   for (float2 *p : g->dead_rings) cudaFree(p);
   for (const SpectrumHost &p : g->spectra)
-    for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold, (void *)p.d_ring})
+    for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold, (void *)p.d_ring, (void *)p.d_win,
+                     (void *)p.d_fbuf})
       if (d) cudaFree(d);
   for (void *p : g->dead_spec) cudaFree(p);
   for (cudaEvent_t e : g->ev_user) cudaEventDestroy(e);
@@ -2458,14 +2471,21 @@ static int source_cap(const xlg_group *g, const HostClient &h) {
   return h.casc ? stage_b_rows((uint64_t)cap, h.b2.geo.L2, h.b2.geo.D2) : cap;
 }
 
-// A spectrum of the band (src = -1) or of client index src's output stream, after the checks of its source
+// A spectrum of the band (src = -1) or of client index src's output stream, after the checks of its source.
+// hop 0 means width; today's spectra are hop = width, reduce = XLG_SPECTRUM_MAX and no window.
 static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_per_row, uint32_t skip_per_row,
-                        uint32_t flags, int *spectrum_id) {
+                        uint32_t flags, uint32_t hop, uint32_t reduce, const float *window, int *spectrum_id) {
   if (width == 0 || width > SPEC_MAX_W || frames_per_row == 0) {
     XL_LOG("spectrum: width %u must be in [1, %d] and frames per row %u at least 1", width, SPEC_MAX_W, frames_per_row);
     return -EINVAL;
   }
-  const uint64_t R = (uint64_t)frames_per_row * width + skip_per_row;
+  if (hop == 0) hop = width;
+  if (8ull * hop < width) {
+    XL_LOG("spectrum: a hop of %u is below width / 8 (%u)", hop, width);
+    return -EINVAL;
+  }
+  // (below 2^64: (2^32 - 1)^2 + 2^32 + 4096)
+  const uint64_t R = (uint64_t)(frames_per_row - 1) * hop + width + skip_per_row;
   if (R >= (1ull << 31)) {
     XL_LOG("spectrum: a row period of %llu samples is not below 2^31", (unsigned long long)R);
     return -EINVAL;
@@ -2474,6 +2494,16 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
     XL_LOG("spectrum: unknown flags 0x%x", flags & ~XLG_SPECTRUM_POWER);
     return -EINVAL;
   }
+  if (reduce != XLG_SPECTRUM_MAX && reduce != XLG_SPECTRUM_MEAN) {
+    XL_LOG("spectrum: unknown reduce mode %u", reduce);
+    return -EINVAL;
+  }
+  if (window != nullptr)
+    for (uint32_t n = 0; n < width; n++)
+      if (!std::isfinite(window[n])) {
+        XL_LOG("spectrum: window weight %u is not finite", n);
+        return -EINVAL;
+      }
   if (g->flags & XLG_TRACK_STATE) {
     XL_LOG("spectrum: an XLG_TRACK_STATE group does not serve spectra");
     return -ENOTSUP;
@@ -2486,12 +2516,19 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
   p.F = (int)frames_per_row;
   p.S = (int)skip_per_row;
   p.R = (int)R;
+  p.H = (int)hop;
+  p.mean = reduce == XLG_SPECTRUM_MEAN;
+  p.ext = p.H != p.W || window != nullptr || p.mean;
   p.src = src;
   // a source's positions count from here: P = 0 in its own stream
   const uint64_t cap = src < 0 ? (uint64_t)g->max_input_len / 2 : (uint64_t)source_cap(g, g->clients[src]);
   p.P = src < 0 ? g->S : 0;
   p.rows_cap = (int)(cap / R + 1);
   p.NR = p.rows_cap + 1;
+  // the frames a block of at most cap samples completes: their last samples are distinct positions of the block,
+  // one frame's at least min(H, W + S) after the previous one's (H within a row, W + S from a row's last frame to
+  // the next row's first)
+  if (p.mean) p.fb_frames = (int)((cap - 1) / std::min<uint64_t>(hop, (uint64_t)width + skip_per_row) + 1);
   // a source's ring holds every sample of the frames a block completes: the block's own and W - 1 before them
   const size_t ring_cap = src < 0 ? 0 : next_pow2((size_t)width - 1 + (size_t)cap);
   p.ring_mask = (unsigned)(ring_cap - 1);
@@ -2506,14 +2543,18 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
   const size_t hold_bytes = (size_t)p.NR * W * sizeof(unsigned);
   if (cudaMalloc(&p.d_tw, W * sizeof(float2)) != cudaSuccess || cudaMalloc(&p.d_map, W * sizeof(int)) != cudaSuccess ||
       cudaMalloc(&p.d_hold, hold_bytes) != cudaSuccess ||
-      (ring_cap > 0 && cudaMalloc(&p.d_ring, ring_cap * sizeof(float2)) != cudaSuccess)) {
-    for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold, (void *)p.d_ring})
+      (ring_cap > 0 && cudaMalloc(&p.d_ring, ring_cap * sizeof(float2)) != cudaSuccess) ||
+      (window != nullptr && cudaMalloc(&p.d_win, W * sizeof(float)) != cudaSuccess) ||
+      (p.fb_frames > 0 && cudaMalloc(&p.d_fbuf, (size_t)p.fb_frames * W * sizeof(float)) != cudaSuccess)) {
+    for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold, (void *)p.d_ring, (void *)p.d_win,
+                     (void *)p.d_fbuf})
       if (d) cudaFree(d);
     XL_LOG("spectrum: out of device memory");
     return -ENOMEM;
   }
   CU_OK(cudaMemcpy(p.d_tw, tw.data(), W * sizeof(float2), cudaMemcpyHostToDevice));
   CU_OK(cudaMemcpy(p.d_map, map.data(), W * sizeof(int), cudaMemcpyHostToDevice));
+  if (window != nullptr) CU_OK(cudaMemcpy(p.d_win, window, W * sizeof(float), cudaMemcpyHostToDevice));
   // (on a group stream, finished before the spectrum exists: the kernels' streams do not wait for the legacy one)
   CU_OK(cudaMemsetAsync(p.d_hold, 0, hold_bytes, g->s_in));
   CU_OK(cudaStreamSynchronize(g->s_in));
@@ -2529,7 +2570,8 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
 extern "C" int xlg_add_spectrum(xlg_group *g, uint32_t width, uint32_t frames_per_row, uint32_t skip_per_row,
                                 uint32_t flags, int *spectrum_id) {
   if (g == nullptr || spectrum_id == nullptr) return -EINVAL;
-  return add_spectrum(g, -1, width, frames_per_row, skip_per_row, flags, spectrum_id);
+  return add_spectrum(g, -1, width, frames_per_row, skip_per_row, flags, width, XLG_SPECTRUM_MAX, nullptr,
+                      spectrum_id);
 }
 
 extern "C" int xlg_add_client_spectrum(xlg_group *g, int client_id, uint32_t width, uint32_t frames_per_row,
@@ -2540,7 +2582,8 @@ extern "C" int xlg_add_client_spectrum(xlg_group *g, int client_id, uint32_t wid
     XL_LOG("client spectrum: client %d does not exist", client_id);
     return -EINVAL;
   }
-  return add_spectrum(g, client_id, width, frames_per_row, skip_per_row, flags, spectrum_id);
+  return add_spectrum(g, client_id, width, frames_per_row, skip_per_row, flags, width, XLG_SPECTRUM_MAX, nullptr,
+                      spectrum_id);
 }
 
 extern "C" int xlg_add_subband_spectrum(xlg_group *g, int subband_id, uint32_t width, uint32_t frames_per_row,
@@ -2551,7 +2594,37 @@ extern "C" int xlg_add_subband_spectrum(xlg_group *g, int subband_id, uint32_t w
     XL_LOG("sub-band spectrum: sub-band %d does not exist", subband_id);
     return -EINVAL;
   }
-  return add_spectrum(g, cid, width, frames_per_row, skip_per_row, flags, spectrum_id);
+  return add_spectrum(g, cid, width, frames_per_row, skip_per_row, flags, width, XLG_SPECTRUM_MAX, nullptr,
+                      spectrum_id);
+}
+
+extern "C" int xlg_add_spectrum_ex(xlg_group *g, int source, int source_id, const xlg_spectrum_desc *desc,
+                                   int *spectrum_id) {
+  if (g == nullptr || spectrum_id == nullptr) return -EINVAL;
+  if (desc == nullptr) {
+    XL_LOG("spectrum: no description");
+    return -EINVAL;
+  }
+  int src = -1;
+  if (source == XLG_SOURCE_CLIENT) {
+    if (source_id < 0 || source_id >= (int)g->clients.size() || !g->clients[source_id].active ||
+        g->clients[source_id].sb) {
+      XL_LOG("client spectrum: client %d does not exist", source_id);
+      return -EINVAL;
+    }
+    src = source_id;
+  } else if (source == XLG_SOURCE_SUBBAND) {
+    src = subband_client(g, source_id);
+    if (src < 0) {
+      XL_LOG("sub-band spectrum: sub-band %d does not exist", source_id);
+      return -EINVAL;
+    }
+  } else if (source != XLG_SOURCE_BAND) {
+    XL_LOG("spectrum: unknown source %d", source);
+    return -EINVAL;
+  }
+  return add_spectrum(g, src, desc->width, desc->frames_per_row, desc->skip_per_row, desc->flags, desc->hop,
+                      desc->reduce, desc->window, spectrum_id);
 }
 
 static SpectrumHost *spectrum_of(xlg_group *g, int id) {
@@ -2567,7 +2640,8 @@ extern "C" int xlg_remove_spectrum(xlg_group *g, int spectrum_id) {
     return -EINVAL;
   }
   // in-flight tickets still read the tables and the hold: freed at the next re-layout, which drains
-  for (void *d : {(void *)p->d_tw, (void *)p->d_map, (void *)p->d_hold, (void *)p->d_ring})
+  for (void *d : {(void *)p->d_tw, (void *)p->d_map, (void *)p->d_hold, (void *)p->d_ring, (void *)p->d_win,
+                   (void *)p->d_fbuf})
     if (d) g->dead_spec.push_back(d);
   *p = SpectrumHost();
   g->dirty = true;
@@ -2624,6 +2698,9 @@ struct Block {
   // spectrum walk: entries, CTAs of the FFT and direct paths, row values to emit, the end of their rows in the arena
   int n_spec = 0, max_spf_ctas = 0, max_spd_ctas = 0, max_spd_groups = 0, max_sp_values = 0;
   size_t spf_smem = 0, spd_smem = 0, sp_used = 0;
+  // the extended spectra, the last n_spx entries: their channel stages' CTAs and the values the fold passes over
+  int n_spx = 0, max_spxf_ctas = 0, max_spxd_ctas = 0, max_spxd_groups = 0, max_fold_values = 0;
+  size_t spxf_smem = 0, spxd_smem = 0;
   int n_spa = 0, max_spa_n = 0;  // appends to spectrum sources' rings, the longest
   // sub-band walk
   int n_sb = 0, max_sb_n1 = 0, max_sb_n2 = 0;
@@ -2736,73 +2813,103 @@ static void walk_banks(Block &b) {
 // source's counts are read here, every block (a re-layout moves its row): a cascade's final row is h.last_n2 at
 // h.b2.fin_off (ho still holds stage A until launch_stage_b), and a sub-band's or bank channel's ho.n_out is
 // zeroed by launch_members after this walk.
-static void walk_spectra(Block &b) {
+static void walk_spectrum(Block &b, int id) {
   xlg_group *g = b.g;
   Slot &s = b.s;
-  s.sp_frames = s.sp_flops = 0;
-  for (int id = 0; id < (int)g->spectra.size(); id++) {
-    SpectrumHost &p = g->spectra[id];
-    b.ho.sp_w[id] = p.active ? p.W : 0;
-    if (!p.active) continue;
-    long long E = b.S + b.n;
-    if (p.src >= 0) {
-      const HostClient &h = g->clients[p.src];
-      const int n_src = h.casc ? h.last_n2 : b.ho.n_out[p.src];
-      if (n_src > 0) {
-        CascBlk &cb = s.spcb.h[b.n_spa++];
-        memset(&cb, 0, sizeof(cb));
-        cb.ring = p.d_ring;
-        cb.a_pos = p.pos;
-        cb.mask = p.ring_mask;
-        cb.a_off = h.casc ? h.b2.fin_off : h.out_off;
-        cb.n1 = n_src;
-        b.max_spa_n = std::max(b.max_spa_n, n_src);
-      }
-      p.pos += n_src;
-      E = p.pos;
+  SpectrumHost &p = g->spectra[id];
+  long long E = b.S + b.n;
+  if (p.src >= 0) {
+    const HostClient &h = g->clients[p.src];
+    const int n_src = h.casc ? h.last_n2 : b.ho.n_out[p.src];
+    if (n_src > 0) {
+      CascBlk &cb = s.spcb.h[b.n_spa++];
+      memset(&cb, 0, sizeof(cb));
+      cb.ring = p.d_ring;
+      cb.a_pos = p.pos;
+      cb.mask = p.ring_mask;
+      cb.a_off = h.casc ? h.b2.fin_off : h.out_off;
+      cb.n1 = n_src;
+      b.max_spa_n = std::max(b.max_spa_n, n_src);
     }
-    const uint64_t d = (uint64_t)(E - p.P), F = (uint64_t)p.F;
-    const uint64_t total = d / (uint64_t)p.R * F + std::min<uint64_t>(F, d % (uint64_t)p.R / (uint64_t)p.W);
-    const int n_frames = (int)(total - (p.rows_done * F + (uint64_t)p.fir));
-    const int n_rows = (int)(total / F - p.rows_done);
-    b.ho.sp_rows[id] = n_rows;
-    b.ho.sp_off[id] = 2 * p.out_off;
-    if (n_frames > 0) {
-      s.spring.h[b.n_spec] = p.src < 0 ? g->ring : p.d_ring;
-      SpecBlk &e = s.spblk.h[b.n_spec++];
-      e.tw = p.d_tw;
-      e.map = p.d_map;
-      e.hold = p.d_hold;
-      e.out = reinterpret_cast<float *>(s.d_out) + 2 * (size_t)p.out_off;
-      e.base = p.P + (long long)(p.rows_done * (uint64_t)p.R);
-      e.mask = p.src < 0 ? b.mask : p.ring_mask;
-      e.W = p.W;
-      e.F = p.F;
-      e.R = p.R;
-      e.NR = p.NR;
-      e.f0 = (unsigned)p.fir;
-      e.n_frames = n_frames;
-      e.n_rows = n_rows;
-      e.slot0 = (int)(p.rows_done % (uint64_t)p.NR);
-      e.power = p.power ? 1 : 0;
-      e.inv_w = 1.0f / (float)p.W;
-      const uint64_t flops = spec_fft(p.W) ? xlg_bank_fft_flops((uint32_t)p.W) : 4ull * p.W * p.W;
-      s.sp_frames += (uint64_t)n_frames;
-      s.sp_flops += (uint64_t)n_frames * (flops + 6ull * p.W);
-      if (spec_fft(p.W)) {
-        b.max_spf_ctas = std::max(b.max_spf_ctas, (n_frames + bank_fft_frames(p.W) - 1) / bank_fft_frames(p.W));
-        b.spf_smem = std::max(b.spf_smem, bank_fft_smem(p.W));
-      } else {
-        b.max_spd_ctas = std::max(b.max_spd_ctas, (n_frames + spec_direct_frames(p.W) - 1) / spec_direct_frames(p.W));
-        b.max_spd_groups = std::max(b.max_spd_groups, spec_direct_groups(p.W));
-        b.spd_smem = std::max(b.spd_smem, spec_direct_smem(p.W));
-      }
-      b.max_sp_values = std::max(b.max_sp_values, n_rows * p.W);
-      b.sp_used = std::max(b.sp_used, (size_t)p.out_off + ((size_t)n_rows * p.W + 1) / 2);
-    }
-    p.rows_done = total / F;
-    p.fir = (int)(total % F);
+    p.pos += n_src;
+    E = p.pos;
   }
+  const uint64_t d = (uint64_t)(E - p.P), F = (uint64_t)p.F;
+  uint64_t total;
+  if (p.ext) {  // frames completed at offset o of a row: none before W, then one more every H, at most F
+    const uint64_t o = d % (uint64_t)p.R;
+    total = d / (uint64_t)p.R * F + (o < (uint64_t)p.W ? 0 : std::min<uint64_t>(F, (o - p.W) / (uint64_t)p.H + 1));
+  } else {
+    total = d / (uint64_t)p.R * F + std::min<uint64_t>(F, d % (uint64_t)p.R / (uint64_t)p.W);
+  }
+  const int n_frames = (int)(total - (p.rows_done * F + (uint64_t)p.fir));
+  const int n_rows = (int)(total / F - p.rows_done);
+  b.ho.sp_rows[id] = n_rows;
+  b.ho.sp_off[id] = 2 * p.out_off;
+  if (n_frames > 0) {
+    s.spring.h[b.n_spec] = p.src < 0 ? g->ring : p.d_ring;
+    SpecBlk &e = s.spblk.h[b.n_spec++];
+    e.tw = p.d_tw;
+    e.map = p.d_map;
+    e.hold = p.d_hold;
+    e.out = reinterpret_cast<float *>(s.d_out) + 2 * (size_t)p.out_off;
+    e.base = p.P + (long long)(p.rows_done * (uint64_t)p.R);
+    e.mask = p.src < 0 ? b.mask : p.ring_mask;
+    e.W = p.W;
+    e.F = p.F;
+    e.R = p.R;
+    e.NR = p.NR;
+    e.f0 = (unsigned)p.fir;
+    e.n_frames = n_frames;
+    e.n_rows = n_rows;
+    e.slot0 = (int)(p.rows_done % (uint64_t)p.NR);
+    e.power = p.power ? 1 : 0;
+    e.inv_w = 1.0f / (float)p.W;
+    const uint64_t flops = spec_fft(p.W) ? xlg_bank_fft_flops((uint32_t)p.W) : 4ull * p.W * p.W;
+    s.sp_frames += (uint64_t)n_frames;
+    s.sp_flops += (uint64_t)n_frames * (flops + 6ull * p.W + (p.d_win ? 2ull * p.W : 0) + (p.mean ? p.W : 0));
+    if (p.ext) {
+      SpecExt &x = s.spext.h[b.n_spx++];
+      x.win = p.d_win;
+      x.fbuf = p.d_fbuf;
+      x.H = p.H;
+      x.mean = p.mean ? 1 : 0;
+      if (spec_fft(p.W)) {
+        b.max_spxf_ctas = std::max(b.max_spxf_ctas, (n_frames + bank_fft_frames(p.W) - 1) / bank_fft_frames(p.W));
+        b.spxf_smem = std::max(b.spxf_smem, bank_fft_smem(p.W));
+      } else {
+        b.max_spxd_ctas =
+            std::max(b.max_spxd_ctas, (n_frames + spec_direct_frames(p.W) - 1) / spec_direct_frames(p.W));
+        b.max_spxd_groups = std::max(b.max_spxd_groups, spec_direct_groups(p.W));
+        b.spxd_smem = std::max(b.spxd_smem, spec_direct_smem(p.W));
+      }
+      if (p.mean)  // values of the rows its frames touch
+        b.max_fold_values = std::max(b.max_fold_values, (int)(((long long)p.fir + n_frames - 1) / p.F + 1) * p.W);
+    } else if (spec_fft(p.W)) {
+      b.max_spf_ctas = std::max(b.max_spf_ctas, (n_frames + bank_fft_frames(p.W) - 1) / bank_fft_frames(p.W));
+      b.spf_smem = std::max(b.spf_smem, bank_fft_smem(p.W));
+    } else {
+      b.max_spd_ctas = std::max(b.max_spd_ctas, (n_frames + spec_direct_frames(p.W) - 1) / spec_direct_frames(p.W));
+      b.max_spd_groups = std::max(b.max_spd_groups, spec_direct_groups(p.W));
+      b.spd_smem = std::max(b.spd_smem, spec_direct_smem(p.W));
+    }
+    b.max_sp_values = std::max(b.max_sp_values, n_rows * p.W);
+    b.sp_used = std::max(b.sp_used, (size_t)p.out_off + ((size_t)n_rows * p.W + 1) / 2);
+  }
+  p.rows_done = total / F;
+  p.fir = (int)(total % F);
+}
+
+// every spectrum, today's first: the table is [plain entries | extended entries]
+static void walk_spectra(Block &b) {
+  xlg_group *g = b.g;
+  b.s.sp_frames = b.s.sp_flops = 0;
+  for (int ext = 0; ext < 2; ext++)
+    for (int id = 0; id < (int)g->spectra.size(); id++) {
+      const SpectrumHost &p = g->spectra[id];
+      if (ext == 0) b.ho.sp_w[id] = p.active ? p.W : 0;
+      if (p.active && p.ext == (ext == 1)) walk_spectrum(b, id);
+    }
 }
 
 // Sub-band members: each class walks its sub-band's n1 new samples (ho.n_out of the sub-band) from the sub-band
@@ -2964,11 +3071,25 @@ static int launch_spectra(Block &b) {
     CU_OK(s.spblk.upload((size_t)b.n_spec, b.cs));
     CU_OK(s.spring.upload((size_t)b.n_spec, b.cs));
   }
+  const int n_plain = b.n_spec - b.n_spx;
   if (b.max_spf_ctas > 0)
-    spectrum_fft_kernel<<<dim3(b.max_spf_ctas, b.n_spec), SPEC_THREADS, b.spf_smem, b.cs>>>(s.spblk.d, s.spring.d);
+    spectrum_fft_kernel<<<dim3(b.max_spf_ctas, n_plain), SPEC_THREADS, b.spf_smem, b.cs>>>(s.spblk.d, s.spring.d);
   if (b.max_spd_ctas > 0)
-    spectrum_direct_kernel<<<dim3(b.max_spd_ctas, b.max_spd_groups, b.n_spec), SPEC_THREADS, b.spd_smem, b.cs>>>(
+    spectrum_direct_kernel<<<dim3(b.max_spd_ctas, b.max_spd_groups, n_plain), SPEC_THREADS, b.spd_smem, b.cs>>>(
         s.spblk.d, s.spring.d);
+  if (b.n_spx > 0) {
+    const SpecBlk *xb = s.spblk.d + n_plain;
+    const float2 *const *xr = s.spring.d + n_plain;
+    CU_OK(s.spext.upload((size_t)b.n_spx, b.cs));
+    if (b.max_spxf_ctas > 0)
+      spectrum_fft_ext_kernel<<<dim3(b.max_spxf_ctas, b.n_spx), SPEC_THREADS, b.spxf_smem, b.cs>>>(xb, xr, s.spext.d);
+    if (b.max_spxd_ctas > 0)
+      spectrum_direct_ext_kernel<<<dim3(b.max_spxd_ctas, b.max_spxd_groups, b.n_spx), SPEC_THREADS, b.spxd_smem,
+                                   b.cs>>>(xb, xr, s.spext.d);
+    if (b.max_fold_values > 0)
+      spectrum_fold_kernel<<<dim3((b.max_fold_values + SPEC_THREADS - 1) / SPEC_THREADS, b.n_spx), SPEC_THREADS, 0,
+                             b.cs>>>(xb, s.spext.d);
+  }
   if (b.max_sp_values > 0)
     spectrum_emit_kernel<<<dim3((b.max_sp_values + SPEC_THREADS - 1) / SPEC_THREADS, b.n_spec), SPEC_THREADS, 0,
                            b.cs>>>(s.spblk.d);

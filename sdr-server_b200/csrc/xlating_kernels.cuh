@@ -1935,4 +1935,147 @@ __global__ void __launch_bounds__(SPEC_THREADS) spectrum_emit_kernel(const SpecB
   b.out[e] = b.power ? v : __fmul_rn(10.f, log10f(v));
 }
 
+// ---------------------------------------------------------------------------
+// Extended spectra (xlg_add_spectrum_ex): a hop H between frame starts, a window and a mean.  Row period
+// R = (F - 1) H + W + S; row r covers the frames x[P + r R + f H ... + W), f < F.  Each frame is windowed before
+// the transform, z[n] = (x[n].x * w[n], x[n].y * w[n]) (one rounded multiply each; no window: z = x), and goes
+// through the same channel stage, spec_power and hold as above.  A max spectrum folds by atomicMax as above.  A
+// mean spectrum's channel stage stores each frame's powers (position space, as the hold) in the spectrum's frame
+// buffer, row j of it for frame j of this block; spectrum_fold_kernel then adds them into the hold in frame order,
+//     s = +0;  s = s + p_f for f = 0 .. F - 1 (rounded adds, one frame after the other, across blocks in block order)
+// and divides a completed row once, v = s / float(F) (correctly rounded).  The hold carries s between blocks as
+// float bits (the empty hold, 0, is +0).  spectrum_emit_kernel then writes and empties the row as for any spectrum.
+// The entries are the tail of the block's SpecBlk table, SpecExt holds what only they need.
+// ---------------------------------------------------------------------------
+struct SpecExt {
+  const float *win;  // W weights, or nullptr: no window
+  float *fbuf;       // mean: the frames' powers, a row of W per frame of this block; max: nullptr
+  int H;             // hop
+  int mean;
+};
+
+__device__ __forceinline__ long long spec_frame_pos(const SpecBlk &b, int H, int j) {
+  const unsigned g = b.f0 + (unsigned)j, rr = g / (unsigned)b.F, ff = g - rr * (unsigned)b.F;
+  return b.base + (long long)rr * b.R + (long long)ff * H;
+}
+
+__device__ __forceinline__ float2 spec_load(const float2 *__restrict__ ring, unsigned mask, long long pos,
+                                            const float *__restrict__ win, int n) {
+  const float2 v = ring[(unsigned)((unsigned long long)pos) & mask];
+  if (win == nullptr) return v;
+  const float w = __ldg(win + n);
+  return make_float2(__fmul_rn(v.x, w), __fmul_rn(v.y, w));
+}
+
+// spectrum_fft_kernel with the hop, the window and the mean's frame buffer
+__global__ void __launch_bounds__(SPEC_THREADS)
+spectrum_fft_ext_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__restrict__ rings,
+                        const SpecExt *__restrict__ ext) {
+  extern __shared__ __align__(16) float2 u[];
+  const SpecBlk b = blk[blockIdx.y];
+  const SpecExt x = ext[blockIdx.y];
+  const float2 *__restrict__ ring = rings[blockIdx.y];
+  if (!spec_fft(b.W)) return;
+  const int W = b.W, F = bank_fft_frames(W);
+  const int j0 = blockIdx.x * F;
+  if (j0 >= b.n_frames) return;
+  const int nf = min(F, b.n_frames - j0), tid = threadIdx.x, lw = 31 - __clz(W);
+  for (int e = tid; e < nf * W; e += SPEC_THREADS) {
+    const int n = e & (W - 1);
+    u[e] = spec_load(ring, b.mask, spec_frame_pos(b, x.H, j0 + (e >> lw)) + n, x.win, n);
+  }
+  __syncthreads();
+  fft_dif_rows<SPEC_THREADS>(u, nf, W, lw, b.tw, tid);
+  if (x.mean) {
+    float *fb = x.fbuf + (size_t)j0 * W;
+    for (int e = tid; e < nf * W; e += SPEC_THREADS) fb[e] = __uint_as_float(spec_power(u[e], b.inv_w));
+    return;
+  }
+  if (W >= SPEC_THREADS) {
+    for (int e = tid; e < nf * W; e += SPEC_THREADS) {
+      const int h = spec_frame(b, j0 + (e >> lw)).hold_row;
+      atomicMax(b.hold + (size_t)h * W + (e & (W - 1)), spec_power(u[e], b.inv_w));
+    }
+    return;
+  }
+  unsigned *pw = reinterpret_cast<unsigned *>(u);
+  for (int e = tid; e < nf * W; e += SPEC_THREADS) pw[2 * e] = spec_power(u[e], b.inv_w);
+  __syncthreads();
+  const int runs = SPEC_THREADS / W, per = (nf + runs - 1) / runs;
+  const int q = tid & (W - 1), f0 = (tid >> lw) * per, f1 = min(nf, f0 + per);
+  int h = -1;
+  unsigned m = 0u;
+  for (int f = f0; f < f1; f++) {
+    const int hf = spec_frame(b, j0 + f).hold_row;
+    if (hf != h) {
+      if (h >= 0) atomicMax(b.hold + (size_t)h * W + q, m);
+      h = hf;
+      m = 0u;
+    }
+    m = max(m, pw[2 * ((f << lw) + q)]);
+  }
+  if (h >= 0) atomicMax(b.hold + (size_t)h * W + q, m);
+}
+
+// spectrum_direct_kernel with the hop, the window and the mean's frame buffer
+__global__ void __launch_bounds__(SPEC_THREADS)
+spectrum_direct_ext_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__restrict__ rings,
+                           const SpecExt *__restrict__ ext) {
+  extern __shared__ __align__(16) float2 sm[];
+  const SpecBlk b = blk[blockIdx.z];
+  const SpecExt xe = ext[blockIdx.z];
+  const float2 *__restrict__ ring = rings[blockIdx.z];
+  const int W = b.W;
+  if (spec_fft(W)) return;
+  const int Fd = spec_direct_frames(W), j0 = blockIdx.x * Fd, k0 = blockIdx.y * SPEC_THREADS;
+  if (j0 >= b.n_frames || k0 >= W) return;
+  const int nf = min(Fd, b.n_frames - j0), tid = threadIdx.x;
+  float2 *tw = sm, *xs = sm + W;
+  for (int i = tid; i < W; i += SPEC_THREADS) tw[i] = b.tw[i];
+  for (int e = tid; e < nf * W; e += SPEC_THREADS) {
+    const int f = e / W, n = e - f * W;
+    xs[e] = spec_load(ring, b.mask, spec_frame_pos(b, xe.H, j0 + f) + n, xe.win, n);
+  }
+  __syncthreads();
+  const int wb = min(W, SPEC_THREADS), f = tid / wb, k = k0 + tid - f * wb;
+  if (f >= nf || k >= W) return;
+  const float2 *x = xs + f * W;
+  float2 acc = make_float2(0.f, 0.f);
+  int t = 0;
+  for (int n = 0; n < W; n++) {
+    const float2 a = x[n], w = tw[t];
+    acc.x = fmaf(a.x, w.x, acc.x);
+    acc.x = fmaf(-a.y, w.y, acc.x);
+    acc.y = fmaf(a.x, w.y, acc.y);
+    acc.y = fmaf(a.y, w.x, acc.y);
+    t += k;
+    if (t >= W) t -= W;
+  }
+  const unsigned p = spec_power(acc, b.inv_w);
+  if (xe.mean)
+    xe.fbuf[(size_t)(j0 + f) * W + k] = __uint_as_float(p);
+  else
+    atomicMax(b.hold + (size_t)spec_frame(b, j0 + f).hold_row * W + k, p);
+}
+
+// CTA (x, s) folds values [x 256, x 256 + 256) of the rows x W that mean spectrum s's frames of this block touch:
+// thread (i, q) adds position q of the block's frames in row i, in frame order, to hold row i and divides the sum
+// by float(F) if the block completes that row (i < n_rows)
+__global__ void __launch_bounds__(SPEC_THREADS)
+spectrum_fold_kernel(const SpecBlk *__restrict__ blk, const SpecExt *__restrict__ ext) {
+  const SpecBlk b = blk[blockIdx.y];
+  const SpecExt x = ext[blockIdx.y];
+  if (!x.mean) return;
+  const int W = b.W, touched = (int)((b.f0 + (unsigned)b.n_frames - 1u) / (unsigned)b.F) + 1;
+  const int e = blockIdx.x * SPEC_THREADS + threadIdx.x;
+  if (e >= touched * W) return;
+  const int i = e / W, q = e - i * W;
+  const long long first = (long long)i * b.F - (long long)b.f0;  // row i's frame 0, as a frame of this block
+  const int j1 = (int)min((long long)b.n_frames, first + b.F);
+  unsigned *hold = b.hold + (size_t)((b.slot0 + i) % b.NR) * W + q;
+  float s = __uint_as_float(*hold);
+  for (int j = (int)max(0ll, first); j < j1; j++) s = __fadd_rn(s, x.fbuf[(size_t)j * W + q]);
+  *hold = __float_as_uint(i < b.n_rows ? __fdiv_rn(s, (float)b.F) : s);
+}
+
 }  // namespace xl

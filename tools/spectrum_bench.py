@@ -1,14 +1,18 @@
 """Spectrum rows (xlg_add_spectrum): the spectrum kernels alone, and what a spectrum adds to a step of clients.
 
-    python tools/spectrum_bench.py [--blocks K] [--warmup W] [--rounds R] [--widths W,...]
+    python tools/spectrum_bench.py [--blocks K] [--warmup W] [--rounds R] [--widths W,...] [--variants V,...]
 
-1. Per width W (one JSON line per width and round): a 61.44 Msps cs16 stream in blocks of 262144 bytes, as in
-   bench.py, feeding one spectrum with the reference tool's parameters (F = fs // W, S = fs % W: one row per
-   second of stream).  Reported: the spectrum span's time per block from a profiled run (CUDA events around the
-   channel stage and the emit pass, xlg_spectrum_profile), its kernel (fft or direct) and counted work.
+1. Per width W and variant (one JSON line each, the variants alternated within every round): a 61.44 Msps cs16
+   stream in blocks of 262144 bytes, as in bench.py, feeding one spectrum with the reference tool's parameters
+   (F = fs // W, S = fs % W: one row per second of stream).  Variants: "plain" (xlg_add_spectrum), "hann" (a Hann
+   window, H = W, max) and "hann_mean" (a Hann window, H = W / 2, the mean: Welch's method at 50 % overlap, with
+   F = 2 fs // W - 1 so that a row still spans about a second).  Reported: the spectrum span's time per block
+   from a profiled run (CUDA events around the channel stages, the fold and the emit pass, xlg_spectrum_profile),
+   its kernel (fft or direct) and counted work.
 2. bench.py's cfg2 workload (256 clients at 48 and 96 ksps on a 2.016 Msps cu8 stream, blocks of 262144 bytes,
-   device inputs and outputs) without and with a W = 1024 spectrum (F = 1968, S = 768), the two alternated in
-   every round: the step time per block between device events (xlg_timer_start / _stop), profiling off.
+   device inputs and outputs) without a spectrum, with a W = 1024 spectrum (F = 1968, S = 768) and with a
+   W = 1024, H = 512 Hann mean spectrum (F = 3935, S = 768), alternated in every round: the step time per block
+   between device events (xlg_timer_start / _stop), profiling off.
 
 The card's name, power limit and clocks are printed first, read in the same call.  Nothing is written to the tree.
 """
@@ -28,11 +32,25 @@ pkg = importlib.import_module("sdr-server_b200")
 FS, FMT, BLOCK = 61440000, "cs16", 262144
 
 
-def kernel_run(W, blocks, warmup, data):
-    F, S = pkg.spectrogram_params(FS, W)
+def hann(W):
+    return (0.5 - 0.5 * np.cos(2 * np.pi * np.arange(W) / W)).astype(np.float32)
+
+
+def add(g, fs, W, variant):
+    """One spectrum of the band in the given variant, at the reference tool's row length."""
+    F, S = pkg.spectrogram_params(fs, W)
+    if variant == "plain":
+        return g.add_spectrum(W, F, S), F, S
+    if variant == "hann":
+        return g.add_spectrum(W, F, S, hop=W, window=hann(W)), F, S
+    F = 2 * F - 1  # (F - 1) W / 2 + W + S = the plain row's F W + S
+    return g.add_spectrum(W, F, S, hop=W // 2, window=hann(W), mean=True), F, S
+
+
+def kernel_run(W, variant, blocks, warmup, data):
     g = pkg.Group(FS, BLOCK)
     try:
-        sid = g.add_spectrum(W, F, S)
+        sid, F, S = add(g, FS, W, variant)
         g.profile_enable(True)
         for i in range(warmup):
             g.wait(g.submit(FMT, data[i % len(data)]))
@@ -44,12 +62,12 @@ def kernel_run(W, blocks, warmup, data):
     finally:
         g.close()
     n = p["spectrum_launches"]
-    return {"W": W, "F": F, "S": S, "kernel": kernel, "blocks": blocks, "launches": n,
+    return {"W": W, "variant": variant, "F": F, "S": S, "kernel": kernel, "blocks": blocks, "launches": n,
             "kernel_us_per_block": 1e3 * p["spectrum_ms"] / max(n, 1), "frames": p["frames"],
             "channel_flops": p["channel_flops"]}
 
 
-def step_run(torch, with_spectrum, blocks, warmup):
+def step_run(torch, spectrum, blocks, warmup):
     import bench
     wl = bench.workload("cfg2", "default")
     host = bench.synth_blocks(wl["fmt"], 8, wl["block_elems"], seed=3)
@@ -63,8 +81,8 @@ def step_run(torch, with_spectrum, blocks, warmup):
             if key not in taps:
                 taps[key] = pkg.create_low_pass_filter(1.0, wl["fs"], c["cutoff"], c["tw"])
             g.add_client(c["decimation"], taps[key], c["center"])
-        if with_spectrum:
-            g.add_spectrum(1024, *pkg.spectrogram_params(wl["fs"], 1024))
+        if spectrum != "none":
+            add(g, wl["fs"], 1024, spectrum)
         code = pkg.FMT[wl["fmt"]]
 
         def feed(k):
@@ -80,7 +98,8 @@ def step_run(torch, with_spectrum, blocks, warmup):
         ms = g.timer_stop()
     finally:
         g.close()
-    return {"workload": "cfg2", "spectrum": "W=1024" if with_spectrum else "none", "blocks": blocks,
+    label = spectrum if spectrum == "none" else f"W=1024 {spectrum}"
+    return {"workload": "cfg2", "spectrum": label, "blocks": blocks,
             "step_us_per_block": 1e3 * ms / blocks}
 
 
@@ -90,6 +109,7 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--widths", default="64,1000,1024,4096")
+    ap.add_argument("--variants", default="plain,hann,hann_mean")
     args = ap.parse_args()
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm",
                            "--format=csv,noheader"], capture_output=True, text=True).stdout.strip().splitlines()[0]
@@ -97,13 +117,14 @@ def main():
     import torch
     rng = np.random.default_rng(0)
     data = [rng.integers(-32768, 32767, BLOCK // 2, dtype=np.int16, endpoint=True) for _ in range(4)]
+    variants = args.variants.split(",")
     for r in range(args.rounds):
         for W in [int(w) for w in args.widths.split(",")]:
-            print(json.dumps({**kernel_run(W, args.blocks, args.warmup, data), "round": r}), flush=True)
+            for v in variants:
+                print(json.dumps({**kernel_run(W, v, args.blocks, args.warmup, data), "round": r}), flush=True)
     for r in range(args.rounds):
-        for with_spectrum in (False, True):
-            print(json.dumps({**step_run(torch, with_spectrum, 10 * args.blocks, args.warmup), "round": r}),
-                  flush=True)
+        for spectrum in ["none"] + [v for v in variants if v != "hann"]:
+            print(json.dumps({**step_run(torch, spectrum, 10 * args.blocks, args.warmup), "round": r}), flush=True)
 
 
 if __name__ == "__main__":
