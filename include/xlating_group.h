@@ -245,10 +245,17 @@ uint64_t xlg_bank_fft_flops(uint32_t K);
  *   S = fs % W; its png_util_set_data turns a dB row into 8-bit grey with (int)(dB + 255) clamped to [0, 255].
  *   A row is returned with the ticket whose block holds the row's last frame sample: a block completes zero,
  *   one or many rows, and a row spans as many blocks as it needs.  Removing a spectrum drops its partial row.
- *   W a power of two from 4 to 4096 runs an FFT per frame; any other W a direct DFT of W complex MACs per input
- *   sample.  Spectrum ids come from a small-integer space of their own; xlg_client_count does not count them.
- *   -EINVAL (logged) for W = 0 or above 4096, F = 0, R >= 2^31 or an unknown flag; -ENOTSUP (logged) on an
- *   XLG_TRACK_STATE group.  A group with a spectrum refuses XLG_PATH_Q15 submits (-ENOTSUP, logged, nothing
+ *   W a power of two from 4 to 4096 runs an FFT per frame; any other W up to 4096 a direct DFT of W complex MACs
+ *   per input sample.  W = 8192, 16384, 32768 and 65536 (wide spectra) run the same FFT at K = W in two passes:
+ *   the first one or two radix-4 stages over the frame, then the rest on each 2048- or 4096-point chunk.  X and
+ *   the rows are exactly those of the FFT at K = W (DESIGN.md section 5).  Besides the hold (cap / R + 2 rows of
+ *   W floats, cap as for xlg_add_spectrum_ex), the twiddles (W + C float2, C the chunk), the row map (W ints) and,
+ *   for a source, its ring (next_pow2(W - 1 + cap) float2), a wide spectrum keeps a scratch of
+ *   ((cap - 1) / min(H, W + S) + 1) x W float2 in HBM (H = W here): the most frames a block completes.  A band
+ *   spectrum makes the input ring keep W - 1 samples of history.
+ *   Spectrum ids come from a small-integer space of their own; xlg_client_count does not count them.
+ *   -EINVAL (logged) for W = 0, W above 65536 or above 4096 and not a power of two, F = 0, R >= 2^31 or an unknown
+ *   flag; -ENOTSUP (logged) on an XLG_TRACK_STATE group.  A group with a spectrum refuses XLG_PATH_Q15 submits (-ENOTSUP, logged, nothing
  *   enqueued).  Attaching or removing a spectrum changes no client's output. */
 int xlg_add_spectrum(xlg_group *g, uint32_t width, uint32_t frames_per_row, uint32_t skip_per_row, uint32_t flags,
                      int *spectrum_id);
@@ -283,7 +290,9 @@ int xlg_add_subband_spectrum(xlg_group *g, int subband_id, uint32_t width, uint3
  * Ids, rows, widths, info, profile, removal and the sources' -EBUSY rules are xlg_add_spectrum's; xlg_reserve
  * counts a spectrum's rows with this R.  A desc with H = W, no window and the max is served exactly as
  * xlg_add_spectrum.  A mean spectrum keeps a frame buffer of ((cap - 1) / min(H, W + S) + 1) x W floats in HBM,
- * cap being max_input_len/2 or the source's row capacity: the most frames a block completes.
+ * cap being max_input_len/2 or the source's row capacity: the most frames a block completes.  A wide spectrum
+ * (W from 8192 to 65536, a power of two) keeps its scratch of as many rows of W float2 as well, and a window
+ * W floats.
  * -EINVAL (logged, nothing changed) for every refusal of xlg_add_spectrum, a NULL desc, an unknown source, client
  * or sub-band id, 8 H < W (more than 7/8 overlap), R >= 2^31, a window weight that is not finite or an unknown
  * reduce; -ENOTSUP (logged) on an XLG_TRACK_STATE group. */
@@ -308,8 +317,8 @@ int xlg_spectrum_width(xlg_group *g, int64_t ticket, int spectrum_id, uint32_t *
 /* Waits for the ticket and copies at most cap_rows of its rows (xlg_spectrum_width floats each) into dst;
  * *n_rows = rows it has. */
 int xlg_read_spectrum(xlg_group *g, int64_t ticket, int spectrum_id, float *dst, size_t cap_rows, size_t *n_rows);
-/* The channel stage serving a spectrum (0 = direct DFT, 1 = FFT) and the rows completed by the blocks submitted
- * so far. */
+/* The channel stage serving a spectrum (0 = direct DFT, 1 = FFT, 2 = wide FFT, W above 4096) and the rows
+ * completed by the blocks submitted so far. */
 int xlg_spectrum_info(const xlg_group *g, int spectrum_id, int *kernel, uint64_t *rows_done);
 /* Size the per-ticket result arenas (device and pinned host) for `output_samples_per_block` complex output
  * samples per block summed over all clients (a client at decimation D produces about max_input_len/2/D + 2).

@@ -565,6 +565,7 @@ class Group:
         `frames_per_row` consecutive `width`-point DFT frames, `skip` samples skipped after each row, half swapped
         as the reference's spectrogram; dB rows, or linear power with power=True.  spectrogram_params(fs, width)
         gives the reference tool's frames_per_row and skip.  Returns a spectrum id.
+        `width` is 1 to 4096, or a power of two from 8192 to 65536 (the wide FFT, the same rows as an FFT at K = width).
         With `hop` (samples between frame starts in a row), `window` (`width` float weights) or mean=True (the
         mean of the frames' powers instead of their max) it is a Welch spectrum (xlg_add_spectrum_ex)."""
         if hop is not None or window is not None or mean:
@@ -581,7 +582,7 @@ class Group:
         """A spectrum of client `cid`'s output stream (xlg_add_client_spectrum): add_spectrum's rows of what
         output() returns for it from the next submitted block on (a cascade client's final row).
         spectrogram_params(client_rate, width) gives the reference tool's parameters for the client's file.
-        hop, window and mean as for add_spectrum."""
+        width (1 to 4096, or a power of two from 8192 to 65536), hop, window and mean as for add_spectrum."""
         if hop is not None or window is not None or mean:
             return self._add_spectrum_ex(1, cid, width, frames_per_row, skip, power, hop, window, mean)
         sid = C.c_int(-1)
@@ -594,8 +595,8 @@ class Group:
     def add_subband_spectrum(self, sbid: int, width: int, frames_per_row: int, skip: int = 0,
                              power: bool = False, hop=None, window=None, mean: bool = False) -> int:
         """A spectrum of sub-band (or bank channel) `sbid`'s rows at fs / decim1 (xlg_add_subband_spectrum),
-        from the next submitted block on: a zoomed waterfall of the sub-band.  hop, window and mean as for
-        add_spectrum."""
+        from the next submitted block on: a zoomed waterfall of the sub-band.  width (1 to 4096, or a power of
+        two from 8192 to 65536), hop, window and mean as for add_spectrum."""
         if hop is not None or window is not None or mean:
             return self._add_spectrum_ex(2, sbid, width, frames_per_row, skip, power, hop, window, mean)
         sid = C.c_int(-1)
@@ -641,7 +642,8 @@ class Group:
         return buf
 
     def spectrum_info(self, sid: int):
-        """(kernel: 0 direct DFT, 1 FFT, rows completed by the blocks submitted so far)."""
+        """(kernel: 0 direct DFT, 1 FFT, 2 wide FFT (width above 4096), rows completed by the blocks submitted
+        so far)."""
         kind, rows = C.c_int(-1), C.c_uint64(0)
         code = self._L.xlg_spectrum_info(self._h, sid, C.byref(kind), C.byref(rows))
         if code != 0:

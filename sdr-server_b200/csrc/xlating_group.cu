@@ -179,7 +179,11 @@ struct SpectrumHost {
   int H = 0;                 // hop (W for today's spectra)
   float *d_win = nullptr;    // W weights, or none
   float *d_fbuf = nullptr;   // mean: fb_frames rows of W, the powers of the frames a block completes
-  int fb_frames = 0;
+  int fb_frames = 0;         // the most frames a block completes (kept for a mean or a wide spectrum)
+  // W above SPEC_MAX_W: served by the two wide passes, plain or extended (ext stays false); d_tw holds the W-point
+  // table, then the C-point one
+  bool wide = false;
+  float2 *d_scratch = nullptr;  // fb_frames rows of W: pass A's output
 };
 
 // members of one sub-band that read the same windows: equal (L2, D2, T2, hist2) and, until their windows have
@@ -257,7 +261,8 @@ struct Slot {
   uint64_t bf_poly = 0, bf_flops = 0;
   BlkTable<SpecBlk> spblk;       // spectra with work in this block
   BlkTable<const float2 *> spring;  // the ring each spblk entry reads
-  BlkTable<SpecExt> spext;       // the extended entries' hop, window and frame buffer (the tail of spblk)
+  BlkTable<SpecExt> spext;       // the extended and wide entries' hop, window and frame buffer (the tail of spblk)
+  BlkTable<SpecWide> spwide;     // the wide entries' scratch and chunk table (the tail of spext)
   BlkTable<CascBlk> spcb;        // spectra of a source: this block's appends to their rings
   uint64_t sp_frames = 0, sp_flops = 0;
   cudaEvent_t ev_spec = nullptr;  // this block's spectra done (the hold rows are updated in block order on it)
@@ -627,6 +632,7 @@ static void slot_free(Slot &s) {
   s.spcb.release();
   s.spring.release();
   s.spext.release();
+  s.spwide.release();
   if (s.d_sbph) cudaFree(s.d_sbph);
   s.d_sbph = nullptr;
   s.d_pscratch = nullptr;
@@ -979,10 +985,11 @@ static int rebuild_banks(xlg_group *g) {
 static int rebuild_spectra(xlg_group *g, size_t &out_total, size_t &max_hist) {
   for (void *p : g->dead_spec) cudaFree(p);
   g->dead_spec.clear();
-  size_t n = 0, n_src = 0, n_ext = 0;
+  size_t n = 0, n_src = 0, n_ext = 0, n_wide = 0;
   for (SpectrumHost &p : g->spectra) {
     if (!p.active) continue;
-    n_ext += p.ext ? 1 : 0;
+    n_ext += p.ext || p.wide ? 1 : 0;
+    n_wide += p.wide ? 1 : 0;
     p.out_off = (int)out_total;
     out_total += ((size_t)p.rows_cap * p.W + 1) / 2;
     out_total = (out_total + 3) & ~(size_t)3;
@@ -998,7 +1005,9 @@ static int rebuild_spectra(xlg_group *g, size_t &out_total, size_t &max_hist) {
   CU_OK(cudaFuncSetAttribute(spectrum_direct_ext_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              (int)spec_direct_smem(SPEC_MAX_W - 1)));
   for (Slot &s : g->slots)
-    if (s.spblk.reserve(n) || s.spring.reserve(n) || s.spcb.reserve(n_src) || s.spext.reserve(n_ext)) return -EIO;
+    if (s.spblk.reserve(n) || s.spring.reserve(n) || s.spcb.reserve(n_src) || s.spext.reserve(n_ext) ||
+        s.spwide.reserve(n_wide))
+      return -EIO;
   return 0;
 }
 
@@ -1954,7 +1963,7 @@ extern "C" void xlg_destroy(xlg_group *g) {
   for (float2 *p : g->dead_rings) cudaFree(p);
   for (const SpectrumHost &p : g->spectra)
     for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold, (void *)p.d_ring, (void *)p.d_win,
-                     (void *)p.d_fbuf})
+                     (void *)p.d_fbuf, (void *)p.d_scratch})
       if (d) cudaFree(d);
   for (void *p : g->dead_spec) cudaFree(p);
   for (cudaEvent_t e : g->ev_user) cudaEventDestroy(e);
@@ -2475,8 +2484,10 @@ static int source_cap(const xlg_group *g, const HostClient &h) {
 // hop 0 means width; today's spectra are hop = width, reduce = XLG_SPECTRUM_MAX and no window.
 static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_per_row, uint32_t skip_per_row,
                         uint32_t flags, uint32_t hop, uint32_t reduce, const float *window, int *spectrum_id) {
-  if (width == 0 || width > SPEC_MAX_W || frames_per_row == 0) {
-    XL_LOG("spectrum: width %u must be in [1, %d] and frames per row %u at least 1", width, SPEC_MAX_W, frames_per_row);
+  if (width == 0 || (width > SPEC_MAX_W && !spec_wide((int)std::min<uint32_t>(width, 1u << 30))) ||
+      frames_per_row == 0) {
+    XL_LOG("spectrum: width %u must be in [1, %d] or a power of two up to %d, and frames per row %u at least 1",
+           width, SPEC_MAX_W, SPEC_WIDE_MAX_W, frames_per_row);
     return -EINVAL;
   }
   if (hop == 0) hop = width;
@@ -2518,7 +2529,8 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
   p.R = (int)R;
   p.H = (int)hop;
   p.mean = reduce == XLG_SPECTRUM_MEAN;
-  p.ext = p.H != p.W || window != nullptr || p.mean;
+  p.wide = spec_wide(p.W);
+  p.ext = !p.wide && (p.H != p.W || window != nullptr || p.mean);
   p.src = src;
   // a source's positions count from here: P = 0 in its own stream
   const uint64_t cap = src < 0 ? (uint64_t)g->max_input_len / 2 : (uint64_t)source_cap(g, g->clients[src]);
@@ -2528,7 +2540,7 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
   // the frames a block of at most cap samples completes: their last samples are distinct positions of the block,
   // one frame's at least min(H, W + S) after the previous one's (H within a row, W + S from a row's last frame to
   // the next row's first)
-  if (p.mean) p.fb_frames = (int)((cap - 1) / std::min<uint64_t>(hop, (uint64_t)width + skip_per_row) + 1);
+  if (p.mean || p.wide) p.fb_frames = (int)((cap - 1) / std::min<uint64_t>(hop, (uint64_t)width + skip_per_row) + 1);
   // a source's ring holds every sample of the frames a block completes: the block's own and W - 1 before them
   const size_t ring_cap = src < 0 ? 0 : next_pow2((size_t)width - 1 + (size_t)cap);
   p.ring_mask = (unsigned)(ring_cap - 1);
@@ -2537,22 +2549,27 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
   for (int j = 0; j < W; j++) {
     // spectrogram.c:156-163: the halves swapped, an odd width's last bin in place
     const int bin = j < half ? half + j : j < 2 * half ? j - half : W - 1;
-    map[j] = spec_fft(W) ? bank_fft_pos(bin, W) : bin;
+    map[j] = spec_fft(W) || p.wide ? bank_fft_pos(bin, W) : bin;
   }
-  const std::vector<float2> tw = twiddle_table(W);
+  std::vector<float2> tw = twiddle_table(W);
+  if (p.wide) {  // pass B's table after the W-point one
+    const std::vector<float2> tc = twiddle_table(spec_wide_chunk(W));
+    tw.insert(tw.end(), tc.begin(), tc.end());
+  }
   const size_t hold_bytes = (size_t)p.NR * W * sizeof(unsigned);
-  if (cudaMalloc(&p.d_tw, W * sizeof(float2)) != cudaSuccess || cudaMalloc(&p.d_map, W * sizeof(int)) != cudaSuccess ||
-      cudaMalloc(&p.d_hold, hold_bytes) != cudaSuccess ||
+  if (cudaMalloc(&p.d_tw, tw.size() * sizeof(float2)) != cudaSuccess ||
+      cudaMalloc(&p.d_map, W * sizeof(int)) != cudaSuccess || cudaMalloc(&p.d_hold, hold_bytes) != cudaSuccess ||
       (ring_cap > 0 && cudaMalloc(&p.d_ring, ring_cap * sizeof(float2)) != cudaSuccess) ||
       (window != nullptr && cudaMalloc(&p.d_win, W * sizeof(float)) != cudaSuccess) ||
-      (p.fb_frames > 0 && cudaMalloc(&p.d_fbuf, (size_t)p.fb_frames * W * sizeof(float)) != cudaSuccess)) {
+      (p.mean && cudaMalloc(&p.d_fbuf, (size_t)p.fb_frames * W * sizeof(float)) != cudaSuccess) ||
+      (p.wide && cudaMalloc(&p.d_scratch, (size_t)p.fb_frames * W * sizeof(float2)) != cudaSuccess)) {
     for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold, (void *)p.d_ring, (void *)p.d_win,
-                     (void *)p.d_fbuf})
+                     (void *)p.d_fbuf, (void *)p.d_scratch})
       if (d) cudaFree(d);
     XL_LOG("spectrum: out of device memory");
     return -ENOMEM;
   }
-  CU_OK(cudaMemcpy(p.d_tw, tw.data(), W * sizeof(float2), cudaMemcpyHostToDevice));
+  CU_OK(cudaMemcpy(p.d_tw, tw.data(), tw.size() * sizeof(float2), cudaMemcpyHostToDevice));
   CU_OK(cudaMemcpy(p.d_map, map.data(), W * sizeof(int), cudaMemcpyHostToDevice));
   if (window != nullptr) CU_OK(cudaMemcpy(p.d_win, window, W * sizeof(float), cudaMemcpyHostToDevice));
   // (on a group stream, finished before the spectrum exists: the kernels' streams do not wait for the legacy one)
@@ -2641,7 +2658,7 @@ extern "C" int xlg_remove_spectrum(xlg_group *g, int spectrum_id) {
   }
   // in-flight tickets still read the tables and the hold: freed at the next re-layout, which drains
   for (void *d : {(void *)p->d_tw, (void *)p->d_map, (void *)p->d_hold, (void *)p->d_ring, (void *)p->d_win,
-                   (void *)p->d_fbuf})
+                   (void *)p->d_fbuf, (void *)p->d_scratch})
     if (d) g->dead_spec.push_back(d);
   *p = SpectrumHost();
   g->dirty = true;
@@ -2652,7 +2669,7 @@ extern "C" int xlg_spectrum_info(const xlg_group *g, int spectrum_id, int *kerne
   if (g == nullptr) return -EINVAL;
   const SpectrumHost *p = spectrum_of(const_cast<xlg_group *>(g), spectrum_id);
   if (p == nullptr) return -EINVAL;
-  if (kernel) *kernel = spec_fft(p->W) ? 1 : 0;
+  if (kernel) *kernel = p->wide ? 2 : spec_fft(p->W) ? 1 : 0;
   if (rows_done) *rows_done = p->rows_done;
   return 0;
 }
@@ -2701,6 +2718,8 @@ struct Block {
   // the extended spectra, the last n_spx entries: their channel stages' CTAs and the values the fold passes over
   int n_spx = 0, max_spxf_ctas = 0, max_spxd_ctas = 0, max_spxd_groups = 0, max_fold_values = 0;
   size_t spxf_smem = 0, spxd_smem = 0;
+  // the wide spectra, after the extended ones: CTAs of their two passes (the fold also covers them)
+  int n_spw = 0, max_spwa_ctas = 0, max_spwb_ctas = 0;
   int n_spa = 0, max_spa_n = 0;  // appends to spectrum sources' rings, the longest
   // sub-band walk
   int n_sb = 0, max_sb_n1 = 0, max_sb_n2 = 0;
@@ -2836,7 +2855,7 @@ static void walk_spectrum(Block &b, int id) {
   }
   const uint64_t d = (uint64_t)(E - p.P), F = (uint64_t)p.F;
   uint64_t total;
-  if (p.ext) {  // frames completed at offset o of a row: none before W, then one more every H, at most F
+  if (p.ext || p.wide) {  // frames completed at offset o of a row: none before W, then one more every H, at most F
     const uint64_t o = d % (uint64_t)p.R;
     total = d / (uint64_t)p.R * F + (o < (uint64_t)p.W ? 0 : std::min<uint64_t>(F, (o - p.W) / (uint64_t)p.H + 1));
   } else {
@@ -2865,15 +2884,27 @@ static void walk_spectrum(Block &b, int id) {
     e.slot0 = (int)(p.rows_done % (uint64_t)p.NR);
     e.power = p.power ? 1 : 0;
     e.inv_w = 1.0f / (float)p.W;
-    const uint64_t flops = spec_fft(p.W) ? xlg_bank_fft_flops((uint32_t)p.W) : 4ull * p.W * p.W;
+    const uint64_t flops = spec_fft(p.W) || p.wide ? xlg_bank_fft_flops((uint32_t)p.W) : 4ull * p.W * p.W;
     s.sp_frames += (uint64_t)n_frames;
     s.sp_flops += (uint64_t)n_frames * (flops + 6ull * p.W + (p.d_win ? 2ull * p.W : 0) + (p.mean ? p.W : 0));
-    if (p.ext) {
-      SpecExt &x = s.spext.h[b.n_spx++];
+    if (p.ext || p.wide) {
+      SpecExt &x = s.spext.h[b.n_spx + b.n_spw];
       x.win = p.d_win;
       x.fbuf = p.d_fbuf;
       x.H = p.H;
       x.mean = p.mean ? 1 : 0;
+    }
+    if (p.mean)  // values of the rows its frames touch
+      b.max_fold_values = std::max(b.max_fold_values, (int)(((long long)p.fir + n_frames - 1) / p.F + 1) * p.W);
+    if (p.wide) {
+      SpecWide &w = s.spwide.h[b.n_spw++];
+      w.scratch = p.d_scratch;
+      w.tw_c = p.d_tw + p.W;
+      const int C = spec_wide_chunk(p.W);
+      b.max_spwa_ctas = std::max(b.max_spwa_ctas, n_frames * (C / SPEC_THREADS));
+      b.max_spwb_ctas = std::max(b.max_spwb_ctas, n_frames * (p.W / C));
+    } else if (p.ext) {
+      b.n_spx++;
       if (spec_fft(p.W)) {
         b.max_spxf_ctas = std::max(b.max_spxf_ctas, (n_frames + bank_fft_frames(p.W) - 1) / bank_fft_frames(p.W));
         b.spxf_smem = std::max(b.spxf_smem, bank_fft_smem(p.W));
@@ -2883,8 +2914,6 @@ static void walk_spectrum(Block &b, int id) {
         b.max_spxd_groups = std::max(b.max_spxd_groups, spec_direct_groups(p.W));
         b.spxd_smem = std::max(b.spxd_smem, spec_direct_smem(p.W));
       }
-      if (p.mean)  // values of the rows its frames touch
-        b.max_fold_values = std::max(b.max_fold_values, (int)(((long long)p.fir + n_frames - 1) / p.F + 1) * p.W);
     } else if (spec_fft(p.W)) {
       b.max_spf_ctas = std::max(b.max_spf_ctas, (n_frames + bank_fft_frames(p.W) - 1) / bank_fft_frames(p.W));
       b.spf_smem = std::max(b.spf_smem, bank_fft_smem(p.W));
@@ -2900,15 +2929,15 @@ static void walk_spectrum(Block &b, int id) {
   p.fir = (int)(total % F);
 }
 
-// every spectrum, today's first: the table is [plain entries | extended entries]
+// every spectrum, today's first: the table is [plain entries | extended entries | wide entries]
 static void walk_spectra(Block &b) {
   xlg_group *g = b.g;
   b.s.sp_frames = b.s.sp_flops = 0;
-  for (int ext = 0; ext < 2; ext++)
+  for (int seg = 0; seg < 3; seg++)
     for (int id = 0; id < (int)g->spectra.size(); id++) {
       const SpectrumHost &p = g->spectra[id];
-      if (ext == 0) b.ho.sp_w[id] = p.active ? p.W : 0;
-      if (p.active && p.ext == (ext == 1)) walk_spectrum(b, id);
+      if (seg == 0) b.ho.sp_w[id] = p.active ? p.W : 0;
+      if (p.active && (p.wide ? 2 : p.ext ? 1 : 0) == seg) walk_spectrum(b, id);
     }
 }
 
@@ -3071,24 +3100,31 @@ static int launch_spectra(Block &b) {
     CU_OK(s.spblk.upload((size_t)b.n_spec, b.cs));
     CU_OK(s.spring.upload((size_t)b.n_spec, b.cs));
   }
-  const int n_plain = b.n_spec - b.n_spx;
+  const int n_plain = b.n_spec - b.n_spx - b.n_spw;
   if (b.max_spf_ctas > 0)
     spectrum_fft_kernel<<<dim3(b.max_spf_ctas, n_plain), SPEC_THREADS, b.spf_smem, b.cs>>>(s.spblk.d, s.spring.d);
   if (b.max_spd_ctas > 0)
     spectrum_direct_kernel<<<dim3(b.max_spd_ctas, b.max_spd_groups, n_plain), SPEC_THREADS, b.spd_smem, b.cs>>>(
         s.spblk.d, s.spring.d);
-  if (b.n_spx > 0) {
+  if (b.n_spx + b.n_spw > 0) {
     const SpecBlk *xb = s.spblk.d + n_plain;
     const float2 *const *xr = s.spring.d + n_plain;
-    CU_OK(s.spext.upload((size_t)b.n_spx, b.cs));
+    CU_OK(s.spext.upload((size_t)(b.n_spx + b.n_spw), b.cs));
     if (b.max_spxf_ctas > 0)
       spectrum_fft_ext_kernel<<<dim3(b.max_spxf_ctas, b.n_spx), SPEC_THREADS, b.spxf_smem, b.cs>>>(xb, xr, s.spext.d);
     if (b.max_spxd_ctas > 0)
       spectrum_direct_ext_kernel<<<dim3(b.max_spxd_ctas, b.max_spxd_groups, b.n_spx), SPEC_THREADS, b.spxd_smem,
                                    b.cs>>>(xb, xr, s.spext.d);
+    if (b.n_spw > 0) {  // the wide entries: pass A into their scratch, then pass B into the hold or frame buffer
+      CU_OK(s.spwide.upload((size_t)b.n_spw, b.cs));
+      spectrum_wide_a_kernel<<<dim3(b.max_spwa_ctas, b.n_spw), SPEC_THREADS, 0, b.cs>>>(
+          xb + b.n_spx, xr + b.n_spx, s.spext.d + b.n_spx, s.spwide.d);
+      spectrum_wide_b_kernel<<<dim3(b.max_spwb_ctas, b.n_spw), SPEC_THREADS, SPEC_WIDE_SMEM, b.cs>>>(
+          xb + b.n_spx, s.spext.d + b.n_spx, s.spwide.d);
+    }
     if (b.max_fold_values > 0)
-      spectrum_fold_kernel<<<dim3((b.max_fold_values + SPEC_THREADS - 1) / SPEC_THREADS, b.n_spx), SPEC_THREADS, 0,
-                             b.cs>>>(xb, s.spext.d);
+      spectrum_fold_kernel<<<dim3((b.max_fold_values + SPEC_THREADS - 1) / SPEC_THREADS, b.n_spx + b.n_spw),
+                             SPEC_THREADS, 0, b.cs>>>(xb, s.spext.d);
   }
   if (b.max_sp_values > 0)
     spectrum_emit_kernel<<<dim3((b.max_sp_values + SPEC_THREADS - 1) / SPEC_THREADS, b.n_spec), SPEC_THREADS, 0,

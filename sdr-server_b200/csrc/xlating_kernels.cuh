@@ -1688,7 +1688,8 @@ bank_cf32_kernel(const BankBlk *__restrict__ blk, const float2 *__restrict__ rin
 // the radix-2 butterfly (a0, a1) -> (a0 + a1, a0 - a1), and every product y * w is
 //     (fmaf(-y.y, w.y, y.x * w.x), fmaf(y.y, w.x, y.x * w.y))     (rounded products, no contraction)
 // W is the direct bank's table read at stride K / L, so the quarter turns stay exact.  Channel k then lies at
-// the digit reversal of k mod K (bank_fft_pos in xlating_group.cu), which the channel table carries.
+// the digit reversal of k mod K (bank_fft_pos in xlating_group.cu), which the channel table carries.  The
+// spectra use the same transform at K up to 65536 (the wide ones in two passes, spectrum_wide_a/b_kernel).
 // ---------------------------------------------------------------------------
 constexpr int BF_THREADS = 256;
 constexpr int BF_N = 2048;  // sums per CTA: BF_N / K frames, one frame at K = 4096
@@ -1792,6 +1793,7 @@ bank_fft_cf32_kernel(const BankBlk *__restrict__ blk, const float2 *__restrict__
 // The hold has NR rows used round-robin by row number (NR exceeds the rows a block touches); the emit pass reads
 // each row the block completed through the row map (out[j] = hold[map[j]]: the reference's half swap, then the
 // FFT path's digit reversal), writes v (XLG_SPECTRUM_POWER) or 10 * log10f(v), and zeroes what it read.
+// Powers of two from 8192 to 65536 are the wide spectra at the end of this file: the FFT path's X at K = W.
 // ---------------------------------------------------------------------------
 constexpr int SPEC_THREADS = 256;
 constexpr int SPEC_MAX_W = 4096;
@@ -2076,6 +2078,110 @@ spectrum_fold_kernel(const SpecBlk *__restrict__ blk, const SpecExt *__restrict_
   float s = __uint_as_float(*hold);
   for (int j = (int)max(0ll, first); j < j1; j++) s = __fadd_rn(s, x.fbuf[(size_t)j * W + q]);
   *hold = __float_as_uint(i < b.n_rows ? __fdiv_rn(s, (float)b.F) : s);
+}
+
+// ---------------------------------------------------------------------------
+// Wide spectra (W a power of two from 8192 to SPEC_WIDE_MAX_W = 65536, plain or extended): X is fft_dif_rows'
+// transform at K = W, bin k at bank_fft_pos(k, W), but a frame does not fit in one CTA's shared memory.  In the
+// decimation in frequency, after the first s radix-4 stages (s = 1 at W <= 16384, s = 2 above) each contiguous
+// chunk of C = W / 4^s points (2048 or 4096) only meets itself, and its remaining stages at L <= C read the W-point
+// table at stride W / L = (W / C)(C / L): they are fft_dif_rows at K = C with the C-point table, twiddle_table(C),
+// which is twiddle_table(W) at stride W / C bit for bit (the double angles differ by a power of two).  So:
+//   spectrum_wide_a_kernel: thread (frame j, column i < C) loads the 4^s points i + m C of frame j (spec_load: the
+//     hop and the window), runs the first s stages' butterflies on them in registers, each with fft_dif_rows'
+//     operations in its order and the W table at stride W / L, and stores them at the same positions of row j of
+//     the spectrum's scratch (HBM, frames of this block x W, read back from L2).
+//   spectrum_wide_b_kernel: CTA (frame j, chunk c) runs fft_dif_rows on chunk c of row j in shared memory
+//     (C float2: 32 KiB at C = 4096) and folds the powers as spectrum_fft_ext_kernel does: atomicMax into the hold
+//     row, or a store to the mean's frame buffer.  Position c C + t is the W-point transform's own position.
+// The entries are the tail of the block's SpecBlk table, [plain | extended | wide], outside every other channel
+// kernel's grid.  Each has a SpecExt (a plain one: H = W, no window, the max), so that spectrum_fold_kernel and
+// spectrum_emit_kernel finish their rows unchanged, and a SpecWide.
+// ---------------------------------------------------------------------------
+constexpr int SPEC_WIDE_MAX_W = 65536;
+__host__ __device__ constexpr bool spec_wide(int W) {
+  return W > SPEC_MAX_W && W <= SPEC_WIDE_MAX_W && (W & (W - 1)) == 0;
+}
+// pass A's radix-4 stages, and the chunk length after them
+__host__ __device__ constexpr int spec_wide_stages(int W) { return W > 16384 ? 2 : 1; }
+__host__ __device__ constexpr int spec_wide_chunk(int W) { return W >> (2 * spec_wide_stages(W)); }
+constexpr size_t SPEC_WIDE_SMEM = 4096 * sizeof(float2);  // pass B: the largest chunk
+
+struct SpecWide {
+  float2 *scratch;     // pass A's rows: a row of W per frame of this block
+  const float2 *tw_c;  // the C-point table
+};
+
+// fft_dif_rows' radix-4 butterfly on (a0, a1, a2, a3) = u[j + q L/4], in place, twiddles tw[q j s]
+__device__ __forceinline__ void dif_bfly4(float2 &a0, float2 &a1, float2 &a2, float2 &a3, const float2 *tw, int js) {
+  const float2 t0 = make_float2(a0.x + a2.x, a0.y + a2.y), t1 = make_float2(a0.x - a2.x, a0.y - a2.y);
+  const float2 t2 = make_float2(a1.x + a3.x, a1.y + a3.y), t3 = make_float2(a1.x - a3.x, a1.y - a3.y);
+  a0 = make_float2(t0.x + t2.x, t0.y + t2.y);
+  a1 = cmul_tw(make_float2(t1.x + t3.y, t1.y - t3.x), __ldg(tw + js));
+  a2 = cmul_tw(make_float2(t0.x - t2.x, t0.y - t2.y), __ldg(tw + 2 * js));
+  a3 = cmul_tw(make_float2(t1.x - t3.y, t1.y + t3.x), __ldg(tw + 3 * js));
+}
+
+// pass A on the 4^NS points i + m C of a frame starting at pos: stage 1 (L = W) on columns i + r C, r < 4^(NS-1),
+// then, for NS = 2, stage 2 (L = W / 4, stride 4) on each quarter's points
+template <int NS>
+__device__ __forceinline__ void spec_wide_pass_a(const float2 *__restrict__ ring, unsigned mask, long long pos,
+                                                 const float *__restrict__ win, const float2 *__restrict__ tw,
+                                                 float2 *__restrict__ row, int i, int C) {
+  constexpr int M = NS == 1 ? 4 : 16, Q = M / 4;
+  float2 a[M];
+#pragma unroll
+  for (int m = 0; m < M; m++) a[m] = spec_load(ring, mask, pos + i + m * C, win, i + m * C);
+#pragma unroll
+  for (int r = 0; r < Q; r++) dif_bfly4(a[r], a[r + Q], a[r + 2 * Q], a[r + 3 * Q], tw, i + r * C);
+  if (NS == 2) {
+#pragma unroll
+    for (int q = 0; q < 4; q++) dif_bfly4(a[4 * q], a[4 * q + 1], a[4 * q + 2], a[4 * q + 3], tw, 4 * i);
+  }
+#pragma unroll
+  for (int m = 0; m < M; m++) row[i + m * C] = a[m];
+}
+
+// CTA (x, s): threads [x 256, x 256 + 256) of wide spectrum s's frames x C columns, C = spec_wide_chunk(W)
+__global__ void __launch_bounds__(SPEC_THREADS)
+spectrum_wide_a_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__restrict__ rings,
+                       const SpecExt *__restrict__ ext, const SpecWide *__restrict__ wide) {
+  const SpecBlk b = blk[blockIdx.y];
+  const SpecExt x = ext[blockIdx.y];
+  const float2 *__restrict__ ring = rings[blockIdx.y];
+  const int W = b.W, C = spec_wide_chunk(W), lc = 31 - __clz(C);
+  const int e = blockIdx.x * SPEC_THREADS + threadIdx.x, j = e >> lc, i = e & (C - 1);
+  if (j >= b.n_frames) return;
+  float2 *row = wide[blockIdx.y].scratch + (size_t)j * W;
+  const long long pos = spec_frame_pos(b, x.H, j);
+  if (spec_wide_stages(W) == 1)
+    spec_wide_pass_a<1>(ring, b.mask, pos, x.win, b.tw, row, i, C);
+  else
+    spec_wide_pass_a<2>(ring, b.mask, pos, x.win, b.tw, row, i, C);
+}
+
+// CTA (x, s): chunk x mod 4^s of frame x / 4^s of wide spectrum s (at least four CTAs per SM: without that bound
+// ptxas aims at eight, 32 registers, and spills)
+__global__ void __launch_bounds__(SPEC_THREADS, 4)
+spectrum_wide_b_kernel(const SpecBlk *__restrict__ blk, const SpecExt *__restrict__ ext,
+                       const SpecWide *__restrict__ wide) {
+  extern __shared__ __align__(16) float2 u[];
+  const SpecBlk b = blk[blockIdx.y];
+  const SpecExt x = ext[blockIdx.y];
+  const SpecWide wd = wide[blockIdx.y];
+  const int W = b.W, ls = 2 * spec_wide_stages(W), C = W >> ls, lc = 31 - __clz(C), tid = threadIdx.x;
+  const int j = blockIdx.x >> ls, c0 = (blockIdx.x & ((1 << ls) - 1)) * C;
+  if (j >= b.n_frames) return;
+  const size_t off = (size_t)j * W + c0;
+  for (int t = tid; t < C; t += SPEC_THREADS) u[t] = wd.scratch[off + t];
+  __syncthreads();
+  fft_dif_rows<SPEC_THREADS>(u, 1, C, lc, wd.tw_c, tid);
+  if (x.mean) {
+    for (int t = tid; t < C; t += SPEC_THREADS) x.fbuf[off + t] = __uint_as_float(spec_power(u[t], b.inv_w));
+    return;
+  }
+  unsigned *hold = b.hold + (size_t)spec_frame(b, j).hold_row * W + c0;
+  for (int t = tid; t < C; t += SPEC_THREADS) atomicMax(hold + t, spec_power(u[t], b.inv_w));
 }
 
 }  // namespace xl

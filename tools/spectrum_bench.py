@@ -8,7 +8,7 @@
    window, H = W, max) and "hann_mean" (a Hann window, H = W / 2, the mean: Welch's method at 50 % overlap, with
    F = 2 fs // W - 1 so that a row still spans about a second).  Reported: the spectrum span's time per block
    from a profiled run (CUDA events around the channel stages, the fold and the emit pass, xlg_spectrum_profile),
-   its kernel (fft or direct) and counted work.
+   its kernel (direct, fft, or wide_fft above W = 4096) and counted work.
 2. bench.py's cfg2 workload (256 clients at 48 and 96 ksps on a 2.016 Msps cu8 stream, blocks of 262144 bytes,
    device inputs and outputs) without a spectrum, with a W = 1024 spectrum (F = 1968, S = 768) and with a
    W = 1024, H = 512 Hann mean spectrum (F = 3935, S = 768), alternated in every round: the step time per block
@@ -58,7 +58,7 @@ def kernel_run(W, variant, blocks, warmup, data):
         for i in range(blocks):
             g.wait(g.submit(FMT, data[i % len(data)]))
         p = g.spectrum_profile_read()
-        kernel = "fft" if g.spectrum_info(sid)[0] == 1 else "direct"
+        kernel = ("direct", "fft", "wide_fft")[g.spectrum_info(sid)[0]]
     finally:
         g.close()
     n = p["spectrum_launches"]
