@@ -38,8 +38,16 @@ extern "C" {
 typedef struct xlg_group xlg_group;
 
 /* input sample formats = the three SDR front-ends (src/sdr_device.c; cu8 RTL-SDR,
- * cs8 HackRF, cs16 Airspy) */
-enum { XLG_FMT_CU8 = 0, XLG_FMT_CS8 = 1, XLG_FMT_CS16 = 2 };
+ * cs8 HackRF, cs16 Airspy), and cf32: interleaved float32 (re, im), the format sdr-server
+ * writes for a client and the spectrogram tool reads.  The ring holds cf32 values bit for bit,
+ * unconverted, so every client, sub-band, bank and spectrum is defined on the submitted samples
+ * exactly as for the other formats; the exact float images of a cu8, cs8 or cs16 block
+ * ((u - 127.5) * 2^-7, s * 2^-7, s * 2^-15) give bit-identical outputs and rows.  The Q15 path
+ * takes no cf32 (XLG_PATH_Q15 with XLG_FMT_CF32: -EINVAL, logged, nothing enqueued).  A host
+ * cf32 block needs staging buffers of 4 bytes per element instead of 2: each slot grows its
+ * device buffer on its first host cf32 block and its pinned buffer on its first pageable one
+ * (-ENOMEM, logged, no ticket, if that allocation fails). */
+enum { XLG_FMT_CU8 = 0, XLG_FMT_CS8 = 1, XLG_FMT_CS16 = 2, XLG_FMT_CF32 = 3 };
 
 /* xlg_create flags */
 #define XLG_OUT_DEVICE 0x1u    /* leave outputs in HBM (no D2H); xlg_output returns device pointers */
@@ -53,7 +61,8 @@ enum { XLG_FMT_CU8 = 0, XLG_FMT_CS8 = 1, XLG_FMT_CS16 = 2 };
                                   per-filter drop-in engine, which moves filters in and out of a group. */
 /* xlg_submit flags */
 #define XLG_INPUT_DEVICE 0x100u /* `input` is a device pointer on the group's GPU (already staged), aligned to one
-                                   complex sample: 2 bytes for cu8 and cs8, 4 for cs16.  A misaligned one is
+                                   complex sample: 2 bytes for cu8 and cs8, 4 for cs16, 8 for cf32 (a
+                                   torch.complex64 tensor's data_ptr() is).  A misaligned one is
                                    refused (-EINVAL, logged) before anything is enqueued; no ticket is taken.
                                    The block may be overwritten once xlg_input_consumed(ticket) (or xlg_wait)
                                    returns. */

@@ -32,8 +32,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 # XLATING_B200_LIB: an A/B measurement switch (another build of the SAME library, e.g. other tile constants)
 LIB_PATH = os.environ.get("XLATING_B200_LIB") or os.path.join(HERE, "lib", "libxlating_b200.so")
 
-FMT = {"cu8": 0, "cs8": 1, "cs16": 2}
-NP_DTYPE = {"cu8": np.uint8, "cs8": np.int8, "cs16": np.int16}
+FMT = {"cu8": 0, "cs8": 1, "cs16": 2, "cf32": 3}
+NP_DTYPE = {"cu8": np.uint8, "cs8": np.int8, "cs16": np.int16, "cf32": np.float32}
 
 XLG_OUT_DEVICE = 0x1
 XLG_NO_RENORM = 0x2
@@ -672,9 +672,17 @@ class Group:
         return hist.value, kind.value
 
     def submit(self, fmt: str, data, flags: int = 0) -> int:
-        """data: numpy array (host) -- or (device_ptr, n_elements) with XLG_INPUT_DEVICE."""
-        if flags & XLG_INPUT_DEVICE:
+        """data: numpy array (host) -- or (device_ptr, n_elements) with XLG_INPUT_DEVICE.  cf32 takes float32
+        (re, im) pairs or complex64, and also a CUDA torch.complex64 tensor, submitted in place through
+        XLG_INPUT_DEVICE."""
+        if fmt == "cf32" and getattr(data, "is_cuda", False):
+            assert str(data.dtype) == "torch.complex64" and data.is_contiguous(), data.dtype
+            ptr, n, flags = data.data_ptr(), 2 * data.numel(), flags | XLG_INPUT_DEVICE
+        elif flags & XLG_INPUT_DEVICE:
             ptr, n = data
+        elif fmt == "cf32" and np.iscomplexobj(data):
+            data = np.ascontiguousarray(data, dtype=np.complex64).view(np.float32)
+            ptr, n = data.ctypes.data, data.size
         else:
             data = np.ascontiguousarray(data, dtype=NP_DTYPE[fmt])
             ptr, n = data.ctypes.data, data.size

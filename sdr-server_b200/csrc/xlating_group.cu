@@ -230,6 +230,7 @@ enum Span {
 
 struct Slot {
   void *d_raw = nullptr, *h_raw = nullptr;
+  size_t d_raw_bytes = 0, h_raw_bytes = 0;
   float2 *d_out = nullptr;
   short2 *d_qout = nullptr;
   float2 *d_phases = nullptr;
@@ -558,7 +559,44 @@ static size_t next_pow2(size_t v) {
   return p;
 }
 
-static int elem_bytes(int fmt) { return fmt == XLG_FMT_CS16 ? 2 : 1; }
+static int elem_bytes(int fmt) { return fmt == XLG_FMT_CF32 ? 4 : fmt == XLG_FMT_CS16 ? 2 : 1; }
+
+static bool page_locked(const void *p) {
+  cudaPointerAttributes attr;
+  if (cudaPointerGetAttributes(&attr, p) == cudaSuccess) return attr.type == cudaMemoryTypeHost;
+  cudaGetLastError();
+  return false;
+}
+
+// A slot's staging buffers hold max_input_len elements of 2 bytes (cs16) from xlg_create on.  A host cf32 block
+// needs 4: the device buffer grows on the slot's first one, the pinned buffer on its first pageable one, so a group
+// that never receives cf32 from the host keeps its footprint.  The slot is idle here (xlg_submit waited for it).
+static int grow_raw_cf32(xlg_group *g, Slot &s, bool pageable) {
+  const size_t bytes = (size_t)g->max_input_len * 4;
+  if (s.d_raw_bytes < bytes) {
+    void *d = nullptr;
+    if (cudaMalloc(&d, bytes) != cudaSuccess) {
+      cudaGetLastError();
+      XL_LOG("no device memory for a %zu-byte cf32 staging buffer", bytes);
+      return -ENOMEM;
+    }
+    cudaFree(s.d_raw);
+    s.d_raw = d;
+    s.d_raw_bytes = bytes;
+  }
+  if (pageable && s.h_raw_bytes < bytes) {
+    void *h = nullptr;
+    if (cudaHostAlloc(&h, bytes, cudaHostAllocDefault) != cudaSuccess) {
+      cudaGetLastError();
+      XL_LOG("no pinned memory for a %zu-byte cf32 staging buffer", bytes);
+      return -ENOMEM;
+    }
+    cudaFreeHost(s.h_raw);
+    s.h_raw = h;
+    s.h_raw_bytes = bytes;
+  }
+  return 0;
+}
 
 // (re)fill a device array; the allocation is reused while it is large enough (a re-layout per attach must not
 // pay a cudaFree + cudaMalloc -- each an implicit device synchronisation -- for every table)
@@ -639,6 +677,7 @@ static void slot_free(Slot &s) {
   s.d_vblk = s.h_vblk = nullptr;
   s.d_endph = nullptr;
   s.d_raw = s.h_raw = nullptr;
+  s.d_raw_bytes = s.h_raw_bytes = 0;
   s.d_out = nullptr;
   s.d_qout = nullptr;
   s.d_phases = nullptr;
@@ -1792,6 +1831,7 @@ extern "C" int xlg_create_ex(int device, uint32_t sampling_freq, uint32_t max_in
   for (Slot &s : g->slots) {
     if (cudaMalloc(&s.d_raw, raw_bytes) != cudaSuccess) return fail(-ENOMEM);
     if (cudaHostAlloc(&s.h_raw, raw_bytes, cudaHostAllocDefault) != cudaSuccess) return fail(-ENOMEM);
+    s.d_raw_bytes = s.h_raw_bytes = raw_bytes;
     cudaEvent_t *evs[] = {&s.ev_h2d, &s.ev_conv, &s.ev_phase, &s.ev_fir, &s.ev_done};
     for (cudaEvent_t *ev : evs)
       if (cudaEventCreateWithFlags(ev, cudaEventDisableTiming) != cudaSuccess) return fail(-EIO);
@@ -3006,12 +3046,7 @@ static int stage_and_convert(Block &b, int fmt, const void *input, uint32_t flag
   const void *d_in = input;
   if (!(flags & XLG_INPUT_DEVICE) && n > 0) {
     const size_t bytes = (size_t)n * 2 * elem_bytes(fmt);
-    cudaPointerAttributes attr;
-    bool pinned = false;
-    if (cudaPointerGetAttributes(&attr, input) == cudaSuccess)
-      pinned = attr.type == cudaMemoryTypeHost;
-    else
-      cudaGetLastError();
+    const bool pinned = page_locked(input);
     const void *src = input;
     if (!pinned) {
       memcpy(s.h_raw, input, bytes);
@@ -3048,8 +3083,11 @@ static int stage_and_convert(Block &b, int fmt, const void *input, uint32_t flag
       launch_convert<0>(b.q15, d_in, g, b.S, n, b.cvs);
     else if (fmt == XLG_FMT_CS8)
       launch_convert<1>(b.q15, d_in, g, b.S, n, b.cvs);
-    else
+    else if (fmt == XLG_FMT_CS16)
       launch_convert<2>(b.q15, d_in, g, b.S, n, b.cvs);
+    else
+      copy_cf32_kernel<<<(n + 255) / 256, 256, 0, b.cvs>>>(static_cast<const float2 *>(d_in), g->ring,
+                                                           (unsigned)(g->ring_cap - 1), b.S, n);
     if (span_end(g, s, SP_CONV, b.cvs)) return -EIO;
     CU_OK(cudaEventRecord(s.ev_conv, b.cvs));
   }
@@ -3505,12 +3543,16 @@ static int copy_back(Block &b) {
 
 extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t input_len, uint32_t flags) {
   if (g == nullptr || (input == nullptr && input_len > 0)) return -EINVAL;
-  if (fmt < XLG_FMT_CU8 || fmt > XLG_FMT_CS16) return -EINVAL;
+  if (fmt < XLG_FMT_CU8 || fmt > XLG_FMT_CF32) return -EINVAL;
+  if (fmt == XLG_FMT_CF32 && (flags & XLG_PATH_Q15)) {
+    XL_LOG("the Q15 path takes no cf32 input; submit cf32 without XLG_PATH_Q15");
+    return -EINVAL;
+  }
   if (input_len > g->max_input_len) {
     XL_LOG("block of %zu elements exceeds max_input_len %u", input_len, g->max_input_len);
     return -EINVAL;
   }
-  // the conversion kernels load one complex sample at a time (uchar2 / char2 / short2); host inputs are staged
+  // the conversion kernels load one complex sample at a time (uchar2 / char2 / short2 / float2); host inputs are staged
   // into an aligned buffer, device inputs are read where they are
   const size_t sample_bytes = 2 * elem_bytes(fmt);
   if ((flags & XLG_INPUT_DEVICE) && input_len > 0 && (uintptr_t)input % sample_bytes != 0) {
@@ -3584,6 +3626,10 @@ extern "C" int64_t xlg_submit(xlg_group *g, int fmt, const void *input, size_t i
                            std::chrono::steady_clock::now() - t_enter).count();
     std::lock_guard<std::mutex> lk(g->mu);
     harvest_locked(g, s);
+  }
+  if (fmt == XLG_FMT_CF32 && !(flags & XLG_INPUT_DEVICE) && input_len >= 2) {
+    const int rc = grow_raw_cf32(g, s, !page_locked(input));
+    if (rc) return rc;
   }
   Block b{g, s, ho, ticket, q15 ? g->qS : g->S, (int)(input_len / 2), q15, (unsigned)(g->ring_cap - 1), g->max_client};
   {

@@ -128,6 +128,15 @@ __global__ void convert_cf32_vec_kernel(const void *__restrict__ raw, float2 *__
   }
 }
 
+// cf32 input: the ring holds the submitted values bit for bit (a copy, no arithmetic: NaN payloads, -0.0 and
+// subnormals pass unchanged), at S mod cap like every conversion
+__global__ void copy_cf32_kernel(const float2 *__restrict__ raw, float2 *__restrict__ ring, unsigned mask,
+                                 long long S, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  ring[(unsigned)((unsigned long long)(S + i)) & mask] = raw[i];
+}
+
 template <int FMT>
 __global__ void convert_q15_kernel(const void *__restrict__ raw, short2 *__restrict__ ring,
                                    unsigned mask, long long S, int n) {
