@@ -314,6 +314,32 @@ typedef struct {
   const float *window; /* width weights, copied; NULL: none */
 } xlg_spectrum_desc;
 int xlg_add_spectrum_ex(xlg_group *g, int source, int source_id, const xlg_spectrum_desc *desc, int *spectrum_id);
+/* Spectra of any width W from 1 to 65536 (DESIGN.md section 5, "Chirp-z spectra"): the arguments, ids, rows,
+ * widths, profile, removal and refusals of xlg_add_spectrum_ex, except its width rule; W = 0 and W above 65536
+ * are still refused (-EINVAL, logged, nothing changed).  A width that xlg_add_spectrum_ex serves (W <= 4096, or a
+ * power of two up to 65536) is served exactly as xlg_add_spectrum_ex serves it: the same kernels, rows and
+ * xlg_spectrum_info kernel.  Every other width runs the chirp-z stage (xlg_spectrum_info kernel 3).  Its rows are
+ * xlg_add_spectrum_ex's (frames, hop, window, max or mean, p with its 1/W, hold, half swap, dB or linear) with the
+ * W-point DFT X of each windowed frame z computed by Bluestein's algorithm at M = next_pow2(2W - 1):
+ *   1. a[n] = z[n] c[n] for n < W, a[n] = 0 for W <= n < M, c[n] = e^{-i pi (n^2 mod 2W) / W} (n^2 in 64 bits);
+ *   2. A = the M-point FFT of a (the FFT path's transform at K = M, in position order bank_fft_pos(k, M));
+ *   3. Y = A Bh position by position, Bh the M-point DFT of b[m] = e^{+i pi (m^2 mod 2W) / W}, |m| < W, wrapped
+ *      mod M and scaled by 1/M;
+ *   4. v = the same M-point FFT of conj(Y) in natural order, so X_k = conj(v[k]) c[k] for k < W.
+ *   Since |c[k]| = 1, p is defined on v[k] itself, p = (v.re / W)^2 + (v.im / W)^2 + 1e-20f as for every spectrum,
+ *   with no final chirp.  c and Bh are computed in double and rounded once to float (xlg_spectrum_any_tables); the
+ *   order of every rounded operation is stated in xlating_kernels.cuh ("Chirp-z spectra").
+ * Besides what an extended spectrum holds (the hold, the row map of W ints, a source's ring, a window, a mean's
+ * frame buffer), a chirp-z spectrum keeps the twiddles, the chirp and Bh ((2 M + C + W) float2, C = M / 16 or
+ * M / 4 at M = 16384), the bin of each position (M ints) and two scratches of fb x M float2 in HBM,
+ * fb = (cap - 1) / min(H, W + S) + 1 the most frames a block completes: at W = 65535 (M = 131072), 2 MiB per
+ * frame.  Its frame costs channel_flops of 2 xlg_bank_fft_flops(M) + 4 W + 4 M + 6 W (the two transforms, the
+ * chirp's and Bh's complex products of 4 instructions, the power), plus 2 W windowed and W for a mean. */
+int xlg_add_spectrum_any(xlg_group *g, int source, int source_id, const xlg_spectrum_desc *desc, int *spectrum_id);
+/* The chirp-z stage's tables for width W (above 4096, at most 65536, not a power of two; else -EINVAL): *m = M,
+ * chirp = c[n] as W (re, im) float pairs and kernel = Bh as M pairs in position order (kernel[bank_fft_pos(k, M)]
+ * is Bh[k]).  chirp and kernel may be NULL (then only *m is set).  Needs no group and no device. */
+int xlg_spectrum_any_tables(uint32_t width, float *chirp, float *kernel, uint32_t *m);
 /* Drops its partial row.  -EINVAL for an unknown id. */
 int xlg_remove_spectrum(xlg_group *g, int spectrum_id);
 /* The rows a spectrum completed in a ticket: *n_rows x W contiguous floats, in pinned host memory, or in HBM for
@@ -326,8 +352,8 @@ int xlg_spectrum_width(xlg_group *g, int64_t ticket, int spectrum_id, uint32_t *
 /* Waits for the ticket and copies at most cap_rows of its rows (xlg_spectrum_width floats each) into dst;
  * *n_rows = rows it has. */
 int xlg_read_spectrum(xlg_group *g, int64_t ticket, int spectrum_id, float *dst, size_t cap_rows, size_t *n_rows);
-/* The channel stage serving a spectrum (0 = direct DFT, 1 = FFT, 2 = wide FFT, W above 4096) and the rows
- * completed by the blocks submitted so far. */
+/* The channel stage serving a spectrum (0 = direct DFT, 1 = FFT, 2 = wide FFT, W above 4096, 3 = chirp-z,
+ * xlg_add_spectrum_any above 4096 and not a power of two) and the rows completed by the blocks submitted so far. */
 int xlg_spectrum_info(const xlg_group *g, int spectrum_id, int *kernel, uint64_t *rows_done);
 /* Size the per-ticket result arenas (device and pinned host) for `output_samples_per_block` complex output
  * samples per block summed over all clients (a client at decimation D produces about max_input_len/2/D + 2).
@@ -484,7 +510,8 @@ typedef struct {
   uint64_t frames;           /* W-point frames transformed (overlapped frames each count) */
   uint64_t channel_flops;    /* FP32 instructions of the channel stages: per frame xlg_bank_fft_flops(W) + 6 W on
                                 the FFT path, 4 W^2 + 6 W on the direct path (an fmaf counts one); 2 W more for a
-                                windowed spectrum's frame and W more for a mean spectrum's (the fold's adds) */
+                                windowed spectrum's frame and W more for a mean spectrum's (the fold's adds); a
+                                chirp-z frame 2 xlg_bank_fft_flops(M) + 4 W + 4 M + 6 W (xlg_add_spectrum_any) */
 } xlg_spectrum_profile;
 int xlg_spectrum_profile_read(xlg_group *g, xlg_spectrum_profile *p, int reset);
 

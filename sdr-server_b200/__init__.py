@@ -56,7 +56,7 @@ DROPIN_EXTENSION_SYMBOLS = ["create_rational_frequency_xlating_filter", "create_
 GROUP_SYMBOLS = [
     "xlg_create", "xlg_create_ex", "xlg_destroy", "xlg_add_client", "xlg_add_client_ex", "xlg_add_client_rational_ex", "xlg_remove_client", "xlg_reserve", "xlg_client_count", "xlg_submit",
     "xlg_wait", "xlg_input_consumed", "xlg_output", "xlg_read_output", "xlg_copy_output", "xlg_alloc_pinned", "xlg_free_pinned", "xlg_wait_stream", "xlg_partition_active", "xlg_timer_start",
-    "xlg_timer_stop", "xlg_profile_enable", "xlg_profile_read", "xlg_client_info", "xlg_add_client_rational", "xlg_poly_profile_read", "xlg_add_client_cascade", "xlg_add_client_cascade_rational", "xlg_cascade_info", "xlg_cascade_profile_read", "xlg_add_subband", "xlg_remove_subband", "xlg_add_client_subband", "xlg_add_client_subband_rational", "xlg_subband_info", "xlg_subband_profile_read", "xlg_add_bank", "xlg_add_bank_subband", "xlg_remove_bank", "xlg_bank_profile_read", "xlg_dropin_stats", "xlg_dropin_stream_stats", "xlg_dropin_stream_times",
+    "xlg_timer_stop", "xlg_profile_enable", "xlg_profile_read", "xlg_client_info", "xlg_add_client_rational", "xlg_poly_profile_read", "xlg_add_client_cascade", "xlg_add_client_cascade_rational", "xlg_cascade_info", "xlg_cascade_profile_read", "xlg_add_subband", "xlg_remove_subband", "xlg_add_client_subband", "xlg_add_client_subband_rational", "xlg_subband_info", "xlg_subband_profile_read", "xlg_add_bank", "xlg_add_bank_subband", "xlg_remove_bank", "xlg_bank_profile_read", "xlg_add_spectrum_any", "xlg_spectrum_any_tables", "xlg_dropin_stats", "xlg_dropin_stream_stats", "xlg_dropin_stream_times",
 ]
 
 
@@ -208,6 +208,10 @@ def lib() -> C.CDLL:
     L.xlg_add_subband_spectrum.restype = C.c_int
     L.xlg_add_spectrum_ex.argtypes = [vp, C.c_int, C.c_int, C.POINTER(XlgSpectrumDesc), C.POINTER(C.c_int)]
     L.xlg_add_spectrum_ex.restype = C.c_int
+    L.xlg_add_spectrum_any.argtypes = [vp, C.c_int, C.c_int, C.POINTER(XlgSpectrumDesc), C.POINTER(C.c_int)]
+    L.xlg_add_spectrum_any.restype = C.c_int
+    L.xlg_spectrum_any_tables.argtypes = [u32, fp, fp, C.POINTER(C.c_uint32)]
+    L.xlg_spectrum_any_tables.restype = C.c_int
     L.xlg_remove_spectrum.argtypes = [vp, C.c_int]
     L.xlg_remove_spectrum.restype = C.c_int
     L.xlg_spectrum_output.argtypes = [vp, C.c_int64, C.c_int, C.POINTER(C.POINTER(C.c_float)), C.POINTER(sz)]
@@ -542,9 +546,10 @@ class Group:
         if code != 0:
             raise ValueError(code)
 
-    def _add_spectrum_ex(self, source, source_id, width, frames_per_row, skip, power, hop, window, mean):
-        """xlg_add_spectrum_ex (hop None: width; window: `width` weights or None; mean: the mean of the row's
-        frames instead of their max)."""
+    def _add_spectrum_ex(self, source, source_id, width, frames_per_row, skip, power, hop, window, mean,
+                         any_width=False):
+        """xlg_add_spectrum_ex, or xlg_add_spectrum_any with any_width (hop None: width; window: `width` weights
+        or None; mean: the mean of the row's frames instead of their max)."""
         w = None
         if window is not None:
             w = np.ascontiguousarray(window, np.float32)
@@ -554,22 +559,25 @@ class Group:
                                0 if hop is None else hop, 1 if mean else 0,
                                None if w is None else w.ctypes.data_as(C.POINTER(C.c_float)))
         sid = C.c_int(-1)
-        code = self._L.xlg_add_spectrum_ex(self._h, source, source_id, C.byref(desc), C.byref(sid))
+        add = self._L.xlg_add_spectrum_any if any_width else self._L.xlg_add_spectrum_ex
+        code = add(self._h, source, source_id, C.byref(desc), C.byref(sid))
         if code != 0:
             raise ValueError(code)
         return sid.value
 
     def add_spectrum(self, width: int, frames_per_row: int, skip: int = 0, power: bool = False,
-                     hop=None, window=None, mean: bool = False) -> int:
+                     hop=None, window=None, mean: bool = False, *, any_width: bool = False) -> int:
         """A spectrum (xlg_add_spectrum) attached before the next submitted block: rows of the max-held power of
         `frames_per_row` consecutive `width`-point DFT frames, `skip` samples skipped after each row, half swapped
         as the reference's spectrogram; dB rows, or linear power with power=True.  spectrogram_params(fs, width)
         gives the reference tool's frames_per_row and skip.  Returns a spectrum id.
         `width` is 1 to 4096, or a power of two from 8192 to 65536 (the wide FFT, the same rows as an FFT at K = width).
         With `hop` (samples between frame starts in a row), `window` (`width` float weights) or mean=True (the
-        mean of the frames' powers instead of their max) it is a Welch spectrum (xlg_add_spectrum_ex)."""
-        if hop is not None or window is not None or mean:
-            return self._add_spectrum_ex(0, 0, width, frames_per_row, skip, power, hop, window, mean)
+        mean of the frames' powers instead of their max) it is a Welch spectrum (xlg_add_spectrum_ex).
+        any_width=True takes every width from 1 to 65536 (xlg_add_spectrum_any): the widths above are served
+        exactly as without it, every other one by the chirp-z stage (spectrum_info kernel 3)."""
+        if any_width or hop is not None or window is not None or mean:
+            return self._add_spectrum_ex(0, 0, width, frames_per_row, skip, power, hop, window, mean, any_width)
         sid = C.c_int(-1)
         code = self._L.xlg_add_spectrum(self._h, width, frames_per_row, skip, XLG_SPECTRUM_POWER if power else 0,
                                         C.byref(sid))
@@ -578,13 +586,15 @@ class Group:
         return sid.value
 
     def add_client_spectrum(self, cid: int, width: int, frames_per_row: int, skip: int = 0,
-                            power: bool = False, hop=None, window=None, mean: bool = False) -> int:
+                            power: bool = False, hop=None, window=None, mean: bool = False, *,
+                            any_width: bool = False) -> int:
         """A spectrum of client `cid`'s output stream (xlg_add_client_spectrum): add_spectrum's rows of what
         output() returns for it from the next submitted block on (a cascade client's final row).
         spectrogram_params(client_rate, width) gives the reference tool's parameters for the client's file.
-        width (1 to 4096, or a power of two from 8192 to 65536), hop, window and mean as for add_spectrum."""
-        if hop is not None or window is not None or mean:
-            return self._add_spectrum_ex(1, cid, width, frames_per_row, skip, power, hop, window, mean)
+        width (1 to 4096, or a power of two from 8192 to 65536), hop, window, mean and any_width as for
+        add_spectrum."""
+        if any_width or hop is not None or window is not None or mean:
+            return self._add_spectrum_ex(1, cid, width, frames_per_row, skip, power, hop, window, mean, any_width)
         sid = C.c_int(-1)
         code = self._L.xlg_add_client_spectrum(self._h, cid, width, frames_per_row, skip,
                                                XLG_SPECTRUM_POWER if power else 0, C.byref(sid))
@@ -593,12 +603,13 @@ class Group:
         return sid.value
 
     def add_subband_spectrum(self, sbid: int, width: int, frames_per_row: int, skip: int = 0,
-                             power: bool = False, hop=None, window=None, mean: bool = False) -> int:
+                             power: bool = False, hop=None, window=None, mean: bool = False, *,
+                             any_width: bool = False) -> int:
         """A spectrum of sub-band (or bank channel) `sbid`'s rows at fs / decim1 (xlg_add_subband_spectrum),
         from the next submitted block on: a zoomed waterfall of the sub-band.  width (1 to 4096, or a power of
-        two from 8192 to 65536), hop, window and mean as for add_spectrum."""
-        if hop is not None or window is not None or mean:
-            return self._add_spectrum_ex(2, sbid, width, frames_per_row, skip, power, hop, window, mean)
+        two from 8192 to 65536), hop, window, mean and any_width as for add_spectrum."""
+        if any_width or hop is not None or window is not None or mean:
+            return self._add_spectrum_ex(2, sbid, width, frames_per_row, skip, power, hop, window, mean, any_width)
         sid = C.c_int(-1)
         code = self._L.xlg_add_subband_spectrum(self._h, sbid, width, frames_per_row, skip,
                                                 XLG_SPECTRUM_POWER if power else 0, C.byref(sid))
@@ -642,8 +653,8 @@ class Group:
         return buf
 
     def spectrum_info(self, sid: int):
-        """(kernel: 0 direct DFT, 1 FFT, 2 wide FFT (width above 4096), rows completed by the blocks submitted
-        so far)."""
+        """(kernel: 0 direct DFT, 1 FFT, 2 wide FFT (width above 4096), 3 chirp-z (any_width, above 4096 and not
+        a power of two), rows completed by the blocks submitted so far)."""
         kind, rows = C.c_int(-1), C.c_uint64(0)
         code = self._L.xlg_spectrum_info(self._h, sid, C.byref(kind), C.byref(rows))
         if code != 0:
@@ -986,6 +997,23 @@ def bank_fft_fits(d1: int, t1: int) -> bool:
 def bank_fft_flops(K: int) -> int:
     """Real FP32 instructions of the butterflies of one K-point FFT bank frame (xlg_bank_fft_flops)."""
     return int(lib().xlg_bank_fft_flops(K))
+
+
+def spectrum_any_tables(width: int):
+    """The chirp-z stage's tables for `width` (above 4096, at most 65536, not a power of two), as the library
+    builds them (xlg_spectrum_any_tables): (chirp: complex64[width], kernel: complex64[M] in the transform's
+    position order, M).  ValueError for any other width."""
+    L = lib()
+    m = C.c_uint32(0)
+    code = L.xlg_spectrum_any_tables(width, None, None, C.byref(m))
+    if code != 0:
+        raise ValueError(code)
+    chirp, kern = np.zeros(width, np.complex64), np.zeros(m.value, np.complex64)
+    fp = C.POINTER(C.c_float)
+    code = L.xlg_spectrum_any_tables(width, chirp.ctypes.data_as(fp), kern.ctypes.data_as(fp), C.byref(m))
+    if code != 0:
+        raise ValueError(code)
+    return chirp, kern, m.value
 
 
 def spectrogram_params(fs: int, width: int):

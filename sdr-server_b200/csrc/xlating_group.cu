@@ -184,6 +184,12 @@ struct SpectrumHost {
   // table, then the C-point one
   bool wide = false;
   float2 *d_scratch = nullptr;  // fb_frames rows of W: pass A's output
+  // xlg_add_spectrum_any above 4096 and not a power of two: the chirp-z passes at M = next_pow2(2W - 1), plain or
+  // extended (ext stays false); d_tw holds the M-point table, the C-point one, the chirp (W) and Bh (M), d_map the
+  // half swap alone (the hold is in natural bin order), d_scratch two sets of fb_frames rows of M
+  bool czt = false;
+  int M = 0;
+  int *d_bin = nullptr;  // the bin of each of the M positions
 };
 
 // members of one sub-band that read the same windows: equal (L2, D2, T2, hist2) and, until their windows have
@@ -264,6 +270,7 @@ struct Slot {
   BlkTable<const float2 *> spring;  // the ring each spblk entry reads
   BlkTable<SpecExt> spext;       // the extended and wide entries' hop, window and frame buffer (the tail of spblk)
   BlkTable<SpecWide> spwide;     // the wide entries' scratch and chunk table (the tail of spext)
+  BlkTable<SpecCzt> spczt;       // the chirp-z entries' scratches and tables (after the wide ones in spext)
   BlkTable<CascBlk> spcb;        // spectra of a source: this block's appends to their rings
   uint64_t sp_frames = 0, sp_flops = 0;
   cudaEvent_t ev_spec = nullptr;  // this block's spectra done (the hold rows are updated in block order on it)
@@ -671,6 +678,7 @@ static void slot_free(Slot &s) {
   s.spring.release();
   s.spext.release();
   s.spwide.release();
+  s.spczt.release();
   if (s.d_sbph) cudaFree(s.d_sbph);
   s.d_sbph = nullptr;
   s.d_pscratch = nullptr;
@@ -1024,11 +1032,12 @@ static int rebuild_banks(xlg_group *g) {
 static int rebuild_spectra(xlg_group *g, size_t &out_total, size_t &max_hist) {
   for (void *p : g->dead_spec) cudaFree(p);
   g->dead_spec.clear();
-  size_t n = 0, n_src = 0, n_ext = 0, n_wide = 0;
+  size_t n = 0, n_src = 0, n_ext = 0, n_wide = 0, n_czt = 0;
   for (SpectrumHost &p : g->spectra) {
     if (!p.active) continue;
-    n_ext += p.ext || p.wide ? 1 : 0;
+    n_ext += p.ext || p.wide || p.czt ? 1 : 0;
     n_wide += p.wide ? 1 : 0;
+    n_czt += p.czt ? 1 : 0;
     p.out_off = (int)out_total;
     out_total += ((size_t)p.rows_cap * p.W + 1) / 2;
     out_total = (out_total + 3) & ~(size_t)3;
@@ -1043,9 +1052,15 @@ static int rebuild_spectra(xlg_group *g, size_t &out_total, size_t &max_hist) {
                              (int)spec_direct_smem(SPEC_MAX_W - 1)));
   CU_OK(cudaFuncSetAttribute(spectrum_direct_ext_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              (int)spec_direct_smem(SPEC_MAX_W - 1)));
+  if (n_czt > 0) {
+    CU_OK(cudaFuncSetAttribute(spectrum_czt_b_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)SPEC_CZT_SMEM));
+    CU_OK(cudaFuncSetAttribute(spectrum_czt_d_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)SPEC_CZT_SMEM));
+  }
   for (Slot &s : g->slots)
     if (s.spblk.reserve(n) || s.spring.reserve(n) || s.spcb.reserve(n_src) || s.spext.reserve(n_ext) ||
-        s.spwide.reserve(n_wide))
+        s.spwide.reserve(n_wide) || s.spczt.reserve(n_czt))
       return -EIO;
   return 0;
 }
@@ -2003,7 +2018,7 @@ extern "C" void xlg_destroy(xlg_group *g) {
   for (float2 *p : g->dead_rings) cudaFree(p);
   for (const SpectrumHost &p : g->spectra)
     for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold, (void *)p.d_ring, (void *)p.d_win,
-                     (void *)p.d_fbuf, (void *)p.d_scratch})
+                     (void *)p.d_fbuf, (void *)p.d_scratch, (void *)p.d_bin})
       if (d) cudaFree(d);
   for (void *p : g->dead_spec) cudaFree(p);
   for (cudaEvent_t e : g->ev_user) cudaEventDestroy(e);
@@ -2520,12 +2535,89 @@ static int source_cap(const xlg_group *g, const HostClient &h) {
   return h.casc ? stage_b_rows((uint64_t)cap, h.b2.geo.L2, h.b2.geo.D2) : cap;
 }
 
+// The chirp-z stage's M and tables for width W (xlating_kernels.cuh, "Chirp-z spectra"): c[n] = e^{-i pi (n^2
+// mod 2W) / W}, n < W, and Bh, the M-point DFT of b[m] = conj(c[|m|]) for |m| < W wrapped mod M, times 1/M, in
+// the position order of the kernels' transform (kern[p] = Bh[bin[p]]); both computed in double and rounded once.
+// The DFT is an iterative radix-2 FFT with each twiddle from cos and sin of its own angle.
+static int czt_m(int W) { return (int)next_pow2(2 * (size_t)W - 1); }
+
+static void czt_tables(int W, std::vector<float2> &chirp, std::vector<float2> &kern, std::vector<int> &bin) {
+  const int M = czt_m(W);
+  const double pi = 3.14159265358979323846;
+  std::vector<double> cr((size_t)W), ci((size_t)W);
+  chirp.resize((size_t)W);
+  for (int n = 0; n < W; n++) {
+    const uint64_t r = (uint64_t)n * (uint64_t)n % (2 * (uint64_t)W);  // n^2 passes 2^31 at n = 46341
+    const double t = pi * (double)r / (double)W;
+    cr[n] = cos(t);
+    ci[n] = -sin(t);
+    chirp[n] = make_float2((float)cr[n], (float)ci[n]);
+  }
+  std::vector<double> re((size_t)M, 0.0), im((size_t)M, 0.0);
+  for (int m = 0; m < W; m++) {
+    re[m] = cr[m];
+    im[m] = -ci[m];
+    if (m > 0) {
+      re[M - m] = cr[m];
+      im[M - m] = -ci[m];
+    }
+  }
+  for (int i = 1, j = 0; i < M; i++) {  // bit reversal, then decimation in time
+    int bit = M >> 1;
+    for (; j & bit; bit >>= 1) j ^= bit;
+    j ^= bit;
+    if (i < j) {
+      std::swap(re[i], re[j]);
+      std::swap(im[i], im[j]);
+    }
+  }
+  for (int len = 2; len <= M; len <<= 1)
+    for (int k = 0; k < len / 2; k++) {
+      const double t = -2.0 * pi * (double)k / (double)len, wr = cos(t), wi = sin(t);
+      for (int i = k; i < M; i += len) {
+        const int h = i + len / 2;
+        const double xr = re[h] * wr - im[h] * wi, xi = re[h] * wi + im[h] * wr;
+        re[h] = re[i] - xr;
+        im[h] = im[i] - xi;
+        re[i] += xr;
+        im[i] += xi;
+      }
+    }
+  kern.resize((size_t)M);
+  bin.resize((size_t)M);
+  for (int k = 0; k < M; k++) {
+    const int p = bank_fft_pos(k, M);
+    bin[p] = k;
+    kern[p] = make_float2((float)(re[k] / M), (float)(im[k] / M));
+  }
+}
+
+extern "C" int xlg_spectrum_any_tables(uint32_t width, float *chirp, float *kernel, uint32_t *m) {
+  if (width <= SPEC_MAX_W || width > SPEC_WIDE_MAX_W || spec_wide((int)width)) return -EINVAL;
+  const int W = (int)width;
+  if (m) *m = (uint32_t)czt_m(W);
+  if (chirp == nullptr && kernel == nullptr) return 0;
+  std::vector<float2> c, k;
+  std::vector<int> bin;
+  czt_tables(W, c, k, bin);
+  if (chirp) memcpy(chirp, c.data(), c.size() * sizeof(float2));
+  if (kernel) memcpy(kernel, k.data(), k.size() * sizeof(float2));
+  return 0;
+}
+
 // A spectrum of the band (src = -1) or of client index src's output stream, after the checks of its source.
-// hop 0 means width; today's spectra are hop = width, reduce = XLG_SPECTRUM_MAX and no window.
+// hop 0 means width; today's spectra are hop = width, reduce = XLG_SPECTRUM_MAX and no window.  any: every width
+// up to 65536, those above 4096 that are not powers of two through the chirp-z stage.
 static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_per_row, uint32_t skip_per_row,
-                        uint32_t flags, uint32_t hop, uint32_t reduce, const float *window, int *spectrum_id) {
-  if (width == 0 || (width > SPEC_MAX_W && !spec_wide((int)std::min<uint32_t>(width, 1u << 30))) ||
-      frames_per_row == 0) {
+                        uint32_t flags, uint32_t hop, uint32_t reduce, const float *window, bool any,
+                        int *spectrum_id) {
+  if (any && (width == 0 || width > SPEC_WIDE_MAX_W || frames_per_row == 0)) {
+    XL_LOG("spectrum: width %u must be in [1, %d], and frames per row %u at least 1", width, SPEC_WIDE_MAX_W,
+           frames_per_row);
+    return -EINVAL;
+  }
+  if (!any && (width == 0 || (width > SPEC_MAX_W && !spec_wide((int)std::min<uint32_t>(width, 1u << 30))) ||
+               frames_per_row == 0)) {
     XL_LOG("spectrum: width %u must be in [1, %d] or a power of two up to %d, and frames per row %u at least 1",
            width, SPEC_MAX_W, SPEC_WIDE_MAX_W, frames_per_row);
     return -EINVAL;
@@ -2570,7 +2662,9 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
   p.H = (int)hop;
   p.mean = reduce == XLG_SPECTRUM_MEAN;
   p.wide = spec_wide(p.W);
-  p.ext = !p.wide && (p.H != p.W || window != nullptr || p.mean);
+  p.czt = p.W > SPEC_MAX_W && !p.wide;  // (only through xlg_add_spectrum_any)
+  p.M = p.czt ? czt_m(p.W) : 0;
+  p.ext = !p.wide && !p.czt && (p.H != p.W || window != nullptr || p.mean);
   p.src = src;
   // a source's positions count from here: P = 0 in its own stream
   const uint64_t cap = src < 0 ? (uint64_t)g->max_input_len / 2 : (uint64_t)source_cap(g, g->clients[src]);
@@ -2580,7 +2674,7 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
   // the frames a block of at most cap samples completes: their last samples are distinct positions of the block,
   // one frame's at least min(H, W + S) after the previous one's (H within a row, W + S from a row's last frame to
   // the next row's first)
-  if (p.mean || p.wide) p.fb_frames = (int)((cap - 1) / std::min<uint64_t>(hop, (uint64_t)width + skip_per_row) + 1);
+  if (p.mean || p.wide || p.czt) p.fb_frames = (int)((cap - 1) / std::min<uint64_t>(hop, (uint64_t)width + skip_per_row) + 1);
   // a source's ring holds every sample of the frames a block completes: the block's own and W - 1 before them
   const size_t ring_cap = src < 0 ? 0 : next_pow2((size_t)width - 1 + (size_t)cap);
   p.ring_mask = (unsigned)(ring_cap - 1);
@@ -2591,10 +2685,17 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
     const int bin = j < half ? half + j : j < 2 * half ? j - half : W - 1;
     map[j] = spec_fft(W) || p.wide ? bank_fft_pos(bin, W) : bin;
   }
-  std::vector<float2> tw = twiddle_table(W);
-  if (p.wide) {  // pass B's table after the W-point one
-    const std::vector<float2> tc = twiddle_table(spec_wide_chunk(W));
+  std::vector<float2> tw = twiddle_table(p.czt ? p.M : W);
+  std::vector<int> czbin;
+  if (p.wide || p.czt) {  // pass B's table after the W- or M-point one
+    const std::vector<float2> tc = twiddle_table(spec_wide_chunk(p.czt ? p.M : W));
     tw.insert(tw.end(), tc.begin(), tc.end());
+  }
+  if (p.czt) {  // then the chirp and Bh
+    std::vector<float2> chirp, kern;
+    czt_tables(W, chirp, kern, czbin);
+    tw.insert(tw.end(), chirp.begin(), chirp.end());
+    tw.insert(tw.end(), kern.begin(), kern.end());
   }
   const size_t hold_bytes = (size_t)p.NR * W * sizeof(unsigned);
   if (cudaMalloc(&p.d_tw, tw.size() * sizeof(float2)) != cudaSuccess ||
@@ -2602,9 +2703,11 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
       (ring_cap > 0 && cudaMalloc(&p.d_ring, ring_cap * sizeof(float2)) != cudaSuccess) ||
       (window != nullptr && cudaMalloc(&p.d_win, W * sizeof(float)) != cudaSuccess) ||
       (p.mean && cudaMalloc(&p.d_fbuf, (size_t)p.fb_frames * W * sizeof(float)) != cudaSuccess) ||
-      (p.wide && cudaMalloc(&p.d_scratch, (size_t)p.fb_frames * W * sizeof(float2)) != cudaSuccess)) {
+      (p.wide && cudaMalloc(&p.d_scratch, (size_t)p.fb_frames * W * sizeof(float2)) != cudaSuccess) ||
+      (p.czt && cudaMalloc(&p.d_scratch, 2 * (size_t)p.fb_frames * p.M * sizeof(float2)) != cudaSuccess) ||
+      (p.czt && cudaMalloc(&p.d_bin, (size_t)p.M * sizeof(int)) != cudaSuccess)) {
     for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold, (void *)p.d_ring, (void *)p.d_win,
-                     (void *)p.d_fbuf, (void *)p.d_scratch})
+                     (void *)p.d_fbuf, (void *)p.d_scratch, (void *)p.d_bin})
       if (d) cudaFree(d);
     XL_LOG("spectrum: out of device memory");
     return -ENOMEM;
@@ -2612,6 +2715,7 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
   CU_OK(cudaMemcpy(p.d_tw, tw.data(), tw.size() * sizeof(float2), cudaMemcpyHostToDevice));
   CU_OK(cudaMemcpy(p.d_map, map.data(), W * sizeof(int), cudaMemcpyHostToDevice));
   if (window != nullptr) CU_OK(cudaMemcpy(p.d_win, window, W * sizeof(float), cudaMemcpyHostToDevice));
+  if (p.czt) CU_OK(cudaMemcpy(p.d_bin, czbin.data(), (size_t)p.M * sizeof(int), cudaMemcpyHostToDevice));
   // (on a group stream, finished before the spectrum exists: the kernels' streams do not wait for the legacy one)
   CU_OK(cudaMemsetAsync(p.d_hold, 0, hold_bytes, g->s_in));
   CU_OK(cudaStreamSynchronize(g->s_in));
@@ -2628,7 +2732,7 @@ extern "C" int xlg_add_spectrum(xlg_group *g, uint32_t width, uint32_t frames_pe
                                 uint32_t flags, int *spectrum_id) {
   if (g == nullptr || spectrum_id == nullptr) return -EINVAL;
   return add_spectrum(g, -1, width, frames_per_row, skip_per_row, flags, width, XLG_SPECTRUM_MAX, nullptr,
-                      spectrum_id);
+                      false, spectrum_id);
 }
 
 extern "C" int xlg_add_client_spectrum(xlg_group *g, int client_id, uint32_t width, uint32_t frames_per_row,
@@ -2640,7 +2744,7 @@ extern "C" int xlg_add_client_spectrum(xlg_group *g, int client_id, uint32_t wid
     return -EINVAL;
   }
   return add_spectrum(g, client_id, width, frames_per_row, skip_per_row, flags, width, XLG_SPECTRUM_MAX, nullptr,
-                      spectrum_id);
+                      false, spectrum_id);
 }
 
 extern "C" int xlg_add_subband_spectrum(xlg_group *g, int subband_id, uint32_t width, uint32_t frames_per_row,
@@ -2652,11 +2756,12 @@ extern "C" int xlg_add_subband_spectrum(xlg_group *g, int subband_id, uint32_t w
     return -EINVAL;
   }
   return add_spectrum(g, cid, width, frames_per_row, skip_per_row, flags, width, XLG_SPECTRUM_MAX, nullptr,
-                      spectrum_id);
+                      false, spectrum_id);
 }
 
-extern "C" int xlg_add_spectrum_ex(xlg_group *g, int source, int source_id, const xlg_spectrum_desc *desc,
-                                   int *spectrum_id) {
+// xlg_add_spectrum_ex, and with any = true xlg_add_spectrum_any
+static int add_spectrum_desc(xlg_group *g, int source, int source_id, const xlg_spectrum_desc *desc, bool any,
+                             int *spectrum_id) {
   if (g == nullptr || spectrum_id == nullptr) return -EINVAL;
   if (desc == nullptr) {
     XL_LOG("spectrum: no description");
@@ -2681,7 +2786,17 @@ extern "C" int xlg_add_spectrum_ex(xlg_group *g, int source, int source_id, cons
     return -EINVAL;
   }
   return add_spectrum(g, src, desc->width, desc->frames_per_row, desc->skip_per_row, desc->flags, desc->hop,
-                      desc->reduce, desc->window, spectrum_id);
+                      desc->reduce, desc->window, any, spectrum_id);
+}
+
+extern "C" int xlg_add_spectrum_ex(xlg_group *g, int source, int source_id, const xlg_spectrum_desc *desc,
+                                   int *spectrum_id) {
+  return add_spectrum_desc(g, source, source_id, desc, false, spectrum_id);
+}
+
+extern "C" int xlg_add_spectrum_any(xlg_group *g, int source, int source_id, const xlg_spectrum_desc *desc,
+                                    int *spectrum_id) {
+  return add_spectrum_desc(g, source, source_id, desc, true, spectrum_id);
 }
 
 static SpectrumHost *spectrum_of(xlg_group *g, int id) {
@@ -2698,7 +2813,7 @@ extern "C" int xlg_remove_spectrum(xlg_group *g, int spectrum_id) {
   }
   // in-flight tickets still read the tables and the hold: freed at the next re-layout, which drains
   for (void *d : {(void *)p->d_tw, (void *)p->d_map, (void *)p->d_hold, (void *)p->d_ring, (void *)p->d_win,
-                   (void *)p->d_fbuf, (void *)p->d_scratch})
+                   (void *)p->d_fbuf, (void *)p->d_scratch, (void *)p->d_bin})
     if (d) g->dead_spec.push_back(d);
   *p = SpectrumHost();
   g->dirty = true;
@@ -2709,7 +2824,7 @@ extern "C" int xlg_spectrum_info(const xlg_group *g, int spectrum_id, int *kerne
   if (g == nullptr) return -EINVAL;
   const SpectrumHost *p = spectrum_of(const_cast<xlg_group *>(g), spectrum_id);
   if (p == nullptr) return -EINVAL;
-  if (kernel) *kernel = p->wide ? 2 : spec_fft(p->W) ? 1 : 0;
+  if (kernel) *kernel = p->czt ? 3 : p->wide ? 2 : spec_fft(p->W) ? 1 : 0;
   if (rows_done) *rows_done = p->rows_done;
   return 0;
 }
@@ -2760,6 +2875,9 @@ struct Block {
   size_t spxf_smem = 0, spxd_smem = 0;
   // the wide spectra, after the extended ones: CTAs of their two passes (the fold also covers them)
   int n_spw = 0, max_spwa_ctas = 0, max_spwb_ctas = 0;
+  // the chirp-z spectra, after the wide ones: CTAs of their pass-A and pass-B launches, pass B's shared memory
+  int n_spc = 0, max_spca_ctas = 0, max_spcb_ctas = 0;
+  size_t spcb_smem = 0;
   int n_spa = 0, max_spa_n = 0;  // appends to spectrum sources' rings, the longest
   // sub-band walk
   int n_sb = 0, max_sb_n1 = 0, max_sb_n2 = 0;
@@ -2895,7 +3013,7 @@ static void walk_spectrum(Block &b, int id) {
   }
   const uint64_t d = (uint64_t)(E - p.P), F = (uint64_t)p.F;
   uint64_t total;
-  if (p.ext || p.wide) {  // frames completed at offset o of a row: none before W, then one more every H, at most F
+  if (p.ext || p.wide || p.czt) {  // frames completed at offset o of a row: none before W, then one more every H, at most F
     const uint64_t o = d % (uint64_t)p.R;
     total = d / (uint64_t)p.R * F + (o < (uint64_t)p.W ? 0 : std::min<uint64_t>(F, (o - p.W) / (uint64_t)p.H + 1));
   } else {
@@ -2924,11 +3042,13 @@ static void walk_spectrum(Block &b, int id) {
     e.slot0 = (int)(p.rows_done % (uint64_t)p.NR);
     e.power = p.power ? 1 : 0;
     e.inv_w = 1.0f / (float)p.W;
-    const uint64_t flops = spec_fft(p.W) || p.wide ? xlg_bank_fft_flops((uint32_t)p.W) : 4ull * p.W * p.W;
+    // a chirp-z frame: two M-point transforms, the chirp's W products and Bh's M (4 instructions each)
+    const uint64_t flops = p.czt ? 2 * xlg_bank_fft_flops((uint32_t)p.M) + 4ull * p.W + 4ull * p.M
+                           : spec_fft(p.W) || p.wide ? xlg_bank_fft_flops((uint32_t)p.W) : 4ull * p.W * p.W;
     s.sp_frames += (uint64_t)n_frames;
     s.sp_flops += (uint64_t)n_frames * (flops + 6ull * p.W + (p.d_win ? 2ull * p.W : 0) + (p.mean ? p.W : 0));
-    if (p.ext || p.wide) {
-      SpecExt &x = s.spext.h[b.n_spx + b.n_spw];
+    if (p.ext || p.wide || p.czt) {
+      SpecExt &x = s.spext.h[b.n_spx + b.n_spw + b.n_spc];
       x.win = p.d_win;
       x.fbuf = p.d_fbuf;
       x.H = p.H;
@@ -2936,7 +3056,21 @@ static void walk_spectrum(Block &b, int id) {
     }
     if (p.mean)  // values of the rows its frames touch
       b.max_fold_values = std::max(b.max_fold_values, (int)(((long long)p.fir + n_frames - 1) / p.F + 1) * p.W);
-    if (p.wide) {
+    if (p.czt) {
+      SpecCzt &c = s.spczt.h[b.n_spc++];
+      const int C = spec_wide_chunk(p.M);
+      const size_t rows = (size_t)p.fb_frames * p.M;
+      c.s1 = p.d_scratch;
+      c.s2 = p.d_scratch + rows;
+      c.tw_c = p.d_tw + p.M;
+      c.chirp = c.tw_c + C;
+      c.kern = c.chirp + p.W;
+      c.bin = p.d_bin;
+      c.M = p.M;
+      b.max_spca_ctas = std::max(b.max_spca_ctas, n_frames * (C / SPEC_THREADS));
+      b.max_spcb_ctas = std::max(b.max_spcb_ctas, n_frames * (p.M / C));
+      b.spcb_smem = std::max(b.spcb_smem, (size_t)C * sizeof(float2));
+    } else if (p.wide) {
       SpecWide &w = s.spwide.h[b.n_spw++];
       w.scratch = p.d_scratch;
       w.tw_c = p.d_tw + p.W;
@@ -2969,15 +3103,15 @@ static void walk_spectrum(Block &b, int id) {
   p.fir = (int)(total % F);
 }
 
-// every spectrum, today's first: the table is [plain entries | extended entries | wide entries]
+// every spectrum, today's first: the table is [plain entries | extended entries | wide entries | chirp-z entries]
 static void walk_spectra(Block &b) {
   xlg_group *g = b.g;
   b.s.sp_frames = b.s.sp_flops = 0;
-  for (int seg = 0; seg < 3; seg++)
+  for (int seg = 0; seg < 4; seg++)
     for (int id = 0; id < (int)g->spectra.size(); id++) {
       const SpectrumHost &p = g->spectra[id];
       if (seg == 0) b.ho.sp_w[id] = p.active ? p.W : 0;
-      if (p.active && (p.wide ? 2 : p.ext ? 1 : 0) == seg) walk_spectrum(b, id);
+      if (p.active && (p.czt ? 3 : p.wide ? 2 : p.ext ? 1 : 0) == seg) walk_spectrum(b, id);
     }
 }
 
@@ -3138,16 +3272,16 @@ static int launch_spectra(Block &b) {
     CU_OK(s.spblk.upload((size_t)b.n_spec, b.cs));
     CU_OK(s.spring.upload((size_t)b.n_spec, b.cs));
   }
-  const int n_plain = b.n_spec - b.n_spx - b.n_spw;
+  const int n_plain = b.n_spec - b.n_spx - b.n_spw - b.n_spc;
   if (b.max_spf_ctas > 0)
     spectrum_fft_kernel<<<dim3(b.max_spf_ctas, n_plain), SPEC_THREADS, b.spf_smem, b.cs>>>(s.spblk.d, s.spring.d);
   if (b.max_spd_ctas > 0)
     spectrum_direct_kernel<<<dim3(b.max_spd_ctas, b.max_spd_groups, n_plain), SPEC_THREADS, b.spd_smem, b.cs>>>(
         s.spblk.d, s.spring.d);
-  if (b.n_spx + b.n_spw > 0) {
+  if (b.n_spx + b.n_spw + b.n_spc > 0) {
     const SpecBlk *xb = s.spblk.d + n_plain;
     const float2 *const *xr = s.spring.d + n_plain;
-    CU_OK(s.spext.upload((size_t)(b.n_spx + b.n_spw), b.cs));
+    CU_OK(s.spext.upload((size_t)(b.n_spx + b.n_spw + b.n_spc), b.cs));
     if (b.max_spxf_ctas > 0)
       spectrum_fft_ext_kernel<<<dim3(b.max_spxf_ctas, b.n_spx), SPEC_THREADS, b.spxf_smem, b.cs>>>(xb, xr, s.spext.d);
     if (b.max_spxd_ctas > 0)
@@ -3160,9 +3294,19 @@ static int launch_spectra(Block &b) {
       spectrum_wide_b_kernel<<<dim3(b.max_spwb_ctas, b.n_spw), SPEC_THREADS, SPEC_WIDE_SMEM, b.cs>>>(
           xb + b.n_spx, s.spext.d + b.n_spx, s.spwide.d);
     }
+    if (b.n_spc > 0) {  // the chirp-z entries: the forward transform and Bh into s2, the second transform
+      const int o = b.n_spx + b.n_spw;
+      CU_OK(s.spczt.upload((size_t)b.n_spc, b.cs));
+      spectrum_czt_a_kernel<<<dim3(b.max_spca_ctas, b.n_spc), SPEC_THREADS, 0, b.cs>>>(xb + o, xr + o,
+                                                                                     s.spext.d + o, s.spczt.d);
+      spectrum_czt_b_kernel<<<dim3(b.max_spcb_ctas, b.n_spc), SPEC_THREADS, b.spcb_smem, b.cs>>>(xb + o, s.spczt.d);
+      spectrum_czt_c_kernel<<<dim3(b.max_spca_ctas, b.n_spc), SPEC_THREADS, 0, b.cs>>>(xb + o, s.spczt.d);
+      spectrum_czt_d_kernel<<<dim3(b.max_spcb_ctas, b.n_spc), SPEC_THREADS, b.spcb_smem, b.cs>>>(xb + o, s.spext.d + o,
+                                                                                                s.spczt.d);
+    }
     if (b.max_fold_values > 0)
-      spectrum_fold_kernel<<<dim3((b.max_fold_values + SPEC_THREADS - 1) / SPEC_THREADS, b.n_spx + b.n_spw),
-                             SPEC_THREADS, 0, b.cs>>>(xb, s.spext.d);
+      spectrum_fold_kernel<<<dim3((b.max_fold_values + SPEC_THREADS - 1) / SPEC_THREADS,
+                                  b.n_spx + b.n_spw + b.n_spc), SPEC_THREADS, 0, b.cs>>>(xb, s.spext.d);
   }
   if (b.max_sp_values > 0)
     spectrum_emit_kernel<<<dim3((b.max_sp_values + SPEC_THREADS - 1) / SPEC_THREADS, b.n_spec), SPEC_THREADS, 0,

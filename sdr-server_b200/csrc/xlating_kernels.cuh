@@ -2193,4 +2193,174 @@ spectrum_wide_b_kernel(const SpecBlk *__restrict__ blk, const SpecExt *__restric
   for (int t = tid; t < C; t += SPEC_THREADS) atomicMax(hold + t, spec_power(u[t], b.inv_w));
 }
 
+// ---------------------------------------------------------------------------
+// Chirp-z spectra (xlg_add_spectrum_any, every W up to 65536 that the entries above do not serve: above 4096 and
+// not a power of two).  Bluestein's identity kn = (k^2 + n^2 - (k - n)^2) / 2 turns the W-point DFT of a frame z
+// (windowed as spec_load does) into a circular convolution of length M = next_pow2(2W - 1) (16384 to 131072),
+// which the wide passes' M-point FFT computes.  With c[n] = e^{-i pi (n^2 mod 2W) / W} (the index in 64 bits),
+// and Bh[p] the M-point DFT of b[m] = e^{+i pi (m^2 mod 2W) / W}, |m| < W, wrapped mod M, scaled by 1/M and
+// stored at the positions p of the transform's output (bin bin[p]; all three tables built in double on the host
+// and rounded once to float), in this order (cmul_tw's rounded products and fmaf for every complex product):
+//   a[n] = cmul_tw(z[n], c[n]) for n < W, +0 for W <= n < M
+//   A    = fft_dif_rows' M-point transform of a (pass A then pass B as for a wide spectrum), in position order
+//   Y[p] = cmul_tw(A[p], Bh[p]);  y[bin[p]] = (Y[p].x, -Y[p].y)         (conj(Y), scattered into natural order)
+//   v    = the same M-point transform of y;  X_k = conj(v[k]) c[k] for k < W
+// |c[k]| = 1, so the rows are defined on v itself: p_k = spec_power(v[k]), with the 1/W of a W-point spectrum;
+// no post-chirp is applied.  Four launches serve every chirp-z entry of a block:
+//   spectrum_czt_a_kernel: thread (frame j, column i < C) loads the 4^s points i + m C (spec_load, then the chirp;
+//     the zero padding is written, never left from an earlier frame), runs pass A's stages and stores them at the
+//     same positions of row j of scratch s1 (M float2 per frame)
+//   spectrum_czt_b_kernel: CTA (frame j, chunk c) runs fft_dif_rows on chunk c of s1's row j, multiplies by Bh,
+//     conjugates and scatters each position p to y[bin[p]] in row j of scratch s2
+//   spectrum_czt_c_kernel: pass A of the second transform, in place on s2's row j
+//   spectrum_czt_d_kernel: CTA (frame j, chunk c) runs fft_dif_rows on chunk c of s2's row j and folds p of every
+//     position whose bin is below W into the hold (atomicMax) or the mean's frame buffer (bins in natural order;
+//     positions of bins >= W are dropped)
+// M = 131072 takes two pass-A stages and 8192-point chunks in 64 KiB of dynamic shared memory, the same split as
+// the wide passes at every other M.  The entries are the tail of the block's table, [plain | extended | wide |
+// chirp-z]: each has a SpecExt (fold and emit finish their rows unchanged) and a SpecCzt.
+// ---------------------------------------------------------------------------
+constexpr int SPEC_CZT_MAX_M = 131072;
+constexpr size_t SPEC_CZT_SMEM = (SPEC_CZT_MAX_M >> 4) * sizeof(float2);  // passes B and D: the largest chunk
+
+struct SpecCzt {
+  float2 *s1, *s2;        // a row of M per frame of this block each: pass A's output, then y
+  const float2 *tw_c;     // the C-point table (SpecBlk.tw is the M-point one)
+  const float2 *chirp;    // c[n], n < W
+  const float2 *kern;     // Bh, in position order
+  const int *bin;         // the bin of each position
+  int M;
+};
+
+// pass A's stages on a[] = the 4^NS points i + m C of an M-point row, in place (spec_wide_pass_a's butterflies)
+template <int NS>
+__device__ __forceinline__ void czt_pass_a(float2 (&a)[NS == 1 ? 4 : 16], const float2 *__restrict__ tw, int i,
+                                           int C) {
+  constexpr int Q = NS == 1 ? 1 : 4;
+#pragma unroll
+  for (int r = 0; r < Q; r++) dif_bfly4(a[r], a[r + Q], a[r + 2 * Q], a[r + 3 * Q], tw, i + r * C);
+  if (NS == 2) {
+#pragma unroll
+    for (int q = 0; q < 4; q++) dif_bfly4(a[4 * q], a[4 * q + 1], a[4 * q + 2], a[4 * q + 3], tw, 4 * i);
+  }
+}
+
+template <int NS>
+__device__ __forceinline__ void czt_load_a(const float2 *__restrict__ ring, unsigned mask, long long pos,
+                                           const float *__restrict__ win, const float2 *__restrict__ chirp, int W,
+                                           const float2 *__restrict__ tw, float2 *__restrict__ row, int i, int C) {
+  constexpr int NP = NS == 1 ? 4 : 16;
+  float2 a[NP];
+#pragma unroll
+  for (int m = 0; m < NP; m++) {
+    const int n = i + m * C;
+    a[m] = n < W ? cmul_tw(spec_load(ring, mask, pos + n, win, n), __ldg(chirp + n)) : make_float2(0.f, 0.f);
+  }
+  czt_pass_a<NS>(a, tw, i, C);
+#pragma unroll
+  for (int m = 0; m < NP; m++) row[i + m * C] = a[m];
+}
+
+template <int NS>
+__device__ __forceinline__ void czt_inplace_a(float2 *__restrict__ row, const float2 *__restrict__ tw, int i, int C) {
+  constexpr int NP = NS == 1 ? 4 : 16;
+  float2 a[NP];
+#pragma unroll
+  for (int m = 0; m < NP; m++) a[m] = row[i + m * C];
+  czt_pass_a<NS>(a, tw, i, C);
+#pragma unroll
+  for (int m = 0; m < NP; m++) row[i + m * C] = a[m];
+}
+
+// CTA (x, s): threads [x 256, x 256 + 256) of chirp-z spectrum s's frames x C columns (first = true: the chirped
+// frames from the ring into s1; else s2 in place)
+template <bool FIRST>
+__device__ __forceinline__ void spectrum_czt_pass_a(const SpecBlk *__restrict__ blk,
+                                                    const float2 *const *__restrict__ rings,
+                                                    const SpecExt *__restrict__ ext, const SpecCzt *__restrict__ czt) {
+  const SpecBlk b = blk[blockIdx.y];
+  const SpecCzt z = czt[blockIdx.y];
+  const int M = z.M, C = spec_wide_chunk(M), lc = 31 - __clz(C);
+  const int e = blockIdx.x * SPEC_THREADS + threadIdx.x, j = e >> lc, i = e & (C - 1);
+  if (j >= b.n_frames) return;
+  if (FIRST) {
+    const SpecExt x = ext[blockIdx.y];
+    const long long pos = spec_frame_pos(b, x.H, j);
+    float2 *row = z.s1 + (size_t)j * M;
+    if (spec_wide_stages(M) == 1)
+      czt_load_a<1>(rings[blockIdx.y], b.mask, pos, x.win, z.chirp, b.W, b.tw, row, i, C);
+    else
+      czt_load_a<2>(rings[blockIdx.y], b.mask, pos, x.win, z.chirp, b.W, b.tw, row, i, C);
+  } else {
+    float2 *row = z.s2 + (size_t)j * M;
+    if (spec_wide_stages(M) == 1)
+      czt_inplace_a<1>(row, b.tw, i, C);
+    else
+      czt_inplace_a<2>(row, b.tw, i, C);
+  }
+}
+
+__global__ void __launch_bounds__(SPEC_THREADS)
+spectrum_czt_a_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__restrict__ rings,
+                      const SpecExt *__restrict__ ext, const SpecCzt *__restrict__ czt) {
+  spectrum_czt_pass_a<true>(blk, rings, ext, czt);
+}
+
+__global__ void __launch_bounds__(SPEC_THREADS)
+spectrum_czt_c_kernel(const SpecBlk *__restrict__ blk, const SpecCzt *__restrict__ czt) {
+  spectrum_czt_pass_a<false>(blk, nullptr, nullptr, czt);
+}
+
+// CTA (x, s): chunk x mod 4^s of frame x / 4^s of chirp-z spectrum s: pass B of the first transform, the product
+// with Bh, the conjugate and the scatter into natural order
+__global__ void __launch_bounds__(SPEC_THREADS, 3)
+spectrum_czt_b_kernel(const SpecBlk *__restrict__ blk, const SpecCzt *__restrict__ czt) {
+  extern __shared__ __align__(16) float2 u[];
+  const SpecBlk b = blk[blockIdx.y];
+  const SpecCzt z = czt[blockIdx.y];
+  const int M = z.M, ls = 2 * spec_wide_stages(M), C = M >> ls, lc = 31 - __clz(C), tid = threadIdx.x;
+  const int j = blockIdx.x >> ls, c0 = (blockIdx.x & ((1 << ls) - 1)) * C;
+  if (j >= b.n_frames) return;
+  const float2 *src = z.s1 + (size_t)j * M + c0;
+  for (int t = tid; t < C; t += SPEC_THREADS) u[t] = src[t];
+  __syncthreads();
+  fft_dif_rows<SPEC_THREADS>(u, 1, C, lc, z.tw_c, tid);
+  float2 *dst = z.s2 + (size_t)j * M;
+  for (int t = tid; t < C; t += SPEC_THREADS) {
+    const float2 y = cmul_tw(u[t], __ldg(z.kern + c0 + t));
+    dst[__ldg(z.bin + c0 + t)] = make_float2(y.x, -y.y);
+  }
+}
+
+// CTA (x, s): chunk x mod 4^s of frame x / 4^s of chirp-z spectrum s: pass B of the second transform and the
+// powers of bins below W into the hold or the mean's frame buffer
+__global__ void __launch_bounds__(SPEC_THREADS, 3)
+spectrum_czt_d_kernel(const SpecBlk *__restrict__ blk, const SpecExt *__restrict__ ext,
+                      const SpecCzt *__restrict__ czt) {
+  extern __shared__ __align__(16) float2 u[];
+  const SpecBlk b = blk[blockIdx.y];
+  const SpecExt x = ext[blockIdx.y];
+  const SpecCzt z = czt[blockIdx.y];
+  const int W = b.W, M = z.M, ls = 2 * spec_wide_stages(M), C = M >> ls, lc = 31 - __clz(C), tid = threadIdx.x;
+  const int j = blockIdx.x >> ls, c0 = (blockIdx.x & ((1 << ls) - 1)) * C;
+  if (j >= b.n_frames) return;
+  const float2 *src = z.s2 + (size_t)j * M + c0;
+  for (int t = tid; t < C; t += SPEC_THREADS) u[t] = src[t];
+  __syncthreads();
+  fft_dif_rows<SPEC_THREADS>(u, 1, C, lc, z.tw_c, tid);
+  if (x.mean) {
+    float *fb = x.fbuf + (size_t)j * W;
+    for (int t = tid; t < C; t += SPEC_THREADS) {
+      const int k = __ldg(z.bin + c0 + t);
+      if (k < W) fb[k] = __uint_as_float(spec_power(u[t], b.inv_w));
+    }
+    return;
+  }
+  unsigned *hold = b.hold + (size_t)spec_frame(b, j).hold_row * W;
+  for (int t = tid; t < C; t += SPEC_THREADS) {
+    const int k = __ldg(z.bin + c0 + t);
+    if (k < W) atomicMax(hold + k, spec_power(u[t], b.inv_w));
+  }
+}
+
 }  // namespace xl

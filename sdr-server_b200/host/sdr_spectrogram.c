@@ -10,6 +10,10 @@
  * collected in order.  The host forms 10 * log10f(v) in float as spectrogram.c:156-163 does, then the pixel as
  * png_util_set_data does, (int)(dB + 255) clamped to [0, 255]: the pixels are a function of the power rows alone.
  *
+ * With -a (not the reference's) the spectrum is xlg_add_spectrum_any's at the same parameters: every -w up to 65536
+ * (and up to fs), widths above 4096 that are not powers of two through the chirp-z stage.  The widths the tool
+ * serves without -a give the same rows, so the same image, with it.
+ *
  * Height: floor(samples / fs), samples being the whole complex samples of the file (its size, or the gzip trailer's
  * size field for .gz, as the reference does), counted in 64 bits (the reference's uint32_t count wraps at 2^32
  * samples).  Exactly the rows whose full period lies in the file.
@@ -46,6 +50,7 @@ static void usage(void) {
   printf("  -d <data_format> data format: cu8, cs16, cf32 (default: cu8)\n");
   printf("  -i <input_file> I/Q input file\n");
   printf("  -o <output_file> spectrogram output\n");
+  printf("  -a  any width up to 65536 (not only up to 4096 or a power of two), through the chirp-z transform\n");
   printf("  -f <fftw_flags> supported values: FFTW_ESTIMATE, FFTW_MEASURE (accepted for compatibility; the transform "
          "runs on the GPU). Default: FFTW_MEASURE\n");
 }
@@ -72,9 +77,12 @@ int main(int argc, char **argv) {
   int width = 1024;
   double fs_arg = 48000;
   const char *data_format = "cu8", *input_file = NULL, *output_file = NULL, *fftw_flags = "FFTW_MEASURE";
-  int opt;
-  while ((opt = getopt(argc, argv, "hw:s:d:i:o:f:")) != -1) {
+  int opt, any_width = 0;
+  while ((opt = getopt(argc, argv, "ahw:s:d:i:o:f:")) != -1) {
     switch (opt) {
+      case 'a':
+        any_width = 1;
+        break;
       case 'h':
         usage();
         return EXIT_SUCCESS;
@@ -130,7 +138,11 @@ int main(int argc, char **argv) {
     return EXIT_FAILURE;
   }
   const uint32_t W = (uint32_t)width;
-  if (W > 65536 || (W > 4096 && (W & (W - 1)) != 0)) {
+  if (any_width && W > 65536) {
+    fprintf(stderr, "-w (%d) is not served: widths up to 65536\n", width);
+    return EXIT_FAILURE;
+  }
+  if (!any_width && (W > 65536 || (W > 4096 && (W & (W - 1)) != 0))) {
     fprintf(stderr, "-w (%d) is not served: widths up to 4096, or powers of two up to 65536\n", width);
     return EXIT_FAILURE;
   }
@@ -238,7 +250,12 @@ int main(int argc, char **argv) {
   int64_t next_read = 0, submitted = 0; /* tickets whose rows were written / tickets submitted */
   int failed = 0;
   int code = xlg_create(0, fs, 2 * BLOCK_SAMPLES, 0, &g);
-  if (code == 0) code = xlg_add_spectrum(g, W, fs / W, fs % W, XLG_SPECTRUM_POWER, &sid);
+  if (code == 0 && any_width) {
+    const xlg_spectrum_desc desc = {W, fs / W, fs % W, XLG_SPECTRUM_POWER, 0, XLG_SPECTRUM_MAX, NULL};
+    code = xlg_add_spectrum_any(g, XLG_SOURCE_BAND, 0, &desc, &sid);
+  } else if (code == 0) {
+    code = xlg_add_spectrum(g, W, fs / W, fs % W, XLG_SPECTRUM_POWER, &sid);
+  }
   if (code != 0) {
     fprintf(stderr, "unable to start the GPU spectrum: %d\n", code);
     failed = 1;

@@ -1,6 +1,7 @@
 """Spectrum rows (xlg_add_spectrum): the spectrum kernels alone, and what a spectrum adds to a step of clients.
 
     python tools/spectrum_bench.py [--blocks K] [--warmup W] [--rounds R] [--widths W,...] [--variants V,...]
+                                   [--no-step]
 
 1. Per width W and variant (one JSON line each, the variants alternated within every round): a 61.44 Msps cs16
    stream in blocks of 262144 bytes, as in bench.py, feeding one spectrum with the reference tool's parameters
@@ -8,11 +9,12 @@
    window, H = W, max) and "hann_mean" (a Hann window, H = W / 2, the mean: Welch's method at 50 % overlap, with
    F = 2 fs // W - 1 so that a row still spans about a second).  Reported: the spectrum span's time per block
    from a profiled run (CUDA events around the channel stages, the fold and the emit pass, xlg_spectrum_profile),
-   its kernel (direct, fft, or wide_fft above W = 4096) and counted work.
+   its kernel (direct, fft, wide_fft at powers of two above W = 4096, or czt: every other width above 4096, served
+   through xlg_add_spectrum_any) and counted work.
 2. bench.py's cfg2 workload (256 clients at 48 and 96 ksps on a 2.016 Msps cu8 stream, blocks of 262144 bytes,
    device inputs and outputs) without a spectrum, with a W = 1024 spectrum (F = 1968, S = 768) and with a
    W = 1024, H = 512 Hann mean spectrum (F = 3935, S = 768), alternated in every round: the step time per block
-   between device events (xlg_timer_start / _stop), profiling off.
+   between device events (xlg_timer_start / _stop), profiling off.  --no-step leaves this part out.
 
 The card's name, power limit and clocks are printed first, read in the same call.  Nothing is written to the tree.
 """
@@ -39,12 +41,13 @@ def hann(W):
 def add(g, fs, W, variant):
     """One spectrum of the band in the given variant, at the reference tool's row length."""
     F, S = pkg.spectrogram_params(fs, W)
+    any_width = W > 4096 and W & (W - 1) != 0  # the chirp-z stage
     if variant == "plain":
-        return g.add_spectrum(W, F, S), F, S
+        return g.add_spectrum(W, F, S, any_width=any_width), F, S
     if variant == "hann":
-        return g.add_spectrum(W, F, S, hop=W, window=hann(W)), F, S
+        return g.add_spectrum(W, F, S, hop=W, window=hann(W), any_width=any_width), F, S
     F = 2 * F - 1  # (F - 1) W / 2 + W + S = the plain row's F W + S
-    return g.add_spectrum(W, F, S, hop=W // 2, window=hann(W), mean=True), F, S
+    return g.add_spectrum(W, F, S, hop=W // 2, window=hann(W), mean=True, any_width=any_width), F, S
 
 
 def kernel_run(W, variant, blocks, warmup, data):
@@ -58,7 +61,7 @@ def kernel_run(W, variant, blocks, warmup, data):
         for i in range(blocks):
             g.wait(g.submit(FMT, data[i % len(data)]))
         p = g.spectrum_profile_read()
-        kernel = ("direct", "fft", "wide_fft")[g.spectrum_info(sid)[0]]
+        kernel = ("direct", "fft", "wide_fft", "czt")[g.spectrum_info(sid)[0]]
     finally:
         g.close()
     n = p["spectrum_launches"]
@@ -110,6 +113,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--widths", default="64,1000,1024,4096")
     ap.add_argument("--variants", default="plain,hann,hann_mean")
+    ap.add_argument("--no-step", action="store_true")
     args = ap.parse_args()
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm",
                            "--format=csv,noheader"], capture_output=True, text=True).stdout.strip().splitlines()[0]
@@ -122,7 +126,7 @@ def main():
         for W in [int(w) for w in args.widths.split(",")]:
             for v in variants:
                 print(json.dumps({**kernel_run(W, v, args.blocks, args.warmup, data), "round": r}), flush=True)
-    for r in range(args.rounds):
+    for r in range(0 if args.no_step else args.rounds):
         for spectrum in ["none"] + [v for v in variants if v != "hann"]:
             print(json.dumps({**step_run(torch, spectrum, 10 * args.blocks, args.warmup), "round": r}), flush=True)
 
