@@ -155,10 +155,20 @@ struct BankHost {
   int taps_off = 0, tw_off = 0, ch_off = 0;
 };
 
+// which channel stages serve a spectrum; also its segment of the per-block tables, in this order:
+// [plain | extended | wide | chirp-z]
+enum SpecKind {
+  SPEC_PLAIN,  // hop W, no window, the max, W <= 4096: spectrum_fft_kernel or spectrum_direct_kernel
+  SPEC_EXT,    // a hop other than W, a window or the mean, W <= 4096: their _ext twins
+  SPEC_WIDE,   // W a power of two above 4096: the two wide passes, plain or extended
+  SPEC_CZT,    // every other W above 4096 (xlg_add_spectrum_any): the chirp-z passes, plain or extended
+};
+
 // a spectrum (xlg_add_spectrum, xlg_add_client_spectrum, xlg_add_subband_spectrum): its device tables and hold
 // rows, and its walk from P in 64-bit stream positions -- the band's, or its source's own, counted from the attach
 struct SpectrumHost {
   bool active = false;
+  SpecKind kind = SPEC_PLAIN;
   bool power = false;        // XLG_SPECTRUM_POWER
   int W = 0, F = 0, S = 0, R = 0;
   long long P = 0;
@@ -174,22 +184,21 @@ struct SpectrumHost {
   int *d_map = nullptr;
   unsigned *d_hold = nullptr;
   int out_off = 0;           // its rows in the slot's arena, in complex samples
-  // xlg_add_spectrum_ex: served by the extended kernels when it has a hop other than W, a window or the mean
-  bool ext = false, mean = false;
+  // xlg_add_spectrum_ex
+  bool mean = false;
   int H = 0;                 // hop (W for today's spectra)
   float *d_win = nullptr;    // W weights, or none
   float *d_fbuf = nullptr;   // mean: fb_frames rows of W, the powers of the frames a block completes
   int fb_frames = 0;         // the most frames a block completes (kept for a mean or a wide spectrum)
-  // W above SPEC_MAX_W: served by the two wide passes, plain or extended (ext stays false); d_tw holds the W-point
-  // table, then the C-point one
-  bool wide = false;
+  // SPEC_WIDE: d_tw holds the W-point table, then the C-point one
   float2 *d_scratch = nullptr;  // fb_frames rows of W: pass A's output
-  // xlg_add_spectrum_any above 4096 and not a power of two: the chirp-z passes at M = next_pow2(2W - 1), plain or
-  // extended (ext stays false); d_tw holds the M-point table, the C-point one, the chirp (W) and Bh (M), d_map the
-  // half swap alone (the hold is in natural bin order), d_scratch two sets of fb_frames rows of M
-  bool czt = false;
+  // SPEC_CZT, at M = next_pow2(2W - 1): d_tw holds the M-point table, the C-point one, the chirp (W) and Bh (M),
+  // d_map the half swap alone (the hold is in natural bin order), d_scratch two sets of fb_frames rows of M
   int M = 0;
   int *d_bin = nullptr;  // the bin of each of the M positions
+
+  // every device buffer it holds (null where it has none)
+  std::array<void *, 8> buffers() const { return {d_tw, d_map, d_hold, d_ring, d_win, d_fbuf, d_scratch, d_bin}; }
 };
 
 // members of one sub-band that read the same windows: equal (L2, D2, T2, hist2) and, until their windows have
@@ -1035,9 +1044,9 @@ static int rebuild_spectra(xlg_group *g, size_t &out_total, size_t &max_hist) {
   size_t n = 0, n_src = 0, n_ext = 0, n_wide = 0, n_czt = 0;
   for (SpectrumHost &p : g->spectra) {
     if (!p.active) continue;
-    n_ext += p.ext || p.wide || p.czt ? 1 : 0;
-    n_wide += p.wide ? 1 : 0;
-    n_czt += p.czt ? 1 : 0;
+    n_ext += p.kind != SPEC_PLAIN ? 1 : 0;
+    n_wide += p.kind == SPEC_WIDE ? 1 : 0;
+    n_czt += p.kind == SPEC_CZT ? 1 : 0;
     p.out_off = (int)out_total;
     out_total += ((size_t)p.rows_cap * p.W + 1) / 2;
     out_total = (out_total + 3) & ~(size_t)3;
@@ -2017,8 +2026,7 @@ extern "C" void xlg_destroy(xlg_group *g) {
     if (h.b2.ring.p) cudaFree(h.b2.ring.p);
   for (float2 *p : g->dead_rings) cudaFree(p);
   for (const SpectrumHost &p : g->spectra)
-    for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold, (void *)p.d_ring, (void *)p.d_win,
-                     (void *)p.d_fbuf, (void *)p.d_scratch, (void *)p.d_bin})
+    for (void *d : p.buffers())
       if (d) cudaFree(d);
   for (void *p : g->dead_spec) cudaFree(p);
   for (cudaEvent_t e : g->ev_user) cudaEventDestroy(e);
@@ -2661,10 +2669,10 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
   p.R = (int)R;
   p.H = (int)hop;
   p.mean = reduce == XLG_SPECTRUM_MEAN;
-  p.wide = spec_wide(p.W);
-  p.czt = p.W > SPEC_MAX_W && !p.wide;  // (only through xlg_add_spectrum_any)
-  p.M = p.czt ? czt_m(p.W) : 0;
-  p.ext = !p.wide && !p.czt && (p.H != p.W || window != nullptr || p.mean);
+  p.kind = spec_wide(p.W) ? SPEC_WIDE : p.W > SPEC_MAX_W ? SPEC_CZT  // (SPEC_CZT only through xlg_add_spectrum_any)
+           : p.H != p.W || window != nullptr || p.mean ? SPEC_EXT : SPEC_PLAIN;
+  const bool wide = p.kind == SPEC_WIDE, czt = p.kind == SPEC_CZT;
+  p.M = czt ? czt_m(p.W) : 0;
   p.src = src;
   // a source's positions count from here: P = 0 in its own stream
   const uint64_t cap = src < 0 ? (uint64_t)g->max_input_len / 2 : (uint64_t)source_cap(g, g->clients[src]);
@@ -2674,7 +2682,7 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
   // the frames a block of at most cap samples completes: their last samples are distinct positions of the block,
   // one frame's at least min(H, W + S) after the previous one's (H within a row, W + S from a row's last frame to
   // the next row's first)
-  if (p.mean || p.wide || p.czt) p.fb_frames = (int)((cap - 1) / std::min<uint64_t>(hop, (uint64_t)width + skip_per_row) + 1);
+  if (p.mean || wide || czt) p.fb_frames = (int)((cap - 1) / std::min<uint64_t>(hop, (uint64_t)width + skip_per_row) + 1);
   // a source's ring holds every sample of the frames a block completes: the block's own and W - 1 before them
   const size_t ring_cap = src < 0 ? 0 : next_pow2((size_t)width - 1 + (size_t)cap);
   p.ring_mask = (unsigned)(ring_cap - 1);
@@ -2683,15 +2691,15 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
   for (int j = 0; j < W; j++) {
     // spectrogram.c:156-163: the halves swapped, an odd width's last bin in place
     const int bin = j < half ? half + j : j < 2 * half ? j - half : W - 1;
-    map[j] = spec_fft(W) || p.wide ? bank_fft_pos(bin, W) : bin;
+    map[j] = spec_fft(W) || wide ? bank_fft_pos(bin, W) : bin;
   }
-  std::vector<float2> tw = twiddle_table(p.czt ? p.M : W);
+  std::vector<float2> tw = twiddle_table(czt ? p.M : W);
   std::vector<int> czbin;
-  if (p.wide || p.czt) {  // pass B's table after the W- or M-point one
-    const std::vector<float2> tc = twiddle_table(spec_wide_chunk(p.czt ? p.M : W));
+  if (wide || czt) {  // pass B's table after the W- or M-point one
+    const std::vector<float2> tc = twiddle_table(spec_wide_chunk(czt ? p.M : W));
     tw.insert(tw.end(), tc.begin(), tc.end());
   }
-  if (p.czt) {  // then the chirp and Bh
+  if (czt) {  // then the chirp and Bh
     std::vector<float2> chirp, kern;
     czt_tables(W, chirp, kern, czbin);
     tw.insert(tw.end(), chirp.begin(), chirp.end());
@@ -2703,11 +2711,10 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
       (ring_cap > 0 && cudaMalloc(&p.d_ring, ring_cap * sizeof(float2)) != cudaSuccess) ||
       (window != nullptr && cudaMalloc(&p.d_win, W * sizeof(float)) != cudaSuccess) ||
       (p.mean && cudaMalloc(&p.d_fbuf, (size_t)p.fb_frames * W * sizeof(float)) != cudaSuccess) ||
-      (p.wide && cudaMalloc(&p.d_scratch, (size_t)p.fb_frames * W * sizeof(float2)) != cudaSuccess) ||
-      (p.czt && cudaMalloc(&p.d_scratch, 2 * (size_t)p.fb_frames * p.M * sizeof(float2)) != cudaSuccess) ||
-      (p.czt && cudaMalloc(&p.d_bin, (size_t)p.M * sizeof(int)) != cudaSuccess)) {
-    for (void *d : {(void *)p.d_tw, (void *)p.d_map, (void *)p.d_hold, (void *)p.d_ring, (void *)p.d_win,
-                     (void *)p.d_fbuf, (void *)p.d_scratch, (void *)p.d_bin})
+      (wide && cudaMalloc(&p.d_scratch, (size_t)p.fb_frames * W * sizeof(float2)) != cudaSuccess) ||
+      (czt && cudaMalloc(&p.d_scratch, 2 * (size_t)p.fb_frames * p.M * sizeof(float2)) != cudaSuccess) ||
+      (czt && cudaMalloc(&p.d_bin, (size_t)p.M * sizeof(int)) != cudaSuccess)) {
+    for (void *d : p.buffers())
       if (d) cudaFree(d);
     XL_LOG("spectrum: out of device memory");
     return -ENOMEM;
@@ -2715,7 +2722,7 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
   CU_OK(cudaMemcpy(p.d_tw, tw.data(), tw.size() * sizeof(float2), cudaMemcpyHostToDevice));
   CU_OK(cudaMemcpy(p.d_map, map.data(), W * sizeof(int), cudaMemcpyHostToDevice));
   if (window != nullptr) CU_OK(cudaMemcpy(p.d_win, window, W * sizeof(float), cudaMemcpyHostToDevice));
-  if (p.czt) CU_OK(cudaMemcpy(p.d_bin, czbin.data(), (size_t)p.M * sizeof(int), cudaMemcpyHostToDevice));
+  if (czt) CU_OK(cudaMemcpy(p.d_bin, czbin.data(), (size_t)p.M * sizeof(int), cudaMemcpyHostToDevice));
   // (on a group stream, finished before the spectrum exists: the kernels' streams do not wait for the legacy one)
   CU_OK(cudaMemsetAsync(p.d_hold, 0, hold_bytes, g->s_in));
   CU_OK(cudaStreamSynchronize(g->s_in));
@@ -2726,37 +2733,6 @@ static int add_spectrum(xlg_group *g, int src, uint32_t width, uint32_t frames_p
   g->dirty = true;  // its rows in the arenas, the input ring's history bound
   *spectrum_id = id;
   return 0;
-}
-
-extern "C" int xlg_add_spectrum(xlg_group *g, uint32_t width, uint32_t frames_per_row, uint32_t skip_per_row,
-                                uint32_t flags, int *spectrum_id) {
-  if (g == nullptr || spectrum_id == nullptr) return -EINVAL;
-  return add_spectrum(g, -1, width, frames_per_row, skip_per_row, flags, width, XLG_SPECTRUM_MAX, nullptr,
-                      false, spectrum_id);
-}
-
-extern "C" int xlg_add_client_spectrum(xlg_group *g, int client_id, uint32_t width, uint32_t frames_per_row,
-                                       uint32_t skip_per_row, uint32_t flags, int *spectrum_id) {
-  if (g == nullptr || spectrum_id == nullptr) return -EINVAL;
-  if (client_id < 0 || client_id >= (int)g->clients.size() || !g->clients[client_id].active ||
-      g->clients[client_id].sb) {
-    XL_LOG("client spectrum: client %d does not exist", client_id);
-    return -EINVAL;
-  }
-  return add_spectrum(g, client_id, width, frames_per_row, skip_per_row, flags, width, XLG_SPECTRUM_MAX, nullptr,
-                      false, spectrum_id);
-}
-
-extern "C" int xlg_add_subband_spectrum(xlg_group *g, int subband_id, uint32_t width, uint32_t frames_per_row,
-                                        uint32_t skip_per_row, uint32_t flags, int *spectrum_id) {
-  if (g == nullptr || spectrum_id == nullptr) return -EINVAL;
-  const int cid = subband_client(g, subband_id);
-  if (cid < 0) {
-    XL_LOG("sub-band spectrum: sub-band %d does not exist", subband_id);
-    return -EINVAL;
-  }
-  return add_spectrum(g, cid, width, frames_per_row, skip_per_row, flags, width, XLG_SPECTRUM_MAX, nullptr,
-                      false, spectrum_id);
 }
 
 // xlg_add_spectrum_ex, and with any = true xlg_add_spectrum_any
@@ -2789,6 +2765,24 @@ static int add_spectrum_desc(xlg_group *g, int source, int source_id, const xlg_
                       desc->reduce, desc->window, any, spectrum_id);
 }
 
+extern "C" int xlg_add_spectrum(xlg_group *g, uint32_t width, uint32_t frames_per_row, uint32_t skip_per_row,
+                                uint32_t flags, int *spectrum_id) {
+  const xlg_spectrum_desc desc = {width, frames_per_row, skip_per_row, flags, 0, XLG_SPECTRUM_MAX, nullptr};
+  return add_spectrum_desc(g, XLG_SOURCE_BAND, 0, &desc, false, spectrum_id);
+}
+
+extern "C" int xlg_add_client_spectrum(xlg_group *g, int client_id, uint32_t width, uint32_t frames_per_row,
+                                       uint32_t skip_per_row, uint32_t flags, int *spectrum_id) {
+  const xlg_spectrum_desc desc = {width, frames_per_row, skip_per_row, flags, 0, XLG_SPECTRUM_MAX, nullptr};
+  return add_spectrum_desc(g, XLG_SOURCE_CLIENT, client_id, &desc, false, spectrum_id);
+}
+
+extern "C" int xlg_add_subband_spectrum(xlg_group *g, int subband_id, uint32_t width, uint32_t frames_per_row,
+                                        uint32_t skip_per_row, uint32_t flags, int *spectrum_id) {
+  const xlg_spectrum_desc desc = {width, frames_per_row, skip_per_row, flags, 0, XLG_SPECTRUM_MAX, nullptr};
+  return add_spectrum_desc(g, XLG_SOURCE_SUBBAND, subband_id, &desc, false, spectrum_id);
+}
+
 extern "C" int xlg_add_spectrum_ex(xlg_group *g, int source, int source_id, const xlg_spectrum_desc *desc,
                                    int *spectrum_id) {
   return add_spectrum_desc(g, source, source_id, desc, false, spectrum_id);
@@ -2812,8 +2806,7 @@ extern "C" int xlg_remove_spectrum(xlg_group *g, int spectrum_id) {
     return -EINVAL;
   }
   // in-flight tickets still read the tables and the hold: freed at the next re-layout, which drains
-  for (void *d : {(void *)p->d_tw, (void *)p->d_map, (void *)p->d_hold, (void *)p->d_ring, (void *)p->d_win,
-                   (void *)p->d_fbuf, (void *)p->d_scratch, (void *)p->d_bin})
+  for (void *d : p->buffers())
     if (d) g->dead_spec.push_back(d);
   *p = SpectrumHost();
   g->dirty = true;
@@ -2824,7 +2817,7 @@ extern "C" int xlg_spectrum_info(const xlg_group *g, int spectrum_id, int *kerne
   if (g == nullptr) return -EINVAL;
   const SpectrumHost *p = spectrum_of(const_cast<xlg_group *>(g), spectrum_id);
   if (p == nullptr) return -EINVAL;
-  if (kernel) *kernel = p->czt ? 3 : p->wide ? 2 : spec_fft(p->W) ? 1 : 0;
+  if (kernel) *kernel = p->kind == SPEC_CZT ? 3 : p->kind == SPEC_WIDE ? 2 : spec_fft(p->W) ? 1 : 0;
   if (rows_done) *rows_done = p->rows_done;
   return 0;
 }
@@ -2843,6 +2836,18 @@ static void launch_convert(bool q15, const void *raw, xlg_group *g, long long S,
     convert_cf32_kernel<FMT><<<blocks, threads, 0, st>>>(raw, g->ring, mask, S, n);
   }
 }
+
+// One spectrum channel-stage launch, grown over the entries it serves: CTAs along x (0: no launch), along y, and
+// dynamic shared memory
+struct SpecLaunch {
+  int ctas = 0, groups = 0;
+  size_t smem = 0;
+  void grow(int c, int gr = 1, size_t sm = 0) {
+    ctas = std::max(ctas, c);
+    groups = std::max(groups, gr);
+    smem = std::max(smem, sm);
+  }
+};
 
 // One block being submitted: where it goes, and what the walks over its clients, banks and sub-bands found (the
 // sizes of each kernel family's launch)
@@ -2867,17 +2872,15 @@ struct Block {
   size_t bk_smem = 0;
   int n_bf = 0, max_bf_ctas = 0;  // FFT banks
   size_t bf_smem = 0;
-  // spectrum walk: entries, CTAs of the FFT and direct paths, row values to emit, the end of their rows in the arena
-  int n_spec = 0, max_spf_ctas = 0, max_spd_ctas = 0, max_spd_groups = 0, max_sp_values = 0;
-  size_t spf_smem = 0, spd_smem = 0, sp_used = 0;
-  // the extended spectra, the last n_spx entries: their channel stages' CTAs and the values the fold passes over
-  int n_spx = 0, max_spxf_ctas = 0, max_spxd_ctas = 0, max_spxd_groups = 0, max_fold_values = 0;
-  size_t spxf_smem = 0, spxd_smem = 0;
-  // the wide spectra, after the extended ones: CTAs of their two passes (the fold also covers them)
-  int n_spw = 0, max_spwa_ctas = 0, max_spwb_ctas = 0;
-  // the chirp-z spectra, after the wide ones: CTAs of their pass-A and pass-B launches, pass B's shared memory
-  int n_spc = 0, max_spca_ctas = 0, max_spcb_ctas = 0;
-  size_t spcb_smem = 0;
+  // spectrum walk: entries, row values to emit, the end of their rows in the arena; the plain entries' FFT and
+  // direct paths
+  int n_spec = 0, max_sp_values = 0;
+  size_t sp_used = 0;
+  SpecLaunch spf, spd;
+  // the extended spectra, then the wide, then the chirp-z ones, the last entries: their counts, the values the fold
+  // passes over, the extended FFT and direct paths, the wide passes A and B, the chirp-z passes A (and C), B (and D)
+  int n_spx = 0, n_spw = 0, n_spc = 0, max_fold_values = 0;
+  SpecLaunch spxf, spxd, spwa, spwb, spca, spcb;
   int n_spa = 0, max_spa_n = 0;  // appends to spectrum sources' rings, the longest
   // sub-band walk
   int n_sb = 0, max_sb_n1 = 0, max_sb_n2 = 0;
@@ -3013,7 +3016,7 @@ static void walk_spectrum(Block &b, int id) {
   }
   const uint64_t d = (uint64_t)(E - p.P), F = (uint64_t)p.F;
   uint64_t total;
-  if (p.ext || p.wide || p.czt) {  // frames completed at offset o of a row: none before W, then one more every H, at most F
+  if (p.kind != SPEC_PLAIN) {  // frames completed at offset o of a row: none before W, then one more every H, at most F
     const uint64_t o = d % (uint64_t)p.R;
     total = d / (uint64_t)p.R * F + (o < (uint64_t)p.W ? 0 : std::min<uint64_t>(F, (o - p.W) / (uint64_t)p.H + 1));
   } else {
@@ -3043,11 +3046,12 @@ static void walk_spectrum(Block &b, int id) {
     e.power = p.power ? 1 : 0;
     e.inv_w = 1.0f / (float)p.W;
     // a chirp-z frame: two M-point transforms, the chirp's W products and Bh's M (4 instructions each)
-    const uint64_t flops = p.czt ? 2 * xlg_bank_fft_flops((uint32_t)p.M) + 4ull * p.W + 4ull * p.M
-                           : spec_fft(p.W) || p.wide ? xlg_bank_fft_flops((uint32_t)p.W) : 4ull * p.W * p.W;
+    const uint64_t flops = p.kind == SPEC_CZT ? 2 * xlg_bank_fft_flops((uint32_t)p.M) + 4ull * p.W + 4ull * p.M
+                           : spec_fft(p.W) || p.kind == SPEC_WIDE ? xlg_bank_fft_flops((uint32_t)p.W)
+                                                                  : 4ull * p.W * p.W;
     s.sp_frames += (uint64_t)n_frames;
     s.sp_flops += (uint64_t)n_frames * (flops + 6ull * p.W + (p.d_win ? 2ull * p.W : 0) + (p.mean ? p.W : 0));
-    if (p.ext || p.wide || p.czt) {
+    if (p.kind != SPEC_PLAIN) {
       SpecExt &x = s.spext.h[b.n_spx + b.n_spw + b.n_spc];
       x.win = p.d_win;
       x.fbuf = p.d_fbuf;
@@ -3056,7 +3060,7 @@ static void walk_spectrum(Block &b, int id) {
     }
     if (p.mean)  // values of the rows its frames touch
       b.max_fold_values = std::max(b.max_fold_values, (int)(((long long)p.fir + n_frames - 1) / p.F + 1) * p.W);
-    if (p.czt) {
+    if (p.kind == SPEC_CZT) {
       SpecCzt &c = s.spczt.h[b.n_spc++];
       const int C = spec_wide_chunk(p.M);
       const size_t rows = (size_t)p.fb_frames * p.M;
@@ -3067,34 +3071,23 @@ static void walk_spectrum(Block &b, int id) {
       c.kern = c.chirp + p.W;
       c.bin = p.d_bin;
       c.M = p.M;
-      b.max_spca_ctas = std::max(b.max_spca_ctas, n_frames * (C / SPEC_THREADS));
-      b.max_spcb_ctas = std::max(b.max_spcb_ctas, n_frames * (p.M / C));
-      b.spcb_smem = std::max(b.spcb_smem, (size_t)C * sizeof(float2));
-    } else if (p.wide) {
+      b.spca.grow(n_frames * (C / SPEC_THREADS));
+      b.spcb.grow(n_frames * (p.M / C), 1, (size_t)C * sizeof(float2));
+    } else if (p.kind == SPEC_WIDE) {
       SpecWide &w = s.spwide.h[b.n_spw++];
       w.scratch = p.d_scratch;
       w.tw_c = p.d_tw + p.W;
       const int C = spec_wide_chunk(p.W);
-      b.max_spwa_ctas = std::max(b.max_spwa_ctas, n_frames * (C / SPEC_THREADS));
-      b.max_spwb_ctas = std::max(b.max_spwb_ctas, n_frames * (p.W / C));
-    } else if (p.ext) {
-      b.n_spx++;
-      if (spec_fft(p.W)) {
-        b.max_spxf_ctas = std::max(b.max_spxf_ctas, (n_frames + bank_fft_frames(p.W) - 1) / bank_fft_frames(p.W));
-        b.spxf_smem = std::max(b.spxf_smem, bank_fft_smem(p.W));
-      } else {
-        b.max_spxd_ctas =
-            std::max(b.max_spxd_ctas, (n_frames + spec_direct_frames(p.W) - 1) / spec_direct_frames(p.W));
-        b.max_spxd_groups = std::max(b.max_spxd_groups, spec_direct_groups(p.W));
-        b.spxd_smem = std::max(b.spxd_smem, spec_direct_smem(p.W));
-      }
-    } else if (spec_fft(p.W)) {
-      b.max_spf_ctas = std::max(b.max_spf_ctas, (n_frames + bank_fft_frames(p.W) - 1) / bank_fft_frames(p.W));
-      b.spf_smem = std::max(b.spf_smem, bank_fft_smem(p.W));
-    } else {
-      b.max_spd_ctas = std::max(b.max_spd_ctas, (n_frames + spec_direct_frames(p.W) - 1) / spec_direct_frames(p.W));
-      b.max_spd_groups = std::max(b.max_spd_groups, spec_direct_groups(p.W));
-      b.spd_smem = std::max(b.spd_smem, spec_direct_smem(p.W));
+      b.spwa.grow(n_frames * (C / SPEC_THREADS));
+      b.spwb.grow(n_frames * (p.W / C));
+    } else {  // the FFT or the direct path, in the plain or the extended kernels
+      const bool x = p.kind == SPEC_EXT;
+      b.n_spx += x ? 1 : 0;
+      const int Ff = bank_fft_frames(p.W), Fd = spec_direct_frames(p.W);
+      if (spec_fft(p.W))
+        (x ? b.spxf : b.spf).grow((n_frames + Ff - 1) / Ff, 1, bank_fft_smem(p.W));
+      else
+        (x ? b.spxd : b.spd).grow((n_frames + Fd - 1) / Fd, spec_direct_groups(p.W), spec_direct_smem(p.W));
     }
     b.max_sp_values = std::max(b.max_sp_values, n_rows * p.W);
     b.sp_used = std::max(b.sp_used, (size_t)p.out_off + ((size_t)n_rows * p.W + 1) / 2);
@@ -3103,7 +3096,7 @@ static void walk_spectrum(Block &b, int id) {
   p.fir = (int)(total % F);
 }
 
-// every spectrum, today's first: the table is [plain entries | extended entries | wide entries | chirp-z entries]
+// every spectrum, by kind: the table is [plain entries | extended entries | wide entries | chirp-z entries]
 static void walk_spectra(Block &b) {
   xlg_group *g = b.g;
   b.s.sp_frames = b.s.sp_flops = 0;
@@ -3111,7 +3104,7 @@ static void walk_spectra(Block &b) {
     for (int id = 0; id < (int)g->spectra.size(); id++) {
       const SpectrumHost &p = g->spectra[id];
       if (seg == 0) b.ho.sp_w[id] = p.active ? p.W : 0;
-      if (p.active && (p.czt ? 3 : p.wide ? 2 : p.ext ? 1 : 0) == seg) walk_spectrum(b, id);
+      if (p.active && p.kind == seg) walk_spectrum(b, id);
     }
 }
 
@@ -3273,36 +3266,36 @@ static int launch_spectra(Block &b) {
     CU_OK(s.spring.upload((size_t)b.n_spec, b.cs));
   }
   const int n_plain = b.n_spec - b.n_spx - b.n_spw - b.n_spc;
-  if (b.max_spf_ctas > 0)
-    spectrum_fft_kernel<<<dim3(b.max_spf_ctas, n_plain), SPEC_THREADS, b.spf_smem, b.cs>>>(s.spblk.d, s.spring.d);
-  if (b.max_spd_ctas > 0)
-    spectrum_direct_kernel<<<dim3(b.max_spd_ctas, b.max_spd_groups, n_plain), SPEC_THREADS, b.spd_smem, b.cs>>>(
+  if (b.spf.ctas > 0)
+    spectrum_fft_kernel<<<dim3(b.spf.ctas, n_plain), SPEC_THREADS, b.spf.smem, b.cs>>>(s.spblk.d, s.spring.d);
+  if (b.spd.ctas > 0)
+    spectrum_direct_kernel<<<dim3(b.spd.ctas, b.spd.groups, n_plain), SPEC_THREADS, b.spd.smem, b.cs>>>(
         s.spblk.d, s.spring.d);
   if (b.n_spx + b.n_spw + b.n_spc > 0) {
     const SpecBlk *xb = s.spblk.d + n_plain;
     const float2 *const *xr = s.spring.d + n_plain;
     CU_OK(s.spext.upload((size_t)(b.n_spx + b.n_spw + b.n_spc), b.cs));
-    if (b.max_spxf_ctas > 0)
-      spectrum_fft_ext_kernel<<<dim3(b.max_spxf_ctas, b.n_spx), SPEC_THREADS, b.spxf_smem, b.cs>>>(xb, xr, s.spext.d);
-    if (b.max_spxd_ctas > 0)
-      spectrum_direct_ext_kernel<<<dim3(b.max_spxd_ctas, b.max_spxd_groups, b.n_spx), SPEC_THREADS, b.spxd_smem,
-                                   b.cs>>>(xb, xr, s.spext.d);
+    if (b.spxf.ctas > 0)
+      spectrum_fft_ext_kernel<<<dim3(b.spxf.ctas, b.n_spx), SPEC_THREADS, b.spxf.smem, b.cs>>>(xb, xr, s.spext.d);
+    if (b.spxd.ctas > 0)
+      spectrum_direct_ext_kernel<<<dim3(b.spxd.ctas, b.spxd.groups, b.n_spx), SPEC_THREADS, b.spxd.smem, b.cs>>>(
+          xb, xr, s.spext.d);
     if (b.n_spw > 0) {  // the wide entries: pass A into their scratch, then pass B into the hold or frame buffer
       CU_OK(s.spwide.upload((size_t)b.n_spw, b.cs));
-      spectrum_wide_a_kernel<<<dim3(b.max_spwa_ctas, b.n_spw), SPEC_THREADS, 0, b.cs>>>(
+      spectrum_wide_a_kernel<<<dim3(b.spwa.ctas, b.n_spw), SPEC_THREADS, 0, b.cs>>>(
           xb + b.n_spx, xr + b.n_spx, s.spext.d + b.n_spx, s.spwide.d);
-      spectrum_wide_b_kernel<<<dim3(b.max_spwb_ctas, b.n_spw), SPEC_THREADS, SPEC_WIDE_SMEM, b.cs>>>(
+      spectrum_wide_b_kernel<<<dim3(b.spwb.ctas, b.n_spw), SPEC_THREADS, SPEC_WIDE_SMEM, b.cs>>>(
           xb + b.n_spx, s.spext.d + b.n_spx, s.spwide.d);
     }
     if (b.n_spc > 0) {  // the chirp-z entries: the forward transform and Bh into s2, the second transform
       const int o = b.n_spx + b.n_spw;
       CU_OK(s.spczt.upload((size_t)b.n_spc, b.cs));
-      spectrum_czt_a_kernel<<<dim3(b.max_spca_ctas, b.n_spc), SPEC_THREADS, 0, b.cs>>>(xb + o, xr + o,
-                                                                                     s.spext.d + o, s.spczt.d);
-      spectrum_czt_b_kernel<<<dim3(b.max_spcb_ctas, b.n_spc), SPEC_THREADS, b.spcb_smem, b.cs>>>(xb + o, s.spczt.d);
-      spectrum_czt_c_kernel<<<dim3(b.max_spca_ctas, b.n_spc), SPEC_THREADS, 0, b.cs>>>(xb + o, s.spczt.d);
-      spectrum_czt_d_kernel<<<dim3(b.max_spcb_ctas, b.n_spc), SPEC_THREADS, b.spcb_smem, b.cs>>>(xb + o, s.spext.d + o,
-                                                                                                s.spczt.d);
+      spectrum_czt_a_kernel<<<dim3(b.spca.ctas, b.n_spc), SPEC_THREADS, 0, b.cs>>>(xb + o, xr + o, s.spext.d + o,
+                                                                                 s.spczt.d);
+      spectrum_czt_b_kernel<<<dim3(b.spcb.ctas, b.n_spc), SPEC_THREADS, b.spcb.smem, b.cs>>>(xb + o, s.spczt.d);
+      spectrum_czt_c_kernel<<<dim3(b.spca.ctas, b.n_spc), SPEC_THREADS, 0, b.cs>>>(xb + o, s.spczt.d);
+      spectrum_czt_d_kernel<<<dim3(b.spcb.ctas, b.n_spc), SPEC_THREADS, b.spcb.smem, b.cs>>>(xb + o, s.spext.d + o,
+                                                                                            s.spczt.d);
     }
     if (b.max_fold_values > 0)
       spectrum_fold_kernel<<<dim3((b.max_fold_values + SPEC_THREADS - 1) / SPEC_THREADS,

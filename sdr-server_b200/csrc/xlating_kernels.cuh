@@ -1802,7 +1802,9 @@ bank_fft_cf32_kernel(const BankBlk *__restrict__ blk, const float2 *__restrict__
 // The hold has NR rows used round-robin by row number (NR exceeds the rows a block touches); the emit pass reads
 // each row the block completed through the row map (out[j] = hold[map[j]]: the reference's half swap, then the
 // FFT path's digit reversal), writes v (XLG_SPECTRUM_POWER) or 10 * log10f(v), and zeroes what it read.
-// Powers of two from 8192 to 65536 are the wide spectra at the end of this file: the FFT path's X at K = W.
+// The two channel stages (spectrum_fft_kernel, spectrum_direct_kernel) share their bodies with the extended
+// spectra's, after SpecExt below.  Powers of two from 8192 to 65536 are the wide spectra at the end of this file:
+// the FFT path's X at K = W.
 // ---------------------------------------------------------------------------
 constexpr int SPEC_THREADS = 256;
 constexpr int SPEC_MAX_W = 4096;
@@ -1848,12 +1850,65 @@ __device__ __forceinline__ unsigned spec_power(float2 X, float inv) {
   return __float_as_uint(__fadd_rn(__fadd_rn(__fmul_rn(cx, cx), __fmul_rn(cy, cy)), 1e-20f));
 }
 
-// CTA (x, s) transforms frames [x F, x F + F) of spectrum s, F = bank_fft_frames(W), one row of W each in shared
-// memory, and folds their powers into the hold (below W = 256 a CTA first takes the max over runs of its frames)
-__global__ void __launch_bounds__(SPEC_THREADS)
-spectrum_fft_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__restrict__ rings) {
+// CTA (x, s) writes values [x 256, x 256 + 256) of the n_rows x W values of the rows spectrum s completed in
+// this block, and empties what it read of the hold
+__global__ void __launch_bounds__(SPEC_THREADS) spectrum_emit_kernel(const SpecBlk *__restrict__ blk) {
+  const SpecBlk b = blk[blockIdx.y];
+  const int e = blockIdx.x * SPEC_THREADS + threadIdx.x;
+  if (e >= b.n_rows * b.W) return;
+  const int i = e / b.W, j = e - i * b.W;
+  unsigned *hold = b.hold + (size_t)((b.slot0 + i) % b.NR) * b.W + b.map[j];
+  const float v = __uint_as_float(*hold);
+  *hold = 0u;
+  b.out[e] = b.power ? v : __fmul_rn(10.f, log10f(v));
+}
+
+// ---------------------------------------------------------------------------
+// Extended spectra (xlg_add_spectrum_ex): a hop H between frame starts, a window and a mean.  Row period
+// R = (F - 1) H + W + S; row r covers the frames x[P + r R + f H ... + W), f < F.  Each frame is windowed before
+// the transform, z[n] = (x[n].x * w[n], x[n].y * w[n]) (one rounded multiply each; no window: z = x), and goes
+// through the same channel stage, spec_power and hold as above: spectrum_fft_ext_kernel and
+// spectrum_direct_ext_kernel are the EXT = true instances of the two stages' bodies below, the plain kernels the
+// EXT = false ones.  A max spectrum folds by atomicMax as above.  A
+// mean spectrum's channel stage stores each frame's powers (position space, as the hold) in the spectrum's frame
+// buffer, row j of it for frame j of this block; spectrum_fold_kernel then adds them into the hold in frame order,
+//     s = +0;  s = s + p_f for f = 0 .. F - 1 (rounded adds, one frame after the other, across blocks in block order)
+// and divides a completed row once, v = s / float(F) (correctly rounded).  The hold carries s between blocks as
+// float bits (the empty hold, 0, is +0).  spectrum_emit_kernel then writes and empties the row as for any spectrum.
+// The entries are the tail of the block's SpecBlk table, SpecExt holds what only they need (the plain kernels read
+// none).
+// ---------------------------------------------------------------------------
+struct SpecExt {
+  const float *win;  // W weights, or nullptr: no window
+  float *fbuf;       // mean: the frames' powers, a row of W per frame of this block; max: nullptr
+  int H;             // hop
+  int mean;
+};
+
+__device__ __forceinline__ long long spec_frame_pos(const SpecBlk &b, int H, int j) {
+  const unsigned g = b.f0 + (unsigned)j, rr = g / (unsigned)b.F, ff = g - rr * (unsigned)b.F;
+  return b.base + (long long)rr * b.R + (long long)ff * H;
+}
+
+__device__ __forceinline__ float2 spec_load(const float2 *__restrict__ ring, unsigned mask, long long pos,
+                                            const float *__restrict__ win, int n) {
+  const float2 v = ring[(unsigned)((unsigned long long)pos) & mask];
+  if (win == nullptr) return v;
+  const float w = __ldg(win + n);
+  return make_float2(__fmul_rn(v.x, w), __fmul_rn(v.y, w));
+}
+
+// The FFT path: CTA (x, s) transforms frames [x F, x F + F) of spectrum s, F = bank_fft_frames(W), one row of W
+// each in shared memory, and folds their powers into the hold (below W = 256 a CTA first takes the max over runs of
+// its frames) or, for a mean, stores them to the frame buffer.  EXT = false: a plain spectrum, hop W, no window
+// and the max, without reading a SpecExt.
+template <bool EXT>
+__device__ __forceinline__ void spectrum_fft_stage(const SpecBlk *__restrict__ blk,
+                                                   const float2 *const *__restrict__ rings,
+                                                   const SpecExt *__restrict__ ext) {
   extern __shared__ __align__(16) float2 u[];
   const SpecBlk b = blk[blockIdx.y];
+  const SpecExt x = EXT ? ext[blockIdx.y] : SpecExt{nullptr, nullptr, b.W, 0};
   const float2 *__restrict__ ring = rings[blockIdx.y];
   if (!spec_fft(b.W)) return;
   const int W = b.W, F = bank_fft_frames(W);
@@ -1861,11 +1916,16 @@ spectrum_fft_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__rest
   if (j0 >= b.n_frames) return;
   const int nf = min(F, b.n_frames - j0), tid = threadIdx.x, lw = 31 - __clz(W);
   for (int e = tid; e < nf * W; e += SPEC_THREADS) {
-    const long long pos = spec_frame(b, j0 + (e >> lw)).pos + (e & (W - 1));
-    u[e] = ring[(unsigned)((unsigned long long)pos) & b.mask];
+    const int n = e & (W - 1);
+    u[e] = spec_load(ring, b.mask, spec_frame_pos(b, x.H, j0 + (e >> lw)) + n, x.win, n);
   }
   __syncthreads();
   fft_dif_rows<SPEC_THREADS>(u, nf, W, lw, b.tw, tid);
+  if (EXT && x.mean) {
+    float *fb = x.fbuf + (size_t)j0 * W;
+    for (int e = tid; e < nf * W; e += SPEC_THREADS) fb[e] = __uint_as_float(spec_power(u[e], b.inv_w));
+    return;
+  }
   if (W >= SPEC_THREADS) {  // at most 8 frames: one atomicMax per power
     for (int e = tid; e < nf * W; e += SPEC_THREADS) {
       const int h = spec_frame(b, j0 + (e >> lw)).hold_row;
@@ -1896,12 +1956,16 @@ spectrum_fft_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__rest
   if (h >= 0) atomicMax(b.hold + (size_t)h * W + q, m);
 }
 
-// CTA (x, y, s) computes bins [y 256, y 256 + 256) of frames [x Fd, x Fd + Fd) of spectrum s,
-// Fd = spec_direct_frames(W): the frames and the table in shared memory, one bin of one frame per thread
-__global__ void __launch_bounds__(SPEC_THREADS)
-spectrum_direct_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__restrict__ rings) {
+// The direct path: CTA (x, y, s) computes bins [y 256, y 256 + 256) of frames [x Fd, x Fd + Fd) of spectrum s,
+// Fd = spec_direct_frames(W): the frames and the table in shared memory, one bin of one frame per thread.  EXT as
+// above.
+template <bool EXT>
+__device__ __forceinline__ void spectrum_direct_stage(const SpecBlk *__restrict__ blk,
+                                                      const float2 *const *__restrict__ rings,
+                                                      const SpecExt *__restrict__ ext) {
   extern __shared__ __align__(16) float2 sm[];
   const SpecBlk b = blk[blockIdx.z];
+  const SpecExt xe = EXT ? ext[blockIdx.z] : SpecExt{nullptr, nullptr, b.W, 0};
   const float2 *__restrict__ ring = rings[blockIdx.z];
   const int W = b.W;
   if (spec_fft(W)) return;
@@ -1912,140 +1976,12 @@ spectrum_direct_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__r
   for (int i = tid; i < W; i += SPEC_THREADS) tw[i] = b.tw[i];
   for (int e = tid; e < nf * W; e += SPEC_THREADS) {
     const int f = e / W;
-    const long long pos = spec_frame(b, j0 + f).pos + (e - f * W);
-    xs[e] = ring[(unsigned)((unsigned long long)pos) & b.mask];
-  }
-  __syncthreads();
-  const int wb = min(W, SPEC_THREADS), f = tid / wb, k = k0 + tid - f * wb;
-  if (f >= nf || k >= W) return;
-  const float2 *x = xs + f * W;
-  float2 acc = make_float2(0.f, 0.f);
-  int t = 0;
-  for (int n = 0; n < W; n++) {
-    const float2 a = x[n], w = tw[t];
-    acc.x = fmaf(a.x, w.x, acc.x);
-    acc.x = fmaf(-a.y, w.y, acc.x);
-    acc.y = fmaf(a.x, w.y, acc.y);
-    acc.y = fmaf(a.y, w.x, acc.y);
-    t += k;
-    if (t >= W) t -= W;
-  }
-  atomicMax(b.hold + (size_t)spec_frame(b, j0 + f).hold_row * W + k, spec_power(acc, b.inv_w));
-}
-
-// CTA (x, s) writes values [x 256, x 256 + 256) of the n_rows x W values of the rows spectrum s completed in
-// this block, and empties what it read of the hold
-__global__ void __launch_bounds__(SPEC_THREADS) spectrum_emit_kernel(const SpecBlk *__restrict__ blk) {
-  const SpecBlk b = blk[blockIdx.y];
-  const int e = blockIdx.x * SPEC_THREADS + threadIdx.x;
-  if (e >= b.n_rows * b.W) return;
-  const int i = e / b.W, j = e - i * b.W;
-  unsigned *hold = b.hold + (size_t)((b.slot0 + i) % b.NR) * b.W + b.map[j];
-  const float v = __uint_as_float(*hold);
-  *hold = 0u;
-  b.out[e] = b.power ? v : __fmul_rn(10.f, log10f(v));
-}
-
-// ---------------------------------------------------------------------------
-// Extended spectra (xlg_add_spectrum_ex): a hop H between frame starts, a window and a mean.  Row period
-// R = (F - 1) H + W + S; row r covers the frames x[P + r R + f H ... + W), f < F.  Each frame is windowed before
-// the transform, z[n] = (x[n].x * w[n], x[n].y * w[n]) (one rounded multiply each; no window: z = x), and goes
-// through the same channel stage, spec_power and hold as above.  A max spectrum folds by atomicMax as above.  A
-// mean spectrum's channel stage stores each frame's powers (position space, as the hold) in the spectrum's frame
-// buffer, row j of it for frame j of this block; spectrum_fold_kernel then adds them into the hold in frame order,
-//     s = +0;  s = s + p_f for f = 0 .. F - 1 (rounded adds, one frame after the other, across blocks in block order)
-// and divides a completed row once, v = s / float(F) (correctly rounded).  The hold carries s between blocks as
-// float bits (the empty hold, 0, is +0).  spectrum_emit_kernel then writes and empties the row as for any spectrum.
-// The entries are the tail of the block's SpecBlk table, SpecExt holds what only they need.
-// ---------------------------------------------------------------------------
-struct SpecExt {
-  const float *win;  // W weights, or nullptr: no window
-  float *fbuf;       // mean: the frames' powers, a row of W per frame of this block; max: nullptr
-  int H;             // hop
-  int mean;
-};
-
-__device__ __forceinline__ long long spec_frame_pos(const SpecBlk &b, int H, int j) {
-  const unsigned g = b.f0 + (unsigned)j, rr = g / (unsigned)b.F, ff = g - rr * (unsigned)b.F;
-  return b.base + (long long)rr * b.R + (long long)ff * H;
-}
-
-__device__ __forceinline__ float2 spec_load(const float2 *__restrict__ ring, unsigned mask, long long pos,
-                                            const float *__restrict__ win, int n) {
-  const float2 v = ring[(unsigned)((unsigned long long)pos) & mask];
-  if (win == nullptr) return v;
-  const float w = __ldg(win + n);
-  return make_float2(__fmul_rn(v.x, w), __fmul_rn(v.y, w));
-}
-
-// spectrum_fft_kernel with the hop, the window and the mean's frame buffer
-__global__ void __launch_bounds__(SPEC_THREADS)
-spectrum_fft_ext_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__restrict__ rings,
-                        const SpecExt *__restrict__ ext) {
-  extern __shared__ __align__(16) float2 u[];
-  const SpecBlk b = blk[blockIdx.y];
-  const SpecExt x = ext[blockIdx.y];
-  const float2 *__restrict__ ring = rings[blockIdx.y];
-  if (!spec_fft(b.W)) return;
-  const int W = b.W, F = bank_fft_frames(W);
-  const int j0 = blockIdx.x * F;
-  if (j0 >= b.n_frames) return;
-  const int nf = min(F, b.n_frames - j0), tid = threadIdx.x, lw = 31 - __clz(W);
-  for (int e = tid; e < nf * W; e += SPEC_THREADS) {
-    const int n = e & (W - 1);
-    u[e] = spec_load(ring, b.mask, spec_frame_pos(b, x.H, j0 + (e >> lw)) + n, x.win, n);
-  }
-  __syncthreads();
-  fft_dif_rows<SPEC_THREADS>(u, nf, W, lw, b.tw, tid);
-  if (x.mean) {
-    float *fb = x.fbuf + (size_t)j0 * W;
-    for (int e = tid; e < nf * W; e += SPEC_THREADS) fb[e] = __uint_as_float(spec_power(u[e], b.inv_w));
-    return;
-  }
-  if (W >= SPEC_THREADS) {
-    for (int e = tid; e < nf * W; e += SPEC_THREADS) {
-      const int h = spec_frame(b, j0 + (e >> lw)).hold_row;
-      atomicMax(b.hold + (size_t)h * W + (e & (W - 1)), spec_power(u[e], b.inv_w));
+    if constexpr (EXT) {
+      const int n = e - f * W;
+      xs[e] = spec_load(ring, b.mask, spec_frame_pos(b, xe.H, j0 + f) + n, xe.win, n);
+    } else {  // (the plain kernel's own load: through spec_frame_pos and spec_load it compiles to more instructions)
+      xs[e] = ring[(unsigned)((unsigned long long)(spec_frame(b, j0 + f).pos + (e - f * W))) & b.mask];
     }
-    return;
-  }
-  unsigned *pw = reinterpret_cast<unsigned *>(u);
-  for (int e = tid; e < nf * W; e += SPEC_THREADS) pw[2 * e] = spec_power(u[e], b.inv_w);
-  __syncthreads();
-  const int runs = SPEC_THREADS / W, per = (nf + runs - 1) / runs;
-  const int q = tid & (W - 1), f0 = (tid >> lw) * per, f1 = min(nf, f0 + per);
-  int h = -1;
-  unsigned m = 0u;
-  for (int f = f0; f < f1; f++) {
-    const int hf = spec_frame(b, j0 + f).hold_row;
-    if (hf != h) {
-      if (h >= 0) atomicMax(b.hold + (size_t)h * W + q, m);
-      h = hf;
-      m = 0u;
-    }
-    m = max(m, pw[2 * ((f << lw) + q)]);
-  }
-  if (h >= 0) atomicMax(b.hold + (size_t)h * W + q, m);
-}
-
-// spectrum_direct_kernel with the hop, the window and the mean's frame buffer
-__global__ void __launch_bounds__(SPEC_THREADS)
-spectrum_direct_ext_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__restrict__ rings,
-                           const SpecExt *__restrict__ ext) {
-  extern __shared__ __align__(16) float2 sm[];
-  const SpecBlk b = blk[blockIdx.z];
-  const SpecExt xe = ext[blockIdx.z];
-  const float2 *__restrict__ ring = rings[blockIdx.z];
-  const int W = b.W;
-  if (spec_fft(W)) return;
-  const int Fd = spec_direct_frames(W), j0 = blockIdx.x * Fd, k0 = blockIdx.y * SPEC_THREADS;
-  if (j0 >= b.n_frames || k0 >= W) return;
-  const int nf = min(Fd, b.n_frames - j0), tid = threadIdx.x;
-  float2 *tw = sm, *xs = sm + W;
-  for (int i = tid; i < W; i += SPEC_THREADS) tw[i] = b.tw[i];
-  for (int e = tid; e < nf * W; e += SPEC_THREADS) {
-    const int f = e / W, n = e - f * W;
-    xs[e] = spec_load(ring, b.mask, spec_frame_pos(b, xe.H, j0 + f) + n, xe.win, n);
   }
   __syncthreads();
   const int wb = min(W, SPEC_THREADS), f = tid / wb, k = k0 + tid - f * wb;
@@ -2063,10 +1999,32 @@ spectrum_direct_ext_kernel(const SpecBlk *__restrict__ blk, const float2 *const 
     if (t >= W) t -= W;
   }
   const unsigned p = spec_power(acc, b.inv_w);
-  if (xe.mean)
+  if (EXT && xe.mean)
     xe.fbuf[(size_t)(j0 + f) * W + k] = __uint_as_float(p);
   else
     atomicMax(b.hold + (size_t)spec_frame(b, j0 + f).hold_row * W + k, p);
+}
+
+__global__ void __launch_bounds__(SPEC_THREADS)
+spectrum_fft_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__restrict__ rings) {
+  spectrum_fft_stage<false>(blk, rings, nullptr);
+}
+
+__global__ void __launch_bounds__(SPEC_THREADS)
+spectrum_direct_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__restrict__ rings) {
+  spectrum_direct_stage<false>(blk, rings, nullptr);
+}
+
+__global__ void __launch_bounds__(SPEC_THREADS)
+spectrum_fft_ext_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__restrict__ rings,
+                        const SpecExt *__restrict__ ext) {
+  spectrum_fft_stage<true>(blk, rings, ext);
+}
+
+__global__ void __launch_bounds__(SPEC_THREADS)
+spectrum_direct_ext_kernel(const SpecBlk *__restrict__ blk, const float2 *const *__restrict__ rings,
+                           const SpecExt *__restrict__ ext) {
+  spectrum_direct_stage<true>(blk, rings, ext);
 }
 
 // CTA (x, s) folds values [x 256, x 256 + 256) of the rows x W that mean spectrum s's frames of this block touch:
@@ -2131,24 +2089,42 @@ __device__ __forceinline__ void dif_bfly4(float2 &a0, float2 &a1, float2 &a2, fl
   a3 = cmul_tw(make_float2(t1.x - t3.y, t1.y + t3.x), __ldg(tw + 3 * js));
 }
 
-// pass A on the 4^NS points i + m C of a frame starting at pos: stage 1 (L = W) on columns i + r C, r < 4^(NS-1),
-// then, for NS = 2, stage 2 (L = W / 4, stride 4) on each quarter's points
+// pass A's stages, in place, on a[m] = the point i + m C (m < 4^NS) of a row of the K-point transform, tw the K-point
+// table: stage 1 (L = K) on columns i + r C, r < 4^(NS-1), then, for NS = 2, stage 2 (L = K / 4, stride 4) on each
+// quarter's points
 template <int NS>
-__device__ __forceinline__ void spec_wide_pass_a(const float2 *__restrict__ ring, unsigned mask, long long pos,
-                                                 const float *__restrict__ win, const float2 *__restrict__ tw,
-                                                 float2 *__restrict__ row, int i, int C) {
-  constexpr int M = NS == 1 ? 4 : 16, Q = M / 4;
-  float2 a[M];
-#pragma unroll
-  for (int m = 0; m < M; m++) a[m] = spec_load(ring, mask, pos + i + m * C, win, i + m * C);
+__device__ __forceinline__ void pass_a_stages(float2 (&a)[NS == 1 ? 4 : 16], const float2 *__restrict__ tw, int i,
+                                              int C) {
+  constexpr int Q = NS == 1 ? 1 : 4;
 #pragma unroll
   for (int r = 0; r < Q; r++) dif_bfly4(a[r], a[r + Q], a[r + 2 * Q], a[r + 3 * Q], tw, i + r * C);
   if (NS == 2) {
 #pragma unroll
     for (int q = 0; q < 4; q++) dif_bfly4(a[4 * q], a[4 * q + 1], a[4 * q + 2], a[4 * q + 3], tw, 4 * i);
   }
+}
+
+// pass A on the 4^NS points i + m C of a frame starting at pos (spec_load: the hop and the window)
+template <int NS>
+__device__ __forceinline__ void spec_wide_pass_a(const float2 *__restrict__ ring, unsigned mask, long long pos,
+                                                 const float *__restrict__ win, const float2 *__restrict__ tw,
+                                                 float2 *__restrict__ row, int i, int C) {
+  constexpr int M = NS == 1 ? 4 : 16;
+  float2 a[M];
+#pragma unroll
+  for (int m = 0; m < M; m++) a[m] = spec_load(ring, mask, pos + i + m * C, win, i + m * C);
+  pass_a_stages<NS>(a, tw, i, C);
 #pragma unroll
   for (int m = 0; m < M; m++) row[i + m * C] = a[m];
+}
+
+// pass B's start: the C points of a chunk at src into shared memory u, then fft_dif_rows on them with the C-point
+// table (the barriers included)
+__device__ __forceinline__ void spec_chunk_fft(float2 *u, const float2 *src, int C, int lc, const float2 *tw_c,
+                                               int tid) {
+  for (int t = tid; t < C; t += SPEC_THREADS) u[t] = src[t];
+  __syncthreads();
+  fft_dif_rows<SPEC_THREADS>(u, 1, C, lc, tw_c, tid);
 }
 
 // CTA (x, s): threads [x 256, x 256 + 256) of wide spectrum s's frames x C columns, C = spec_wide_chunk(W)
@@ -2182,9 +2158,7 @@ spectrum_wide_b_kernel(const SpecBlk *__restrict__ blk, const SpecExt *__restric
   const int j = blockIdx.x >> ls, c0 = (blockIdx.x & ((1 << ls) - 1)) * C;
   if (j >= b.n_frames) return;
   const size_t off = (size_t)j * W + c0;
-  for (int t = tid; t < C; t += SPEC_THREADS) u[t] = wd.scratch[off + t];
-  __syncthreads();
-  fft_dif_rows<SPEC_THREADS>(u, 1, C, lc, wd.tw_c, tid);
+  spec_chunk_fft(u, wd.scratch + off, C, lc, wd.tw_c, tid);
   if (x.mean) {
     for (int t = tid; t < C; t += SPEC_THREADS) x.fbuf[off + t] = __uint_as_float(spec_power(u[t], b.inv_w));
     return;
@@ -2232,19 +2206,6 @@ struct SpecCzt {
   int M;
 };
 
-// pass A's stages on a[] = the 4^NS points i + m C of an M-point row, in place (spec_wide_pass_a's butterflies)
-template <int NS>
-__device__ __forceinline__ void czt_pass_a(float2 (&a)[NS == 1 ? 4 : 16], const float2 *__restrict__ tw, int i,
-                                           int C) {
-  constexpr int Q = NS == 1 ? 1 : 4;
-#pragma unroll
-  for (int r = 0; r < Q; r++) dif_bfly4(a[r], a[r + Q], a[r + 2 * Q], a[r + 3 * Q], tw, i + r * C);
-  if (NS == 2) {
-#pragma unroll
-    for (int q = 0; q < 4; q++) dif_bfly4(a[4 * q], a[4 * q + 1], a[4 * q + 2], a[4 * q + 3], tw, 4 * i);
-  }
-}
-
 template <int NS>
 __device__ __forceinline__ void czt_load_a(const float2 *__restrict__ ring, unsigned mask, long long pos,
                                            const float *__restrict__ win, const float2 *__restrict__ chirp, int W,
@@ -2256,7 +2217,7 @@ __device__ __forceinline__ void czt_load_a(const float2 *__restrict__ ring, unsi
     const int n = i + m * C;
     a[m] = n < W ? cmul_tw(spec_load(ring, mask, pos + n, win, n), __ldg(chirp + n)) : make_float2(0.f, 0.f);
   }
-  czt_pass_a<NS>(a, tw, i, C);
+  pass_a_stages<NS>(a, tw, i, C);
 #pragma unroll
   for (int m = 0; m < NP; m++) row[i + m * C] = a[m];
 }
@@ -2267,7 +2228,7 @@ __device__ __forceinline__ void czt_inplace_a(float2 *__restrict__ row, const fl
   float2 a[NP];
 #pragma unroll
   for (int m = 0; m < NP; m++) a[m] = row[i + m * C];
-  czt_pass_a<NS>(a, tw, i, C);
+  pass_a_stages<NS>(a, tw, i, C);
 #pragma unroll
   for (int m = 0; m < NP; m++) row[i + m * C] = a[m];
 }
@@ -2321,10 +2282,7 @@ spectrum_czt_b_kernel(const SpecBlk *__restrict__ blk, const SpecCzt *__restrict
   const int M = z.M, ls = 2 * spec_wide_stages(M), C = M >> ls, lc = 31 - __clz(C), tid = threadIdx.x;
   const int j = blockIdx.x >> ls, c0 = (blockIdx.x & ((1 << ls) - 1)) * C;
   if (j >= b.n_frames) return;
-  const float2 *src = z.s1 + (size_t)j * M + c0;
-  for (int t = tid; t < C; t += SPEC_THREADS) u[t] = src[t];
-  __syncthreads();
-  fft_dif_rows<SPEC_THREADS>(u, 1, C, lc, z.tw_c, tid);
+  spec_chunk_fft(u, z.s1 + (size_t)j * M + c0, C, lc, z.tw_c, tid);
   float2 *dst = z.s2 + (size_t)j * M;
   for (int t = tid; t < C; t += SPEC_THREADS) {
     const float2 y = cmul_tw(u[t], __ldg(z.kern + c0 + t));
@@ -2344,10 +2302,7 @@ spectrum_czt_d_kernel(const SpecBlk *__restrict__ blk, const SpecExt *__restrict
   const int W = b.W, M = z.M, ls = 2 * spec_wide_stages(M), C = M >> ls, lc = 31 - __clz(C), tid = threadIdx.x;
   const int j = blockIdx.x >> ls, c0 = (blockIdx.x & ((1 << ls) - 1)) * C;
   if (j >= b.n_frames) return;
-  const float2 *src = z.s2 + (size_t)j * M + c0;
-  for (int t = tid; t < C; t += SPEC_THREADS) u[t] = src[t];
-  __syncthreads();
-  fft_dif_rows<SPEC_THREADS>(u, 1, C, lc, z.tw_c, tid);
+  spec_chunk_fft(u, z.s2 + (size_t)j * M + c0, C, lc, z.tw_c, tid);
   if (x.mean) {
     float *fb = x.fbuf + (size_t)j * W;
     for (int t = tid; t < C; t += SPEC_THREADS) {
