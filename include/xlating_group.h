@@ -242,6 +242,26 @@ int xlg_add_bank_fft(xlg_group *g, uint32_t decim1, const float *taps1, size_t t
 /* Real FP32 instructions of the butterflies of one K-point FFT bank frame (K a power of two): 28 per radix-4
  * butterfly (16 adds and 3 complex products of 4), 4 per radix-2 butterfly.  The planner costs FFT banks by it. */
 uint64_t xlg_bank_fft_flops(uint32_t K);
+/* Extension: chirp-z bank sub-bands (DESIGN.md section 5, "Chirp-z banks").  A bank of any even K = 2 * decim1
+ * up to 4096 whose channels are defined exactly as xlg_add_bank's; only the rounding differs.  A K that
+ * xlg_add_bank_fft takes is served exactly as it serves it (the same kernel and rows, stage_a_kind 8).  Every other
+ * K runs the chirp-z stage (stage_a_kind 9): each frame's polyphase sums, placed at (p + r_m) mod K as an FFT bank
+ * places them, go through Bluestein's algorithm at M = next_pow2(2K - 1) (16 to 8192) in one kernel:
+ *   1. a[n] = u[n] c[n] for n < K, a[n] = 0 for K <= n < M, c[n] = e^{-i pi (n^2 mod 2K) / K} (n^2 in 64 bits);
+ *   2. A = the M-point FFT of a (the FFT bank's transform at K = M, in position order bank_fft_pos(k, M));
+ *   3. Y = A Bh position by position, Bh the chirp-z spectrum's table at W = K (scaled by 1/M);
+ *   4. v = the same M-point FFT of conj(Y) in natural order;
+ *   5. y_k = c[k mod K] conj(v[k mod K]).
+ * c and Bh are computed in double and rounded once (xlg_bank_any_tables); the order of every rounded operation is
+ * stated in xlating_kernels.cuh ("Chirp-z banks").  Ids, xlg_add_bank_subband, xlg_remove_bank, members and
+ * xlg_reserve work as for every bank.  -EINVAL (logged, nothing changed) for decim1 or taps1_len of 0, K above
+ * 4096, fs % K != 0, or more than max(16 * K, 16384) taps; -ENOTSUP (logged) on an XLG_TRACK_STATE group.  A
+ * group with one refuses XLG_PATH_Q15 submits, as for every bank.  Its frames count in xlg_bank_fft_profile. */
+int xlg_add_bank_any(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, int *bank_id);
+/* The chirp-z bank stage's tables for K (even, at most 4096, not a power of two; else -EINVAL): *m = M, chirp =
+ * c[n] as K (re, im) float pairs and kernel = Bh as M pairs in position order, xlg_spectrum_any_tables' tables at
+ * width K.  chirp and kernel may be NULL (then only *m is set).  Needs no group and no device. */
+int xlg_bank_any_tables(uint32_t K, float *chirp, float *kernel, uint32_t *m);
 /* Extension: spectrum rows (DESIGN.md section 5, "Spectrum rows"): the reference spectrogram tool's rows
  * (src/spectrogram/spectrogram.c) of the band, served beside the clients.
  *   A spectrum of width W, frames_per_row F and skip_per_row S attached before the next submitted block, at
@@ -493,13 +513,15 @@ typedef struct {
 } xlg_bank_profile;
 int xlg_bank_profile_read(xlg_group *g, xlg_bank_profile *p, int reset);
 
-/* FFT banks (xlg_add_bank_fft), counted like xlg_profile's while profiling is enabled.  xlg_bank_profile counts
- * direct banks only. */
+/* FFT and chirp-z banks (xlg_add_bank_fft, xlg_add_bank_any), counted like xlg_profile's while profiling is
+ * enabled.  xlg_bank_profile counts direct banks only. */
 typedef struct {
-  double fft_ms;             /* the FFT bank kernel */
+  double fft_ms;             /* the FFT and chirp-z bank kernels (one span per block) */
   uint64_t fft_launches;
   uint64_t poly_macs;        /* real-by-complex MACs of the polyphase sums: sum n1 * T1 */
-  uint64_t butterfly_flops;  /* real FP32 instructions of the butterflies: sum n1 * xlg_bank_fft_flops(K) */
+  uint64_t butterfly_flops;  /* real FP32 instructions of the butterflies: sum n1 * xlg_bank_fft_flops(K); a
+                                chirp-z bank of C materialised channels n1 * (2 xlg_bank_fft_flops(M) + 4 K + 4 M
+                                + 4 C) (the two transforms, the chirp's, Bh's and the final chirp's products) */
 } xlg_bank_fft_profile;
 int xlg_bank_fft_profile_read(xlg_group *g, xlg_bank_fft_profile *p, int reset);
 

@@ -56,7 +56,7 @@ DROPIN_EXTENSION_SYMBOLS = ["create_rational_frequency_xlating_filter", "create_
 GROUP_SYMBOLS = [
     "xlg_create", "xlg_create_ex", "xlg_destroy", "xlg_add_client", "xlg_add_client_ex", "xlg_add_client_rational_ex", "xlg_remove_client", "xlg_reserve", "xlg_client_count", "xlg_submit",
     "xlg_wait", "xlg_input_consumed", "xlg_output", "xlg_read_output", "xlg_copy_output", "xlg_alloc_pinned", "xlg_free_pinned", "xlg_wait_stream", "xlg_partition_active", "xlg_timer_start",
-    "xlg_timer_stop", "xlg_profile_enable", "xlg_profile_read", "xlg_client_info", "xlg_add_client_rational", "xlg_poly_profile_read", "xlg_add_client_cascade", "xlg_add_client_cascade_rational", "xlg_cascade_info", "xlg_cascade_profile_read", "xlg_add_subband", "xlg_remove_subband", "xlg_add_client_subband", "xlg_add_client_subband_rational", "xlg_subband_info", "xlg_subband_profile_read", "xlg_add_bank", "xlg_add_bank_subband", "xlg_remove_bank", "xlg_bank_profile_read", "xlg_add_spectrum_any", "xlg_spectrum_any_tables", "xlg_dropin_stats", "xlg_dropin_stream_stats", "xlg_dropin_stream_times",
+    "xlg_timer_stop", "xlg_profile_enable", "xlg_profile_read", "xlg_client_info", "xlg_add_client_rational", "xlg_poly_profile_read", "xlg_add_client_cascade", "xlg_add_client_cascade_rational", "xlg_cascade_info", "xlg_cascade_profile_read", "xlg_add_subband", "xlg_remove_subband", "xlg_add_client_subband", "xlg_add_client_subband_rational", "xlg_subband_info", "xlg_subband_profile_read", "xlg_add_bank", "xlg_add_bank_subband", "xlg_remove_bank", "xlg_bank_profile_read", "xlg_add_spectrum_any", "xlg_spectrum_any_tables", "xlg_add_bank_any", "xlg_bank_any_tables", "xlg_dropin_stats", "xlg_dropin_stream_stats", "xlg_dropin_stream_times",
 ]
 
 
@@ -200,6 +200,10 @@ def lib() -> C.CDLL:
     L.xlg_bank_fft_profile_read.restype = C.c_int
     L.xlg_bank_fft_flops.argtypes = [u32]
     L.xlg_bank_fft_flops.restype = C.c_uint64
+    L.xlg_add_bank_any.argtypes = [vp, u32, fp, sz, C.POINTER(C.c_int)]
+    L.xlg_add_bank_any.restype = C.c_int
+    L.xlg_bank_any_tables.argtypes = [u32, fp, fp, C.POINTER(C.c_uint32)]
+    L.xlg_bank_any_tables.restype = C.c_int
     L.xlg_add_spectrum.argtypes = [vp, u32, u32, u32, u32, C.POINTER(C.c_int)]
     L.xlg_add_spectrum.restype = C.c_int
     L.xlg_add_client_spectrum.argtypes = [vp, C.c_int, u32, u32, u32, u32, C.POINTER(C.c_int)]
@@ -520,14 +524,15 @@ class Group:
             raise ValueError(code)
         return bid.value
 
-    def add_bank_fft(self, decim1: int, taps1) -> int:
+    def add_bank_fft(self, decim1: int, taps1, *, any_k: bool = False) -> int:
         """An FFT bank (xlg_add_bank_fft): add_bank's channels, cut by a K-point FFT per frame instead of a direct
-        sum per channel (K = 2 * decim1 a power of two up to 4096; bank_fft_fits bounds taps1).  Returns a bank
-        id from add_bank's id space."""
+        sum per channel (K = 2 * decim1 a power of two up to 4096; bank_fft_fits bounds taps1).  any_k=True takes
+        every even K up to 4096 (xlg_add_bank_any; bank_any_fits bounds taps1): the K above are served as without
+        it, every other K by the chirp-z stage.  Returns a bank id from add_bank's id space."""
         t1 = np.ascontiguousarray(taps1, dtype=np.float32)
         bid = C.c_int(-1)
-        code = self._L.xlg_add_bank_fft(self._h, decim1, t1.ctypes.data_as(C.POINTER(C.c_float)), len(t1),
-                                        C.byref(bid))
+        add = self._L.xlg_add_bank_any if any_k else self._L.xlg_add_bank_fft
+        code = add(self._h, decim1, t1.ctypes.data_as(C.POINTER(C.c_float)), len(t1), C.byref(bid))
         if code != 0:
             raise ValueError(code)
         return bid.value
@@ -999,6 +1004,42 @@ def bank_fft_flops(K: int) -> int:
     return int(lib().xlg_bank_fft_flops(K))
 
 
+def bank_any_fits(d1: int, t1: int) -> bool:
+    """Whether xlg_add_bank_any takes a bank on the kernel's side (fs % K is the group's check): K = 2 * d1 at
+    most 4096 and at most max(16 * K, 16384) taps, bank_fft_max_taps in csrc/xlating_kernels.cuh."""
+    K = 2 * d1
+    return d1 >= 1 and K <= 4096 and 1 <= t1 <= max(16 * K, 16384)
+
+
+def bank_any_m(K: int) -> int:
+    """M = next_pow2(2K - 1), the chirp-z bank stage's transform length."""
+    return 1 << (2 * K - 2).bit_length()
+
+
+def bank_any_flops(K: int, channels: int) -> int:
+    """Real FP32 instructions of one chirp-z bank frame's channel stage with `channels` materialised channels:
+    2 * bank_fft_flops(M) + 4 K + 4 M + 4 C (xlg_bank_fft_profile's butterfly_flops)."""
+    M = bank_any_m(K)
+    return 2 * bank_fft_flops(M) + 4 * K + 4 * M + 4 * channels
+
+
+def bank_any_tables(K: int):
+    """The chirp-z bank stage's tables for K (even, at most 4096, not a power of two), as the library builds
+    them (xlg_bank_any_tables): (chirp: complex64[K], kernel: complex64[M] in the transform's position order, M).
+    ValueError for any other K."""
+    L = lib()
+    m = C.c_uint32(0)
+    code = L.xlg_bank_any_tables(K, None, None, C.byref(m))
+    if code != 0:
+        raise ValueError(code)
+    chirp, kern = np.zeros(K, np.complex64), np.zeros(m.value, np.complex64)
+    fp = C.POINTER(C.c_float)
+    code = L.xlg_bank_any_tables(K, chirp.ctypes.data_as(fp), kern.ctypes.data_as(fp), C.byref(m))
+    if code != 0:
+        raise ValueError(code)
+    return chirp, kern, m.value
+
+
 def spectrum_any_tables(width: int):
     """The chirp-z stage's tables for `width` (above 4096, at most 65536, not a power of two), as the library
     builds them (xlg_spectrum_any_tables): (chirp: complex64[width], kernel: complex64[M] in the transform's
@@ -1033,7 +1074,7 @@ def spectrogram_pixels(rows) -> np.ndarray:
     return np.clip(np.trunc(v), 0, 255).astype(np.uint8)
 
 
-def subband_plan(fs: int, clients, bank: bool = False, fft: bool = False):
+def subband_plan(fs: int, clients, bank: bool = False, fft: bool = False, any_k: bool = False):
     """Sub-band clients for `clients`, a list of (center, rate).  For every D1 >= 2 that divides fs with
     fs1 = fs / D1 even, fs1 > 2 * max rate and every rate dividing fs1: sub-band centres fs1 / 2 apart from
     the lowest client centre up across the occupied span, each client assigned to the nearest one (so its
@@ -1057,9 +1098,15 @@ def subband_plan(fs: int, clients, bank: bool = False, fft: bool = False):
 
     fft=True (with bank=True) also considers FFT banks (Group.add_bank_fft) where bank_fft_fits: their channel
     stage costs bank_fft_flops(K) / D1 per input sample instead of 8 * C.  At each D1 the cheaper kernel is
-    taken (the direct one on a tie), and the plan carries "kernel": "direct" or "fft"."""
+    taken (the direct one on a tie), and the plan carries "kernel": "direct" or "fft".
+
+    any_k=True (with fft=True) also considers chirp-z banks (Group.add_bank_fft(..., any_k=True)) at every D1
+    whose K = 2 * D1 is not a power of two, where bank_any_fits: their channel stage costs bank_any_flops(K, C) / D1
+    per input sample, and "kernel" is "czt" where one is taken (ties keep the earlier kernel)."""
     if fft and not bank:
         raise ValueError("fft=True plans banks: it needs bank=True")
+    if any_k and not fft:
+        raise ValueError("any_k=True plans chirp-z banks: it needs fft=True")
     centers = [int(c) for c, _ in clients]
     rates = [int(r) for _, r in clients]
     rmax = max(rates)
@@ -1091,6 +1138,8 @@ def subband_plan(fs: int, clients, bank: bool = False, fft: bool = False):
                 stages = [(8.0 * len(used), "direct")] if bank_fits(d1, t1.size) else []
                 if fft and bank_fft_fits(d1, t1.size):
                     stages.append((bank_fft_flops(2 * d1) / d1, "fft"))
+                elif any_k and bank_any_fits(d1, t1.size):
+                    stages.append((bank_any_flops(2 * d1, len(used)) / d1, "czt"))
                 if not stages:
                     continue
                 stage, kernel = min(stages, key=lambda c: c[0])  # (a tie keeps the direct bank)

@@ -140,16 +140,23 @@ struct HostClient {
   int chan = 0;                  // its channel k in [-D1, D1)
 };
 
-// a channel bank (xlg_add_bank, xlg_add_bank_fft): reversed padded taps, twiddles, and the walk of an integer
-// client (D1, T1) attached at P
+// which kernel serves a bank's channel stage; also its per-block table (Slot::bkblk, bfblk, bzblk)
+enum BankKind {
+  BANK_DIRECT,  // xlg_add_bank: bank_cf32_kernel
+  BANK_FFT,     // xlg_add_bank_fft, and xlg_add_bank_any at a power-of-two K: bank_fft_cf32_kernel
+  BANK_CZT,     // xlg_add_bank_any at every other K: bank_czt_cf32_kernel
+};
+
+// a channel bank (xlg_add_bank, xlg_add_bank_fft, xlg_add_bank_any): reversed padded taps, twiddles, and the
+// walk of an integer client (D1, T1) attached at P
 struct BankHost {
   bool active = false;
-  bool fft = false;          // its channel stage: bank_fft_cf32_kernel instead of bank_cf32_kernel
+  BankKind kind = BANK_DIRECT;
   uint32_t D1 = 0;
   size_t T1 = 0;
   int K = 0, tpad = 0;
   std::vector<float> taps;   // h[T1-1-j] at j, zero to tpad
-  std::vector<float2> tw;    // e^{-2 pi i j / K}
+  std::vector<float2> tw;    // e^{-2 pi i j / K}; BANK_CZT: e^{-2 pi i j / M}, then c (K) and Bh (M)
   long long P = 0, hist = 0;
   std::vector<int> cids;     // its materialised channels' client indices (the layout's)
   int taps_off = 0, tw_off = 0, ch_off = 0;
@@ -274,7 +281,8 @@ struct Slot {
   BlkTable<BankBlk> bkblk;       // banks with channels: this block's windows, counts and channel tables
   uint64_t bk_poly = 0, bk_dft = 0;
   BlkTable<BankBlk> bfblk;       // the same for the FFT banks
-  uint64_t bf_poly = 0, bf_flops = 0;
+  BlkTable<BankBlk> bzblk;       // and for the chirp-z banks
+  uint64_t bf_poly = 0, bf_flops = 0;  // FFT and chirp-z banks
   BlkTable<SpecBlk> spblk;       // spectra with work in this block
   BlkTable<const float2 *> spring;  // the ring each spblk entry reads
   BlkTable<SpecExt> spext;       // the extended and wide entries' hop, window and frame buffer (the tail of spblk)
@@ -682,6 +690,7 @@ static void slot_free(Slot &s) {
   s.sbblk.release();
   s.bkblk.release();
   s.bfblk.release();
+  s.bzblk.release();
   s.spblk.release();
   s.spcb.release();
   s.spring.release();
@@ -1002,7 +1011,7 @@ static int bank_fft_pos(int k, int K) {
 // the channel tables of the banks that have channels, and the per-slot tables.
 static int rebuild_banks(xlg_group *g) {
   g->bank_live.clear();
-  size_t n_fft = 0;
+  size_t n_fft = 0, n_czt = 0;
   std::vector<float> taps;
   std::vector<float2> tw;
   std::vector<int2> chans;
@@ -1015,10 +1024,14 @@ static int rebuild_banks(xlg_group *g) {
     if (k.cids.empty()) continue;
     k.ch_off = (int)chans.size();
     for (int i : k.cids) {
-      const int c = g->clients[i].chan;
-      chans.push_back(make_int2(k.fft ? bank_fft_pos(c, k.K) : (c + k.K) % k.K, g->clients[i].out_off));
+      const int c = g->clients[i].chan, kk = (c + k.K) % k.K;
+      const int x = k.kind == BANK_FFT ? bank_fft_pos(c, k.K)
+                    : k.kind == BANK_CZT ? bank_fft_pos(kk, bank_czt_m(k.K)) | kk << 16  // (position, k mod K)
+                                         : kk;
+      chans.push_back(make_int2(x, g->clients[i].out_off));
     }
-    n_fft += k.fft ? 1 : 0;
+    n_fft += k.kind == BANK_FFT ? 1 : 0;
+    n_czt += k.kind == BANK_CZT ? 1 : 0;
     k.taps_off = (int)taps.size();
     taps.insert(taps.end(), k.taps.begin(), k.taps.end());
     k.tw_off = (int)tw.size();
@@ -1027,12 +1040,16 @@ static int rebuild_banks(xlg_group *g) {
   }
   if (g->bank_live.empty()) return 0;
   CU_OK(cudaFuncSetAttribute(bank_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTileMaxSmem));
+  if (n_czt > 0)
+    CU_OK(cudaFuncSetAttribute(bank_czt_cf32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)bank_czt_smem(BZ_N)));
   if (dev_assign(&g->d_bktaps, &g->cap_bktaps, taps.data(), taps.size() * sizeof(float)) ||
       dev_assign(&g->d_bktw, &g->cap_bktw, tw.data(), tw.size() * sizeof(float2)) ||
       dev_assign(&g->d_bkch, &g->cap_bkch, chans.data(), chans.size() * sizeof(int2)))
     return -EIO;
   for (Slot &s : g->slots)
-    if (s.bkblk.reserve(g->bank_live.size() - n_fft) || s.bfblk.reserve(n_fft)) return -EIO;
+    if (s.bkblk.reserve(g->bank_live.size() - n_fft - n_czt) || s.bfblk.reserve(n_fft) || s.bzblk.reserve(n_czt))
+      return -EIO;
   return 0;
 }
 
@@ -1294,7 +1311,8 @@ static int rebuild_layout(xlg_group *g) {
       continue;
     }
     if (h.bank >= 0) {
-      h.kind = g->banks[h.bank].fft ? 8 : 7;  // a bank channel: bank_cf32_kernel (8: bank_fft_cf32_kernel) writes it
+      // a bank channel: bank_cf32_kernel writes it (8: bank_fft_cf32_kernel, 9: bank_czt_cf32_kernel)
+      h.kind = g->banks[h.bank].kind == BANK_CZT ? 9 : g->banks[h.bank].kind == BANK_FFT ? 8 : 7;
       continue;
     }
     h.kind = h.L > 1 ? 3 : 0;
@@ -2397,9 +2415,13 @@ static std::vector<float2> twiddle_table(int K) {
   return tw;
 }
 
-// A bank (fft: its channel stage is bank_fft_cf32_kernel's) after the checks of its kernel
-static int add_bank(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, bool fft, int *bank_id) {
-  const char *what = fft ? "FFT bank" : "bank";
+static void czt_tables(int W, std::vector<float2> &chirp, std::vector<float2> &kern, std::vector<int> &bin);
+
+// A bank whose channel stage is `kind`'s kernel, after the checks of that kernel
+static int add_bank(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, BankKind kind,
+                    int *bank_id) {
+  const bool fft = kind != BANK_DIRECT;
+  const char *what = kind == BANK_CZT ? "chirp-z bank" : fft ? "FFT bank" : "bank";
   if (g == nullptr || bank_id == nullptr) return -EINVAL;
   if (decim1 == 0 || taps1_len == 0 || taps1 == nullptr) {
     XL_LOG("%s: decimation %u and tap count %zu must both be at least 1", what, decim1, taps1_len);
@@ -2412,12 +2434,16 @@ static int add_bank(xlg_group *g, uint32_t decim1, const float *taps1, size_t ta
   }
   if (fft) {
     const uint32_t K = 2 * decim1;
-    if ((K & (K - 1)) != 0 || K > 4096) {
+    if (kind == BANK_FFT && ((K & (K - 1)) != 0 || K > 4096)) {
       XL_LOG("FFT bank: K = 2 x decimation %u = %u is not a power of two up to 4096", decim1, K);
       return -EINVAL;
     }
+    if (K > 4096) {
+      XL_LOG("chirp-z bank: K = 2 x decimation %u = %u exceeds 4096", decim1, K);
+      return -EINVAL;
+    }
     if (taps1_len > (size_t)bank_fft_max_taps((int)K)) {
-      XL_LOG("FFT bank: %zu taps at decimation %u exceed the kernel's bound of %lld", taps1_len, decim1,
+      XL_LOG("%s: %zu taps at decimation %u exceed the kernel's bound of %lld", what, taps1_len, decim1,
              bank_fft_max_taps((int)K));
       return -EINVAL;
     }
@@ -2431,14 +2457,23 @@ static int add_bank(xlg_group *g, uint32_t decim1, const float *taps1, size_t ta
   }
   BankHost k;
   k.active = true;
-  k.fft = fft;
+  k.kind = kind;
   k.D1 = decim1;
   k.T1 = taps1_len;
   k.K = 2 * (int)decim1;
   k.tpad = bank_tpad(k.K, (int)taps1_len);
   k.taps.assign((size_t)k.tpad, 0.f);
   for (size_t j = 0; j < taps1_len; j++) k.taps[j] = taps1[taps1_len - 1 - j];
-  k.tw = twiddle_table(k.K);
+  if (kind == BANK_CZT) {  // the M-point table, then c and Bh
+    std::vector<float2> chirp, kern;
+    std::vector<int> bin;
+    czt_tables(k.K, chirp, kern, bin);
+    k.tw = twiddle_table(bank_czt_m(k.K));
+    k.tw.insert(k.tw.end(), chirp.begin(), chirp.end());
+    k.tw.insert(k.tw.end(), kern.begin(), kern.end());
+  } else {
+    k.tw = twiddle_table(k.K);
+  }
   k.P = g->S;
   k.hist = (long long)taps1_len - 1;  // a fresh filter's history: T1 - 1 samples, zero before P
   int id = 0;
@@ -2451,11 +2486,17 @@ static int add_bank(xlg_group *g, uint32_t decim1, const float *taps1, size_t ta
 }
 
 extern "C" int xlg_add_bank(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, int *bank_id) {
-  return add_bank(g, decim1, taps1, taps1_len, false, bank_id);
+  return add_bank(g, decim1, taps1, taps1_len, BANK_DIRECT, bank_id);
 }
 
 extern "C" int xlg_add_bank_fft(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, int *bank_id) {
-  return add_bank(g, decim1, taps1, taps1_len, true, bank_id);
+  return add_bank(g, decim1, taps1, taps1_len, BANK_FFT, bank_id);
+}
+
+extern "C" int xlg_add_bank_any(xlg_group *g, uint32_t decim1, const float *taps1, size_t taps1_len, int *bank_id) {
+  const uint32_t K = 2 * decim1;
+  const bool fft = decim1 <= 2048 && (K & (K - 1)) == 0;  // a K that xlg_add_bank_fft takes
+  return add_bank(g, decim1, taps1, taps1_len, fft ? BANK_FFT : BANK_CZT, bank_id);
 }
 
 extern "C" uint64_t xlg_bank_fft_flops(uint32_t K) {
@@ -2600,9 +2641,8 @@ static void czt_tables(int W, std::vector<float2> &chirp, std::vector<float2> &k
   }
 }
 
-extern "C" int xlg_spectrum_any_tables(uint32_t width, float *chirp, float *kernel, uint32_t *m) {
-  if (width <= SPEC_MAX_W || width > SPEC_WIDE_MAX_W || spec_wide((int)width)) return -EINVAL;
-  const int W = (int)width;
+// czt_tables(W) into the caller's buffers (xlg_spectrum_any_tables, xlg_bank_any_tables)
+static int czt_tables_query(int W, float *chirp, float *kernel, uint32_t *m) {
   if (m) *m = (uint32_t)czt_m(W);
   if (chirp == nullptr && kernel == nullptr) return 0;
   std::vector<float2> c, k;
@@ -2611,6 +2651,16 @@ extern "C" int xlg_spectrum_any_tables(uint32_t width, float *chirp, float *kern
   if (chirp) memcpy(chirp, c.data(), c.size() * sizeof(float2));
   if (kernel) memcpy(kernel, k.data(), k.size() * sizeof(float2));
   return 0;
+}
+
+extern "C" int xlg_spectrum_any_tables(uint32_t width, float *chirp, float *kernel, uint32_t *m) {
+  if (width <= SPEC_MAX_W || width > SPEC_WIDE_MAX_W || spec_wide((int)width)) return -EINVAL;
+  return czt_tables_query((int)width, chirp, kernel, m);
+}
+
+extern "C" int xlg_bank_any_tables(uint32_t K, float *chirp, float *kernel, uint32_t *m) {
+  if (K < 2 || K > 4096 || K % 2 != 0 || (K & (K - 1)) == 0) return -EINVAL;
+  return czt_tables_query((int)K, chirp, kernel, m);
 }
 
 // A spectrum of the band (src = -1) or of client index src's output stream, after the checks of its source.
@@ -2872,6 +2922,8 @@ struct Block {
   size_t bk_smem = 0;
   int n_bf = 0, max_bf_ctas = 0;  // FFT banks
   size_t bf_smem = 0;
+  int n_bz = 0, max_bz_ctas = 0;  // chirp-z banks
+  size_t bz_smem = 0;
   // spectrum walk: entries, row values to emit, the end of their rows in the arena; the plain entries' FFT and
   // direct paths
   int n_spec = 0, max_sp_values = 0;
@@ -2959,7 +3011,8 @@ static void walk_banks(Block &b) {
       b.ho.out_off[i] = g->clients[i].out_off;
     }
     if (k.cids.empty()) continue;
-    BankBlk &e = k.fft ? s.bfblk.h[b.n_bf++] : s.bkblk.h[b.n_bk++];
+    BankBlk &e = k.kind == BANK_CZT ? s.bzblk.h[b.n_bz++] : k.kind == BANK_FFT ? s.bfblk.h[b.n_bf++]
+                                                                              : s.bkblk.h[b.n_bk++];
     e.taps = g->d_bktaps + k.taps_off;
     e.tw = g->d_bktw + k.tw_off;
     e.chans = g->d_bkch + k.ch_off;
@@ -2973,7 +3026,15 @@ static void walk_banks(Block &b) {
     e.tpad = k.tpad;
     e.n_ch = (int)k.cids.size();
     e.r0 = (int)(((first - k.P) % k.K + k.K) % k.K);
-    if (k.fft) {
+    if (k.kind == BANK_CZT) {
+      const int M = bank_czt_m(k.K);
+      b.max_bz_ctas = std::max(b.max_bz_ctas, (n1 + bank_czt_frames(M) - 1) / bank_czt_frames(M));
+      b.bz_smem = std::max(b.bz_smem, bank_czt_smem(M));
+      s.bf_poly += (uint64_t)n1 * k.T1;
+      s.bf_flops += (uint64_t)n1 * (2 * xlg_bank_fft_flops((uint32_t)M) + 4ull * k.K + 4ull * M + 4ull * e.n_ch);
+      continue;
+    }
+    if (k.kind == BANK_FFT) {
       b.max_bf_ctas = std::max(b.max_bf_ctas, (n1 + bank_fft_frames(k.K) - 1) / bank_fft_frames(k.K));
       b.bf_smem = std::max(b.bf_smem, bank_fft_smem(k.K));
       s.bf_poly += (uint64_t)n1 * k.T1;
@@ -3230,7 +3291,7 @@ static int stage_and_convert(Block &b, int fmt, const void *input, uint32_t flag
 }
 
 // Banks: after the conversions the FIR kernels wait for, not after the pre-pass (they have no oscillator); the
-// direct banks, then the FFT banks
+// direct banks, then the FFT and chirp-z banks in one span
 static int launch_banks(Block &b) {
   xlg_group *g = b.g;
   Slot &s = b.s;
@@ -3241,10 +3302,17 @@ static int launch_banks(Block &b) {
         s.bkblk.d, g->ring, s.d_out);
     if (span_end(g, s, SP_BANK, b.cs)) return -EIO;
   }
-  if (b.n_bf == 0 || b.max_bf_ctas <= 0) return 0;
+  const bool bf = b.n_bf > 0 && b.max_bf_ctas > 0, bz = b.n_bz > 0 && b.max_bz_ctas > 0;
+  if (!bf && !bz) return 0;
   if (span_begin(g, s, SP_BANK_FFT, b.cs)) return -EIO;
-  CU_OK(s.bfblk.upload((size_t)b.n_bf, b.cs));
-  bank_fft_cf32_kernel<<<dim3(b.max_bf_ctas, b.n_bf), BF_THREADS, b.bf_smem, b.cs>>>(s.bfblk.d, g->ring, s.d_out);
+  if (bf) {
+    CU_OK(s.bfblk.upload((size_t)b.n_bf, b.cs));
+    bank_fft_cf32_kernel<<<dim3(b.max_bf_ctas, b.n_bf), BF_THREADS, b.bf_smem, b.cs>>>(s.bfblk.d, g->ring, s.d_out);
+  }
+  if (bz) {
+    CU_OK(s.bzblk.upload((size_t)b.n_bz, b.cs));
+    bank_czt_cf32_kernel<<<dim3(b.max_bz_ctas, b.n_bz), BZ_THREADS, b.bz_smem, b.cs>>>(s.bzblk.d, g->ring, s.d_out);
+  }
   return span_end(g, s, SP_BANK_FFT, b.cs);
 }
 

@@ -1742,6 +1742,22 @@ __device__ __forceinline__ void fft_dif_rows(float2 *u, int nf, int K, int lk, c
   }
 }
 
+// Phase p's polyphase sum of the frame whose window starts at stream position w: two fmaf chains from +0 over
+// the taps j = p, p + K, ... below T1, the window's samples before the attach point read as zero (taps and ring
+// through the L1: T1 is too long to stage)
+__device__ __forceinline__ float2 bank_phase_sum(const BankBlk &b, const float2 *__restrict__ ring, long long w,
+                                                 int p) {
+  float2 acc = make_float2(0.f, 0.f);
+  for (int j = p; j < b.T1; j += b.K) {
+    const long long pos = w + j;
+    const float2 xv = pos < b.zb ? make_float2(0.f, 0.f) : ring[(unsigned)((unsigned long long)pos) & b.mask];
+    const float hv = __ldg(b.taps + j);
+    acc.x = fmaf(xv.x, hv, acc.x);
+    acc.y = fmaf(xv.y, hv, acc.y);
+  }
+  return acc;
+}
+
 // CTA (x, b) computes frames [x F, x F + F) of bank b, F = bank_fft_frames(K): the rotated sums of each frame in
 // a row of K in shared memory (taps and window read through the L1: T1 is too long to stage), the FFT of every
 // row, then the materialised channels' samples, a channel's frames consecutively.  chans[c].x is the channel's
@@ -1753,19 +1769,11 @@ bank_fft_cf32_kernel(const BankBlk *__restrict__ blk, const float2 *__restrict__
   const int K = b.K, F = bank_fft_frames(K);
   const int f0 = blockIdx.x * F;
   if (f0 >= b.n1) return;
-  const int nf = min(F, b.n1 - f0), T1 = b.T1, tid = threadIdx.x;
+  const int nf = min(F, b.n1 - f0), tid = threadIdx.x;
   const int lk = 31 - __clz(K);
   for (int e = tid; e < nf * K; e += BF_THREADS) {
     const int f = e >> lk, p = e & (K - 1);
-    const long long w = b.first + (long long)(f0 + f) * b.D1;
-    float2 acc = make_float2(0.f, 0.f);
-    for (int j = p; j < T1; j += K) {
-      const long long pos = w + j;
-      const float2 xv = pos < b.zb ? make_float2(0.f, 0.f) : ring[(unsigned)((unsigned long long)pos) & b.mask];
-      const float hv = __ldg(b.taps + j);
-      acc.x = fmaf(xv.x, hv, acc.x);
-      acc.y = fmaf(xv.y, hv, acc.y);
-    }
+    const float2 acc = bank_phase_sum(b, ring, b.first + (long long)(f0 + f) * b.D1, p);
     const int r = (int)(((long long)b.r0 + (long long)(f0 + f) * b.D1) & (K - 1));
     u[(f << lk) + ((p + r) & (K - 1))] = acc;
   }
@@ -1776,6 +1784,91 @@ bank_fft_cf32_kernel(const BankBlk *__restrict__ blk, const float2 *__restrict__
     if (f >= nf) continue;
     const int2 ch = b.chans[c];
     out[ch.y + f0 + f] = u[(f << lk) + ch.x];
+  }
+}
+
+// ---------------------------------------------------------------------------
+// Chirp-z banks (xlg_add_bank_any, K = 2 * D1 even, at most 4096 and not a power of two).  The channels are the
+// bank's above; the channel stage is the K-point DFT of the FFT bank's placed sums u (u[(p + r_m) mod K] = v[m][p],
+// r_m = (s_m - P) mod K in 64 bits, taken with %), computed by Bluestein's identity kn = (k^2 + n^2 - (k - n)^2) / 2
+// as a circular convolution of length M = next_pow2(2K - 1) (16 to 8192).  With c[n] = e^{-i pi (n^2 mod 2K) / K}
+// (period K: K is even) and Bh the chirp-z spectrum's table at W = K (the M-point DFT of conj(c[|m|]), |m| < K,
+// wrapped mod M, times 1/M, in position order), in this order (cmul_tw for every complex product):
+//   a[n] = cmul_tw(u[n], c[n]) for n < K, +0 for K <= n < M
+//   A    = fft_dif_rows' M-point transform of a, in position order
+//   Y[p] = cmul_tw(A[p], Bh[p]);  y[bin(p)] = (Y[p].x, -Y[p].y)   (conj(Y) in natural order; bin = fft_bin)
+//   v    = the same M-point transform of y, in position order
+//   y_k  = cmul_tw((v[q].x, -v[q].y), c[k mod K]),  q = bank_fft_pos(k mod K, M)
+// All tables are built in double on the host and rounded once (czt_tables in xlating_group.cu).  FP32
+// instructions per frame: 2 xlg_bank_fft_flops(M) + 4 K + 4 M + 4 C for C materialised channels.
+// ---------------------------------------------------------------------------
+constexpr int BZ_THREADS = 256;
+constexpr int BZ_N = 8192;                // points per CTA: BZ_N / M frames, one frame at M = 8192
+constexpr int BZ_ST = BZ_N / BZ_THREADS;  // float2 a thread holds while conj(Y) moves to natural order
+__host__ __device__ constexpr int bank_czt_m(int K) {  // next_pow2(2K - 1)
+  int m = 1;
+  while (m < 2 * K - 1) m <<= 1;
+  return m;
+}
+__host__ __device__ constexpr int bank_czt_frames(int M) { return BZ_N / M; }
+__host__ __device__ constexpr size_t bank_czt_smem(int M) { return (size_t)bank_czt_frames(M) * M * 8; }
+
+// the bin whose transform output lies at position p of a row of M = 2^lm: bank_fft_pos's inverse (the base-4
+// digits of p, most significant first, are the bin's from the least significant, then the radix-2 stage's bit)
+__device__ __forceinline__ int fft_bin(int p, int lm) {
+  int k = 0, sh = 0, l = lm;
+  for (; l >= 2; l -= 2, sh += 2) k |= ((p >> (l - 2)) & 3) << sh;
+  return l == 1 ? k | ((p & 1) << sh) : k;
+}
+
+// CTA (x, b) computes frames [x F, x F + F) of chirp-z bank b, F = bank_czt_frames(M), each in a row of M in
+// shared memory.  b.tw holds the M-point table, then c (K) and Bh (M); chans[c].x is the channel's position in
+// the second transform's row in its low 16 bits and k mod K above them.  conj(Y) reaches natural order through
+// registers: each thread holds its BZ_ST points across a barrier, then stores them at their bins.
+__global__ void __launch_bounds__(BZ_THREADS, 2)
+bank_czt_cf32_kernel(const BankBlk *__restrict__ blk, const float2 *__restrict__ ring, float2 *__restrict__ out) {
+  extern __shared__ __align__(16) float2 u[];
+  const BankBlk b = blk[blockIdx.y];
+  const int K = b.K, M = bank_czt_m(K), F = bank_czt_frames(M);
+  const int f0 = blockIdx.x * F;
+  if (f0 >= b.n1) return;
+  const int nf = min(F, b.n1 - f0), tid = threadIdx.x, lm = 31 - __clz(M);
+  const float2 *chirp = b.tw + M, *kern = chirp + K;
+  for (int e = tid; e < nf * M; e += BZ_THREADS) {
+    const int f = e >> lm, n = e & (M - 1);
+    if (n >= K) {
+      u[e] = make_float2(0.f, 0.f);
+      continue;
+    }
+    const int r = (int)(((long long)b.r0 + (long long)(f0 + f) * b.D1) % K);
+    const int p = n >= r ? n - r : n - r + K;  // the phase placed at n
+    u[e] = cmul_tw(bank_phase_sum(b, ring, b.first + (long long)(f0 + f) * b.D1, p), __ldg(chirp + n));
+  }
+  __syncthreads();
+  fft_dif_rows<BZ_THREADS>(u, nf, M, lm, b.tw, tid);
+  float2 st[BZ_ST];
+#pragma unroll
+  for (int i = 0; i < BZ_ST; i++) {
+    const int e = tid + i * BZ_THREADS;
+    if (e < nf * M) {
+      const float2 y = cmul_tw(u[e], __ldg(kern + (e & (M - 1))));
+      st[i] = make_float2(y.x, -y.y);
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < BZ_ST; i++) {
+    const int e = tid + i * BZ_THREADS;
+    if (e < nf * M) u[(e & ~(M - 1)) + fft_bin(e & (M - 1), lm)] = st[i];
+  }
+  __syncthreads();
+  fft_dif_rows<BZ_THREADS>(u, nf, M, lm, b.tw, tid);
+  for (int e = tid; e < b.n_ch * F; e += BZ_THREADS) {
+    const int c = e / F, f = e - c * F;
+    if (f >= nf) continue;
+    const int2 ch = b.chans[c];
+    const float2 v = u[(f << lm) + (ch.x & 0xffff)];
+    out[ch.y + f0 + f] = cmul_tw(make_float2(v.x, -v.y), __ldg(chirp + (ch.x >> 16)));
   }
 }
 

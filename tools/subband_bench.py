@@ -15,7 +15,8 @@ Plans, alternated within every round: "single" (one client each: client_plan's t
 rational_plan's as a rational client where the rate does not divide fs), "cascade" (cascade_plan) and
 "subband" (subband_plan; at the last three rates its members resample by a rational L2 / M2), "bank"
 (subband_plan(bank=True): the same kind of members on the channels of one bank) and "bank_fft"
-(subband_plan(bank=True, fft=True): the same with a direct or an FFT bank, whichever the planner costs lower).
+(subband_plan(bank=True, fft=True): the same with a direct or an FFT bank, whichever the planner costs lower)
+and "bank_any" (subband_plan(bank=True, fft=True, any_k=True): chirp-z banks of any even K are candidates too).
 
 Per workload and plan (one JSON line each): input MS/s and step time over K pipelined blocks (CUDA events,
 xlg_timer_*), algorithmic real FMAs per input sample from the shapes, and from a profiled run of its own (one
@@ -49,7 +50,7 @@ WORKLOADS = {  # fs, format, clients, rates
     "10M_256": (10000000, "cs16", 256, (48000,)),
     "20M_256": (20000000, "cs8", 256, (48000,)),
 }
-PLANS = ("single", "cascade", "subband", "bank", "bank_fft")
+PLANS = ("single", "cascade", "subband", "bank", "bank_fft", "bank_any")
 SAMPLED = 3
 
 
@@ -104,13 +105,14 @@ def build(name, plan, profile):
                  if p["interp2"] > 1 else cascade_oracle(p["d1"], p["taps1"], c, p["d2"], p["taps2"], fs, BLOCK))
             oracles.append((ids[k], lambda x, o=o: o.process_cf32(fmt, x)))
     else:
-        banked = plan in ("bank", "bank_fft")
-        p = (pkg.subband_plan(fs, clients, bank=True, fft=True) if plan == "bank_fft" else
-             pkg.subband_plan(fs, clients, bank=banked))
+        banked = plan in ("bank", "bank_fft", "bank_any")
+        p = (pkg.subband_plan(fs, clients, bank=True, fft=True, any_k=plan == "bank_any")
+             if plan in ("bank_fft", "bank_any") else pkg.subband_plan(fs, clients, bank=banked))
         shape = {"d1": p["d1"], "subbands": len(p["subbands"]), "kernel": p.get("kernel")}
         if banked:
-            add = g.add_bank_fft if p.get("kernel") == "fft" else g.add_bank
-            bid = add(p["d1"], p["taps1"])
+            kernel = p.get("kernel")
+            bid = (g.add_bank_fft(p["d1"], p["taps1"], any_k=kernel == "czt") if kernel in ("fft", "czt") else
+                   g.add_bank(p["d1"], p["taps1"]))
             sids = [g.add_bank_subband(bid, sb["channel"]) for sb in p["subbands"]]
         else:
             sids = [g.add_subband(p["d1"], p["taps1"], sb["center"]) for sb in p["subbands"]]
